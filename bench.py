@@ -14,7 +14,7 @@ A "step" = one pass of the hot path over a batch of `--tiles` synthetic rectifie
            per path = 192 B per left-reference voxel for the two views) / its CUDA-event duration.
 `cpu_baseline`: the reference's own `mgm` binary (oracle/_ref, built from the reference sources)
            on a bounded sample of the same workload, on this box's host cores.
-`outputs_verified`: every output tile of the last timed step (8 tiles in flight) and of the last end-to-end step is
+`outputs_verified`: every output tile of the last timed step (--slots tiles in flight) and of the last end-to-end step is
            compared bit for bit with a serial re-run of the same tile.
 `extra_configs`: the other BASELINE.json configurations and the rest of the hot path, each with value / e2e / roofline /
            cpu_baseline: C3 (`mgm_multi`, 256 labels), C4 (a FIXED queue of 256 tiles 1026x1026x192 pulled dynamically by
@@ -49,7 +49,8 @@ def parse():
     ap.add_argument("--size", type=int, default=1024)
     ap.add_argument("--dmin", type=int, default=-64)
     ap.add_argument("--dmax", type=int, default=63)
-    ap.add_argument("--slots", type=int, default=8, help="tiles in flight per GPU (one 8.5 GiB workspace each at the default shape)")
+    ap.add_argument("--slots", type=int, default=4, help="tiles in flight per GPU (one 8.5 GiB workspace each at the default shape; "
+                    "4 leave room on an 80 GB H100 for the wider workspaces of the extra configurations)")
     ap.add_argument("--cpu-procs", type=int, default=0, help="concurrent reference processes (0 = calibrate: all host cores, 1/2, 1/4)")
     ap.add_argument("--cpu-rows", type=int, default=32, help="rows of the CPU sample strips")
     ap.add_argument("--no-cpu", action="store_true")
@@ -58,7 +59,36 @@ def parse():
     ap.add_argument("--nan-border", type=float, default=0.0,
                     help="fraction of the tile width turned into no-data strips (0 = the BASELINE workload; > 0 exercises the "
                          "no-data sentinel range, which can widen the right view's slab: DESIGN.md, limits)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed (disparity, confidence, mask of every "
+                         "tile; a fixed, seeded pixel sample when the whole would exceed 64 MB) as DIR/<name>.npy in float32, all finite: "
+                         "the disparity's rejected (NaN) pixels are written as 0 and flagged 0 in DIR/disp_valid.npy")
     return ap.parse_args()
+
+
+DUMP_BYTES = 56 * 2 ** 20    # the arrays written by --dump-outputs stay below 64 MB in all
+
+
+def dump_outputs(path, arrays, with_nan=()):
+    """arrays: {name: [per-tile (H, W) tensors]} -> DIR/<name>.npy, float32 [tiles, n].  n = every pixel when that fits in
+    DUMP_BYTES, else the same seeded sample of n pixel indices in every tile (also written, as sample_index.npy).
+    Every written value is finite: the arrays named in with_nan (the disparity marks rejected pixels with NaN) are written
+    with 0 at their non-finite pixels, and DIR/<name>_valid.npy holds 1 where the value is finite, 0 where it is not."""
+    os.makedirs(path, exist_ok=True)
+    tiles = len(next(iter(arrays.values())))
+    npix = next(iter(arrays.values()))[0].numel()
+    n = min(npix, DUMP_BYTES // (4 * tiles * (len(arrays) + len(with_nan)) + 8))
+    idx = np.arange(npix) if n == npix else np.sort(np.random.default_rng(0).choice(npix, n, replace=False))
+    np.save(os.path.join(path, "sample_index.npy"), idx.astype(np.float64))
+    for name, ts in arrays.items():
+        out = np.stack([t.reshape(-1).cpu().numpy()[idx] for t in ts]).astype(np.float32)
+        valid = np.isfinite(out)
+        if name in with_nan:
+            np.save(os.path.join(path, name + "_valid.npy"), valid.astype(np.float32))
+            out = np.where(valid, out, np.float32(0))
+        elif not valid.all():
+            raise ValueError("--dump-outputs: %s holds %d non-finite values" % (name, int((~valid).sum())))
+        np.save(os.path.join(path, name + ".npy"), out)
 
 
 def config(a, world):
@@ -70,7 +100,7 @@ def config(a, world):
         "tile": [a.size, a.size], "dmin": a.dmin, "dmax": a.dmax, "labels": a.dmax - a.dmin + 1,
         "tiles_per_gpu_per_step": a.tiles, "tiles_in_flight": a.slots, "parallelism": "tile-shard x%d" % world,
         "nan_border": a.nan_border,
-        "l2": "per-tile working set %.1f GiB (8 float path volumes per view) >> 126 MB L2; inputs differ per tile" % (
+        "l2": "per-tile working set %.1f GiB (8 float path volumes per view) >> 50 MB L2; inputs differ per tile" % (
             2 * 8 * 4.0 * a.size * a.size * (32 * ((a.dmax - a.dmin + 32) // 32)) / 2 ** 30 * 1.0625),
     }
 
@@ -292,6 +322,8 @@ def run_ours(a, rank, world, local_rank):
     tw1 = time.perf_counter()
     launches = eng.kernel_launches() - l0
     ms = max_over_ranks(e0.elapsed_time(e1))
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, {"disp": d_disp, "conf": d_conf, "mask": d_mask}, with_nan=("disp",))
     # stage durations of the LAST tile of each workspace while the tiles overlap (diagnostic: how much the
     # memory-bound WTA stretches when it shares the SMs with the next tile's aggregation)
     overlapped = {}
@@ -369,22 +401,12 @@ def run_ours(a, rank, world, local_rank):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except (OSError, ValueError):
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", 3350.0))
     achieved = alg_bytes / (agg * 1e-3) / 1e9
-    traffic, traffic_src = None, "not captured for this shape"
-    if (W, H, D) == (1024, 1024, 128):      # the committed ncu capture is of this configuration
-        try:
-            tj = json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))["aggregate_kernel"]
-            traffic = float(tj["bytes"])
-            traffic_src = "profiles/traffic.json: %s" % tj.get("source", tj.get("capture", "ncu dram__bytes_read + dram__bytes_write per launch"))
-        except (OSError, ValueError, KeyError):
-            traffic = None
     roofline = {"bound": "hbm", "kernel": "aggregate_kernel (8 passes x 2 views, one persistent launch)",
                 "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                "peak_source": "MEASURED_PEAKS.json hbm_gbs (measured)" if "hbm_gbs" in peaks else "fallback 6650 GB/s",
-                "traffic": traffic, "traffic_source": traffic_src,
-                "frac_of_peak_on_real_traffic": (traffic / (agg * 1e-3) / 1e9 / peak) if traffic else None,
-                "algorithmic_bytes_per_launch": alg_bytes, "kernel_ms": agg,
+                "peak_source": "MEASURED_PEAKS.json hbm_gbs (measured)" if "hbm_gbs" in peaks else "H100 SXM data sheet, 3350 GB/s",
+                "traffic": None, "algorithmic_bytes_per_launch": alg_bytes, "kernel_ms": agg,
                 "tile_ms_serial": float(np.mean(tot_ms[1:])), "stage_ms": stage,
                 "stage_ms_overlapped": overlapped, "how": "serial single-tile launches after the timed region, CUDA events recorded by the library on the launching stream"}
 
@@ -392,6 +414,13 @@ def run_ours(a, rank, world, local_rank):
     if sampler:
         clocks = sampler.window(tw0, tw1)
         sampler.stop()
+        clocks["device"] = torch.cuda.get_device_name(dev)
+        try:       # an absolute rate means little without the power limit the card ran under
+            clocks["power_limit_w"] = float(subprocess.run(
+                ["nvidia-smi", "-i", str(local_rank), "--query-gpu=power.limit", "--format=csv,noheader,nounits"],
+                capture_output=True, text=True, timeout=30).stdout.strip())
+        except (OSError, ValueError, subprocess.SubprocessError):
+            clocks["power_limit_w"] = None
 
     # ---- CPU baseline beside it (rank 0, N=1 only): the reference binary on a bounded sample
     cpu = None

@@ -1,4 +1,4 @@
-/* s2pb200.h -- C ABI of the B200-native stereo engine that drops in behind s2p.
+/* s2pb200.h -- C ABI of the H100-native stereo engine that drops in behind s2p.
  *
  * Plain C, plain pointers and sizes, no torch / numpy types.  The library
  * (s2p_b200/libs2pb200.so, sources in s2p_b200/csrc/) is loaded with
@@ -6,7 +6,7 @@
  * (s2p/triangulation.py:18-20, s2p/sift.py:25-26).  INTEGRATION.md shows the
  * binding a maintainer of the reference would add.
  *
- * What each entry point replaces in the reference (paths under /root/reference):
+ * What each entry point replaces in the reference (paths relative to the root of the s2p sources):
  *
  *   s2pb_mgm()           the `mgm` / `mgm_multi` subprocess + the three
  *                        plambda/backflow subprocesses of create_rejection_mask

@@ -14,6 +14,8 @@ Only tests/, ``__graft_entry__.smoke()`` and ``bench.py``'s cpu_baseline /
 never does.
 """
 import ctypes
+import hashlib
+import json
 import os
 import subprocess
 import tempfile
@@ -348,3 +350,155 @@ def ref_disp_to_lonlatalt(disp, mask_rect, mask_orig, H1, H2, rpc1, rpc2, img_bb
 
 def have_ref_triangulation():
     return os.path.exists(os.path.join(REF_DIR, "libdisp_to_h_ref.so"))
+
+
+# ---------------------------------------------------------------- recorded outputs of the reference programs
+#
+# Where oracle/_ref is built, the reference programs run live.  Elsewhere (oracle/_ref needs the reference's sources) the
+# comparisons use what those programs produced when their outputs were recorded, keyed by a digest of the program, its
+# arguments and its inputs:
+#   tests/golden/ref_outputs.json   per call, a digest of every output (the bit-exact comparisons)
+#   tests/golden/ref_samples.npz    per call and output, the NaN mask and the values on a fixed, seeded sample of pixels (the
+#                                   comparisons with a tolerance)
+# S2PB_RECORD_REF=1 with oracle/_ref built rewrites the entries of the calls that run.
+
+GOLDEN = os.path.join(os.path.dirname(HERE), "tests", "golden")
+RECORDED = os.path.join(GOLDEN, "ref_outputs.json")
+RECORDED_SAMPLES = os.path.join(GOLDEN, "ref_samples.npz")
+SAMPLE = 512
+_recorded_db = None
+
+
+def digest(a):
+    """Digest of an array's values with every NaN alike and -0 == +0: equal digests <=> tests/util.same."""
+    a = np.ascontiguousarray(a)
+    if a.dtype.kind == "f":
+        a = np.where(np.isnan(a), np.nan, a + a.dtype.type(0)).astype(a.dtype)
+    return hashlib.sha256(("%s%s" % (a.dtype.str, a.shape)).encode() + a.tobytes()).hexdigest()[:32]
+
+
+def call_key(program, args, inputs):
+    h = hashlib.sha256(repr((program, args)).encode())
+    for x in inputs:
+        h.update(digest(x).encode())
+    return "%s:%s" % (program, h.hexdigest()[:24])
+
+
+def params_tuple(params):
+    return tuple(getattr(params, f) for f, _ in params._fields_)
+
+
+def _db():
+    global _recorded_db
+    if _recorded_db is None:
+        exact = json.load(open(RECORDED)) if os.path.exists(RECORDED) else {}
+        samples = dict(np.load(RECORDED_SAMPLES)) if os.path.exists(RECORDED_SAMPLES) else {}
+        _recorded_db = (exact, samples)
+    return _recorded_db
+
+
+def _missing(key):
+    return LookupError("no recorded output of the reference for %s (record it where oracle/_ref is built: S2PB_RECORD_REF=1)" % key)
+
+
+def recorded(key, live):
+    """live: a callable running the reference -> {name: array}, or None when the program is not built.
+    -> {name: digest} (compare with digest(ours))."""
+    exact, _ = _db()
+    if live is None:
+        if key not in exact:
+            raise _missing(key)
+        return exact[key]
+    out = {k: digest(v) for k, v in live().items()}
+    if os.environ.get("S2PB_RECORD_REF") == "1":
+        exact[key] = out
+        merged = json.load(open(RECORDED)) if os.path.exists(RECORDED) else {}     # (other processes may have recorded too)
+        merged[key] = out
+        with open(RECORDED, "w") as f:
+            json.dump(merged, f, indent=0, sort_keys=True)
+    return out
+
+
+class Sampled:
+    """A reference output kept as its NaN mask and its values on a fixed sample of pixels (all pixels when run live)."""
+
+    def __init__(self, shape, nan, idx, val):
+        self.shape, self.nan, self.idx, self.val = tuple(shape), nan, idx, val
+
+    def values_of(self, ours):
+        """ours, flattened over the pixels (a trailing axis of another shape is kept), at the sampled pixels"""
+        ours = np.asarray(ours)
+        npix = int(np.prod(self.nan.shape))
+        return ours.reshape(npix, -1)[self.idx].reshape((len(self.idx),) + ours.shape[self.nan.ndim:])
+
+
+def recorded_sampled(key, live):
+    """As recorded(), for the comparisons with a tolerance: -> {name: Sampled}.  The NaN mask is over the first two axes."""
+    _, samples = _db()
+    if live is not None:
+        out = {}
+        for k, v in live().items():
+            v = np.asarray(v)
+            nan = np.isnan(v) if v.ndim == 2 else np.isnan(v).any(axis=tuple(range(2, v.ndim)))
+            npix = nan.size
+            out[k] = Sampled(v.shape, nan, np.arange(npix), v.reshape((npix,) + v.shape[2:]))
+            if os.environ.get("S2PB_RECORD_REF") == "1":
+                idx = np.sort(np.random.default_rng(0).choice(npix, min(SAMPLE, npix), replace=False))
+                samples["%s/%s/shape" % (key, k)] = np.array(v.shape)
+                samples["%s/%s/nan" % (key, k)] = np.packbits(nan.ravel())
+                samples["%s/%s/idx" % (key, k)] = idx
+                samples["%s/%s/val" % (key, k)] = v.reshape((npix,) + v.shape[2:])[idx]
+        if os.environ.get("S2PB_RECORD_REF") == "1":
+            np.savez_compressed(RECORDED_SAMPLES, **samples)
+        return out
+    names = sorted({n.split("/")[-2] for n in samples if n.startswith(key + "/")})
+    if not names:
+        raise _missing(key)
+    out = {}
+    for k in names:
+        g = lambda f: samples["%s/%s/%s" % (key, k, f)]
+        shape = tuple(int(s) for s in g("shape"))
+        nan = np.unpackbits(g("nan"))[:shape[0] * shape[1]].reshape(shape[:2]).astype(bool)
+        out[k] = Sampled(shape, nan, g("idx"), g("val"))
+    return out
+
+
+def ref_mgm_outputs(im1, im2, dmin, dmax, params, wl=None, wr=None, want_pkr=False, binary=None):
+    """run_ref at OMP_NUM_THREADS=1, live or recorded -> {disp, conf, dispR[, pkrL, pkrR]: digest}"""
+    binary = binary or ("mgm" if params.scales < 0 else "mgm_multi")
+    ins = [im1, im2] + ([wl, wr] if wl is not None else [])
+    key = call_key(binary, (int(dmin), int(dmax), params_tuple(params), want_pkr), ins)
+    names = ("disp", "conf", "dispR") + (("pkrL", "pkrR") if want_pkr else ())
+    live = None
+    if os.access(os.path.join(REF_DIR, binary), os.X_OK):
+        def live():
+            r = run_ref(im1, im2, dmin, dmax, params, threads=1, binary=binary, wl=wl, wr=wr, want_pkr=want_pkr)
+            return {k: r[k] for k in names}
+    return recorded(key, live)
+
+
+def ref_homography_sampled(src, H, w, h):
+    """run_ref_homography, live or recorded -> Sampled"""
+    key = call_key("homography", (tuple(np.asarray(H, np.float64).ravel().tolist()), int(w), int(h)), [src])
+    return recorded_sampled(key, (lambda: {"out": run_ref_homography(src, H, w, h)}) if have_ref_homography() else None)["out"]
+
+
+def ref_disp_to_lonlatalt_sampled(disp, mask_rect, mask_orig, H1, H2, rpc1, rpc2, img_bbx):
+    """ref_disp_to_lonlatalt, live or recorded -> (Sampled lon/lat/alt, Sampled reprojection error)"""
+    rpcs = tuple(bytes(r).hex() for r in (rpc1, rpc2))
+    args = (tuple(np.asarray(H1, np.float64).ravel().tolist()), tuple(np.asarray(H2, np.float64).ravel().tolist()), rpcs,
+            tuple(float(x) for x in img_bbx))
+    key = call_key("disp_to_lonlatalt", args, [disp, mask_rect, mask_orig])
+    live = None
+    if have_ref_triangulation():
+        def live():
+            out, err = ref_disp_to_lonlatalt(disp, mask_rect, mask_orig, H1, H2, rpc1, rpc2, img_bbx)
+            return {"lonlatalt": out, "err": err}
+    r = recorded_sampled(key, live)
+    return r["lonlatalt"], r["err"]
+
+
+def ref_rejection_mask_output(disp, im1, im2):
+    """ref_rejection_mask, live or recorded -> digest of the mask"""
+    key = call_key("plambda+backflow", (), [disp, im1, im2])
+    return recorded(key, (lambda: {"mask": ref_rejection_mask(disp, im1, im2)}) if have_ref_mask() else None)["mask"]

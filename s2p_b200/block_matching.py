@@ -1,7 +1,7 @@
 """Drop-in for ``s2p.block_matching`` (boundary #1 of SURVEY.md section 8b).
 
 ``compute_disparity_map`` keeps the reference's signature, file contract and exceptions
-(s2p/block_matching.py:35-336) but, for ``algo in {'mgm', 'mgm_multi', 'mgm_multi_lsd'}``, runs the B200 engine
+(s2p/block_matching.py:35-336) but, for ``algo in {'mgm', 'mgm_multi', 'mgm_multi_lsd'}``, runs the H100 engine
 through the C ABI instead of spawning the ``mgm`` / ``mgm_multi`` binaries and the three
 ``plambda`` / ``backflow`` processes of ``create_rejection_mask``.  Any other ``algo`` is handed to
 the original s2p implementation when that package is importable.
@@ -112,7 +112,7 @@ def compute_disparity_map(im1, im2, disp, mask, algo, disp_min=None, disp_max=No
     if algo not in _NATIVE:
         fn = _original_compute_disparity_map()
         if fn is None:
-            raise NotImplementedError("algo %r is not served by the B200 engine and the s2p package "
+            raise NotImplementedError("algo %r is not served by the H100 engine and the s2p package "
                                       "is not importable to fall through to" % algo)
         return fn(im1, im2, disp, mask, algo, disp_min, disp_max, timeout, max_disp_range, extra_params)
 

@@ -3,7 +3,7 @@
 ``rectification.rectify_pair`` (s2p/rectification.py:281-382) is host algebra on 3x3 matrices and at most a
 few hundred points; its only heavy work is the two calls ``common.image_apply_homography(out, im, H, w, h)``
 (:379-380), each of which spawns the ``homography`` binary (s2p/common.py:159-180).  This module keeps that
-function's signature and file contract and runs the B200 warp instead.  ``install()`` swaps it into an
+function's signature and file contract and runs the H100 warp instead.  ``install()`` swaps it into an
 importable ``s2p`` so that ``rectify_pair`` and ``s2p/__init__.py:276`` use it unchanged.
 """
 import subprocess

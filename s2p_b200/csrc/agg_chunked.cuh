@@ -21,8 +21,8 @@
 // Status: scripts/chunked_emulator.py replays this file's indexing on the CPU (ring slots, guards, staging slots,
 // range words, previous-band ring) and equals the oracle bit for bit for every TSGM and slab width; it found the
 // chunk-edge case of term() below (a neighbour whose span starts right after / ends right before my chunk), which
-// the first GPU run showed as 1.5 % differing pixels on the 512-slot level.  The corrected kernel has not run on a
-// GPU yet, and version 1 is not faster than the dense kernel (see DESIGN.md section 7).
+// the first GPU run showed as 1.5 % differing pixels on the 512-slot level.  The corrected kernel is bit-identical on the
+// GPU (tests/test_gpu_parity.py) but not faster than the dense kernel on ragged levels (DESIGN.md section 3.3).
 #pragma once
 #include "agg_kernel.cuh"
 

@@ -47,4 +47,4 @@ template <> int agg_launch_lpl<kLPL>(int tsgm, const AggParams &P, int sm_count,
 
 }  // namespace s2pb
 static_assert(s2pb::AggSmem<S2PB_LPL, false>::bytes <= 227 * 1024 && s2pb::AggSmem<S2PB_LPL, true>::bytes <= 227 * 1024,
-              "aggregation CTA exceeds the 227 KB of shared memory of an sm_100 SM");
+              "aggregation CTA exceeds the 227 KB of shared memory of an sm_90 SM");

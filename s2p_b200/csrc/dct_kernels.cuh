@@ -7,7 +7,7 @@
 // are (nearly) zero relative to their row: no-data pixels (NaN -> 0, main_mgm.cc:172-173) come back as +-1e-13-ish
 // noise, and the census transform then compares noise with noise.  Two reference builds that differ only in the
 // summation order of their DCT agree with each other within rounding-noise statistics, but the identity does not
-// (profiles/r02_nodata_spread.md), so the engine reproduces the round trip with the reference's own arithmetic:
+// (scripts/nodata_spread.py), so the engine reproduces the round trip with the reference's own arithmetic:
 //   * transforms are dense matrix products in double, terms added in ascending index order, multiply and add rounded
 //     separately (what the oracle build's DCT does; real fftw builds use other orders and differ among themselves);
 //   * the coefficient tables are computed on the HOST with libm's cos / sin (device cos differs in the last bit);
@@ -67,8 +67,8 @@ __global__ void rt_flag_kernel(const float *__restrict__ img, int w, int h, floa
 // rowlist == nullptr).  The sum runs in ascending i with separately rounded multiply and add, from 0.0, like a plain C
 // loop compiled without contraction.  T is [n][n] row-major.  64 outputs x 32 rows per block of 128 threads, 4 x 4 per
 // thread: a thread's four T values and four X values of one i are two 16-byte shared loads each, i.e. four loads per
-// sixteen multiply-add pairs (the first version's 4 x 2 tile with 8-byte loads needed six per eight and was bound by them:
-// 41 % of the FP64 rate, profiles/r02_ncu_dct_kernels.txt).  512 work items on a 1024 x 1024 image for the 148 SMs.
+// sixteen multiply-add pairs (a 4 x 2 tile with 8-byte loads needs six per eight and is bound by them).  512 work items on a
+// 1024 x 1024 image for the 132 SMs.
 // IN = float (image rows) or double.  DIVN: divide the sum by n (the forward transform's normalisation, shear.c:62-63).
 // `mul` (optional, [n]): the output is multiplied by mul[o] (the phase factor cos(o a));
 // `mul2`/`Y2` (optional): a second output Y2[r][o-1] = y * mul2[o] for o >= 1 and Y2[r][n-1] = 0 (the antisymmetric

@@ -497,7 +497,7 @@ __device__ __forceinline__ void parabola3(float v0, float v1, float v2, float &v
 // Which slots a lane of the WTA warp owns.  The sums are element-wise, so the WTA is free to choose: blocked (lane*LPL + e, one
 // 8-/16-byte request per lane) when LPL is a multiple of 4 or is 2, interleaved (32*e + lane, LPL 4-byte requests of 128 contiguous
 // bytes) for LPL = 3, 5, 6 -- a blocked lane stride of 12/20/24 bytes makes every request touch all of the pixel's 32-byte sectors
-// (3-5x the L2->SM traffic; wta_kernel<5> ran at 0.54 of HBM peak against 0.79-0.85 for LPL 4/8/16, profiles/r02_all_kernels.md).
+// (3-5x the L2->SM traffic of LPL 4/8/16).
 // Both enumerate a lane's slots in ascending order, which is all the first-/last-minimum rules below need.
 template <int LPL> struct WtaMap {
     static constexpr bool interleaved = (LPL == 3 || LPL == 5 || LPL == 6);

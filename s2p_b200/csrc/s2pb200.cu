@@ -100,7 +100,7 @@ struct Slot {
 };
 struct s2pb_ctx {
     int device = 0;
-    int sm_count = 148;
+    int sm_count = 132;
     std::vector<Slot> slots;
     int *abort_flag = nullptr;     // pinned + mapped: the host raises it on timeout
     int *scratch_flag = nullptr;   // pinned + mapped: device -> host one-word answers
@@ -273,8 +273,8 @@ extern "C" s2pb_ctx *s2pb_create(int device)
     if (cudaSetDevice(device) != cudaSuccess) { fail(S2PB_ERR_CUDA, "cudaSetDevice(%d) failed", device); return nullptr; }
     cudaDeviceProp prop;
     if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) { fail(S2PB_ERR_CUDA, "cudaGetDeviceProperties failed"); return nullptr; }
-    if (prop.major != 10) {
-        fail(S2PB_ERR_UNSUPPORTED, "device %d is sm_%d%d; this library carries sm_100a code only", device, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0) {
+        fail(S2PB_ERR_UNSUPPORTED, "device %d is sm_%d%d; this library carries sm_90a code only", device, prop.major, prop.minor);
         return nullptr;
     }
     s2pb_ctx *ctx = new s2pb_ctx;
@@ -1158,9 +1158,9 @@ static int mgm_enqueue(s2pb_ctx *ctx, Slot &s, const float *d_im1, const float *
     CK(cudaEventRecord(s.ev[2], st));
     // ---- 8-pass MGM of both views in one persistent launch (two when the views' slabs differ in width)
     // With another tile's aggregation queued or running (tiles in flight) the launch takes one CTA per SM instead of two, so two
-    // tiles' aggregations share the SMs: a pass is a chain of bands, 296 CTAs on 16 pass-views run it 18 bands deep and about a
-    // fifth of the launch is the chain filling and draining (measured by ignoring the hand-off: 3.39 -> 2.53 ms); two launches of
-    // 148 CTAs run 9 deep.  A/B on B200, C2 with 8 tiles in flight: 226.5 -> 236.9 Mpix/s (alone: 3.39 ms with 296, 3.96 with 148).
+    // tiles' aggregations share the SMs: a pass is a chain of bands, two CTAs per SM on 16 pass-views run it twice as many
+    // bands deep as one CTA per SM does, and a good part of each launch is the chain filling and draining.  (This policy was
+    // chosen by measurement on the GPU the engine was first written for and has not been re-measured on the H100.)
     if (LPLv[0] == LPLv[1]) rc = launch_aggregate(ctx, s, 2, w, h, LPL, p->P1, p->P2, p->ndir, p->tsgm, lut, st, general, wgt, wide[0] ? gminv : nullptr,
                                                   0, other_aggregation_pending(ctx, s) ? 1 : 0);
     else {

@@ -1,4 +1,4 @@
-"""numpy-level handle on the B200 stereo engine (one context per process and GPU).
+"""numpy-level handle on the H100 stereo engine (one context per process and GPU).
 
 ``Engine.mgm`` is the in-memory equivalent of what s2p obtains from the `mgm`
 subprocess plus ``create_rejection_mask`` (s2p/block_matching.py:18-32,155-188):

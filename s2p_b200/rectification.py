@@ -5,7 +5,7 @@ Everything in ``rectify_pair`` except the two image warps is 3x3 algebra on at m
 similarities, disparity range) and needs s2p's own geometry modules (rpcm, estimation, rpc_utils); it stays
 the reference's numpy code.  Only ``common.image_apply_homography`` (:379-380) is heavy, and
 ``s2p_b200.common`` replaces it.  ``rectify_pair`` below therefore is the reference's function running with the
-B200 warp installed.  ``rectify_pair_and_match`` goes one step further: the same host algebra, then both warps AND the matcher in
+H100 warp installed.  ``rectify_pair_and_match`` goes one step further: the same host algebra, then both warps AND the matcher in
 one device call, the rectified pair never leaving the GPU (the opt-in of INTEGRATION.md section 2b).
 """
 from . import common
@@ -55,7 +55,7 @@ def rectify_pair_and_match(im1, im2, rpc1, rpc2, x, y, w, h, out1, out2, disp, m
 
 def install():
     """Patch an importable s2p: both boundaries (matcher and warp) and the two "next" rows already served
-    (mask erosion, n-view merge) go to the B200 engine."""
+    (mask erosion, n-view merge) go to the H100 engine."""
     from . import block_matching, fusion, masking, triangulation
     common.install()
     block_matching.install()

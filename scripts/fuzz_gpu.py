@@ -1,5 +1,5 @@
 """Fuzz the CUDA matcher (through the C ABI) against the CPU oracle on random shapes, ranges and parameters:
-mgm and mgm_multi, every distance, weights, MINDIFF, all refinements.  Needs a B200.
+mgm and mgm_multi, every distance, weights, MINDIFF, all refinements.  Needs an H100.
 usage: python scripts/fuzz_gpu.py [N] [seed]"""
 import os
 import sys

@@ -67,9 +67,12 @@ def main():
         with Image.open(os.path.join(REF, "input_pair", name)) as im:
             rpcs.append(np.array(im.tag_v2[50844], np.float64))
     assert rpcs[0].size == 92 and rpcs[1].size == 92
-    np.savez_compressed(os.path.join(os.path.dirname(os.path.abspath(__file__)), "real_pair.npz"),
-                        crop1=c1.astype(np.uint16), xy1=np.array(xy1), crop2=c2.astype(np.uint16), xy2=np.array(xy2),
-                        H1=H1, H2=H2, rectified_ref=rect_ref, rectified_disp=rect_disp, rpc1=rpcs[0], rpc2=rpcs[1])
+    # three files, none larger than 1 MB (tests/util.py load_real_pair joins them)
+    out = lambda name: os.path.join(os.path.dirname(os.path.abspath(__file__)), name)
+    np.savez_compressed(out("real_pair.npz"), crop1=c1.astype(np.uint16), xy1=np.array(xy1), crop2=c2.astype(np.uint16),
+                        xy2=np.array(xy2), H1=H1, H2=H2, rpc1=rpcs[0], rpc2=rpcs[1])
+    np.savez_compressed(out("real_pair_rectified_ref.npz"), rectified_ref=rect_ref)
+    np.savez_compressed(out("real_pair_rectified_disp.npz"), rectified_disp=rect_disp)
 
 
 if __name__ == "__main__":

@@ -1,4 +1,16 @@
+import os
+
 import numpy as np
+
+GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
+
+
+def load_real_pair():
+    """The real-imagery fixture (tests/golden/make_golden_real_pair.py), stored in three files of less than 1 MB each."""
+    z = {}
+    for name in ("real_pair", "real_pair_rectified_ref", "real_pair_rectified_disp"):
+        z.update(np.load(os.path.join(GOLD, name + ".npz")))
+    return z
 
 
 def same(a, b):
