@@ -60,8 +60,8 @@ struct CkSmem {
         meta_off = ring_off + sizeof(float) * warps * kCkRing * vstride;            // float min, int ea, int eb per slot
         r0_off = meta_off + 12 * warps * kCkRing;                                   // float [r0n][vstride]
         r0m_off = r0_off + sizeof(float) * r0n * vstride;                           // float [r0n]
-        cst_off = (r0m_off + sizeof(float) * r0n + 15) / 16 * 16;                   // half [warps][stage][DP]
-        rng_off = cst_off + sizeof(__half) * warps * stage * dp;                    // 2 words per (warp, stage): lo, hi
+        cst_off = (r0m_off + sizeof(float) * r0n + 15) / 16 * 16;                   // u8 [warps][stage][DP] (cost codes)
+        rng_off = cst_off + sizeof(uint8_t) * warps * stage * dp;                   // 2 words per (warp, stage): lo, hi
         r0rng_off = rng_off + 8 * warps * stage;                                    // 2 words per previous-band slot
         bytes = r0rng_off + 8 * r0n;
     }
@@ -101,7 +101,7 @@ __device__ __forceinline__ void run_band_chunked(const PassDesc &pd, const short
     float *meta = reinterpret_cast<float *>(smem + SM.meta_off);
     float *r0 = reinterpret_cast<float *>(smem + SM.r0_off);
     float *r0m = reinterpret_cast<float *>(smem + SM.r0m_off);
-    const __half *cst = reinterpret_cast<const __half *>(smem + SM.cst_off) + (size_t)k * kCkStage * DP;
+    const uint8_t *cst = reinterpret_cast<const uint8_t *>(smem + SM.cst_off) + (size_t)k * kCkStage * DP;
     const unsigned *rng = reinterpret_cast<const unsigned *>(smem + SM.rng_off) + k * kCkStage * 2;
     const unsigned *r0rng = reinterpret_cast<const unsigned *>(smem + SM.r0rng_off);
     float *myring = ring + (size_t)k * kCkRing * VS;
@@ -120,9 +120,9 @@ __device__ __forceinline__ void run_band_chunked(const PassDesc &pd, const short
     __syncwarp();
 
     // ---- staging: my scanline's costs and range words; (warp 0) the previous band's vectors and minima
-    const char *csrc = reinterpret_cast<const char *>(pd.C) + rowbase * (long long)(DP * 2);
-    const long long cstep = strideI * (DP * 2);
-    const unsigned cdst = smem_s + (unsigned)SM.cst_off + (unsigned)(k * kCkStage * DP * 2);
+    const char *csrc = reinterpret_cast<const char *>(pd.C) + rowbase * (long long)DP;
+    const long long cstep = strideI * DP;
+    const unsigned cdst = smem_s + (unsigned)SM.cst_off + (unsigned)(k * kCkStage * DP);
     const unsigned rdst = smem_s + (unsigned)SM.rng_off + (unsigned)(k * kCkStage * 8);
     long long pidx = rowbase;                                // pixel index of the pixel to stage next
     int jc = 0;
@@ -153,8 +153,8 @@ __device__ __forceinline__ void run_band_chunked(const PassDesc &pd, const short
             const unsigned slot = (unsigned)(jc & (kCkStage - 1));
             const int sh = (int)((pidx & 1) * 16);
             const int ea = ((int)(short)((nl0 >> sh) & 0xffff) - gmin) >> 5, eb = ((int)(short)((nh0 >> sh) & 0xffff) - gmin) >> 5;
-            for (int c = 4 * ea + lane; c <= 4 * eb + 3; c += 32)            // a chunk of 32 halfs = four 16-byte pieces
-                cp_async16_s(cdst + slot * (unsigned)(DP * 2) + 16 * c, csrc + 16 * c);
+            for (int c = 2 * ea + lane; c <= 2 * eb + 1; c += 32)            // a chunk of 32 codes = two 16-byte pieces
+                cp_async16_s(cdst + slot * (unsigned)DP + 16 * c, csrc + 16 * c);
             // the 4-byte words that hold lo[pidx] and hi[pidx] (2-byte elements): the half is picked at use time
             if (lane == 0) cp_async4_s(rdst + slot * 8, reinterpret_cast<const char *>(lo_img) + ((pidx * 2) & ~3LL));
             if (lane == 1) cp_async4_s(rdst + slot * 8 + 4, reinterpret_cast<const char *>(hi_img) + ((pidx * 2) & ~3LL));
@@ -250,14 +250,14 @@ __device__ __forceinline__ void run_band_chunked(const PassDesc &pd, const short
                 if (useCn) nC = nb_at(i, false);
                 if (useE) nE = nb_at(i + 1, false);
             }
-            const __half *cp = cst + (size_t)slot * DP;
+            const uint8_t *cp = cst + (size_t)slot * DP;
             float *mine = myring + (i & (kCkRing - 1)) * VS + kCkPad;
             float lm = S2PB_INF;
             for (int e = 0; e < NC; e++) {
                 const int kk = 32 * e + lane;
                 float L = S2PB_INF;
                 if (e >= ea && e <= eb) {
-                    float c = __half2float(cp[kk]);
+                    float c = cost_decode(cp[kk]);
                     if (SCALED) { if (c >= 0.f && c < 64.f) c = lut[(int)c]; }
                     L = c;
                     if (!border) {

@@ -8,8 +8,8 @@
 //
 // HBM layout (per view):
 //   census  u64  [H][W]
-//   C       f16  [H][W][DP]   popcount of the census XOR (exact in f16), +INF = label
-//                             outside the pixel's range or outside the image
+//   C       u8   [H][W][DP]   popcount of the census XOR as an 8-bit code, 0xFF = +INF = label outside the
+//                             pixel's range or outside the image (cost_encode / cost_decode below)
 //           f32  [H][W][DP]   instead, for the "general" flavour (GEN): the other distances of the reference's
 //                             table (ad, sd, ncc, btad, btsd) and / or per-pixel regularity weights (-wl / -wr)
 //   L_p     f32  [H][W][DP]   one volume per scan pass p (kept separate so that the
@@ -167,45 +167,126 @@ template <int LPL> __device__ __forceinline__ void st_vec_out(float *p, const fl
     st_vec<LPL>(p, v);
 #endif
 }
-// raw f16 bits of a lane's LPL costs
-template <int LPL> struct HalfPack { unsigned short h[LPL]; };
-template <int LPL> __device__ __forceinline__ HalfPack<LPL> ld_cost(const __half *p)
+// ------------------------------------------------------------------ 8-bit census cost codes
+//
+// The census cost volume stores one byte per slot: code = the popcount (0..127; census windows give at most 48),
+// kCostInf (0xFF) = +INF.  Any code with its top bit set decodes to +INF, which lets the packed decoder find INF slots
+// with one sign-replicating byte permute.  Every producer and consumer goes through the helpers below; decoding gives
+// exactly (float)code.
+constexpr unsigned kCostInf = 0xFFu;
+constexpr int kCostMaxCode = 127;     // largest finite cost the format holds
+__host__ __device__ __forceinline__ unsigned cost_encode(unsigned cnt, bool finite) { return finite ? cnt : kCostInf; }
+__device__ __forceinline__ unsigned char cost_encode_f(float c) { return isinf(c) ? (unsigned char)kCostInf : (unsigned char)(int)c; }
+__device__ __forceinline__ float cost_decode(unsigned code) { return (code & 0x80u) ? S2PB_INF : (float)code; }
+// four codes of one word (byte j = slot j) -> their values.  Per pair of slots: the halfs 0x64vv (= 1024 + v exactly) from
+// one byte permute, an all-ones mask where the code is INF from a sign-replicating permute, 0x7C00 (half +INF) selected
+// under it, then 1024 subtracted for both in half2 arithmetic; the f16 -> f32 conversion is the one a stored f16 needed.
+// prmt.b32 in its default mode: a selector nibble with its top bit set replicates the sign of the selected byte (__byte_perm
+// keeps only the low three bits of each nibble)
+__device__ __forceinline__ unsigned prmt(unsigned a, unsigned b, unsigned sel)
 {
-    HalfPack<LPL> r;
-    if constexpr (LPL % 8 == 0) {
+    unsigned r;
+    asm("prmt.b32 %0, %1, %2, %3;" : "=r"(r) : "r"(a), "r"(b), "r"(sel));
+    return r;
+}
+template <int N> __device__ __forceinline__ void cost_decode_word(unsigned w, float *c)
+{
+    const __half2 k1024 = __half2half2(__ushort_as_half((unsigned short)0x6400));
 #pragma unroll
-        for (int q = 0; q < LPL / 8; q++) {
-            uint4 t = __ldg(reinterpret_cast<const uint4 *>(p) + q);
-            unsigned w[4] = {t.x, t.y, t.z, t.w};
+    for (int j = 0; j < N; j += 2) {
+        const unsigned h = prmt(w, 0x6464u, j == 0 ? 0x4140u : 0x4342u);     // 0x64 b(j+1) 0x64 b(j)
+        const unsigned m = prmt(w, 0u, j == 0 ? 0x9988u : 0xbbaau);          // sign of b(j), b(j+1) over their halfs
+        unsigned sel = (h & ~m) | (0x7c007c00u & m);
+        const __half2 v = __hsub2(*reinterpret_cast<const __half2 *>(&sel), k1024);
+        c[j] = __low2float(v);
+        if (j + 1 < N) c[j + 1] = __high2float(v);
+    }
+}
+// encode a lane's LPL slots: byte e = cnt[e] where bit e of `fin` is set, else kCostInf
+template <int LPL> struct CostPack { unsigned w[(LPL + 3) / 4]; };
+template <int LPL> __device__ __forceinline__ CostPack<LPL> cost_pack(const unsigned (&cnt)[LPL], unsigned fin)
+{
+    CostPack<LPL> r;
 #pragma unroll
-            for (int k = 0; k < 4; k++) { r.h[8 * q + 2 * k] = w[k] & 0xffff; r.h[8 * q + 2 * k + 1] = w[k] >> 16; }
-        }
-    } else if constexpr (LPL % 4 == 0) {
+    for (int q = 0; q < (LPL + 3) / 4; q++) {
+        unsigned v = 0;
 #pragma unroll
-        for (int q = 0; q < LPL / 4; q++) {
-            uint2 t = __ldg(reinterpret_cast<const uint2 *>(p) + q);
-            r.h[4 * q] = t.x & 0xffff; r.h[4 * q + 1] = t.x >> 16; r.h[4 * q + 2] = t.y & 0xffff; r.h[4 * q + 3] = t.y >> 16;
-        }
-    } else if constexpr (LPL % 2 == 0) {
-#pragma unroll
-        for (int q = 0; q < LPL / 2; q++) {
-            unsigned t = __ldg(reinterpret_cast<const unsigned *>(p) + q);
-            r.h[2 * q] = t & 0xffff; r.h[2 * q + 1] = t >> 16;
-        }
-    } else {
-#pragma unroll
-        for (int q = 0; q < LPL; q++) r.h[q] = __ldg(reinterpret_cast<const unsigned short *>(p) + q);
+        for (int j = 0; j < 4 && 4 * q + j < LPL; j++) v |= cost_encode(cnt[4 * q + j], (fin >> (4 * q + j)) & 1u) << (8 * j);
+        r.w[q] = v;
     }
     return r;
 }
-// cost value of a stored f16: the popcount itself (census 5x5: ratio = 1, one code word) or
-// the reference's scaled cost through a 64-entry table (mgm_costvolume.h:90-91)
-__device__ __forceinline__ float cost_value(unsigned short hbits, const float *__restrict__ lut)
+template <int LPL> __device__ __forceinline__ unsigned cost_code(const CostPack<LPL> &p, int e) { return (p.w[e / 4] >> (8 * (e & 3))) & 0xffu; }
+template <int LPL> __device__ __forceinline__ void cost_unpack(const CostPack<LPL> &p, float (&c)[LPL])
 {
-    float c = __half2float(__ushort_as_half(hbits));
+#pragma unroll
+    for (int q = 0; q < LPL / 4; q++) cost_decode_word<4>(p.w[q], c + 4 * q);
+    if constexpr (LPL % 4 != 0) cost_decode_word<LPL % 4>(p.w[LPL / 4], c + 4 * (LPL / 4));
+}
+// a lane's LPL codes, widest aligned access (GLOBAL: read-only path; else a plain load, e.g. from shared memory)
+template <int LPL, bool GLOBAL> __device__ __forceinline__ CostPack<LPL> ld_cost(const uint8_t *p)
+{
+    CostPack<LPL> r;
+    if constexpr (LPL % 16 == 0) {
+#pragma unroll
+        for (int q = 0; q < LPL / 16; q++) {
+            const uint4 t = GLOBAL ? __ldg(reinterpret_cast<const uint4 *>(p) + q) : reinterpret_cast<const uint4 *>(p)[q];
+            r.w[4 * q] = t.x; r.w[4 * q + 1] = t.y; r.w[4 * q + 2] = t.z; r.w[4 * q + 3] = t.w;
+        }
+    } else if constexpr (LPL % 8 == 0) {
+#pragma unroll
+        for (int q = 0; q < LPL / 8; q++) {
+            const uint2 t = GLOBAL ? __ldg(reinterpret_cast<const uint2 *>(p) + q) : reinterpret_cast<const uint2 *>(p)[q];
+            r.w[2 * q] = t.x; r.w[2 * q + 1] = t.y;
+        }
+    } else if constexpr (LPL % 4 == 0) {
+#pragma unroll
+        for (int q = 0; q < LPL / 4; q++) r.w[q] = GLOBAL ? __ldg(reinterpret_cast<const unsigned *>(p) + q) : reinterpret_cast<const unsigned *>(p)[q];
+    } else {
+        // 1, 2, 3, 5, 6 labels per lane: a lane's codes are only 1- or 2-byte aligned
+#pragma unroll
+        for (int q = 0; q < (LPL + 3) / 4; q++) r.w[q] = 0;
+        if constexpr (LPL % 2 == 0) {
+#pragma unroll
+            for (int q = 0; q < LPL / 2; q++) {
+                const unsigned short t = GLOBAL ? __ldg(reinterpret_cast<const unsigned short *>(p) + q) : reinterpret_cast<const unsigned short *>(p)[q];
+                r.w[q / 2] |= (unsigned)t << (16 * (q & 1));
+            }
+        } else {
+#pragma unroll
+            for (int q = 0; q < LPL; q++) r.w[q / 4] |= (unsigned)(GLOBAL ? __ldg(p + q) : p[q]) << (8 * (q & 3));
+        }
+    }
+    return r;
+}
+// store a lane's LPL codes, widest aligned access
+template <int LPL> __device__ __forceinline__ void st_cost(uint8_t *p, const CostPack<LPL> &v)
+{
+    if constexpr (LPL % 16 == 0) {
+#pragma unroll
+        for (int q = 0; q < LPL / 16; q++) reinterpret_cast<uint4 *>(p)[q] = make_uint4(v.w[4 * q], v.w[4 * q + 1], v.w[4 * q + 2], v.w[4 * q + 3]);
+    } else if constexpr (LPL % 8 == 0) {
+#pragma unroll
+        for (int q = 0; q < LPL / 8; q++) reinterpret_cast<uint2 *>(p)[q] = make_uint2(v.w[2 * q], v.w[2 * q + 1]);
+    } else if constexpr (LPL % 4 == 0) {
+#pragma unroll
+        for (int q = 0; q < LPL / 4; q++) reinterpret_cast<unsigned *>(p)[q] = v.w[q];
+    } else if constexpr (LPL % 2 == 0) {
+#pragma unroll
+        for (int q = 0; q < LPL / 2; q++) reinterpret_cast<unsigned short *>(p)[q] = (unsigned short)(v.w[q / 2] >> (16 * (q & 1)));
+    } else {
+#pragma unroll
+        for (int q = 0; q < LPL; q++) p[q] = (uint8_t)(v.w[q / 4] >> (8 * (q & 3)));
+    }
+}
+// cost value of a stored code: the popcount itself (census 5x5: ratio = 1, one code word) or
+// the reference's scaled cost through a 64-entry table (mgm_costvolume.h:90-91)
+__device__ __forceinline__ float cost_scaled(float c, const float *__restrict__ lut)
+{
     if (lut != nullptr && c >= 0.f && c < 64.f) c = lut[(int)c];
     return c;
 }
+__device__ __forceinline__ float cost_value(unsigned code, const float *__restrict__ lut) { return cost_scaled(cost_decode(code), lut); }
 
 // ------------------------------------------------------------------ MGM aggregation
 
@@ -221,8 +302,8 @@ __device__ __forceinline__ float cost_value(unsigned short hbits, const float *_
 // owns TWO adjacent scanlines: the lower one reads the upper one's last results straight from registers,
 // the two pixels of a step are independent instruction streams (ILP 2), and only every second scanline
 // boundary goes through a shared-memory ring to the next warp.  The CTA advances in lock step, one
-// __syncthreads per pixel step.  Everything that comes from global memory -- the f16 costs of the warp's
-// two scanlines (one 16-byte cp.async per lane and step) and, for the band's first scanline, the previous
+// __syncthreads per pixel step.  Everything that comes from global memory -- the 8-bit cost codes of the warp's
+// two scanlines (at most one 16-byte cp.async per lane and step up to 8 labels per lane) and, for the band's first scanline, the previous
 // band's aggregated vectors (re-read from L2 behind a release/acquire progress counter) -- is staged into
 // shared memory kStage-1 steps ahead, so no global-memory latency sits on the lock-step critical path.
 // CTAs are persistent and pull (band, pass-view) items from a global queue ordered band-major, which
@@ -233,7 +314,7 @@ struct PassDesc {
     int strideS, strideI;
     int type;
     int nBands;
-    const void *C;   // __half (census popcounts) or float (GEN) [H][W][DP]
+    const void *C;   // u8 codes (census popcounts) or float (GEN) [H][W][DP]
     const float *W;  // GEN: this view's regularity weight image (-wl / -wr), nullptr = all ones
     float *L;
     float *Lmin;     // minima of the band-closing scanlines only (read back by the next band)
@@ -253,7 +334,7 @@ struct AggParams {
 // because pixel 0 is staged ahead of the pipeline); shallower for the widest volumes.  (16 labels per lane would
 // still fit 227 KB with 8 stages, but measured no faster: 32.7 vs 31.9 ms on the C3-like mgm_multi tile.)
 template <int LPL, bool GEN = false> struct StageCfg {
-#ifdef S2PB_STAGE          // (A/B builds: depth of the f16 flavour's pipeline for up to 12 labels per lane)
+#ifdef S2PB_STAGE          // (A/B builds: depth of the census flavour's pipeline for up to 12 labels per lane)
     static constexpr int kStage = GEN ? ((LPL <= 4) ? 8 : (LPL <= 8) ? 4 : 2) : ((LPL <= 12) ? S2PB_STAGE : 2);
 #else
     static constexpr int kStage = GEN ? ((LPL <= 4) ? 8 : (LPL <= 8) ? 4 : 2) : ((LPL <= 12) ? 8 : 2);
@@ -282,36 +363,6 @@ template <int NBYTES> __device__ __forceinline__ void warp_cp_async(void *smem, 
         int c = lane + 32 * q;
         if (CH % 32 == 0 || c < CH) cp_async16((char *)smem + 16 * c, (const char *)gmem + 16 * c);
     }
-}
-// a lane's LPL f16 costs from shared memory (widest aligned access)
-template <int LPL> __device__ __forceinline__ HalfPack<LPL> lds_cost(const __half *p)
-{
-    HalfPack<LPL> r;
-    if constexpr (LPL % 8 == 0) {
-#pragma unroll
-        for (int q = 0; q < LPL / 8; q++) {
-            uint4 t = reinterpret_cast<const uint4 *>(p)[q];
-            unsigned w[4] = {t.x, t.y, t.z, t.w};
-#pragma unroll
-            for (int k = 0; k < 4; k++) { r.h[8 * q + 2 * k] = w[k] & 0xffff; r.h[8 * q + 2 * k + 1] = w[k] >> 16; }
-        }
-    } else if constexpr (LPL % 4 == 0) {
-#pragma unroll
-        for (int q = 0; q < LPL / 4; q++) {
-            uint2 t = reinterpret_cast<const uint2 *>(p)[q];
-            r.h[4 * q] = t.x & 0xffff; r.h[4 * q + 1] = t.x >> 16; r.h[4 * q + 2] = t.y & 0xffff; r.h[4 * q + 3] = t.y >> 16;
-        }
-    } else if constexpr (LPL % 2 == 0) {
-#pragma unroll
-        for (int q = 0; q < LPL / 2; q++) {
-            unsigned t = reinterpret_cast<const unsigned *>(p)[q];
-            r.h[2 * q] = t & 0xffff; r.h[2 * q + 1] = t >> 16;
-        }
-    } else {
-#pragma unroll
-        for (int q = 0; q < LPL; q++) r.h[q] = reinterpret_cast<const unsigned short *>(p)[q];
-    }
-    return r;
 }
 // x / 3 with two fmas: bit-identical to IEEE division for every finite x >= 0
 // (exhaustively verified on the CPU: tests/test_host_logic.py::test_div3_trick)
@@ -344,17 +395,17 @@ template <int LPL> __device__ __forceinline__ float nb_term(const NbVec<LPL> &n,
     return fmin3f(n.v[e], v1, mP2) - n.m;
 }
 
-// shared memory carve-up of one CTA (floats first, then halfs; every block 16-byte aligned)
+// shared memory carve-up of one CTA (floats first, then cost codes; every block 16-byte aligned)
 template <int LPL, bool GEN = false> struct AggSmem {
     static constexpr int DP = 32 * LPL;
     static constexpr int kStage = StageCfg<LPL, GEN>::kStage, kR0 = StageCfg<LPL, GEN>::kR0;
-    static constexpr size_t kCostBytes = GEN ? sizeof(float) : sizeof(__half);
+    static constexpr size_t kCostBytes = GEN ? sizeof(float) : sizeof(uint8_t);
     static constexpr int kRing = SyncCfg<LPL>::kRing;
     static constexpr size_t ring_off = 0;                                            // float [kNWC][kRing][DP]
     static constexpr size_t ringm_off = ring_off + sizeof(float) * kNWC * kRing * DP; // float [kNWC][kRing]
     static constexpr size_t r0_off = ringm_off + sizeof(float) * kNWC * kRing;        // float [kR0][DP]   previous band
     static constexpr size_t r0m_off = r0_off + sizeof(float) * kR0 * DP;              // float [kR0]
-    static constexpr size_t cst_off = r0m_off + sizeof(float) * kR0;                  // half | float [kNW][kStage][DP]
+    static constexpr size_t cst_off = r0m_off + sizeof(float) * kR0;                  // u8 | float [kNW][kStage][DP]
     static constexpr size_t wst_off = cst_off + kCostBytes * kNW * kStage * DP;       // float [kNW][kStage]  (GEN: weights)
     static constexpr size_t bytes = wst_off + (GEN ? sizeof(float) * kNW * kStage : 0);
 };
@@ -392,7 +443,7 @@ __device__ __forceinline__ void run_band(const PassDesc &pd, int band, float P1,
     constexpr int LEAD = useE ? 1 : 0;    // newest previous-scanline pixel needed at position i is i+LEAD
     constexpr int U = useE ? 3 : 2;       // window / history registers rotate with period U: the step loop is unrolled by U
     using SM = AggSmem<LPL, GEN>;
-    using CT = typename std::conditional<GEN, float, __half>::type;      // stored cost element
+    using CT = typename std::conditional<GEN, float, uint8_t>::type;     // stored cost element
     constexpr int kStage = SM::kStage, kR0 = SM::kR0, S = kStage - 1, kRing = SM::kRing;
     constexpr bool SYNC2 = SyncCfg<LPL>::sync2;
     constexpr int WSK = SYNC2 ? 2 * SKEW + 1 : 2 * SKEW;   // pixels by which a warp's upper scanline trails the previous warp's
@@ -425,7 +476,7 @@ __device__ __forceinline__ void run_band(const PassDesc &pd, int band, float P1,
     const float *wstA = reinterpret_cast<float *>(smem + SM::wst_off) + (2 * k) * kStage, *wstB = wstA + kStage;   // GEN only
     const bool weighted = GEN && pd.W != nullptr;
 
-    // ---- staging cursors.  Costs: lanes 0-15 copy scanline A, lanes 16-31 scanline B, 16 bytes each.
+    // ---- staging cursors.  Costs: lanes 0-15 copy scanline A, lanes 16-31 scanline B, 16-byte pieces.
     const int rsel = lane >> 4, q16 = lane & 15;
     const bool live_st = rsel ? liveB : liveA;
     const char *csrc = reinterpret_cast<const char *>(pd.C) + (rowbaseA + (long long)rsel * pd.strideS) * CB + 16 * q16;
@@ -494,12 +545,11 @@ __device__ __forceinline__ void run_band(const PassDesc &pd, int band, float P1,
         if constexpr (GEN) {
             ld_vec<LPL>(p, c);
         } else {
-            HalfPack<LPL> cp = lds_cost<LPL>(p);
+            cost_unpack<LPL>(ld_cost<LPL, false>(p), c);
+            if (SCALED) {
 #pragma unroll
-            for (int e = 0; e < LPL; e++) {
-                float cc = __half2float(__ushort_as_half(cp.h[e]));
-                if (SCALED) { if (cc >= 0.f && cc < 64.f) cc = lut[(int)cc]; }   // an idle scanline reads unstaged shared memory: never index with it
-                c[e] = cc;
+                for (int e = 0; e < LPL; e++)
+                    if (c[e] >= 0.f && c[e] < 64.f) c[e] = lut[(int)c[e]];   // an idle scanline reads unstaged shared memory: never index with it
             }
         }
     };

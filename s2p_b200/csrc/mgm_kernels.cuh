@@ -56,13 +56,12 @@ __global__ void has_nan_kernel(const float *__restrict__ in, int n, int *flag)
 // With ZOOMFACTOR = 2 (mgm_costvolume.cc:145-154) label o compares cu(x) with the census of the matched image
 // shifted by (o mod 2)/2 pixel, at column x + floor(o/2): cv = shift 0, cv1 = shift 1/2.
 // NARROW: the census codes fit 32 bits (3x3 and 5x5 windows: 8 and 24 bits), so one POPC on the low words does it.
-// The Hamming distance goes to f16 without a conversion instruction: the half with bits 0x6400 + v is 1024 + v exactly
-// (v < 1024), and subtracting 1024 in half2 arithmetic leaves v -- two labels per HADD2 instead of an I2F and an F2F each, which
-// share the quarter-rate pipe with POPC (that pipe, not issue, bounded the round-1 kernel: four such operations per label).
+// The Hamming distance is stored as its 8-bit code (agg_kernel.cuh), four labels per 32-bit word, with no conversion
+// instruction on the quarter-rate pipe that POPC uses.
 template <int LPL, bool ZOOM2, bool NARROW>
 __global__ void cost_kernel(const uint64_t *__restrict__ cu, const uint64_t *__restrict__ cv, const uint64_t *__restrict__ cv1,
                             int w, int h,
-                            const short *__restrict__ lo, const short *__restrict__ hi, int gmin, __half *__restrict__ C)
+                            const short *__restrict__ lo, const short *__restrict__ hi, int gmin, uint8_t *__restrict__ C)
 {
     constexpr int DP = 32 * LPL;
     int lane = threadIdx.x & 31;
@@ -93,30 +92,7 @@ __global__ void cost_kernel(const uint64_t *__restrict__ cu, const uint64_t *__r
         }
         // no label of the range has a distance: the whole range is 0 (mgm_costvolume.cc:166-171); cnt is 0 there already
         const unsigned fin = __any_sync(0xffffffffu, okm != 0) ? okm : inm;
-        __half *dst = C + p * DP + lane * LPL;
-        if constexpr (LPL % 2 == 0) {          // packed stores: 4, 8 or 16 bytes per lane
-            unsigned wds[LPL / 2];
-#pragma unroll
-            for (int e = 0; e < LPL / 2; e++) {
-                unsigned pk = 0x64006400u + (cnt[2 * e] | (cnt[2 * e + 1] << 16));
-                __half2 hv = __hsub2(*reinterpret_cast<__half2 *>(&pk), __half2half2(__ushort_as_half((unsigned short)0x6400)));
-                const unsigned m = ((fin >> (2 * e)) & 1u ? 0x0000ffffu : 0u) | ((fin >> (2 * e + 1)) & 1u ? 0xffff0000u : 0u);
-                wds[e] = (*reinterpret_cast<unsigned *>(&hv) & m) | (0x7c007c00u & ~m);
-            }
-            if constexpr (LPL % 8 == 0) {
-#pragma unroll
-                for (int q = 0; q < LPL / 8; q++) reinterpret_cast<uint4 *>(dst)[q] = make_uint4(wds[4 * q], wds[4 * q + 1], wds[4 * q + 2], wds[4 * q + 3]);
-            } else if constexpr (LPL % 4 == 0) {
-#pragma unroll
-                for (int q = 0; q < LPL / 4; q++) reinterpret_cast<uint2 *>(dst)[q] = make_uint2(wds[2 * q], wds[2 * q + 1]);
-            } else {
-#pragma unroll
-                for (int q = 0; q < LPL / 2; q++) reinterpret_cast<unsigned *>(dst)[q] = wds[q];
-            }
-        } else {
-#pragma unroll
-            for (int e = 0; e < LPL; e++) dst[e] = (fin >> e) & 1u ? __float2half_rn((float)cnt[e]) : __ushort_as_half((unsigned short)0x7c00);
-        }
+        st_cost<LPL>(C + p * DP + lane * LPL, cost_pack<LPL>(cnt, fin));     // 4 codes per 32-bit word
     }
 }
 
@@ -131,7 +107,7 @@ constexpr int kCostStripThreads = 128;
 template <int LPL>
 __global__ void __launch_bounds__(kCostStripThreads) cost_strip_kernel(const uint64_t *__restrict__ cu, const uint64_t *__restrict__ cv, int w, int h,
                                                                        const short *__restrict__ lo, const short *__restrict__ hi, int gmin,
-                                                                       __half *__restrict__ C)
+                                                                       uint8_t *__restrict__ C)
 {
     constexpr int DP = 32 * LPL, T = 32, NW = T + DP, CS = NW + 4;
     __shared__ __align__(16) unsigned codes[kCostStripThreads / 32][4][CS];
@@ -156,7 +132,7 @@ __global__ void __launch_bounds__(kCostStripThreads) cost_strip_kernel(const uin
         if (xi < w) { a_i = reinterpret_cast<const unsigned *>(cu)[2 * (row + xi)]; l_i = lo[row + xi]; h_i = hi[row + xi]; }
         __syncwarp();
         const int npx = (w - x0 < T) ? w - x0 : T;
-        __half *dst = C + (row + x0) * DP + lane * LPL;
+        uint8_t *dst = C + (row + x0) * DP + lane * LPL;
         for (int i = 0; i < npx; i++, dst += DP) {
             const unsigned a = __shfl_sync(0xffffffffu, a_i, i);
             const int l = __shfl_sync(0xffffffffu, l_i, i), hgh = __shfl_sync(0xffffffffu, h_i, i);
@@ -189,29 +165,7 @@ __global__ void __launch_bounds__(kCostStripThreads) cost_strip_kernel(const uin
                 cnt[e] = none ? 0u : (unsigned)__popc(a ^ cw[e]);
                 if (o >= flo && o <= fhi) fin |= 1u << e;
             }
-            if constexpr (LPL % 2 == 0) {
-                unsigned wds[LPL / 2];
-#pragma unroll
-                for (int e = 0; e < LPL / 2; e++) {
-                    unsigned pk = 0x64006400u + (cnt[2 * e] | (cnt[2 * e + 1] << 16));
-                    __half2 hv = __hsub2(*reinterpret_cast<__half2 *>(&pk), __half2half2(__ushort_as_half((unsigned short)0x6400)));
-                    const unsigned m = ((fin >> (2 * e)) & 1u ? 0x0000ffffu : 0u) | ((fin >> (2 * e + 1)) & 1u ? 0xffff0000u : 0u);
-                    wds[e] = (*reinterpret_cast<unsigned *>(&hv) & m) | (0x7c007c00u & ~m);
-                }
-                if constexpr (LPL % 8 == 0) {
-#pragma unroll
-                    for (int q = 0; q < LPL / 8; q++) reinterpret_cast<uint4 *>(dst)[q] = make_uint4(wds[4 * q], wds[4 * q + 1], wds[4 * q + 2], wds[4 * q + 3]);
-                } else if constexpr (LPL % 4 == 0) {
-#pragma unroll
-                    for (int q = 0; q < LPL / 4; q++) reinterpret_cast<uint2 *>(dst)[q] = make_uint2(wds[2 * q], wds[2 * q + 1]);
-                } else {
-#pragma unroll
-                    for (int q = 0; q < LPL / 2; q++) reinterpret_cast<unsigned *>(dst)[q] = wds[q];
-                }
-            } else {
-#pragma unroll
-                for (int e = 0; e < LPL; e++) dst[e] = (fin >> e) & 1u ? __float2half_rn((float)cnt[e]) : __ushort_as_half((unsigned short)0x7c00);
-            }
+            st_cost<LPL>(dst, cost_pack<LPL>(cnt, fin));
         }
     }
 }
@@ -396,7 +350,7 @@ __global__ void unpad_cost_kernel(const float *__restrict__ C, size_t npix, int 
 template <bool ZOOM2>
 __global__ void cost_chunked_kernel(const uint64_t *__restrict__ cu, const uint64_t *__restrict__ cv, const uint64_t *__restrict__ cv1,
                                     int w, int h, const short *__restrict__ lo, const short *__restrict__ hi, int gmin, int DP,
-                                    __half *__restrict__ C)
+                                    uint8_t *__restrict__ C)
 {
     const int lane = threadIdx.x & 31;
     const size_t npix = (size_t)w * h;
@@ -407,50 +361,51 @@ __global__ void cost_chunked_kernel(const uint64_t *__restrict__ cu, const uint6
         const uint64_t a = cu[p];
         const int l = lo[p], hgh = hi[p];
         const int ea = (l - gmin) >> 5, eb = (hgh - gmin) >> 5;
-        __half *dst = C + p * DP;
+        uint8_t *dst = C + p * DP;
         bool anyfinite = false;
         for (int e = ea; e <= eb; e++) {
             const int o = gmin + 32 * e + lane;
-            float v = S2PB_INF;
+            unsigned cnt = 0;
+            bool ok = false;
             if (o >= l && o <= hgh) {
                 int q = x + o;
                 const uint64_t *codes = cv;
                 if (ZOOM2) { q = x + (o >> 1); if (o & 1) codes = cv1; }
-                if (q >= 0 && q < w) { v = (float)__popcll(a ^ codes[row + q]); anyfinite = true; }
+                if (q >= 0 && q < w) { cnt = __popcll(a ^ codes[row + q]); ok = anyfinite = true; }
             }
-            dst[32 * e + lane] = __float2half_rn(v);
+            dst[32 * e + lane] = (uint8_t)cost_encode(cnt, ok);
         }
         if (!__any_sync(0xffffffffu, anyfinite)) {
             for (int e = ea; e <= eb; e++) {
                 const int o = gmin + 32 * e + lane;
-                if (o >= l && o <= hgh) dst[32 * e + lane] = __float2half_rn(0.f);
+                if (o >= l && o <= hgh) dst[32 * e + lane] = (uint8_t)cost_encode(0, true);
             }
         }
     }
 }
 
-// float volume (stage-level API) -> f16 slab with +INF padding, and back
-__global__ void pack_cost_kernel(const float *__restrict__ Cin, size_t npix, int D, int DP, __half *__restrict__ C)
+// float volume (stage-level API; integer costs in [0, kCostMaxCode] or +INF) -> code slab with +INF padding, and back
+__global__ void pack_cost_kernel(const float *__restrict__ Cin, size_t npix, int D, int DP, uint8_t *__restrict__ C)
 {
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= npix * DP) return;
     size_t p = i / DP; int k = (int)(i % DP);
-    C[i] = __float2half_rn(k < D ? Cin[p * D + k] : S2PB_INF);
+    C[i] = cost_encode_f(k < D ? Cin[p * D + k] : S2PB_INF);
 }
-__global__ void unpack_cost_kernel(const __half *__restrict__ C, size_t npix, int D, int DP, const float *__restrict__ lut,
+__global__ void unpack_cost_kernel(const uint8_t *__restrict__ C, size_t npix, int D, int DP, const float *__restrict__ lut,
                                    float *__restrict__ Cout)
 {
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= npix * D) return;
     size_t p = i / D; int k = (int)(i % D);
-    Cout[i] = cost_value(__half_as_ushort(C[p * DP + k]), lut);
+    Cout[i] = cost_value(C[p * DP + k], lut);
 }
 
 // ------------------------------------------------------------------ WTA + consensus + sub-pixel
 
 struct WtaParams {
     const float *L[kMaxPasses];
-    const void *C;            // __half slab, or float slab for the general flavour (GEN)
+    const void *C;            // u8 code slab, or float slab for the general flavour (GEN)
     const short *lo, *hi;     // per-pixel label range (labels, not slots)
     const float *lut;
     int ndir, gmin, fix_overcount, refine;
@@ -608,13 +563,13 @@ __device__ __forceinline__ void wta_pixels(const WtaParams &P, float *sSrow)
         int am[kMaxPasses];
 #pragma unroll
         for (int e = 0; e < LPL; e++) s[e] = 0.f;
-        // the pixel's range and (f16 flavour) its costs are requested first: they are consumed last, and a warp's pixel is one
+        // the pixel's range and (census flavour) its costs are requested first: they are consumed last, and a warp's pixel is one
         // dependent chain -- next to the aggregation kernel only four warps per SM run this kernel, so its rate there is
         // 1 / chain length, and every global load that waits at the end of the chain is ~1000 cycles of it
         const int plo = __ldg(P.lo + p), phi = __ldg(P.hi + p);
         constexpr bool early_cost = !GEN && !WtaMap<LPL>::interleaved && LPL <= 8;      // (wider: no registers to spare)
-        HalfPack<early_cost ? LPL : 1> cpk;
-        if constexpr (early_cost) cpk = ld_cost<LPL>(reinterpret_cast<const __half *>(P.C) + p * DP + lane * LPL);
+        CostPack<early_cost ? LPL : 1> cpk;
+        if constexpr (early_cost) cpk = ld_cost<LPL, true>(reinterpret_cast<const uint8_t *>(P.C) + p * DP + lane * LPL);
         // the passes' vectors are requested four at a time before any is consumed (memory-level parallelism
         // within the register budget that lets this kernel share an SM with the aggregation kernel)
 #pragma unroll
@@ -632,16 +587,16 @@ __device__ __forceinline__ void wta_pixels(const WtaParams &P, float *sSrow)
         float c[LPL];
         if constexpr (GEN) wta_ld_pass<LPL>(reinterpret_cast<const float *>(P.C) + p * DP, lane, c);
         else if constexpr (WtaMap<LPL>::interleaved) {
-            const unsigned short *cp = reinterpret_cast<const unsigned short *>(P.C) + p * DP + lane;
+            const uint8_t *cp = reinterpret_cast<const uint8_t *>(P.C) + p * DP + lane;
 #pragma unroll
             for (int e = 0; e < LPL; e++) c[e] = cost_value(__ldg(cp + 32 * e), P.lut);
-        } else if constexpr (early_cost) {
-#pragma unroll
-            for (int e = 0; e < LPL; e++) c[e] = cost_value(cpk.h[e], P.lut);
         } else {
-            HalfPack<LPL> cp = ld_cost<LPL>(reinterpret_cast<const __half *>(P.C) + p * DP + lane * LPL);
+            // (one code at a time: the packed decoder's temporaries cost this register-capped kernel spills)
+            CostPack<LPL> cp;
+            if constexpr (early_cost) cp = cpk;
+            else cp = ld_cost<LPL, true>(reinterpret_cast<const uint8_t *>(P.C) + p * DP + lane * LPL);
 #pragma unroll
-            for (int e = 0; e < LPL; e++) c[e] = cost_value(cp.h[e], P.lut);
+            for (int e = 0; e < LPL; e++) c[e] = cost_value(cost_code(cp, e), P.lut);
         }
         wta_finish<LPL>(P, p, lane, s, am, c, sSrow, plo, phi);
     }
@@ -665,7 +620,7 @@ __global__ void __launch_bounds__(kWtaThreads) wta_chunked_kernel(const WtaParam
     extern __shared__ float sS_all[];                    // [warps][DP]
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     float *sS = sS_all + (size_t)wib * DP;
-    const __half *C = reinterpret_cast<const __half *>(P.C);
+    const uint8_t *C = reinterpret_cast<const uint8_t *>(P.C);
     size_t warp = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = ((size_t)gridDim.x * blockDim.x) >> 5;
     for (size_t p = warp; p < P.npix; p += nwarps) {
         const int lo = P.lo[p] - P.gmin, hi = P.hi[p] - P.gmin;      // slots
@@ -686,7 +641,7 @@ __global__ void __launch_bounds__(kWtaThreads) wta_chunked_kernel(const WtaParam
                     if (v < pm[d]) { pm[d] = v; pa[d] = kk; } else if (v == pm[d]) pa[d] = kk;
                     s += v;
                 }
-            const float c = cost_value(__half_as_ushort(C[p * DP + kk]), P.lut);
+            const float c = cost_value(C[p * DP + kk], P.lut);
             if (P.fix_overcount == 1) s = fmaf(-(float)(P.ndir - 1), c, s);
             if (isfinite(s) && best > s) { best = s; bidx = kk; }
             sS[kk] = s;

@@ -60,7 +60,7 @@ struct ViewWS {
     RtState *rtstate;
     short *lo, *hi;        // per-pixel label range
     uint64_t *census;
-    void *C;               // [H][W][DP] costs: __half (census popcounts) or float (general flavour)
+    void *C;               // [H][W][DP] costs: u8 codes (census popcounts, agg_kernel.cuh) or float (general flavour)
     float *L[kMaxPasses];
     float *Lmin[kMaxPasses];
     int *progress;         // [kMaxPasses][maxBands]
@@ -70,7 +70,7 @@ struct Slot {
     void *base = nullptr;
     size_t bytes = 0;
     int w = 0, h = 0, DP = 0, ndir = 0;
-    int cbytes = 2;               // bytes per stored cost: 2 = f16 census popcounts, 4 = float (general flavour)
+    int cbytes = 1;               // bytes per stored cost: 1 = 8-bit census codes, 4 = float (general flavour)
     ViewWS v[2];
     int *next_item = nullptr;
     float *lut = nullptr;
@@ -202,7 +202,7 @@ static int slot_io_ensure(Slot &s, size_t npix)
     return S2PB_OK;
 }
 
-static int slot_ensure(s2pb_ctx *ctx, Slot &s, int w, int h, int DP, int ndir, int cbytes = 2)
+static int slot_ensure(s2pb_ctx *ctx, Slot &s, int w, int h, int DP, int ndir, int cbytes = 1)
 {
     Slot probe;
     slot_layout(probe, w, h, DP, ndir, cbytes, false);
@@ -485,7 +485,7 @@ static void fill_pass(PassDesc &pd, int pass, int w, int h)
 }
 
 // Enqueue the 8-pass aggregation of `nviews` views of slot s in ONE persistent launch.
-// S2PB_CHUNKED=1 in the environment routes the f16-cost aggregation of mgm_multi's levels to the experimental
+// S2PB_CHUNKED=1 in the environment routes the census-cost aggregation of mgm_multi's levels to the experimental
 // chunk-skipping kernel (agg_chunked.cuh)
 // (1 = aggregation and WTA, 2 = aggregation only, 3 = WTA only: to isolate a difference)
 static int chunked_mode() { static int v = -1; if (v < 0) { const char *e = getenv("S2PB_CHUNKED"); v = e ? atoi(e) : 0; } return v; }
@@ -547,7 +547,7 @@ static int launch_aggregate(s2pb_ctx *ctx, Slot &s, int nviews, int w, int h, in
 // S2PB_COST_STRIP=0: the per-pixel cost kernel for every shape (A/B)
 static bool cost_strip_enabled() { static int v = -1; if (v < 0) { const char *e = getenv("S2PB_COST_STRIP"); v = e ? atoi(e) : 1; } return v != 0; }
 template <int LPL> static void launch_cost_t(const uint64_t *cu, const uint64_t *cv, const uint64_t *cv1, int zoom, bool narrow, int w, int h,
-                                             const short *lo, const short *hi, int gmin, __half *C, int sm, cudaStream_t st)
+                                             const short *lo, const short *hi, int gmin, uint8_t *C, int sm, cudaStream_t st)
 {
     if constexpr (LPL <= 8) {
         if (zoom != 2 && narrow && cost_strip_enabled()) { cost_strip_kernel<LPL><<<sm * 16, kCostStripThreads, 0, st>>>(cu, cv, w, h, lo, hi, gmin, C); return; }
@@ -584,7 +584,7 @@ static int launch_cost(s2pb_ctx *ctx, int LPL, int census_win, const uint64_t *c
                        int gmin, void *C, cudaStream_t st, const uint64_t *cv1 = nullptr, int zoom = 1)
 {
     const bool narrow = census_win <= 5;
-    LPL_SWITCH(LPL, launch_cost_t<K>(cu, cv, cv1, zoom, narrow, w, h, lo, hi, gmin, (__half *)C, ctx->sm_count, st));
+    LPL_SWITCH(LPL, launch_cost_t<K>(cu, cv, cv1, zoom, narrow, w, h, lo, hi, gmin, (uint8_t *)C, ctx->sm_count, st));
     CK(cudaGetLastError());
     ctx->launches++;
     return S2PB_OK;
@@ -833,7 +833,7 @@ static int mgm_call_level(s2pb_ctx *ctx, Slot &s, Level &L, int zoom, const s2pb
             return fail(S2PB_ERR_UNSUPPORTED, "a %dx%d level needs %d labels in its volume; %s", w, h, D,
                         general ? "512 are supported for the float-cost flavour" : "2048 are supported");
     }
-    rc = slot_ensure(ctx, s, w, h, 32 * LPL, p->ndir, general ? 4 : 2);
+    rc = slot_ensure(ctx, s, w, h, 32 * LPL, p->ndir, general ? 4 : 1);
     if (rc != S2PB_OK) return rc;
     TRACE(st, "level %dx%d zoom %d: hull L [%d,%d] R [%d,%d] -> LPL %d%s", w, h, zoom, gminv[0], gmaxv[0], gminv[1], gmaxv[1], LPL,
           general ? " (general flavour)" : "");
@@ -882,9 +882,9 @@ static int mgm_call_level(s2pb_ctx *ctx, Slot &s, Level &L, int zoom, const s2pb
             rc = launch_cost_gen(ctx, LPL, G, st);
         } else if (chunked_cost_enabled(32 * LPL)) {      // only the chunks of each pixel's span
             if (zoom == 2) cost_chunked_kernel<true><<<ctx->sm_count * 8, 256, 0, st>>>(s.v[vi].census, cen_rt[1 - vi], cen_half[1 - vi], w, h,
-                                                                                  lo[vi], hi[vi], gminv[vi], 32 * LPL, (__half *)s.v[vi].C);
+                                                                                  lo[vi], hi[vi], gminv[vi], 32 * LPL, (uint8_t *)s.v[vi].C);
             else cost_chunked_kernel<false><<<ctx->sm_count * 8, 256, 0, st>>>(s.v[vi].census, cen_rt[1 - vi], nullptr, w, h,
-                                                                               lo[vi], hi[vi], gminv[vi], 32 * LPL, (__half *)s.v[vi].C);
+                                                                               lo[vi], hi[vi], gminv[vi], 32 * LPL, (uint8_t *)s.v[vi].C);
             ctx->launches++;
             rc = cudaGetLastError() == cudaSuccess ? S2PB_OK : fail(S2PB_ERR_CUDA, "cost_chunked_kernel launch failed");
         } else {
@@ -1099,7 +1099,7 @@ static int mgm_enqueue(s2pb_ctx *ctx, Slot &s, const float *d_im1, const float *
                             general ? 512 : 2048, general ? " by the float-cost flavour" : "");
         }
     const int LPL = LPLv[0] > LPLv[1] ? LPLv[0] : LPLv[1];
-    int rc = slot_ensure(ctx, s, w, h, 32 * LPL, p->ndir, general ? 4 : 2);
+    int rc = slot_ensure(ctx, s, w, h, 32 * LPL, p->ndir, general ? 4 : 1);
     if (rc != S2PB_OK) return rc;
 
     float lut_h[64];
@@ -1147,7 +1147,7 @@ static int mgm_enqueue(s2pb_ctx *ctx, Slot &s, const float *d_im1, const float *
             rc = launch_cost_gen(ctx, LPLv[vi], G, st);
         } else if (wide[vi]) {
             cost_chunked_kernel<false><<<ctx->sm_count * 8, 256, 0, st>>>(s.v[vi].census, s.v[1 - vi].census_rt, nullptr, w, h, s.v[vi].lo, s.v[vi].hi,
-                                                                        gminv[vi], 32 * LPLv[vi], (__half *)s.v[vi].C);
+                                                                        gminv[vi], 32 * LPLv[vi], (uint8_t *)s.v[vi].C);
             ctx->launches++;
             rc = cudaGetLastError() == cudaSuccess ? S2PB_OK : fail(S2PB_ERR_CUDA, "cost_chunked_kernel launch failed");
         } else {
@@ -1529,7 +1529,7 @@ extern "C" int s2pb_costvolume(s2pb_ctx *ctx, const float *u, const float *v, in
     cudaStream_t st = ctx->slots[0].stream;
     DevBuf du, dv, cu, cv, dlo, dhi, dC, dCf, dlut;
     ALLOC(du, npix * 4); ALLOC(dv, npix * 4); ALLOC(cu, npix * 8); ALLOC(cv, npix * 8);
-    ALLOC(dC, npix * DP * 2); ALLOC(dCf, npix * D * 4); ALLOC(dlut, 256);
+    ALLOC(dC, npix * DP); ALLOC(dCf, npix * D * 4); ALLOC(dlut, 256);
     int rc = upload_ranges(lo, hi, npix, gmin, D, dlo, dhi, st);
     if (rc != S2PB_OK) return rc;
     CK(cudaMemcpyAsync(du.p, u, npix * 4, cudaMemcpyHostToDevice, st));
@@ -1541,13 +1541,13 @@ extern "C" int s2pb_costvolume(s2pb_ctx *ctx, const float *u, const float *v, in
     census_kernel<<<grid2d(w, h, b2), b2, 0, st>>>(du.as<float>(), w, h, win / 2, cu.as<uint64_t>());
     census_kernel<<<grid2d(w, h, b2), b2, 0, st>>>(dv.as<float>(), w, h, win / 2, cv.as<uint64_t>());
     ctx->launches += 2;
-    rc = launch_cost(ctx, LPL, win, cu.as<uint64_t>(), cv.as<uint64_t>(), w, h, dlo.as<short>(), dhi.as<short>(), gmin, dC.as<__half>(), st);
+    rc = launch_cost(ctx, LPL, win, cu.as<uint64_t>(), cv.as<uint64_t>(), w, h, dlo.as<short>(), dhi.as<short>(), gmin, dC.as<uint8_t>(), st);
     if (rc != S2PB_OK) return rc;
     float lut_h[64];
     const float *lut = nullptr;
     if (cost_lut(win, lut_h)) { CK(cudaMemcpyAsync(dlut.p, lut_h, 256, cudaMemcpyHostToDevice, st)); lut = dlut.as<float>(); }
     size_t tot = npix * D;
-    unpack_cost_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(dC.as<__half>(), npix, D, DP, lut, dCf.as<float>());
+    unpack_cost_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(dC.as<uint8_t>(), npix, D, DP, lut, dCf.as<float>());
     ctx->launches++;
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync(C, dCf.p, tot * 4, cudaMemcpyDeviceToHost, st));
@@ -1666,11 +1666,15 @@ extern "C" int s2pb_aggregate(s2pb_ctx *ctx, const float *C, const int32_t *lo, 
     if (LPL < 0) return fail(S2PB_ERR_UNSUPPORTED, "too many labels");
     const int DP = 32 * LPL;
     size_t npix = (size_t)w * h, tot = npix * D;
-    for (size_t i = 0; i < tot; i++) {   // the device slab stores costs as f16 (exact for census popcounts)
+    bool fits_code = true;               // the device slab stores 8-bit cost codes (agg_kernel.cuh): integers up to kCostMaxCode
+    for (size_t i = 0; i < tot; i++) {
         float c = C[i];
         if (!(c == INFINITY || (c >= 0.f && c <= 2048.f && c == floorf(c))))
             return fail(S2PB_ERR_UNSUPPORTED, "cost %g at %zu is not an integer in [0,2048] or +inf", c, i);
+        if (c > (float)kCostMaxCode && c != INFINITY) fits_code = false;
     }
+    // larger integer costs: the float-cost flavour, which with unit weights computes the same values
+    if (!fits_code) return s2pb_aggregate_w(ctx, C, lo, hi, w, h, gmin, D, P1, P2, ndir, tsgm, fix_overcount, nullptr, S, disp, cost, conf);
     Slot &s = ctx->slots[0];
     cudaStream_t st = s.stream;
     int rc = slot_ensure(ctx, s, w, h, DP, ndir);
@@ -1682,7 +1686,7 @@ extern "C" int s2pb_aggregate(s2pb_ctx *ctx, const float *C, const int32_t *lo, 
     if (rc != S2PB_OK) return rc;
     CK(cudaMemcpyAsync(dCf.p, C, tot * 4, cudaMemcpyHostToDevice, st));
     size_t totp = npix * DP;
-    pack_cost_kernel<<<(unsigned)((totp + 255) / 256), 256, 0, st>>>(dCf.as<float>(), npix, D, DP, (__half *)s.v[0].C);
+    pack_cost_kernel<<<(unsigned)((totp + 255) / 256), 256, 0, st>>>(dCf.as<float>(), npix, D, DP, (uint8_t *)s.v[0].C);
     ctx->launches++;
     CK(cudaGetLastError());
     rc = launch_aggregate(ctx, s, 1, w, h, LPL, P1, P2, ndir, tsgm, nullptr, st);

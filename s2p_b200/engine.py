@@ -241,7 +241,7 @@ class Engine:
         return out
 
     def costvolume(self, u, v, lo, hi, gmin, D, win=5, cost=None):
-        """cost=None: the census / f16 path of the hot matcher; otherwise one of _lib.COSTS through the general path."""
+        """cost=None: the census / 8-bit cost path of the hot matcher; otherwise one of _lib.COSTS through the general path."""
         u, v = _f32(u), _f32(v)
         h, w = u.shape
         lo = np.ascontiguousarray(lo, np.int32)

@@ -30,7 +30,7 @@ def fill_pass(p, w, h):
 
 
 def run_pass(pd, C, lo_img, hi_img, gmin, DP, tsgm, P1, P2, L, Lmin):
-    """C: [npix, DP] float32 costs (the f16 slab's values), lo_img / hi_img: int16 [npix] labels.  Fills L [npix, DP], Lmin [npix]."""
+    """C: [npix, DP] float32 costs (the census slab's values), lo_img / hi_img: int16 [npix] labels.  Fills L [npix, DP], Lmin [npix]."""
     TYPE = pd["type"]
     useA = True if TYPE == 0 else tsgm == 4
     useCn = tsgm >= 2 if TYPE == 0 else tsgm >= 3

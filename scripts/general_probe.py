@@ -1,5 +1,5 @@
 """Stage timings of the general matcher flavour (float cost slab, optional -wl/-wr weights) on one C2 tile,
-next to the census / f16 hot path.  Usage on the GPU box: python scripts/general_probe.py"""
+next to the census / 8-bit cost hot path.  Usage on the GPU box: python scripts/general_probe.py"""
 import os
 import sys
 
