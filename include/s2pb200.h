@@ -186,6 +186,16 @@ int s2pb_disp_to_lonlatalt(s2pb_ctx *ctx, double *lonlatalt, float *err, const f
                            const double ha[9], const double hb[9], const s2pb_rpc *rpca, const s2pb_rpc *rpcb,
                            const float orig_img_bounding_box[4]);
 
+/* The 3D outlier filter of s2p.triangulation.filter_xyz (s2p/triangulation.py:275-343): same argument lists as
+ * lib/disp_to_h.so's count_3d_neighbors and remove_isolated_3d_points (c/disp_to_h.c:152-230), plus the context.
+ * xyz: nx*ny points of three doubles, row-major.  count[y*nx+x] = number of points of the (2p+1)^2 window, clipped at
+ * the border, whose squared distance (differences in double, rounded to float, summed in float) is < r*r.
+ * remove_isolated_3d_points rejects the points with count < n, saves every rejected point joined to a kept one by a chain
+ * of close points within (2q+1)^2 windows, and writes NaN into the three coordinates of the rest, in place.
+ * Synchronous on the context's stream. */
+int s2pb_count_3d_neighbors(s2pb_ctx *ctx, int32_t *count, const double *xyz, int nx, int ny, float r, int p);
+int s2pb_remove_isolated_3d_points(s2pb_ctx *ctx, double *xyz, int nx, int ny, float r, int p, int n, int q);
+
 /* masking.erosion (s2p/masking.py:87-97 = `morsi diskR erosion`, c/morsi.c:54-66,280-298) on a 0/1 mask */
 int s2pb_erode_mask(s2pb_ctx *ctx, const uint8_t *in, uint8_t *out, int w, int h, float radius);
 

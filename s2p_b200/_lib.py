@@ -62,6 +62,8 @@ _SIGNATURES = {
     "s2pb_merge_n": (c_int, [c_void_p, POINTER(c_void_p), POINTER(c_double), c_int, c_int, c_int, c_int, c_double, _f]),
     "s2pb_disp_to_lonlatalt": (c_int, [c_void_p, POINTER(c_double), _f, _f, _f, _f, c_int, c_int, _f, c_int, c_int,
                                        POINTER(c_double), POINTER(c_double), c_void_p, c_void_p, _f]),
+    "s2pb_count_3d_neighbors": (c_int, [c_void_p, POINTER(c_int32), POINTER(c_double), c_int, c_int, c_float, c_int]),
+    "s2pb_remove_isolated_3d_points": (c_int, [c_void_p, POINTER(c_double), c_int, c_int, c_float, c_int, c_int, c_int]),
     "s2pb_erode_mask": (c_int, [c_void_p, POINTER(c_uint8), POINTER(c_uint8), c_int, c_int, c_float]),
     "s2pb_census": (c_int, [c_void_p, _f, c_int, c_int, c_int, POINTER(c_uint64)]),
     "s2pb_costvolume": (c_int, [c_void_p, _f, _f, c_int, c_int, POINTER(c_int32), POINTER(c_int32), c_int, c_int, c_int, _f]),

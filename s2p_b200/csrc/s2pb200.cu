@@ -11,9 +11,11 @@
 #include "homography_kernels.cuh"
 #include "fusion_kernels.cuh"
 #include "triangulation_kernels.cuh"
+#include "pointcloud_kernels.cuh"
 #include "agg_dispatch.h"
 #include "agg_chunked.cuh"
 
+#include <algorithm>
 #include <atomic>
 #include <chrono>
 #include <list>
@@ -2069,5 +2071,87 @@ extern "C" int s2pb_disp_to_lonlatalt(s2pb_ctx *ctx, double *lonlatalt, float *e
     CK(cudaMemcpyAsync(lonlatalt, d_out.p, npix * 24, cudaMemcpyDeviceToHost, st));
     CK(cudaMemcpyAsync(err, d_err.p, npix * 4, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
+    return S2PB_OK;
+}
+
+// ------------------------------------------------------------------ 3D outlier filter of triangulation (section 8f)
+
+// count_3d_neighbors (c/disp_to_h.c:152-174) of a device cloud into a device count image
+static int pc_count_enqueue(s2pb_ctx *ctx, cudaStream_t st, const double *xyz, int nx, int ny, float r, int p, int *count)
+{
+    if (p < 0) { CK(cudaMemsetAsync(count, 0, (size_t)nx * ny * 4, st)); return S2PB_OK; }     // empty windows
+    p = std::min(p, std::max(nx, ny));                                  // a wider window is the whole image
+    const long long side = kPcTile + 2LL * p;
+    const size_t smem = (size_t)std::min<long long>(side, nx) * std::min<long long>(side, ny) * 24;    // one CTA's clipped footprint
+    int optin = 0;
+    CK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx->device));
+    const dim3 b(kPcTile, kPcTile), g = grid2d(nx, ny, b);
+    if (smem <= (size_t)optin) {
+        CK(cudaFuncSetAttribute(pc_count_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        pc_count_kernel<true><<<g, b, smem, st>>>(xyz, nx, ny, r, p, count);
+    } else {
+        pc_count_kernel<false><<<g, b, 0, st>>>(xyz, nx, ny, r, p, count);
+    }
+    ctx->launches++;
+    CK(cudaGetLastError());
+    return S2PB_OK;
+}
+
+// Same argument list as the reference's count_3d_neighbors (c/disp_to_h.c:152), plus the context.
+extern "C" int s2pb_count_3d_neighbors(s2pb_ctx *ctx, int32_t *count, const double *xyz, int nx, int ny, float r, int p)
+{
+    if (!ctx || !count || !xyz || nx < 1 || ny < 1) return fail(S2PB_ERR_ARG, "bad argument");
+    const size_t npix = (size_t)nx * ny;
+    if (npix > INT32_MAX) return fail(S2PB_ERR_UNSUPPORTED, "at most 2^31 - 1 points");
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t st = ctx->slots[0].stream;
+    pool_release_all(ctx);
+    double *d_xyz = (double *)pool_take(ctx, npix * 24);
+    int *d_count = (int *)pool_take(ctx, npix * 4);
+    if (!d_xyz || !d_count) { pool_release_all(ctx); return fail(S2PB_ERR_NOMEM, "cudaMalloc failed for the point-cloud buffers"); }
+    CK(cudaMemcpyAsync(d_xyz, xyz, npix * 24, cudaMemcpyHostToDevice, st));
+    int rc = pc_count_enqueue(ctx, st, d_xyz, nx, ny, r, p, d_count);
+    if (rc != S2PB_OK) { cudaStreamSynchronize(st); pool_release_all(ctx); return rc; }
+    CK(cudaMemcpyAsync(count, d_count, npix * 4, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    pool_release_all(ctx);
+    return S2PB_OK;
+}
+
+// Same argument list as the reference's remove_isolated_3d_points (c/disp_to_h.c:177-184), plus the context; in place on
+// the host cloud.  Rejection by count, then the closure of the reference's "mercy" sweeps as connected components
+// (pointcloud_kernels.cuh): label, link, flatten, mark the saved components, NaN the rest.
+extern "C" int s2pb_remove_isolated_3d_points(s2pb_ctx *ctx, double *xyz, int nx, int ny, float r, int p, int n, int q)
+{
+    if (!ctx || !xyz || nx < 1 || ny < 1) return fail(S2PB_ERR_ARG, "bad argument");
+    const size_t npix = (size_t)nx * ny;
+    if (npix > INT32_MAX) return fail(S2PB_ERR_UNSUPPORTED, "at most 2^31 - 1 points");
+    if (n <= 0) return S2PB_OK;                                         // a count is never negative: nothing is rejected
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t st = ctx->slots[0].stream;
+    pool_release_all(ctx);
+    double *d_xyz = (double *)pool_take(ctx, npix * 24);
+    int *d_count = (int *)pool_take(ctx, npix * 4), *d_lab = (int *)pool_take(ctx, npix * 4), *d_saved = (int *)pool_take(ctx, npix * 4);
+    if (!d_xyz || !d_count || !d_lab || !d_saved) { pool_release_all(ctx); return fail(S2PB_ERR_NOMEM, "cudaMalloc failed for the point-cloud buffers"); }
+    CK(cudaMemcpyAsync(d_xyz, xyz, npix * 24, cudaMemcpyHostToDevice, st));
+    int rc = pc_count_enqueue(ctx, st, d_xyz, nx, ny, r, p, d_count);
+    if (rc != S2PB_OK) { cudaStreamSynchronize(st); pool_release_all(ctx); return rc; }
+    const unsigned g1 = (unsigned)((npix + 255) / 256);
+    const dim3 b2(32, 8), g2 = grid2d(nx, ny, b2);
+    pc_label_kernel<<<g1, 256, 0, st>>>(d_count, (int)npix, n, d_lab, d_saved);
+    ctx->launches++;
+    if (q >= 0) {                                                       // q < 0: empty windows, nothing is saved
+        q = std::min(q, std::max(nx, ny));
+        pc_link_kernel<<<g2, b2, 0, st>>>(d_xyz, nx, ny, r, q, d_lab);
+        cc_flatten_kernel<<<g1, 256, 0, st>>>((int)npix, d_lab);
+        pc_mark_kernel<<<g2, b2, 0, st>>>(d_xyz, nx, ny, r, q, d_lab, d_saved);
+        ctx->launches += 3;
+    }
+    pc_reject_kernel<<<g1, 256, 0, st>>>((int)npix, d_lab, d_saved, d_xyz);
+    ctx->launches++;
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(xyz, d_xyz, npix * 24, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    pool_release_all(ctx);
     return S2PB_OK;
 }

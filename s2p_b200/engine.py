@@ -7,6 +7,7 @@ CUDA is initialised lazily in the calling process, so a forked
 ``multiprocessing`` worker (s2p/parallel.py:80) creates its own context.
 """
 import ctypes
+import operator
 import os
 
 import numpy as np
@@ -231,6 +232,42 @@ class Engine:
         u8 = lambda a: a.ctypes.data_as(ctypes.POINTER(ctypes.c_uint8))
         _lib.check(self._L.s2pb_erode_mask(self._ctx, u8(m), u8(out), w, h, float(radius)))
         return out
+
+    # ------------------------------------------------------------------ 3D outlier filter of triangulation
+    @staticmethod
+    def _cloud(xyz):
+        """The array the reference's ctypes call receives, np.ascontiguousarray(xyz), with the checks its
+        ndpointer(c_double, shape=(h, w, 3)) argument type makes."""
+        a = np.ascontiguousarray(xyz)
+        if a.ndim != 3 or a.shape[2] != 3:
+            raise ValueError("expecting a 3-channels image with shape (h, w, 3), got shape %s" % (a.shape,))
+        if a.dtype != np.float64:
+            raise TypeError("the point cloud must be float64, got %s" % a.dtype)
+        return a
+
+    def count_3d_neighbors(self, xyz, r, p):
+        """-> (h, w) int32: per point, the points of its (2p+1)^2 window closer than r (c/disp_to_h.c:152-174).
+        r is rounded to float32, as the reference's c_float argument is."""
+        a = self._cloud(xyz)
+        h, w = a.shape[:2]
+        out = np.zeros((h, w), np.int32)
+        if a.size:
+            _lib.check(self._L.s2pb_count_3d_neighbors(self._ctx, out.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)),
+                                                        a.ctypes.data_as(ctypes.POINTER(ctypes.c_double)), w, h, float(r),
+                                                        operator.index(p)))
+        return out
+
+    def remove_isolated_3d_points(self, xyz, r, p, n, q=1):
+        """NaN into the isolated points of np.ascontiguousarray(xyz), in place (c/disp_to_h.c:177-230): a C-contiguous
+        float64 xyz is itself modified.  -> that array."""
+        a = self._cloud(xyz)
+        h, w = a.shape[:2]
+        if not a.flags.writeable:
+            raise ValueError("the point cloud is read-only")
+        if a.size:
+            _lib.check(self._L.s2pb_remove_isolated_3d_points(self._ctx, a.ctypes.data_as(ctypes.POINTER(ctypes.c_double)), w, h,
+                                                               float(r), operator.index(p), operator.index(n), operator.index(q)))
+        return a
 
     # ------------------------------------------------------------------ stages (parity tests)
     def census(self, img, win=5):

@@ -5,6 +5,9 @@ The reference triangulates through ``lib/disp_to_h.so`` loaded with ctypes (s2p/
 byref(rpc2), bbx)`` (:134-143).  ``s2pb_disp_to_lonlatalt`` takes the same argument list (plus the context) and
 ``RPCStruct`` below has the layout of the reference's ``struct rpc`` / ``RPCStruct``; ``install()`` swaps the
 library handle of an importable ``s2p.triangulation`` for an adapter that forwards the very same call.
+
+The 3D outlier filter of the same library, ``count_3d_neighbors`` and ``remove_isolated_3d_points`` (c/disp_to_h.c:143-230),
+which ``filter_xyz`` runs on the cloud of a tile (s2p/triangulation.py:275-343), goes through the adapter too.
 """
 import ctypes
 from ctypes import c_double
@@ -69,8 +72,29 @@ def disp_to_lonlatalt(disp, mask_rect, mask_orig, H1, H2, rpc1, rpc2, img_bbx, d
     return out, err
 
 
+def count_3d_neighbors(xyz, r, p, engine=None):
+    """s2p.triangulation.count_3d_neighbors: -> (h, w) int32, per point the number of points of its (2p+1)^2 window
+    (clipped at the border, itself included) closer than r units."""
+    return (engine or get_engine()).count_3d_neighbors(xyz, r, p)
+
+
+def remove_isolated_3d_points(xyz, r, p, n, q=1, engine=None):
+    """s2p.triangulation.remove_isolated_3d_points: NaN into the points with fewer than n neighbours closer than r in
+    their (2p+1)^2 window, except those joined to a kept point by a chain of close points within (2q+1)^2 windows.
+    In place on np.ascontiguousarray(xyz), as the reference: a C-contiguous float64 xyz is modified, another is not."""
+    (engine or get_engine()).remove_isolated_3d_points(xyz, r, p, n, q)
+
+
+def filter_xyz(xyz, r, n, img_gsd, engine=None):
+    """s2p.triangulation.filter_xyz: remove_isolated_3d_points with p = ceil(r / img_gsd) and q = 1."""
+    p = np.ceil(r / img_gsd).astype(int)
+    remove_isolated_3d_points(xyz, r, p, n, engine=engine)
+
+
 class _LibAdapter:
-    """Stands in for ``s2p.triangulation.lib``: ``disp_to_lonlatalt`` goes to the GPU, anything else to the original."""
+    """Stands in for ``s2p.triangulation.lib``: ``disp_to_lonlatalt``, ``count_3d_neighbors`` and
+    ``remove_isolated_3d_points`` go to the GPU, anything else to the original.  Each takes the positional arguments of
+    the library function and writes into the arrays it is given."""
 
     def __init__(self, original):
         self._original = original
@@ -80,11 +104,28 @@ class _LibAdapter:
             lonlatalt[...] = out
             err[...] = e
 
-        call.argtypes = None        # s2p assigns .argtypes before calling (s2p/triangulation.py:118)
-        self.disp_to_lonlatalt = call
+        def count(out, xyz, w, h, r, p):
+            _check_cloud(xyz, w, h)
+            out[...] = count_3d_neighbors(xyz, np.float32(r), p)
+
+        def remove(xyz, w, h, r, p, n, q):
+            _check_cloud(xyz, w, h)
+            remove_isolated_3d_points(xyz, np.float32(r), p, n, q)
+
+        # s2p assigns .argtypes before calling (s2p/triangulation.py:118,293,324)
+        for name, fn in (("disp_to_lonlatalt", call), ("count_3d_neighbors", count), ("remove_isolated_3d_points", remove)):
+            fn.argtypes = None
+            setattr(self, name, fn)
 
     def __getattr__(self, name):
         return getattr(self._original, name)
+
+
+def _check_cloud(xyz, w, h):
+    """what the ndpointer(c_double, shape=(h, w, 3)) argument type s2p assigns would check, and that xyz is the memory
+    the library would write to"""
+    if not isinstance(xyz, np.ndarray) or xyz.dtype != np.float64 or xyz.shape != (h, w, 3) or not xyz.flags.c_contiguous:
+        raise TypeError("expecting a C-contiguous float64 array of shape (%d, %d, 3)" % (h, w))
 
 
 def install():
