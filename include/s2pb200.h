@@ -18,6 +18,8 @@
  *                        3rdparty/homography/main.cpp:65-177)
  *   s2pb_mgm_batch()     the per-(tile,pair) fan-out of stereo_matching through
  *                        parallel.launch_calls (s2p/__init__.py:166-196,586-591)
+ *   s2pb_sgbm()          the `sgbm` subprocess (OpenCV 2's StereoSGBM, 3rdparty/sgbm) + create_rejection_mask
+ *                        (s2p/block_matching.py:116-134)
  *
  * Conventions: all images are single-band, row-major, C-contiguous float32,
  * NaN = no data.  Disparity d at ref pixel (x,y) means the match is at
@@ -141,6 +143,24 @@ int s2pb_mgm_batch(s2pb_ctx *ctx, int n, const float *const *im1, const float *c
 int s2pb_reserve(s2pb_ctx *ctx, int nslots, int w, int h, int nlabels);
 int s2pb_num_slots(const s2pb_ctx *ctx);
 int s2pb_sync(s2pb_ctx *ctx);
+
+/* ---- the `sgbm` matcher (3rdparty/sgbm/sgbm.cpp + stereosgbm.cpp) ----------------- */
+/* The binary's argv after dmin dmax (`sgbm im1 im2 disp cost dmin dmax win P1 P2 lr`).  What it hardcodes stays
+ * constant: fullDP, preFilterCap 63, uniquenessRatio 10, speckle window 50 and range 1, median 3x3. */
+typedef struct s2pb_sgbm_params {
+    int32_t win;             /* SADwindow    odd window side                                      */
+    int32_t P1;              /* P1           <= 0: 2 (stereosgbm.cpp:334)                         */
+    int32_t P2;              /* P2           <= 0: 5; at least P1 + 1                             */
+    int32_t lr_diff;         /* LRdiff       disp12MaxDiff; <= 0: 1                               */
+} s2pb_sgbm_params;
+/* what s2p passes: win 3, P1 8, P2 32, lr_diff 1 */
+int s2pb_sgbm_default_params(s2pb_sgbm_params *p);
+/* Bit for bit the disparity the `sgbm` binary writes (NaN = rejected; the padding of its crop trick taken as zero),
+ * then the rejection mask of s2pb_mgm.  disp: w*h float32; mask: w*h uint8 or NULL.  Host buffers, pageable or
+ * page-locked; synchronous.  S2PB_ERR_ARG: dmin >= dmax or an even / non-positive win, as the binary.
+ * S2PB_ERR_UNSUPPORTED: disparities x16 outside int16, or win^2 * 189 + 2 * P2 > 32767 or P2 > 4096 (int16 path costs). */
+int s2pb_sgbm(s2pb_ctx *ctx, const float *im1, const float *im2, int w, int h, int dmin, int dmax,
+              const s2pb_sgbm_params *p, float *disp, uint8_t *mask);
 
 /* ---- rectification warp ---------------------------------------------------- */
 /* dst(j,i) = src sampled at H^-1 (j,i,1), order-5 B-spline with the reference's

@@ -26,6 +26,11 @@ class MgmParams(ctypes.Structure):
     ]
 
 
+class SgbmParams(ctypes.Structure):
+    """Mirror of ``s2pb_sgbm_params``: the `sgbm` binary's argv after dmin dmax."""
+    _fields_ = [("win", c_int32), ("P1", c_int32), ("P2", c_int32), ("lr_diff", c_int32)]
+
+
 COSTS = ("census", "ad", "sd", "ncc", "btad", "btsd")   # S2PB_COST_* = index; the reference's `-t` names
 
 
@@ -59,6 +64,8 @@ _SIGNATURES = {
     "s2pb_homography": (c_int, [c_void_p, _f, c_int, c_int, POINTER(c_double), _f, c_int, c_int]),
     "s2pb_rectify_match": (c_int, [c_void_p, _f, c_int, c_int, POINTER(c_double), _f, c_int, c_int, POINTER(c_double), c_int, c_int,
                                    c_int, c_int, POINTER(MgmParams), _f, _f, _f, _f, POINTER(c_uint8), _f]),
+    "s2pb_sgbm_default_params": (c_int, [POINTER(SgbmParams)]),
+    "s2pb_sgbm": (c_int, [c_void_p, _f, _f, c_int, c_int, c_int, c_int, POINTER(SgbmParams), _f, POINTER(c_uint8)]),
     "s2pb_merge_n": (c_int, [c_void_p, POINTER(c_void_p), POINTER(c_double), c_int, c_int, c_int, c_int, c_double, _f]),
     "s2pb_disp_to_lonlatalt": (c_int, [c_void_p, POINTER(c_double), _f, _f, _f, _f, c_int, c_int, _f, c_int, c_int,
                                        POINTER(c_double), POINTER(c_double), c_void_p, c_void_p, _f]),

@@ -3,8 +3,11 @@
 ``compute_disparity_map`` keeps the reference's signature, file contract and exceptions
 (s2p/block_matching.py:35-336) but, for ``algo in {'mgm', 'mgm_multi', 'mgm_multi_lsd'}``, runs the H100 engine
 through the C ABI instead of spawning the ``mgm`` / ``mgm_multi`` binaries and the three
-``plambda`` / ``backflow`` processes of ``create_rejection_mask``.  Any other ``algo`` is handed to
-the original s2p implementation when that package is importable.
+``plambda`` / ``backflow`` processes of ``create_rejection_mask``.  ``algo == 'sgbm'`` with both
+disparity bounds given (as s2p always passes them) runs the engine's bit-exact restatement of the
+``sgbm`` binary with s2p's arguments (win 3, P1 8, P2 32, lr 1) and writes no confidence file, as the
+reference does.  Any other ``algo`` (and ``sgbm`` with a bound of None) is handed to the original s2p
+implementation when that package is importable.
 
     disp  -> float32 TIFF, NaN = rejected
     '<disp stem>_confidence.tif' -> float32 TIFF, consensus 0..nb_directions (read at s2p/__init__.py:263-265)
@@ -29,6 +32,7 @@ except Exception:
         pass
 
 _NATIVE = ("mgm", "mgm_multi", "mgm_multi_lsd")
+SGBM_ARGS = dict(win=3, P1=8, P2=32, lr_diff=1)    # `sgbm ... dmin dmax 3 8 32 1`, s2p/block_matching.py:116-134
 
 
 def disparity_bounds(width, disp_min, disp_max, max_disp_range=None):
@@ -109,6 +113,8 @@ def compute_disparity_map(im1, im2, disp, mask, algo, disp_min=None, disp_max=No
     Raises MaxDisparityRangeError, subprocess.TimeoutExpired (``timeout`` seconds exceeded, as
     ``common.run(timeout=)`` does for the mgm binaries) or subprocess.CalledProcessError.
     """
+    if algo == "sgbm" and disp_min is not None and disp_max is not None:
+        return _sgbm(im1, im2, disp, mask, disp_min, disp_max, max_disp_range)
     if algo not in _NATIVE:
         fn = _original_compute_disparity_map()
         if fn is None:
@@ -137,6 +143,24 @@ def compute_disparity_map(im1, im2, disp, mask, algo, disp_min=None, disp_max=No
         raise subprocess.CalledProcessError(-e.code, cmd, output=str(e)) from e
     rio.write_float_tiff(disp, out["disp"])
     rio.write_float_tiff(confidence_path(disp, algo), out["conf"])
+    rio.write_mask_png(mask, out["mask"])
+
+
+def _sgbm(im1, im2, disp, mask, disp_min, disp_max, max_disp_range):
+    """The reference's 'sgbm' branch (s2p/block_matching.py:116-134): the binary, then create_rejection_mask."""
+    width, _ = rio.image_size(im1)
+    disp_min, disp_max = disparity_bounds(width, disp_min, disp_max, max_disp_range)
+    cmd = ["s2pb200:sgbm", im1, im2, disp, str(disp_min), str(disp_max)] + [str(v) for v in SGBM_ARGS.values()]
+    print("\nRUN: %s" % " ".join(cmd))
+    a, b = rio.read_band(im1), rio.read_band(im2)
+    if a.shape != b.shape:
+        raise subprocess.CalledProcessError(1, cmd, output="rectified images differ in size")
+    eng = get_engine()
+    try:
+        out = eng.sgbm(a, b, disp_min, disp_max, eng.sgbm_params(**SGBM_ARGS), want_mask=True)
+    except S2pbError as e:
+        raise subprocess.CalledProcessError(-e.code, cmd, output=str(e)) from e
+    rio.write_float_tiff(disp, out["disp"])
     rio.write_mask_png(mask, out["mask"])
 
 

@@ -13,7 +13,7 @@ import os
 import numpy as np
 
 from . import _lib
-from ._lib import MgmParams, S2pbError  # noqa: F401  (re-exported)
+from ._lib import MgmParams, S2pbError, SgbmParams  # noqa: F401  (re-exported)
 
 
 def default_params(algo="mgm", **overrides):
@@ -110,6 +110,32 @@ class Engine:
         if want_right:
             out["disp_right"] = right
         return out
+
+    # ------------------------------------------------------------------ sgbm
+    @staticmethod
+    def sgbm_params(**overrides):
+        """What s2p passes to the `sgbm` binary (win 3, P1 8, P2 32, lr_diff 1), then the overrides."""
+        p = SgbmParams()
+        _lib.check(_lib.lib().s2pb_sgbm_default_params(ctypes.byref(p)))
+        for k, v in overrides.items():
+            if not hasattr(p, k):
+                raise TypeError("unknown sgbm parameter %r" % k)
+            setattr(p, k, int(v))
+        return p
+
+    def sgbm(self, im1, im2, dmin, dmax, params=None, want_mask=True):
+        """-> dict(disp, mask): what `sgbm im1 im2 disp cost dmin dmax win P1 P2 lr` writes (NaN = rejected), then
+        create_rejection_mask on the float inputs (mask None when ``want_mask`` is false).  No confidence image."""
+        p = params or self.sgbm_params()
+        im1, im2 = _f32(im1), _f32(im2)
+        if im1.shape != im2.shape or im1.ndim != 2:
+            raise ValueError("im1 and im2 must be 2-D arrays of the same shape")
+        h, w = im1.shape
+        disp = np.empty((h, w), np.float32)
+        mask = np.empty((h, w), np.uint8) if want_mask else None
+        _lib.check(self._L.s2pb_sgbm(self._ctx, _fp(im1), _fp(im2), w, h, int(dmin), int(dmax), ctypes.byref(p), _fp(disp),
+                                     mask.ctypes.data_as(ctypes.POINTER(ctypes.c_uint8)) if want_mask else None))
+        return dict(disp=disp, mask=mask)
 
     def mgm_batch(self, refs, secs, dmin, dmax, params=None, want_mask=True, out=None):
         """n same-shaped pairs pipelined over the context's workspaces (s2pb_reserve first for overlap).
