@@ -1,4 +1,4 @@
-// agg_chunked.cu -- instantiations and launcher of the experimental chunk-skipping aggregation (agg_chunked.cuh).
+// agg_chunked.cu -- instantiations and launcher of the chunk-skipping aggregation (agg_chunked.cuh).
 #include "agg_chunked.cuh"
 #include "agg_dispatch.h"
 

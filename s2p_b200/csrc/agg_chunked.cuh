@@ -1,5 +1,7 @@
-// agg_chunked.cuh -- EXPERIMENTAL (off by default, S2PB_CHUNKED=1 selects it): the MGM
-// aggregation for volumes whose pixels use a small part of the slab, i.e. the fine levels of mgm_multi.
+// agg_chunked.cuh -- the MGM aggregation for slabs wider than 512 slots, which the register-resident kernel of agg_kernel.cuh
+// cannot hold: a level of mgm_multi whose label hull exceeds 512 labels, or `mgm` with more than 512 labels.  It computes only
+// the 32-label chunks that hold each pixel's label range, which is what it was first written for: volumes whose pixels use a
+// small part of the slab, i.e. the fine levels of mgm_multi.
 //
 // Why.  update_dmin_dmax gives most pixels of a fine level 17..40 labels but hands the parent's full range to every
 // pixel next to a rejected one, so the dense slab spans up to 512 labels while the mean range is ~65
@@ -13,16 +15,16 @@
 //   * one scanline per warp (16 warps per CTA) and the neighbours' vectors live in SHARED memory, read with
 //     offsets -1 / 0 / +1 (no shuffles, no register windows); every stored vector carries its chunk span and an
 //     +INF guard on both sides of the span, chunks of a neighbour outside its span read as +INF;
-//   * the chunks a pixel does not compute are either written as +INF to the global L volume (fill_inf: the dense WTA
-//     kernel then works on the result) or left untouched (the chunk-skipping WTA of mgm_kernels.cuh never reads
-//     them; the band hand-off then carries the previous band's spans as well).
+//   * the chunks a pixel does not compute are left untouched in the global L volume (the chunk-skipping WTA of
+//     mgm_kernels.cuh never reads them; the band hand-off carries the previous band's spans as well).
 // The label range of a pixel only enters through its span; slots of an active chunk outside the range hold +INF
 // costs and therefore +INF results, exactly as in the dense kernel.
 // Status: scripts/chunked_emulator.py replays this file's indexing on the CPU (ring slots, guards, staging slots,
 // range words, previous-band ring) and equals the oracle bit for bit for every TSGM and slab width; it found the
 // chunk-edge case of term() below (a neighbour whose span starts right after / ends right before my chunk), which
 // the first GPU run showed as 1.5 % differing pixels on the 512-slot level.  The corrected kernel is bit-identical on the
-// GPU (tests/test_gpu_parity.py) but not faster than the dense kernel on ragged levels (DESIGN.md section 3.3).
+// GPU (tests/test_gpu_parity.py) but not faster than the dense kernel on ragged levels (DESIGN.md section 3.3), so slabs of
+// up to 512 slots stay with the dense kernel.
 #pragma once
 #include "agg_kernel.cuh"
 
@@ -45,8 +47,6 @@ struct ChunkedParams {
     const short *lo[kMaxPV], *hi[kMaxPV];   // per pass-view: the view's per-pixel label range
     int gmin[kMaxPV];                       // ... and the label of slot 0
     int DP;                                 // slots per pixel (multiple of 32, <= 2048)
-    int fill_inf;                           // 1: write +INF to the chunks a pixel skips (the dense WTA kernel then works on the
-                                            // result); 0: leave them untouched (the chunk-skipping WTA never reads them)
 };
 
 // shared memory carve-up for a run-time DP
@@ -69,7 +69,7 @@ struct CkSmem {
 
 template <int TSGM, int TYPE, bool SCALED, int STAGE>
 __device__ __forceinline__ void run_band_chunked(const PassDesc &pd, const short *__restrict__ lo_img, const short *__restrict__ hi_img,
-                                                 int gmin, int DP, bool fill_inf, int band, float P1, float P2,
+                                                 int gmin, int DP, int band, float P1, float P2,
                                                  const float *__restrict__ lut, const int *abort_flag, unsigned char *smem)
 {
     constexpr bool useA = (TYPE == 0) ? true : (TSGM == 4);
@@ -281,8 +281,8 @@ __device__ __forceinline__ void run_band_chunked(const PassDesc &pd, const short
                     }
                     mine[kk] = L;
                     lm = fminf(lm, L);
+                    out[kk] = L;
                 }
-                if (fill_inf || (e >= ea && e <= eb)) out[kk] = L;          // +INF for the chunks outside my span, if asked for
             }
             const float m = warp_min_f32(lm);
             if (lane == 0) {
@@ -324,8 +324,8 @@ __global__ void __launch_bounds__(kCkThreads) aggregate_chunked_kernel(const __g
         const int band = item / P.A.nPV, pvi = item - band * P.A.nPV;
         const PassDesc &pd = P.A.pv[pvi];
         if (band >= (pd.nS + kCkWarps - 1) / kCkWarps) continue;
-        if (pd.type == 0) run_band_chunked<TSGM, 0, SCALED, STAGE>(pd, P.lo[pvi], P.hi[pvi], P.gmin[pvi], P.DP, P.fill_inf != 0, band, P.A.P1, P.A.P2, P.A.lut, P.A.abort_flag, smem);
-        else run_band_chunked<TSGM, 1, SCALED, STAGE>(pd, P.lo[pvi], P.hi[pvi], P.gmin[pvi], P.DP, P.fill_inf != 0, band, P.A.P1, P.A.P2, P.A.lut, P.A.abort_flag, smem);
+        if (pd.type == 0) run_band_chunked<TSGM, 0, SCALED, STAGE>(pd, P.lo[pvi], P.hi[pvi], P.gmin[pvi], P.DP, band, P.A.P1, P.A.P2, P.A.lut, P.A.abort_flag, smem);
+        else run_band_chunked<TSGM, 1, SCALED, STAGE>(pd, P.lo[pvi], P.hi[pvi], P.gmin[pvi], P.DP, band, P.A.P1, P.A.P2, P.A.lut, P.A.abort_flag, smem);
     }
 }
 

@@ -343,7 +343,7 @@ __global__ void unpad_cost_kernel(const float *__restrict__ C, size_t npix, int 
     Cout[i] = C[p * DP + k];
 }
 
-// Companion of agg_chunked.cuh (slabs wider than 512 slots; S2PB_CHUNKED=1 for a measurement on narrower ones): the census cost volume written only on the 32-slot
+// Companion of agg_chunked.cuh (slabs wider than 512 slots): the census cost volume written only on the 32-slot
 // chunks [ea, eb] that hold a pixel's label range (slot 32*e + lane); the chunk-skipping aggregation and WTA never
 // read the others.  Same values as cost_kernel on those chunks, including +INF on the slots of an active chunk that
 // lie outside the range and the all-invalid -> 0 rule (mgm_costvolume.cc:166-171).
@@ -610,7 +610,7 @@ __global__ void __launch_bounds__(kWtaThreads) __maxnreg__((LPL <= 4) ? 64 : 128
     else wta_pixels<LPL, GEN, 0>(P, sSrow);
 }
 
-// Companion of agg_chunked.cuh (slabs wider than 512 slots; S2PB_CHUNKED=1 for a measurement on narrower ones): the same WTA for
+// Companion of agg_chunked.cuh (slabs wider than 512 slots): the same WTA for
 // slabs whose pixels use few of their 32-label chunks.  A warp owns a pixel and only reads the chunks [ea, eb] that hold its
 // label range (slot 32*e + lane), so a 40-label pixel of a 512-slot slab reads 2 x 128 B per pass instead of 2 KB.
 // Per lane it keeps, for every pass, the running minimum and the LAST slot attaining it, and for S the running
