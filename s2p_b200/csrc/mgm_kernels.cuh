@@ -238,85 +238,95 @@ __device__ __forceinline__ float ncc_finish(float prod, float n, float2 a, float
     return (1.f - cl) * 64.f;
 }
 
+// The costs of LPL labels of one pixel for one lane, label o0 + e in element e: +INF outside [l, hgh] or where the matched
+// column (or an NCC tap) leaves the image.  -> whether one of them is finite (the caller applies the all-invalid rule).
+template <int LPL>
+__device__ __forceinline__ bool cost_gen_labels(const CostGenParams &P, size_t p, int x, int y, int l, int hgh, int o0, float (&c)[LPL])
+{
+    const int w = P.w, hw = P.win / 2;
+    const size_t row = p - x;
+    bool anyfinite = false;
+    if (P.cost == kCostNCC) {
+        // cross term of every label of this lane at once: the taps run in the reference's order (x-major) for each
+        // label, the reference image's tap is loaded once per tap instead of once per tap and label
+        int q[LPL];
+        const float *vq[LPL];
+        bool ok[LPL];
+        const bool pin = x - hw >= 0 && x + hw < w && y - hw >= 0 && y + hw < P.h;
+#pragma unroll
+        for (int e = 0; e < LPL; e++) {
+            const int o = o0 + e;
+            q[e] = x + o;
+            bool half = false;
+            if (P.zoom == 2) { q[e] = x + (o >> 1); half = (o & 1) != 0; }
+            vq[e] = half ? P.v1 : P.v0;
+            c[e] = S2PB_INF;
+            const bool inrange = o >= l && o <= hgh && q[e] >= 0 && q[e] < w;          // else the slot stays +INF
+            ok[e] = inrange && pin && q[e] - hw >= 0 && q[e] + hw < w;                  // else a tap is outside: +INF
+            if (ok[e]) c[e] = 0.f;
+        }
+        for (int i = -hw; i <= hw; i++)
+            for (int j = -hw; j <= hw; j++) {
+                const size_t r = (size_t)(y + j) * w;
+                const float ut = pin ? P.u[r + x + i] : 0.f;
+#pragma unroll
+                for (int e = 0; e < LPL; e++)
+                    if (ok[e]) c[e] = fmaf(ut, vq[e][r + q[e] + i], c[e]);
+            }
+        const float n = (float)(P.win * P.win);
+        const float2 sa = pin ? P.su[p] : make_float2(0.f, 0.f);
+#pragma unroll
+        for (int e = 0; e < LPL; e++)
+            if (ok[e]) {
+                const float2 sb = (vq[e] == P.v1 ? P.sv1 : P.sv0)[row + q[e]];
+                c[e] = ncc_finish(c[e], n, sa, sb);
+                if (isfinite(c[e])) anyfinite = true;
+            }
+    } else
+#pragma unroll
+    for (int e = 0; e < LPL; e++) {
+        const int o = o0 + e;
+        float val = S2PB_INF;
+        if (o >= l && o <= hgh) {
+            int q = x + o;
+            bool half = false;
+            if (P.zoom == 2) { q = x + (o >> 1); half = (o & 1) != 0; }       // floor(o/2), goodmod(o,2)
+            if (q >= 0 && q < w) {
+                if (P.cost == kCostCensus) {
+                    const uint64_t *codes = half ? P.cv1 : P.cv0;
+                    val = P.lut[__popcll(P.cu[p] ^ codes[row + q])];
+                } else {
+                    const float *v = half ? P.v1 : P.v0;
+                    if (P.cost == kCostBTAD || P.cost == kCostBTSD) {
+                        const float b = bt_cost(P.u, v, w, row, x, q);
+                        val = (P.cost == kCostBTAD) ? b : b * b;
+                    } else {
+                        float d = P.u[p] - v[row + q];
+                        d = (d > -d) ? d : -d;
+                        val = (P.cost == kCostAD) ? d : d * d;
+                    }
+                }
+                if (isfinite(val)) anyfinite = true;
+            }
+        }
+        c[e] = val;
+    }
+    return anyfinite;
+}
+
 // one warp per pixel, lanes over labels (slot k <-> label gmin + k), like cost_kernel
 template <int LPL>
 __global__ void cost_gen_kernel(const CostGenParams P)
 {
     constexpr int DP = 32 * LPL;
-    const int lane = threadIdx.x & 31, w = P.w, hw = P.win / 2;
+    const int lane = threadIdx.x & 31, w = P.w;
     const size_t npix = (size_t)w * P.h;
     size_t warp = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = ((size_t)gridDim.x * blockDim.x) >> 5;
     for (size_t p = warp; p < npix; p += nwarps) {
         const int x = (int)(p % w), y = (int)(p / w);
-        const size_t row = p - x;
         const int l = P.lo[p], hgh = P.hi[p];
         float c[LPL];
-        bool anyfinite = false;
-        if (P.cost == kCostNCC) {
-            // cross term of every label of this lane at once: the taps run in the reference's order (x-major) for each
-            // label, the reference image's tap is loaded once per tap instead of once per tap and label
-            int q[LPL];
-            const float *vq[LPL];
-            bool ok[LPL];
-            const bool pin = x - hw >= 0 && x + hw < w && y - hw >= 0 && y + hw < P.h;
-#pragma unroll
-            for (int e = 0; e < LPL; e++) {
-                const int o = P.gmin + lane * LPL + e;
-                q[e] = x + o;
-                bool half = false;
-                if (P.zoom == 2) { q[e] = x + (o >> 1); half = (o & 1) != 0; }
-                vq[e] = half ? P.v1 : P.v0;
-                c[e] = S2PB_INF;
-                const bool inrange = o >= l && o <= hgh && q[e] >= 0 && q[e] < w;          // else the slot stays +INF
-                ok[e] = inrange && pin && q[e] - hw >= 0 && q[e] + hw < w;                  // else a tap is outside: +INF
-                if (ok[e]) c[e] = 0.f;
-            }
-            for (int i = -hw; i <= hw; i++)
-                for (int j = -hw; j <= hw; j++) {
-                    const size_t r = (size_t)(y + j) * w;
-                    const float ut = pin ? P.u[r + x + i] : 0.f;
-#pragma unroll
-                    for (int e = 0; e < LPL; e++)
-                        if (ok[e]) c[e] = fmaf(ut, vq[e][r + q[e] + i], c[e]);
-                }
-            const float n = (float)(P.win * P.win);
-            const float2 sa = pin ? P.su[p] : make_float2(0.f, 0.f);
-#pragma unroll
-            for (int e = 0; e < LPL; e++)
-                if (ok[e]) {
-                    const float2 sb = (vq[e] == P.v1 ? P.sv1 : P.sv0)[row + q[e]];
-                    c[e] = ncc_finish(c[e], n, sa, sb);
-                    if (isfinite(c[e])) anyfinite = true;
-                }
-        } else
-#pragma unroll
-        for (int e = 0; e < LPL; e++) {
-            const int o = P.gmin + lane * LPL + e;
-            float val = S2PB_INF;
-            if (o >= l && o <= hgh) {
-                int q = x + o;
-                bool half = false;
-                if (P.zoom == 2) { q = x + (o >> 1); half = (o & 1) != 0; }       // floor(o/2), goodmod(o,2)
-                if (q >= 0 && q < w) {
-                    if (P.cost == kCostCensus) {
-                        const uint64_t *codes = half ? P.cv1 : P.cv0;
-                        val = P.lut[__popcll(P.cu[p] ^ codes[row + q])];
-                    } else {
-                        const float *v = half ? P.v1 : P.v0;
-                        if (P.cost == kCostBTAD || P.cost == kCostBTSD) {
-                            const float b = bt_cost(P.u, v, w, row, x, q);
-                            val = (P.cost == kCostBTAD) ? b : b * b;
-                        } else {
-                            float d = P.u[p] - v[row + q];
-                            d = (d > -d) ? d : -d;
-                            val = (P.cost == kCostAD) ? d : d * d;
-                        }
-                    }
-                    if (isfinite(val)) anyfinite = true;
-                }
-            }
-            c[e] = val;
-        }
+        const bool anyfinite = cost_gen_labels<LPL>(P, p, x, y, l, hgh, P.gmin + lane * LPL, c);
         if (!__any_sync(0xffffffffu, anyfinite)) {        // mgm_costvolume.cc:166-171
 #pragma unroll
             for (int e = 0; e < LPL; e++) {
@@ -379,6 +389,33 @@ __global__ void cost_chunked_kernel(const uint64_t *__restrict__ cu, const uint6
             for (int e = ea; e <= eb; e++) {
                 const int o = gmin + 32 * e + lane;
                 if (o >= l && o <= hgh) dst[32 * e + lane] = (uint8_t)cost_encode(0, true);
+            }
+        }
+    }
+}
+
+// The same for the general flavour: cost_gen_kernel's float costs, written only on the chunks [ea, eb] of each pixel's span
+// (slot 32*e + lane), +INF on the slots of an active chunk outside the range; the other chunks are left untouched.
+__global__ void cost_gen_chunked_kernel(const CostGenParams P, int DP)
+{
+    const int lane = threadIdx.x & 31, w = P.w;
+    const size_t npix = (size_t)w * P.h;
+    size_t warp = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = ((size_t)gridDim.x * blockDim.x) >> 5;
+    for (size_t p = warp; p < npix; p += nwarps) {
+        const int x = (int)(p % w), y = (int)(p / w);
+        const int l = P.lo[p], hgh = P.hi[p];
+        const int ea = (l - P.gmin) >> 5, eb = (hgh - P.gmin) >> 5;
+        float *dst = P.C + p * DP;
+        bool anyfinite = false;
+        for (int e = ea; e <= eb; e++) {
+            float c[1];
+            if (cost_gen_labels<1>(P, p, x, y, l, hgh, P.gmin + 32 * e + lane, c)) anyfinite = true;
+            dst[32 * e + lane] = c[0];
+        }
+        if (!__any_sync(0xffffffffu, anyfinite)) {        // mgm_costvolume.cc:166-171
+            for (int e = ea; e <= eb; e++) {
+                const int o = P.gmin + 32 * e + lane;
+                if (o >= l && o <= hgh) dst[32 * e + lane] = 0.f;
             }
         }
     }
@@ -614,13 +651,13 @@ __global__ void __launch_bounds__(kWtaThreads) __maxnreg__((LPL <= 4) ? 64 : 128
 // slabs whose pixels use few of their 32-label chunks.  A warp owns a pixel and only reads the chunks [ea, eb] that hold its
 // label range (slot 32*e + lane), so a 40-label pixel of a 512-slot slab reads 2 x 128 B per pass instead of 2 KB.
 // Per lane it keeps, for every pass, the running minimum and the LAST slot attaining it, and for S the running
-// first minimum; S itself goes to shared memory for the sub-pixel fit.  Same arithmetic as wta_kernel.
+// first minimum; S itself goes to shared memory for the sub-pixel fit.  Same arithmetic as wta_kernel<LPL, GEN>.
+template <bool GEN>
 __global__ void __launch_bounds__(kWtaThreads) wta_chunked_kernel(const WtaParams P, int DP)
 {
     extern __shared__ float sS_all[];                    // [warps][DP]
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     float *sS = sS_all + (size_t)wib * DP;
-    const uint8_t *C = reinterpret_cast<const uint8_t *>(P.C);
     size_t warp = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = ((size_t)gridDim.x * blockDim.x) >> 5;
     for (size_t p = warp; p < P.npix; p += nwarps) {
         const int lo = P.lo[p] - P.gmin, hi = P.hi[p] - P.gmin;      // slots
@@ -641,7 +678,8 @@ __global__ void __launch_bounds__(kWtaThreads) wta_chunked_kernel(const WtaParam
                     if (v < pm[d]) { pm[d] = v; pa[d] = kk; } else if (v == pm[d]) pa[d] = kk;
                     s += v;
                 }
-            const float c = cost_value(C[p * DP + kk], P.lut);
+            const float c = GEN ? reinterpret_cast<const float *>(P.C)[p * DP + kk]
+                                : cost_value(reinterpret_cast<const uint8_t *>(P.C)[p * DP + kk], P.lut);
             if (P.fix_overcount == 1) s = fmaf(-(float)(P.ndir - 1), c, s);
             if (isfinite(s) && best > s) { best = s; bidx = kk; }
             sS[kk] = s;

@@ -2,9 +2,12 @@
 staging slots, the 4-byte range words, the previous band's ring.  Warps run one after the other inside a step and
 bands one after the other, so this checks the kernel's indexing and masking logic, not its synchronisation.  The
 sum of the emulated pass volumes is compared with the oracle's aggregated volume (bit for bit).
+EMU_GENERAL=1 replays the general flavour (GEN): float costs, a weight image, penalties P*w rounded as the kernel does,
+with the kernel's warps and pipeline depth for the slab (ck_warps / ck_stage).
 usage: python scripts/chunked_emulator.py [DP] [h] [w] [tsgm] [seed]"""
 import os
 import sys
+from fractions import Fraction
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
@@ -20,6 +23,24 @@ if os.environ.get("EMU_WARPS"):          # the configurations of the slabs wider
     R0 = 2 * STAGE
 FIXED = os.environ.get("EMU_BUGGY") != "1"      # EMU_BUGGY=1 reproduces the first version of the kernel (chunk-edge bug)
 FILL_INF = os.environ.get("EMU_FILL_INF") == "1"   # 1: the variant that writes +INF to the skipped chunks of the global volume
+GENERAL = os.environ.get("EMU_GENERAL") == "1"
+
+
+def fma32(a, b, c):
+    """fmaf on float32 values: a*b is exact in float64, and the float64 sum rounds to the float32 result unless it lands on
+    a float32 midpoint (low 29 bits of the float64 = 1 followed by zeros); those few are redone exactly"""
+    a, b, c = np.broadcast_arrays(np.atleast_1d(np.asarray(a, F)), np.atleast_1d(np.asarray(b, F)), np.atleast_1d(np.asarray(c, F)))
+    r64 = a.astype(np.float64) * b.astype(np.float64) + c.astype(np.float64)
+    r = r64.astype(F)
+    tie = (r64.view(np.uint64) & np.uint64(0x1FFFFFFF)) == np.uint64(0x10000000)
+    if tie.any():
+        for i in zip(*np.nonzero(tie)):
+            x = Fraction(float(a[i])) * Fraction(float(b[i])) + Fraction(float(c[i]))
+            if x != Fraction(float(r64[i])):
+                lo_, hi_ = np.nextafter(F(r64[i]), F(-np.inf)), np.nextafter(F(r64[i]), F(np.inf))
+                lo_, hi_ = (lo_, r[i]) if r[i] > r64[i] else (r[i], hi_)
+                r[i] = lo_ if x < Fraction(float(r64[i])) else hi_
+    return r if r.size > 1 else r[0]
 
 
 def fill_pass(p, w, h):
@@ -29,8 +50,9 @@ def fill_pass(p, w, h):
     return dict(nS=t[0], nI=t[1], base=t[2], strideS=t[3], strideI=t[4], type=t[5])
 
 
-def run_pass(pd, C, lo_img, hi_img, gmin, DP, tsgm, P1, P2, L, Lmin):
-    """C: [npix, DP] float32 costs (the census slab's values), lo_img / hi_img: int16 [npix] labels.  Fills L [npix, DP], Lmin [npix]."""
+def run_pass(pd, C, lo_img, hi_img, gmin, DP, tsgm, P1, P2, L, Lmin, W=None):
+    """C: [npix, DP] float32 costs (the census slab's values), lo_img / hi_img: int16 [npix] labels, W: float32 [npix] weights
+    (GENERAL only, None = unweighted).  Fills L [npix, DP], Lmin [npix]."""
     TYPE = pd["type"]
     useA = True if TYPE == 0 else tsgm == 4
     useCn = tsgm >= 2 if TYPE == 0 else tsgm >= 3
@@ -54,6 +76,7 @@ def run_pass(pd, C, lo_img, hi_img, gmin, DP, tsgm, P1, P2, L, Lmin):
         r0[:, PAD + DP:] = INF
         cst = np.full((W_, STAGE, DP), F(333.0), F)
         rng = np.zeros((W_, STAGE, 2), np.uint32)
+        wst = np.full((W_, STAGE), F(999.0), F)
         r0rng = np.zeros((R0, 2), np.uint32)
         st = []
         for k in range(W_):
@@ -83,6 +106,8 @@ def run_pass(pd, C, lo_img, hi_img, gmin, DP, tsgm, P1, P2, L, Lmin):
                 cst[k, slot, 32 * ea:32 * (eb + 1)] = C[w["pidx"], 32 * ea:32 * (eb + 1)]      # only the chunks of the span
                 rng[k, slot, 0] = lo_words[(w["pidx"] * 2 & ~3) // 4]
                 rng[k, slot, 1] = hi_words[(w["pidx"] * 2 & ~3) // 4]
+                if W is not None:
+                    wst[k, slot] = W[w["pidx"]]
                 w["pidx"] += sI
             w["jc"] += 1
             w["nw"] = [w["nw"][1], w["nw"][2], range_words(k, w["jc"] + 2)]
@@ -117,7 +142,7 @@ def run_pass(pd, C, lo_img, hi_img, gmin, DP, tsgm, P1, P2, L, Lmin):
             slot = j & (RING - 1)
             return ring[k - 1, slot], F(meta[k - 1, slot, 0]), int(meta[k - 1, slot, 1]), int(meta[k - 1, slot, 2])
 
-        def term(n, e, kk):
+        def term(n, e, kk, ordn, wv, P1w):
             v, m, ea, eb = n
             a, c0, b = np.full(32, INF, F), np.full(32, INF, F), np.full(32, INF, F)
             if ea <= e <= eb:
@@ -126,6 +151,9 @@ def run_pass(pd, C, lo_img, hi_img, gmin, DP, tsgm, P1, P2, L, Lmin):
                 b[31] = v[PAD + kk[31] + 1]
             elif FIXED and e == eb + 1:          # lane 0's left neighbour is the last element of its span
                 a[0] = v[PAD + kk[0] - 1]
+            if GENERAL:        # P1*w: mul then add for the 1st / 2nd neighbour of the list, fma for the 3rd / 4th; P2*w: fma
+                v1 = fma32(F(P1), wv, np.minimum(a, b)) if ordn >= 2 else np.minimum(a, b) + P1w
+                return np.minimum(np.minimum(c0, v1), fma32(F(P2), wv, m)) - m
             v1 = np.minimum(a, b) + F(P1)
             return np.minimum(np.minimum(c0, v1), m + F(P2)) - m
 
@@ -160,6 +188,8 @@ def run_pass(pd, C, lo_img, hi_img, gmin, DP, tsgm, P1, P2, L, Lmin):
                     nE = nb_at(k, i + 1, False) if useE else None
                 mine = ring[k, i & (RING - 1)]
                 lm = np.full(32, INF, F)
+                wv = wst[k, slot] if W is not None else F(1.0)
+                P1w = F(P1) * wv
                 outv = np.full(DP, INF, F) if FILL_INF else L[w["outpix"]].copy()
                 for e in range(NC):
                     kk = 32 * e + lane
@@ -167,28 +197,28 @@ def run_pass(pd, C, lo_img, hi_img, gmin, DP, tsgm, P1, P2, L, Lmin):
                         c = cst[k, slot, kk]
                         Lv = c.copy()
                         if not border:
-                            if TYPE == 0:
-                                acc = term(nA, e, kk)
+                            if TYPE == 0:         # the reference's neighbour list: A, Cn, B, E
+                                acc = term(nA, e, kk, 0, wv, P1w)
                                 if tsgm == 2:
                                     acc = acc * F(0.5)
                                 if useCn:
-                                    tt = term(nC, e, kk)
+                                    tt = term(nC, e, kk, 1, wv, P1w)
                                     acc = acc + (tt * F(0.5) if tsgm == 2 else tt)
                                 if useB:
-                                    acc = acc + term(nB, e, kk)
+                                    acc = acc + term(nB, e, kk, 2, wv, P1w)
                                 if useE:
-                                    acc = acc + term(nE, e, kk)
-                            else:
-                                acc = term(nE, e, kk)
+                                    acc = acc + term(nE, e, kk, 3, wv, P1w)
+                            else:                 # E, B, Cn, A
+                                acc = term(nE, e, kk, 0, wv, P1w)
                                 if tsgm == 2:
                                     acc = acc * F(0.5)
                                 if useB:
-                                    tt = term(nB, e, kk)
+                                    tt = term(nB, e, kk, 1, wv, P1w)
                                     acc = acc + (tt * F(0.5) if tsgm == 2 else tt)
                                 if useCn:
-                                    acc = acc + term(nC, e, kk)
+                                    acc = acc + term(nC, e, kk, 2, wv, P1w)
                                 if useA:
-                                    acc = acc + term(nA, e, kk)
+                                    acc = acc + term(nA, e, kk, 3, wv, P1w)
                             if tsgm == 3:
                                 acc = acc / F(3)
                             if tsgm == 4:
@@ -208,8 +238,12 @@ def run_pass(pd, C, lo_img, hi_img, gmin, DP, tsgm, P1, P2, L, Lmin):
 
 
 def main():
+    global W_, STAGE, R0
     a = [int(x) for x in sys.argv[1:6]] + [512, 40, 48, 3, 0][len(sys.argv) - 1:]
     DP, h, w, tsgm, seed = a
+    if GENERAL and not os.environ.get("EMU_WARPS"):      # ck_warps / ck_stage of the general flavour
+        W_, STAGE = (8 if DP <= 1024 else 2), 2
+        R0 = 2 * STAGE
     rng_ = np.random.default_rng(seed)
     npix = h * w
     gmin = -DP // 2
@@ -223,18 +257,24 @@ def main():
     lo, hi = lo.astype(np.int32), hi.astype(np.int32)
     C = np.full((h, w, DP), np.inf, np.float32)
     vals = rng_.integers(0, 25, (h, w, DP)).astype(np.float32)
+    Wimg = None
+    P1, P2 = 8.0, 32.0
+    if GENERAL:        # costs with fractions (as ad / btad / ncc give), LSD-like weights, penalties whose products are inexact
+        vals = rng_.uniform(0, 40, (h, w, DP)).astype(np.float32)
+        Wimg = np.maximum(rng_.uniform(0, 1, (h, w)) ** 2, 0.1).astype(np.float32)
+        Wimg[rng_.random((h, w)) < 0.5] = 1.0
+        P1, P2 = 12.0, 48.0
     k = np.arange(DP)[None, None, :] + gmin
     inr = (k >= lo[..., None]) & (k <= hi[..., None])
     C[inr] = vals[inr]
-    P1, P2 = 8.0, 32.0
-    So, do, co, fo = O.port.aggregate(C, lo, hi, gmin, P1, P2, 8, tsgm)
+    So, do, co, fo = O.port.aggregate(C, lo, hi, gmin, P1, P2, 8, tsgm, weights=Wimg)
     Cf = C.reshape(npix, DP)
     lo16, hi16 = lo.reshape(-1).astype(np.int16), hi.reshape(-1).astype(np.int16)
     Ls = []
     for p in range(8):
         L = np.full((npix, DP), np.float32(-1.0), np.float32)
         Lmin = np.zeros(npix, np.float32)
-        run_pass(fill_pass(p, w, h), Cf, lo16, hi16, gmin, DP, tsgm, P1, P2, L, Lmin)
+        run_pass(fill_pass(p, w, h), Cf, lo16, hi16, gmin, DP, tsgm, P1, P2, L, Lmin, None if Wimg is None else Wimg.reshape(-1))
         Ls.append(L)
         print("pass", p, "done", flush=True)
     Ssum = np.zeros((npix, DP), np.float32)
@@ -243,7 +283,8 @@ def main():
     Ssum = (np.float64(-7.0) * Cf.astype(np.float64) + Ssum.astype(np.float64)).astype(np.float32)     # fmaf(-7, C, S)
     So = So.reshape(npix, DP)
     ok = (Ssum == So) | (np.isnan(Ssum) & np.isnan(So)) | (~inr.reshape(npix, DP))
-    print("DP %d %dx%d tsgm %d: %d of %d in-range voxels differ" % (DP, w, h, tsgm, int((~ok).sum()), int(inr.sum())))
+    print("%sDP %d %dx%d tsgm %d (%d warps, %d stages): %d of %d in-range voxels differ" % (
+        "general, " if GENERAL else "", DP, w, h, tsgm, W_, STAGE, int((~ok).sum()), int(inr.sum())))
     # chunks outside every pixel's span must hold +INF in the emulated global volume
     ea, eb = (lo.reshape(-1) - gmin) >> 5, (hi.reshape(-1) - gmin) >> 5
     e_of = (np.arange(DP) >> 5)[None, :]
@@ -253,7 +294,7 @@ def main():
     else:
         print("skipped chunks untouched:", bool(np.all(Ls[0][outside] == np.float32(-1.0))))
     if os.environ.get("EMU_WTA", "1") == "1":
-        main_wta(DP, h, w, tsgm, seed, Ls, Cf, lo.reshape(-1), hi.reshape(-1), gmin)
+        main_wta(DP, h, w, tsgm, seed, Ls, Cf, lo.reshape(-1), hi.reshape(-1), gmin, Wimg, P1, P2)
 
 
 def vfit3(v0, v1, v2):
@@ -316,12 +357,12 @@ def wta_chunked(Ls, Cf, lo, hi, gmin, DP, ndir=8, refine=1):
     return disp, conf
 
 
-def main_wta(DP, h, w, tsgm, seed, Ls, Cf, lo, hi, gmin):
+def main_wta(DP, h, w, tsgm, seed, Ls, Cf, lo, hi, gmin, Wimg=None, P1=8.0, P2=32.0):
     """compare the emulated chunk-skipping WTA (on the emulated pass volumes, garbage outside the spans) with the oracle"""
     import ctypes
     npix = h * w
     C3 = Cf.reshape(h, w, DP)
-    So, do, co, fo = O.port.aggregate(C3, lo.reshape(h, w), hi.reshape(h, w), gmin, 8.0, 32.0, 8, tsgm)
+    So, do, co, fo = O.port.aggregate(C3, lo.reshape(h, w), hi.reshape(h, w), gmin, P1, P2, 8, tsgm, weights=Wimg)
     d_ref, c_ref = do.reshape(-1).copy(), co.reshape(-1).copy()
     lo32, hi32 = np.ascontiguousarray(lo, np.int32), np.ascontiguousarray(hi, np.int32)
     pf = lambda a, t=ctypes.c_float: a.ctypes.data_as(ctypes.POINTER(t))
