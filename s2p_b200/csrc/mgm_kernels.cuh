@@ -647,6 +647,101 @@ __global__ void __launch_bounds__(kWtaThreads) __maxnreg__((LPL <= 4) ? 64 : 128
     else wta_pixels<LPL, GEN, 0>(P, sSrow);
 }
 
+// The same WTA reading only the labels that can still win (DESIGN.md 3.2).  Census flavour, unit weights: every message of
+// the aggregation is >= 0, so L_p[d] >= C[d] in every pass and S[d] >= C[d].  With T = S[d0] of one probe slot d0 (any slot
+// gives a valid bound; the first slot holding the pixel's smallest cost code is the probe), a slot with C[d] > T is neither
+// the winner, nor a tie for it, nor any pass's arg-minimum (min L_p <= L_p[d0] <= T).  A lane requests its LPL slots of the
+// pass vectors only when one of them, or a neighbour of one (the sub-pixel fit reads S[k-1], S[k+1]), has C <= T; the others
+// read +INF, which is what the sums, minima and comparisons below make of a slot that cannot win.  Outputs are those of
+// wta_kernel bit for bit.  Eight passes, blocked slots, no dense S and no PKR image (both read slots that cannot win).
+//
+// The probe would put one more round trip (C -> L_p[d0] -> pass vectors) on a pixel's dependent chain, so the codes, range
+// and probe values of the warp's NEXT pixel are requested while the current pixel's vectors are in flight.
+template <int LPL> __device__ __forceinline__ unsigned wta_probe_key(const CostPack<LPL> &cp, int lane)
+{   // (smallest code << 9) | first slot holding it
+    unsigned key = 0xffffffffu;
+#pragma unroll
+    for (int e = 0; e < LPL; e++) key = min(key, (cost_code(cp, e) << 9) | (unsigned)(lane * LPL + e));
+    return __reduce_min_sync(0xffffffffu, key);
+}
+// S of the probe slot from lanes 0-7's L_p[d0], with wta_finish's arithmetic: passes added in order, then the overcount fix
+__device__ __forceinline__ float wta_probe_sum(const WtaParams &P, float pv, unsigned key)
+{
+    float t = 0.f;
+#pragma unroll
+    for (int q = 0; q < kMaxPasses; q++) t += __shfl_sync(0xffffffffu, pv, q);
+    if (P.fix_overcount == 1) t = fmaf(-(float)(kMaxPasses - 1), cost_value(key >> 9, P.lut), t);
+    return t;
+}
+template <int LPL>
+__global__ void __launch_bounds__(kWtaThreads) __maxnreg__((LPL <= 4) ? 64 : 128) wta_pruned_kernel(const WtaParams P)
+{
+    static_assert(!WtaMap<LPL>::interleaved && LPL <= 8, "blocked slots, codes held in registers");
+    constexpr int DP = 32 * LPL;
+    __shared__ float sS[kWtaThreads / 32][DP];
+    float *sSrow = sS[threadIdx.x >> 5];
+    const int lane = threadIdx.x & 31;
+    // (32-bit pixel counters and the range in one word: the next pixel's state lives beside the current one's in 64 registers)
+    const unsigned warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = (gridDim.x * blockDim.x) >> 5;
+    const unsigned npix = (unsigned)P.npix;
+    if (warp >= npix) return;
+    const float *probe = P.L[0];                 // lanes 0-7: the pass this lane probes
+#pragma unroll
+    for (int q = 1; q < kMaxPasses; q++) if (lane == q) probe = P.L[q];
+    unsigned p = warp;
+    unsigned range = ((unsigned)(unsigned short)__ldg(P.lo + p)) | ((unsigned)(unsigned short)__ldg(P.hi + p) << 16);
+    CostPack<LPL> cpk = ld_cost<LPL, true>(reinterpret_cast<const uint8_t *>(P.C) + (size_t)p * DP + lane * LPL);
+    unsigned key = wta_probe_key<LPL>(cpk, lane);
+    float pv = lane < kMaxPasses ? __ldcg(probe + (size_t)p * DP + (key & 511u)) : 0.f;
+    for (;;) {
+        const unsigned pn = p + nwarps;
+        const bool more = pn < npix;
+        unsigned nrange = range;
+        CostPack<LPL> ncpk = cpk;
+        if (more) {
+            nrange = ((unsigned)(unsigned short)__ldg(P.lo + pn)) | ((unsigned)(unsigned short)__ldg(P.hi + pn) << 16);
+            ncpk = ld_cost<LPL, true>(reinterpret_cast<const uint8_t *>(P.C) + (size_t)pn * DP + lane * LPL);
+        }
+        // the integer costs of census 5x5 make S >= C exact; the scaled costs of 3x3 / 7x7 round in the eight additions and
+        // the overcount fix, by less than 2^-18 of S in all, so the bound is taken 2^-16 wider
+        const float T = wta_probe_sum(P, pv, key) * (1.f + 1.f / 65536.f);
+        unsigned m = 0;
+#pragma unroll
+        for (int e = 0; e < LPL; e++) if (cost_value(cost_code(cpk, e), P.lut) <= T) m |= 1u << e;
+        const unsigned left = __shfl_up_sync(0xffffffffu, m, 1), right = __shfl_down_sync(0xffffffffu, m, 1);
+        // (a pixel always has a finite S at its probe; were it not so, nothing is pruned)
+        const bool ld = m != 0 || (lane > 0 && ((left >> (LPL - 1)) & 1u)) || (lane < 31 && (right & 1u)) || !(T < S2PB_INF);
+        float s[LPL];
+        int am[kMaxPasses];
+#pragma unroll
+        for (int e = 0; e < LPL; e++) s[e] = 0.f;
+        unsigned nkey = key;
+        float npv = 0.f;
+#pragma unroll
+        for (int g = 0; g < kMaxPasses; g += 4) {
+            float v[4][LPL];
+#pragma unroll
+            for (int q = 0; q < 4; q++) {
+#pragma unroll
+                for (int e = 0; e < LPL; e++) v[q][e] = S2PB_INF;
+                if (ld) wta_ld_pass<LPL>(P.L[g + q] + (size_t)p * DP, lane, v[q]);
+            }
+            if (g == 0 && more) {
+                nkey = wta_probe_key<LPL>(ncpk, lane);
+                if (lane < kMaxPasses) npv = __ldcg(probe + (size_t)pn * DP + (nkey & 511u));
+            }
+#pragma unroll
+            for (int q = 0; q < 4; q++) am[g + q] = wta_add_pass<LPL>(v[q], lane, s);
+        }
+        float c[LPL];
+#pragma unroll
+        for (int e = 0; e < LPL; e++) c[e] = cost_value(cost_code(cpk, e), P.lut);
+        wta_finish<LPL>(P, p, lane, s, am, c, sSrow, (short)(range & 0xffffu), (short)(range >> 16));
+        if (!more) break;
+        p = pn; range = nrange; cpk = ncpk; key = nkey; pv = npv;
+    }
+}
+
 // Companion of agg_chunked.cuh (slabs wider than 512 slots): the same WTA for
 // slabs whose pixels use few of their 32-label chunks.  A warp owns a pixel and only reads the chunks [ea, eb] that hold its
 // label range (slot 32*e + lane), so a 40-label pixel of a 512-slot slab reads 2 x 128 B per pass instead of 2 KB.

@@ -105,6 +105,7 @@ struct Slot {
 struct s2pb_ctx {
     int device = 0;
     int sm_count = 132;
+    bool wta_prune = true;         // S2PB_WTA_PRUNE=0 (read when the context is created): wta_kernel for every shape (A/B)
     std::vector<Slot> slots;
     int *abort_flag = nullptr;     // pinned + mapped: the host raises it on timeout
     int *scratch_flag = nullptr;   // pinned + mapped: device -> host one-word answers
@@ -325,6 +326,7 @@ extern "C" s2pb_ctx *s2pb_create(int device)
     s2pb_ctx *ctx = new s2pb_ctx;
     ctx->device = device;
     ctx->sm_count = prop.multiProcessorCount;
+    if (const char *e = getenv("S2PB_WTA_PRUNE")) ctx->wta_prune = atoi(e) != 0;
     if (cudaHostAlloc((void **)&ctx->abort_flag, 16 * sizeof(int), cudaHostAllocMapped) != cudaSuccess) {
         fail(S2PB_ERR_CUDA, "cudaHostAlloc failed"); delete ctx; return nullptr;
     }
@@ -596,8 +598,15 @@ template <int LPL> static void launch_cost_t(const uint64_t *cu, const uint64_t 
         else cost_kernel<LPL, false, false><<<sm * 8, 256, 0, st>>>(cu, cv, cv1, w, h, lo, hi, gmin, C);
     }
 }
-template <int LPL> static void launch_wta_t(const WtaParams &P, int sm, cudaStream_t st, bool general)
+// prune: the census flavour's eight-pass WTA without a dense S or PKR output reads only the labels that can still win
+template <int LPL> static void launch_wta_t(const WtaParams &P, int sm, cudaStream_t st, bool general, bool prune)
 {
+    if constexpr (LPL == 1 || LPL == 2 || LPL == 4 || LPL == 8) {
+        if (prune && !general && P.ndir == kMaxPasses && P.S == nullptr && P.pkr == nullptr) {
+            wta_pruned_kernel<LPL><<<sm * 16, kWtaThreads, 0, st>>>(P);
+            return;
+        }
+    }
     if (general) wta_kernel<LPL, true><<<sm * 16, kWtaThreads, 0, st>>>(P);
     else wta_kernel<LPL, false><<<sm * 16, kWtaThreads, 0, st>>>(P);
 }
@@ -643,7 +652,7 @@ static int launch_wta(s2pb_ctx *ctx, int LPL, const WtaParams &P, cudaStream_t s
         ctx->launches++;
         return S2PB_OK;
     }
-    LPL_SWITCH(LPL, launch_wta_t<K>(P, ctx->sm_count, st, general));
+    LPL_SWITCH(LPL, launch_wta_t<K>(P, ctx->sm_count, st, general, ctx->wta_prune));
     CK(cudaGetLastError());
     ctx->launches++;
     return S2PB_OK;
