@@ -673,6 +673,14 @@ __device__ __forceinline__ float wta_probe_sum(const WtaParams &P, float pv, uns
     if (P.fix_overcount == 1) t = fmaf(-(float)(kMaxPasses - 1), cost_value(key >> 9, P.lut), t);
     return t;
 }
+// m: which of the lane's LPL slots can still win.  The lane requests its slots when one of them or a neighbour of one (the
+// sub-pixel fit reads S[k-1], S[k+1]) is in m; the dilation across lanes is two shuffles.  (A pixel always has a finite S at
+// its probe; were it not so, nothing is pruned.)
+template <int LPL> __device__ __forceinline__ bool wta_lane_reads(unsigned m, int lane, float T)
+{
+    const unsigned left = __shfl_up_sync(0xffffffffu, m, 1), right = __shfl_down_sync(0xffffffffu, m, 1);
+    return m != 0 || (lane > 0 && ((left >> (LPL - 1)) & 1u)) || (lane < 31 && (right & 1u)) || !(T < S2PB_INF);
+}
 template <int LPL>
 __global__ void __launch_bounds__(kWtaThreads) __maxnreg__((LPL <= 4) ? 64 : 128) wta_pruned_kernel(const WtaParams P)
 {
@@ -708,9 +716,7 @@ __global__ void __launch_bounds__(kWtaThreads) __maxnreg__((LPL <= 4) ? 64 : 128
         unsigned m = 0;
 #pragma unroll
         for (int e = 0; e < LPL; e++) if (cost_value(cost_code(cpk, e), P.lut) <= T) m |= 1u << e;
-        const unsigned left = __shfl_up_sync(0xffffffffu, m, 1), right = __shfl_down_sync(0xffffffffu, m, 1);
-        // (a pixel always has a finite S at its probe; were it not so, nothing is pruned)
-        const bool ld = m != 0 || (lane > 0 && ((left >> (LPL - 1)) & 1u)) || (lane < 31 && (right & 1u)) || !(T < S2PB_INF);
+        const bool ld = wta_lane_reads<LPL>(m, lane, T);
         float s[LPL];
         int am[kMaxPasses];
 #pragma unroll
@@ -739,6 +745,109 @@ __global__ void __launch_bounds__(kWtaThreads) __maxnreg__((LPL <= 4) ? 64 : 128
         wta_finish<LPL>(P, p, lane, s, am, c, sSrow, (short)(range & 0xffffu), (short)(range >> 16));
         if (!more) break;
         p = pn; range = nrange; cpk = ncpk; key = nkey; pv = npv;
+    }
+}
+
+// The same WTA in two stages (DESIGN.md 3.2).  Pass 0 is read under the mask above.  S[d] >= L_0[d] too, so passes 1-7 are read
+// only where L_0[d] <= T, dilated by one slot (the winner, its ties and the fit), or where C[d] <= L_q[d0]: a pass-q
+// arg-minimum d* has C[d*] <= L_q[d*] = min L_q <= L_q[d0], so every pass's consensus slot is read.  Lanes 0-7 hold L_q[d0]
+// from the probe.  L_q >= C holds without rounding (L_q = fl(C + x), x >= 0), so that term needs no slack.
+//
+// Pass 0 would put one more round trip on a pixel's chain, so a warp works three pixels deep: pixel p+1's probe and pass 0 are
+// requested while p's passes 1-7 are in flight, and pixel p+2's codes and range one pixel ahead of its probe.  Passes 1-7 are
+// requested together (one round trip; the pruned lanes leave registers for all seven under the 64-register cap), so a pixel
+// waits on one round trip where wta_pruned_kernel waits on two (its passes four at a time).
+template <int LPL> __device__ __forceinline__ void wta_ld_pass_if(const float *px, int lane, bool ld, float (&v)[LPL])
+{
+#pragma unroll
+    for (int e = 0; e < LPL; e++) v[e] = S2PB_INF;
+    if (ld) wta_ld_pass<LPL>(px, lane, v);
+}
+template <int LPL> __device__ __forceinline__ bool wta_lane_reads_c(const WtaParams &P, const CostPack<LPL> &cp, int lane, float T)
+{
+    unsigned m = 0;
+#pragma unroll
+    for (int e = 0; e < LPL; e++) if (cost_value(cost_code(cp, e), P.lut) <= T) m |= 1u << e;
+    return wta_lane_reads<LPL>(m, lane, T);
+}
+__device__ __forceinline__ unsigned wta_range(const WtaParams &P, unsigned p)
+{
+    return ((unsigned)(unsigned short)__ldg(P.lo + p)) | ((unsigned)(unsigned short)__ldg(P.hi + p) << 16);
+}
+template <int LPL>
+__global__ void __launch_bounds__(kWtaThreads) __maxnreg__((LPL <= 4) ? 64 : 128) wta_pruned2_kernel(const WtaParams P)
+{
+    static_assert(!WtaMap<LPL>::interleaved && LPL <= 8, "blocked slots, codes held in registers");
+    constexpr int DP = 32 * LPL;
+    __shared__ float sS[kWtaThreads / 32][DP];
+    float *sSrow = sS[threadIdx.x >> 5];
+    const int lane = threadIdx.x & 31;
+    const unsigned warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = (gridDim.x * blockDim.x) >> 5;
+    const unsigned npix = (unsigned)P.npix;
+    if (warp >= npix) return;
+    const float *probe = P.L[0];                 // lanes 0-7: the pass this lane probes
+#pragma unroll
+    for (int q = 1; q < kMaxPasses; q++) if (lane == q) probe = P.L[q];
+    const uint8_t *codes = reinterpret_cast<const uint8_t *>(P.C) + lane * LPL;
+    // pixel p: range, codes, probe values, bound, pass 0 requested; pixel p1: range and codes requested
+    unsigned p = warp;
+    unsigned range = wta_range(P, p);
+    CostPack<LPL> cpk = ld_cost<LPL, true>(codes + (size_t)p * DP);
+    const unsigned key = wta_probe_key<LPL>(cpk, lane);
+    float pv = lane < kMaxPasses ? __ldcg(probe + (size_t)p * DP + (key & 511u)) : 0.f;
+    // (the slack of wta_pruned_kernel: the scaled costs round in the sums)
+    float T = wta_probe_sum(P, pv, key) * (1.f + 1.f / 65536.f);
+    float v0[LPL];
+    wta_ld_pass_if<LPL>(P.L[0] + (size_t)p * DP, lane, wta_lane_reads_c<LPL>(P, cpk, lane, T), v0);
+    unsigned p1 = p + nwarps;
+    unsigned range1 = range;
+    CostPack<LPL> cpk1 = cpk;
+    if (p1 < npix) { range1 = wta_range(P, p1); cpk1 = ld_cost<LPL, true>(codes + (size_t)p1 * DP); }
+    for (;;) {
+        const bool more1 = p1 < npix;
+        const unsigned p2 = p1 + nwarps;
+        unsigned range2 = range1;
+        CostPack<LPL> cpk2 = cpk1;
+        unsigned key1 = 0;
+        float pv1 = 0.f;
+        if (more1) {
+            if (p2 < npix) { range2 = wta_range(P, p2); cpk2 = ld_cost<LPL, true>(codes + (size_t)p2 * DP); }
+            key1 = wta_probe_key<LPL>(cpk1, lane);
+            if (lane < kMaxPasses) pv1 = __ldcg(probe + (size_t)p1 * DP + (key1 & 511u));
+        }
+        float s[LPL];
+        int am[kMaxPasses];
+#pragma unroll
+        for (int e = 0; e < LPL; e++) s[e] = 0.f;
+        am[0] = wta_add_pass<LPL>(v0, lane, s);
+        unsigned m = 0;
+        float cmin = S2PB_INF;
+#pragma unroll
+        for (int e = 0; e < LPL; e++) {
+            if (v0[e] <= T) m |= 1u << e;
+            cmin = fminf(cmin, cost_value(cost_code(cpk, e), P.lut));
+        }
+        const bool ld = wta_lane_reads<LPL>(m, lane, T);
+        // (every lane takes part in the shuffles: no short-circuit around them)
+        unsigned ldq = 0;
+#pragma unroll
+        for (int q = 1; q < kMaxPasses; q++) if (cmin <= __shfl_sync(0xffffffffu, pv, q)) ldq |= 1u << q;
+        float v[kMaxPasses - 1][LPL];
+#pragma unroll
+        for (int q = 1; q < kMaxPasses; q++) wta_ld_pass_if<LPL>(P.L[q] + (size_t)p * DP, lane, ld || ((ldq >> q) & 1u), v[q - 1]);
+        float T1 = T;
+        if (more1) {
+            T1 = wta_probe_sum(P, pv1, key1) * (1.f + 1.f / 65536.f);
+            wta_ld_pass_if<LPL>(P.L[0] + (size_t)p1 * DP, lane, wta_lane_reads_c<LPL>(P, cpk1, lane, T1), v0);
+        }
+#pragma unroll
+        for (int q = 1; q < kMaxPasses; q++) am[q] = wta_add_pass<LPL>(v[q - 1], lane, s);
+        float c[LPL];
+#pragma unroll
+        for (int e = 0; e < LPL; e++) c[e] = cost_value(cost_code(cpk, e), P.lut);
+        wta_finish<LPL>(P, p, lane, s, am, c, sSrow, (short)(range & 0xffffu), (short)(range >> 16));
+        if (!more1) break;
+        p = p1; p1 = p2; range = range1; range1 = range2; cpk = cpk1; cpk1 = cpk2; pv = pv1; T = T1;
     }
 }
 

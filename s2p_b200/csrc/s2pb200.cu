@@ -105,7 +105,8 @@ struct Slot {
 struct s2pb_ctx {
     int device = 0;
     int sm_count = 132;
-    bool wta_prune = true;         // S2PB_WTA_PRUNE=0 (read when the context is created): wta_kernel for every shape (A/B)
+    int wta_prune = 2;             // S2PB_WTA_PRUNE (read when the context is created, A/B): 0 wta_kernel for every shape,
+                                   // 1 the one-stage wta_pruned_kernel, 2 (the default) the two-stage wta_pruned2_kernel (DESIGN.md 6)
     std::vector<Slot> slots;
     int *abort_flag = nullptr;     // pinned + mapped: the host raises it on timeout
     int *scratch_flag = nullptr;   // pinned + mapped: device -> host one-word answers
@@ -326,7 +327,7 @@ extern "C" s2pb_ctx *s2pb_create(int device)
     s2pb_ctx *ctx = new s2pb_ctx;
     ctx->device = device;
     ctx->sm_count = prop.multiProcessorCount;
-    if (const char *e = getenv("S2PB_WTA_PRUNE")) ctx->wta_prune = atoi(e) != 0;
+    if (const char *e = getenv("S2PB_WTA_PRUNE")) ctx->wta_prune = atoi(e);
     if (cudaHostAlloc((void **)&ctx->abort_flag, 16 * sizeof(int), cudaHostAllocMapped) != cudaSuccess) {
         fail(S2PB_ERR_CUDA, "cudaHostAlloc failed"); delete ctx; return nullptr;
     }
@@ -598,12 +599,14 @@ template <int LPL> static void launch_cost_t(const uint64_t *cu, const uint64_t 
         else cost_kernel<LPL, false, false><<<sm * 8, 256, 0, st>>>(cu, cv, cv1, w, h, lo, hi, gmin, C);
     }
 }
-// prune: the census flavour's eight-pass WTA without a dense S or PKR output reads only the labels that can still win
-template <int LPL> static void launch_wta_t(const WtaParams &P, int sm, cudaStream_t st, bool general, bool prune)
+// prune (s2pb_ctx::wta_prune): the census flavour's eight-pass WTA without a dense S or PKR output reads only the labels that
+// can still win
+template <int LPL> static void launch_wta_t(const WtaParams &P, int sm, cudaStream_t st, bool general, int prune)
 {
     if constexpr (LPL == 1 || LPL == 2 || LPL == 4 || LPL == 8) {
-        if (prune && !general && P.ndir == kMaxPasses && P.S == nullptr && P.pkr == nullptr) {
-            wta_pruned_kernel<LPL><<<sm * 16, kWtaThreads, 0, st>>>(P);
+        if (prune != 0 && !general && P.ndir == kMaxPasses && P.S == nullptr && P.pkr == nullptr) {
+            if (prune == 1) wta_pruned_kernel<LPL><<<sm * 16, kWtaThreads, 0, st>>>(P);
+            else wta_pruned2_kernel<LPL><<<sm * 16, kWtaThreads, 0, st>>>(P);
             return;
         }
     }

@@ -9,7 +9,10 @@ pixel's 128-slot pass vector hold a (dilated) survivor, and asserts on every pix
 survivors alone equal those from the full vector.  `check_claims` with pass volumes does the same for the eight pass arg-minima with pass
 volumes from a plain numpy restatement of the scan (small strips only: it is a per-pixel Python loop).
 
-    python scripts/wta_prune_model.py [--rows 300:396] [--seeds 0,1] [--size 1024] [--views LR]
+The two-stage mask (`two_stage`) reads pass 0 under that mask and passes 1-7 only where L_0[d] <= S[d0] (dilated) or
+C[d] <= L_q[d0]; `--two-stage` counts it per pass with those pass volumes (slow: minutes per strip and view).
+
+    python scripts/wta_prune_model.py [--rows 300:396] [--seeds 0,1] [--size 1024] [--views LR] [--two-stage]
 """
 import argparse
 import os
@@ -91,20 +94,38 @@ def probe_value(C, S, rule):
     return t
 
 
+def dilate(s):
+    d = s.copy()
+    d[..., 1:] |= s[..., :-1]
+    d[..., :-1] |= s[..., 1:]
+    return d
+
+
 def survivors(C, T):
     """{d : C[d] <= T} dilated by one slot on each side, clipped to the slab.  T is taken 2^-16 wider, like the kernel's:
     the scaled costs of census 3x3 / 7x7 round in the sums (the integer costs of 5x5 do not)."""
     s = C <= (T * np.float32(1 + 2.0 ** -16))[..., None]
-    d = s.copy()
-    d[..., 1:] |= s[..., :-1]
-    d[..., :-1] |= s[..., 1:]
-    return s, d
+    return s, dilate(s)
+
+
+def two_stage(C, T, Ls):
+    """The slots each pass is read on by the two-stage WTA (wta_pruned2_kernel) -> eight [h][w][D] masks.  Pass 0: the
+    dilated survivors of C.  Passes 1-7: {d : L_0[d] <= T} from what was read of pass 0, dilated (S >= L_0 like S >= C, same
+    slack), and {d : C[d] <= L_q[d0]} with d0 the probe slot (first arg-minimum of C): every arg-minimum of L_q lies there."""
+    _, d0 = survivors(C, T)
+    L0 = np.where(d0, Ls[0], INF)
+    d1 = dilate(L0 <= (T * np.float32(1 + 2.0 ** -16))[..., None])
+    k0 = np.argmin(C, axis=-1)[..., None]
+    return [d0] + [d1 | (C <= np.take_along_axis(L, k0, -1)) for L in Ls[1:]]
 
 
 def check_claims(C, S, dil, Ls=None):
     """winner, fit values and (with the pass volumes) the eight last arg-minima from the survivors only equal those from
-    the full vectors, on every pixel.  A slot with C = +INF has L_p = +INF whether it is read or not."""
-    dil = dil | np.isinf(C)
+    the full vectors, on every pixel.  A slot with C = +INF has L_p = +INF whether it is read or not.  dil: one mask for
+    every pass, or a list of eight (two_stage): a slot missed by any pass sums to +INF."""
+    per_pass = isinstance(dil, (list, tuple))
+    dils = [d | np.isinf(C) for d in (dil if per_pass else [dil] * 8)]
+    dil = np.logical_and.reduce(dils)
     Sp = np.where(dil, S, INF)
     k = first_min(S)
     assert np.array_equal(first_min(Sp), k), "winner differs"
@@ -114,8 +135,8 @@ def check_claims(C, S, dil, Ls=None):
         a = np.take_along_axis(S, kk[..., None], -1)
         b = np.take_along_axis(Sp, kk[..., None], -1)
         assert np.array_equal(a, b, equal_nan=True), "fit value %+d differs" % o
-    for L in Ls or ():
-        Lp = np.where(dil, L, INF)
+    for L, dq in zip(Ls or (), dils):
+        Lp = np.where(dq, L, INF)
         last = lambda V: D - 1 - np.argmax((V == V.min(-1, keepdims=True))[..., ::-1], axis=-1)
         assert np.array_equal(last(L), last(Lp)), "pass arg-minimum differs"
 
@@ -156,14 +177,44 @@ def strip_volumes(seed, size, rows, dmin, dmax, nan_border, view):
 RULES = (("cmin", 1), ("best", 1), ("cmin+prev", 2))
 
 
+def sector_fraction(d):
+    h, w, D = d.shape
+    return d.reshape(h, w, D // 8, 8).any(-1).mean()
+
+
+def two_stage_fractions(C, S):
+    """-> (per-pass 32-byte sector fractions of the two-stage mask, that of the one-stage mask), probes not included; checks
+    winner, fit and the eight arg-minima of the two-stage mask on every pixel"""
+    Ls = pass_volumes(C)
+    fin = np.isfinite(S)
+    assert np.array_equal(sum_passes(Ls, C)[fin], S[fin]), "numpy pass volumes do not sum to the oracle's S"
+    T = probe_value(C, S, "cmin")
+    masks = two_stage(C, T, Ls)
+    check_claims(C, S, masks, Ls)
+    return [sector_fraction(d) for d in masks], sector_fraction(survivors(C, T)[1])
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--rows", default="300:396")
     ap.add_argument("--seeds", default="0")
     ap.add_argument("--size", type=int, default=1024)
     ap.add_argument("--views", default="LR")
+    ap.add_argument("--two-stage", action="store_true", help="per-pass sector fractions of the two-stage mask")
     a = ap.parse_args()
     rows = tuple(int(x) for x in a.rows.split(":"))
+    if a.two_stage:
+        print("| tile | view | one stage, every pass | two stages: pass 0 | passes 1-7 | mean of 8 | mean + probes |")
+        print("|---|---|---|---|---|---|---|")
+        for nanb in (0.0, 0.05):
+            for seed in (int(s) for s in a.seeds.split(",")):
+                for view in a.views:
+                    C, S = strip_volumes(seed, a.size, rows, -64, 63, nanb, view)
+                    f, f1 = two_stage_fractions(C, S)
+                    print("| seed %d%s | %s | %.3f | %.3f | %.3f-%.3f | %.3f | %.3f |" % (
+                        seed, " nodata" if nanb else "", view, f1, f[0], min(f[1:]), max(f[1:]), np.mean(f),
+                        np.mean(f) + 1 / (C.shape[-1] // 8)), flush=True)
+        return
     # "unpruned pixels": S[d0] >= the largest finite C, recognisable before any mask work -- they read every sector
     print("| tile | view | probe | survivors | 16 B pieces | 32 B sectors | 64 B pairs | unpruned pixels | sectors + probes |")
     print("|---|---|---|---|---|---|---|---|---|")
