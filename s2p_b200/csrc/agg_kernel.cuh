@@ -44,22 +44,11 @@ constexpr int kAggThreads = kNWC * 32;
 // after every odd step separates the two; the ring is 8 deep so that a slot is not reused within that slack.
 // Volumes of 4 labels per lane or fewer keep the barrier after every step.  (Chosen on the GPU the engine was first
 // written for; the H100 A/B at 6 labels per lane is in DESIGN.md section 6.)
-#ifndef S2PB_SYNC2
-#define S2PB_SYNC2 1
-#endif
-// Every warp runs its own three loops -- ramp-up, interior, ramp-down -- so that the interior steps carry no fast / slow
-// test and the compiler keeps one register assignment through the interior loop.
-#ifndef S2PB_SPLIT_LOOP
-#define S2PB_SPLIT_LOOP 1
-#endif
 template <int LPL> struct SyncCfg {
-    static constexpr bool sync2 = S2PB_SYNC2 && LPL > 4 && LPL <= 8;
+    static constexpr bool sync2 = LPL > 4 && LPL <= 8;
     static constexpr int kRing = sync2 ? 8 : 4;      // ring slots per compute warp for handing vectors to the next warp
 };
-#ifndef S2PB_PUBLISH
-#define S2PB_PUBLISH 8        // (a knob for A/B builds: fewer publications = fewer ld.acquire polls by the next band)
-#endif
-constexpr int kPublish = S2PB_PUBLISH;   // a band publishes its progress every kPublish pixels
+constexpr int kPublish = 8;   // a band publishes its progress every kPublish pixels
 
 // ------------------------------------------------------------------ small helpers
 
@@ -144,28 +133,6 @@ template <int LPL> __device__ __forceinline__ void st_vec(float *p, const float 
 #pragma unroll
         for (int q = 0; q < LPL; q++) p[q] = v[q];
     }
-}
-// the pass volumes are written once and read back gigabytes later: S2PB_STREAM_STORES=1 (an A/B build knob, off by
-// default) marks their stores evict-first so that they do not displace the cost rows and band hand-off rows in L2
-#ifndef S2PB_STREAM_STORES
-#define S2PB_STREAM_STORES 0
-#endif
-template <int LPL> __device__ __forceinline__ void st_vec_out(float *p, const float (&v)[LPL])
-{
-#if S2PB_STREAM_STORES
-    if constexpr (LPL % 4 == 0) {
-#pragma unroll
-        for (int q = 0; q < LPL / 4; q++) __stcs(reinterpret_cast<float4 *>(p) + q, make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]));
-    } else if constexpr (LPL % 2 == 0) {
-#pragma unroll
-        for (int q = 0; q < LPL / 2; q++) __stcs(reinterpret_cast<float2 *>(p) + q, make_float2(v[2 * q], v[2 * q + 1]));
-    } else {
-#pragma unroll
-        for (int q = 0; q < LPL; q++) __stcs(p + q, v[q]);
-    }
-#else
-    st_vec<LPL>(p, v);
-#endif
 }
 // ------------------------------------------------------------------ 8-bit census cost codes
 //
@@ -334,11 +301,7 @@ struct AggParams {
 // because pixel 0 is staged ahead of the pipeline); shallower for the widest volumes.  (16 labels per lane would
 // still fit 227 KB with 8 stages, but measured no faster: 32.7 vs 31.9 ms on the C3-like mgm_multi tile.)
 template <int LPL, bool GEN = false> struct StageCfg {
-#ifdef S2PB_STAGE          // (A/B builds: depth of the census flavour's pipeline for up to 12 labels per lane)
-    static constexpr int kStage = GEN ? ((LPL <= 4) ? 8 : (LPL <= 8) ? 4 : 2) : ((LPL <= 12) ? S2PB_STAGE : 2);
-#else
     static constexpr int kStage = GEN ? ((LPL <= 4) ? 8 : (LPL <= 8) ? 4 : 2) : ((LPL <= 12) ? 8 : 2);
-#endif
     static constexpr int kR0 = 2 * kStage;
 };
 
@@ -525,12 +488,10 @@ __device__ __forceinline__ void run_band(const PassDesc &pd, int band, float P1,
         if (stage_prev) {
             if (jp < nI) {
                 int spins = 0;
-#ifndef S2PB_DIAG_NOPOLL      // timing diagnostics only (results are wrong): never wait for the previous band
                 while (avail < jp + 1) {
                     avail = ld_acquire(prev_progress);
                     if (((++spins) & 1023) == 0 && *(volatile const int *)abort_flag) break;
                 }
-#endif
                 const unsigned slot = (unsigned)(jp & (kR0 - 1));
                 warp_cp_async_s<DP * 4>(r0_s + slot * (DP * 4), psrc, lane);
                 if (lane == 0) cp_async4_s(r0m_s + slot * 4, pmsrc);
@@ -690,7 +651,7 @@ __device__ __forceinline__ void run_band(const PassDesc &pd, int band, float P1,
                 hNew.m = mAm;
                 fill_edges<LPL>(hNew, lane);
                 if (MSG) nb_message<LPL>(hNew, P1, P2);
-                st_vec_out<LPL>(outA, LA);
+                st_vec<LPL>(outA, LA);
                 outA += lstep;
             }
             if (actB) {
@@ -704,7 +665,7 @@ __device__ __forceinline__ void run_band(const PassDesc &pd, int band, float P1,
                     fill_edges<LPL>(wAB, lane);
                 }
                 if (usePrev) st_vec<LPL>(myring + (iB & (kRing - 1)) * DP, MSG ? wAB.v : LB);
-                st_vec_out<LPL>(outB, LB);
+                st_vec<LPL>(outB, LB);
                 outB += lstep;
                 if (!MSG && lane == 0 && usePrev) myringm[iB & (kRing - 1)] = mBm;
                 if (publish) {
@@ -717,24 +678,16 @@ __device__ __forceinline__ void run_band(const PassDesc &pd, int band, float P1,
                 }
             }
         }
-#ifdef S2PB_DIAG_NOBAR         // timing diagnostics only (results are wrong): no CTA barrier per step
-        __syncwarp();
-#else
         if (!SYNC2 || (t & 1)) __syncthreads();
         else __syncwarp();      // the staging slot the lanes just read is overwritten by the next step's cp.async
-#endif
     };
     // a step is FAST for this warp when A is at an interior pixel with B one SKEW behind, also interior
     const bool can_fast = liveA && liveB && prevA;
     const int fast_lo = k * WSK + SKEW + 1, fast_hi = k * WSK + nI - 2;     // t range: iB >= 1 and iA <= nI-2
-    auto do_step = [&](const int t, NbVec<LPL> &xB, NbVec<LPL> &xC, NbVec<LPL> &xE, NbVec<LPL> &hNew, NbVec<LPL> &hC, NbVec<LPL> &hE) {
-        if (can_fast && t >= fast_lo && t <= fast_hi) step(std::true_type{}, t, xB, xC, xE, hNew, hC, hE);
-        else step(std::false_type{}, t, xB, xC, xE, hNew, hC, hE);
-    };
 
-#if S2PB_SPLIT_LOOP
     // every warp runs its own three loops -- ramp-up, interior, ramp-down -- so that the interior steps carry no
-    // fast / slow test; the barrier sequence is the same for all warps
+    // fast / slow test and the compiler keeps one register assignment through the interior loop; the barrier sequence
+    // is the same for all warps
     auto group = [&](auto fast_c, const int t) {
         if constexpr (U == 2) {
             step(fast_c, t, x1, x0, x2, h0, h1, h2);
@@ -756,18 +709,6 @@ __device__ __forceinline__ void run_band(const PassDesc &pd, int band, float P1,
     for (; t < ta; t += U) group(std::false_type{}, t);
     for (; t < tb; t += U) group(std::true_type{}, t);
     for (; t < nsteps; t += U) group(std::false_type{}, t);
-#else
-    for (int t = 0; t < nsteps; t += U) {
-        if constexpr (U == 2) {
-            do_step(t, x1, x0, x2, h0, h1, h2);
-            do_step(t + 1, x0, x1, x2, h1, h0, h2);
-        } else {
-            do_step(t, x1, x2, x0, h0, h1, h2);
-            do_step(t + 1, x2, x0, x1, h1, h2, h0);
-            do_step(t + 2, x0, x1, x2, h2, h0, h1);
-        }
-    }
-#endif
     cp_async_wait<0>();
 }
 

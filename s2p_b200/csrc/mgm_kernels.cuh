@@ -650,13 +650,20 @@ __global__ void __launch_bounds__(kWtaThreads) __maxnreg__((LPL <= 4) ? 64 : 128
 // The same WTA reading only the labels that can still win (DESIGN.md 3.2).  Census flavour, unit weights: every message of
 // the aggregation is >= 0, so L_p[d] >= C[d] in every pass and S[d] >= C[d].  With T = S[d0] of one probe slot d0 (any slot
 // gives a valid bound; the first slot holding the pixel's smallest cost code is the probe), a slot with C[d] > T is neither
-// the winner, nor a tie for it, nor any pass's arg-minimum (min L_p <= L_p[d0] <= T).  A lane requests its LPL slots of the
-// pass vectors only when one of them, or a neighbour of one (the sub-pixel fit reads S[k-1], S[k+1]), has C <= T; the others
-// read +INF, which is what the sums, minima and comparisons below make of a slot that cannot win.  Outputs are those of
-// wta_kernel bit for bit.  Eight passes, blocked slots, no dense S and no PKR image (both read slots that cannot win).
+// the winner, nor a tie for it, nor any pass's arg-minimum (min L_p <= L_p[d0] <= T).  The pixel is read in two stages:
+// - pass 0: a lane requests its LPL slots only when one of them, or a neighbour of one (the sub-pixel fit reads S[k-1],
+//   S[k+1]), has C <= T;
+// - passes 1-7: S[d] >= L_0[d] too, so only where L_0[d] <= T, dilated in the same way, or where C[d] <= L_q[d0]: a pass-q
+//   arg-minimum d* has C[d*] <= L_q[d*] = min L_q <= L_q[d0], so every pass's consensus slot is read.  Lanes 0-7 hold L_q[d0]
+//   from the probe.  L_q >= C holds without rounding (L_q = fl(C + x), x >= 0), so that term needs no slack.
+// The other slots read +INF, which is what the sums, minima and comparisons of wta_finish make of a slot that cannot win.
+// Outputs are those of wta_kernel bit for bit.  Eight passes, blocked slots, no dense S and no PKR image (both read slots
+// that cannot win).
 //
-// The probe would put one more round trip (C -> L_p[d0] -> pass vectors) on a pixel's dependent chain, so the codes, range
-// and probe values of the warp's NEXT pixel are requested while the current pixel's vectors are in flight.
+// The probe and pass 0 would each put one more round trip on a pixel's dependent chain (C -> L_p[d0] -> pass 0 -> passes
+// 1-7), so a warp works three pixels deep: pixel p+1's probe and pass 0 are requested while p's passes 1-7 are in flight, and
+// pixel p+2's codes and range one pixel ahead of its probe.  Passes 1-7 are requested together (one round trip; the pruned
+// lanes leave registers for all seven under the 64-register cap), so a pixel waits on one round trip, not two.
 template <int LPL> __device__ __forceinline__ unsigned wta_probe_key(const CostPack<LPL> &cp, int lane)
 {   // (smallest code << 9) | first slot holding it
     unsigned key = 0xffffffffu;
@@ -681,82 +688,6 @@ template <int LPL> __device__ __forceinline__ bool wta_lane_reads(unsigned m, in
     const unsigned left = __shfl_up_sync(0xffffffffu, m, 1), right = __shfl_down_sync(0xffffffffu, m, 1);
     return m != 0 || (lane > 0 && ((left >> (LPL - 1)) & 1u)) || (lane < 31 && (right & 1u)) || !(T < S2PB_INF);
 }
-template <int LPL>
-__global__ void __launch_bounds__(kWtaThreads) __maxnreg__((LPL <= 4) ? 64 : 128) wta_pruned_kernel(const WtaParams P)
-{
-    static_assert(!WtaMap<LPL>::interleaved && LPL <= 8, "blocked slots, codes held in registers");
-    constexpr int DP = 32 * LPL;
-    __shared__ float sS[kWtaThreads / 32][DP];
-    float *sSrow = sS[threadIdx.x >> 5];
-    const int lane = threadIdx.x & 31;
-    // (32-bit pixel counters and the range in one word: the next pixel's state lives beside the current one's in 64 registers)
-    const unsigned warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = (gridDim.x * blockDim.x) >> 5;
-    const unsigned npix = (unsigned)P.npix;
-    if (warp >= npix) return;
-    const float *probe = P.L[0];                 // lanes 0-7: the pass this lane probes
-#pragma unroll
-    for (int q = 1; q < kMaxPasses; q++) if (lane == q) probe = P.L[q];
-    unsigned p = warp;
-    unsigned range = ((unsigned)(unsigned short)__ldg(P.lo + p)) | ((unsigned)(unsigned short)__ldg(P.hi + p) << 16);
-    CostPack<LPL> cpk = ld_cost<LPL, true>(reinterpret_cast<const uint8_t *>(P.C) + (size_t)p * DP + lane * LPL);
-    unsigned key = wta_probe_key<LPL>(cpk, lane);
-    float pv = lane < kMaxPasses ? __ldcg(probe + (size_t)p * DP + (key & 511u)) : 0.f;
-    for (;;) {
-        const unsigned pn = p + nwarps;
-        const bool more = pn < npix;
-        unsigned nrange = range;
-        CostPack<LPL> ncpk = cpk;
-        if (more) {
-            nrange = ((unsigned)(unsigned short)__ldg(P.lo + pn)) | ((unsigned)(unsigned short)__ldg(P.hi + pn) << 16);
-            ncpk = ld_cost<LPL, true>(reinterpret_cast<const uint8_t *>(P.C) + (size_t)pn * DP + lane * LPL);
-        }
-        // the integer costs of census 5x5 make S >= C exact; the scaled costs of 3x3 / 7x7 round in the eight additions and
-        // the overcount fix, by less than 2^-18 of S in all, so the bound is taken 2^-16 wider
-        const float T = wta_probe_sum(P, pv, key) * (1.f + 1.f / 65536.f);
-        unsigned m = 0;
-#pragma unroll
-        for (int e = 0; e < LPL; e++) if (cost_value(cost_code(cpk, e), P.lut) <= T) m |= 1u << e;
-        const bool ld = wta_lane_reads<LPL>(m, lane, T);
-        float s[LPL];
-        int am[kMaxPasses];
-#pragma unroll
-        for (int e = 0; e < LPL; e++) s[e] = 0.f;
-        unsigned nkey = key;
-        float npv = 0.f;
-#pragma unroll
-        for (int g = 0; g < kMaxPasses; g += 4) {
-            float v[4][LPL];
-#pragma unroll
-            for (int q = 0; q < 4; q++) {
-#pragma unroll
-                for (int e = 0; e < LPL; e++) v[q][e] = S2PB_INF;
-                if (ld) wta_ld_pass<LPL>(P.L[g + q] + (size_t)p * DP, lane, v[q]);
-            }
-            if (g == 0 && more) {
-                nkey = wta_probe_key<LPL>(ncpk, lane);
-                if (lane < kMaxPasses) npv = __ldcg(probe + (size_t)pn * DP + (nkey & 511u));
-            }
-#pragma unroll
-            for (int q = 0; q < 4; q++) am[g + q] = wta_add_pass<LPL>(v[q], lane, s);
-        }
-        float c[LPL];
-#pragma unroll
-        for (int e = 0; e < LPL; e++) c[e] = cost_value(cost_code(cpk, e), P.lut);
-        wta_finish<LPL>(P, p, lane, s, am, c, sSrow, (short)(range & 0xffffu), (short)(range >> 16));
-        if (!more) break;
-        p = pn; range = nrange; cpk = ncpk; key = nkey; pv = npv;
-    }
-}
-
-// The same WTA in two stages (DESIGN.md 3.2).  Pass 0 is read under the mask above.  S[d] >= L_0[d] too, so passes 1-7 are read
-// only where L_0[d] <= T, dilated by one slot (the winner, its ties and the fit), or where C[d] <= L_q[d0]: a pass-q
-// arg-minimum d* has C[d*] <= L_q[d*] = min L_q <= L_q[d0], so every pass's consensus slot is read.  Lanes 0-7 hold L_q[d0]
-// from the probe.  L_q >= C holds without rounding (L_q = fl(C + x), x >= 0), so that term needs no slack.
-//
-// Pass 0 would put one more round trip on a pixel's chain, so a warp works three pixels deep: pixel p+1's probe and pass 0 are
-// requested while p's passes 1-7 are in flight, and pixel p+2's codes and range one pixel ahead of its probe.  Passes 1-7 are
-// requested together (one round trip; the pruned lanes leave registers for all seven under the 64-register cap), so a pixel
-// waits on one round trip where wta_pruned_kernel waits on two (its passes four at a time).
 template <int LPL> __device__ __forceinline__ void wta_ld_pass_if(const float *px, int lane, bool ld, float (&v)[LPL])
 {
 #pragma unroll
@@ -775,13 +706,14 @@ __device__ __forceinline__ unsigned wta_range(const WtaParams &P, unsigned p)
     return ((unsigned)(unsigned short)__ldg(P.lo + p)) | ((unsigned)(unsigned short)__ldg(P.hi + p) << 16);
 }
 template <int LPL>
-__global__ void __launch_bounds__(kWtaThreads) __maxnreg__((LPL <= 4) ? 64 : 128) wta_pruned2_kernel(const WtaParams P)
+__global__ void __launch_bounds__(kWtaThreads) __maxnreg__((LPL <= 4) ? 64 : 128) wta_pruned_kernel(const WtaParams P)
 {
     static_assert(!WtaMap<LPL>::interleaved && LPL <= 8, "blocked slots, codes held in registers");
     constexpr int DP = 32 * LPL;
     __shared__ float sS[kWtaThreads / 32][DP];
     float *sSrow = sS[threadIdx.x >> 5];
     const int lane = threadIdx.x & 31;
+    // (32-bit pixel counters and the range in one word: the state of three pixels shares the register cap)
     const unsigned warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = (gridDim.x * blockDim.x) >> 5;
     const unsigned npix = (unsigned)P.npix;
     if (warp >= npix) return;
@@ -795,7 +727,8 @@ __global__ void __launch_bounds__(kWtaThreads) __maxnreg__((LPL <= 4) ? 64 : 128
     CostPack<LPL> cpk = ld_cost<LPL, true>(codes + (size_t)p * DP);
     const unsigned key = wta_probe_key<LPL>(cpk, lane);
     float pv = lane < kMaxPasses ? __ldcg(probe + (size_t)p * DP + (key & 511u)) : 0.f;
-    // (the slack of wta_pruned_kernel: the scaled costs round in the sums)
+    // the integer costs of census 5x5 make S >= C exact; the scaled costs of 3x3 / 7x7 round in the eight additions and the
+    // overcount fix, by less than 2^-18 of S in all, so the bound is taken 2^-16 wider
     float T = wta_probe_sum(P, pv, key) * (1.f + 1.f / 65536.f);
     float v0[LPL];
     wta_ld_pass_if<LPL>(P.L[0] + (size_t)p * DP, lane, wta_lane_reads_c<LPL>(P, cpk, lane, T), v0);

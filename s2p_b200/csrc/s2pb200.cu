@@ -105,8 +105,8 @@ struct Slot {
 struct s2pb_ctx {
     int device = 0;
     int sm_count = 132;
-    int wta_prune = 2;             // S2PB_WTA_PRUNE (read when the context is created, A/B): 0 wta_kernel for every shape,
-                                   // 1 the one-stage wta_pruned_kernel, 2 (the default) the two-stage wta_pruned2_kernel (DESIGN.md 6)
+    bool wta_prune = true;         // S2PB_WTA_PRUNE (read when the context is created): 0 wta_kernel for every shape, the
+                                   // same-device reference of wta_pruned_kernel (DESIGN.md 3.2); unset or any other value prunes
     std::vector<Slot> slots;
     int *abort_flag = nullptr;     // pinned + mapped: the host raises it on timeout
     int *scratch_flag = nullptr;   // pinned + mapped: device -> host one-word answers
@@ -327,7 +327,7 @@ extern "C" s2pb_ctx *s2pb_create(int device)
     s2pb_ctx *ctx = new s2pb_ctx;
     ctx->device = device;
     ctx->sm_count = prop.multiProcessorCount;
-    if (const char *e = getenv("S2PB_WTA_PRUNE")) ctx->wta_prune = atoi(e);
+    if (const char *e = getenv("S2PB_WTA_PRUNE")) ctx->wta_prune = atoi(e) != 0;
     if (cudaHostAlloc((void **)&ctx->abort_flag, 16 * sizeof(int), cudaHostAllocMapped) != cudaSuccess) {
         fail(S2PB_ERR_CUDA, "cudaHostAlloc failed"); delete ctx; return nullptr;
     }
@@ -583,30 +583,25 @@ static int launch_aggregate(s2pb_ctx *ctx, Slot &s, int nviews, int w, int h, in
     return S2PB_OK;
 }
 
-// S2PB_COST_STRIP=0: the per-pixel cost kernel for every shape (A/B)
-static bool cost_strip_enabled() { static int v = -1; if (v < 0) { const char *e = getenv("S2PB_COST_STRIP"); v = e ? atoi(e) : 1; } return v != 0; }
+// census 3x3 / 5x5 up to 8 labels per lane: the strip-staged kernel; 7x7, the half-pixel pass and 12 / 16 labels per lane: the
+// per-pixel one
 template <int LPL> static void launch_cost_t(const uint64_t *cu, const uint64_t *cv, const uint64_t *cv1, int zoom, bool narrow, int w, int h,
                                              const short *lo, const short *hi, int gmin, uint8_t *C, int sm, cudaStream_t st)
 {
-    if constexpr (LPL <= 8) {
-        if (zoom != 2 && narrow && cost_strip_enabled()) { cost_strip_kernel<LPL><<<sm * 16, kCostStripThreads, 0, st>>>(cu, cv, w, h, lo, hi, gmin, C); return; }
-    }
     if (zoom == 2) {
         if (narrow) cost_kernel<LPL, true, true><<<sm * 8, 256, 0, st>>>(cu, cv, cv1, w, h, lo, hi, gmin, C);
         else cost_kernel<LPL, true, false><<<sm * 8, 256, 0, st>>>(cu, cv, cv1, w, h, lo, hi, gmin, C);
-    } else {
-        if (narrow) cost_kernel<LPL, false, true><<<sm * 8, 256, 0, st>>>(cu, cv, cv1, w, h, lo, hi, gmin, C);
-        else cost_kernel<LPL, false, false><<<sm * 8, 256, 0, st>>>(cu, cv, cv1, w, h, lo, hi, gmin, C);
-    }
+    } else if (!narrow) cost_kernel<LPL, false, false><<<sm * 8, 256, 0, st>>>(cu, cv, cv1, w, h, lo, hi, gmin, C);
+    else if constexpr (LPL <= 8) cost_strip_kernel<LPL><<<sm * 16, kCostStripThreads, 0, st>>>(cu, cv, w, h, lo, hi, gmin, C);
+    else cost_kernel<LPL, false, true><<<sm * 8, 256, 0, st>>>(cu, cv, cv1, w, h, lo, hi, gmin, C);
 }
 // prune (s2pb_ctx::wta_prune): the census flavour's eight-pass WTA without a dense S or PKR output reads only the labels that
 // can still win
-template <int LPL> static void launch_wta_t(const WtaParams &P, int sm, cudaStream_t st, bool general, int prune)
+template <int LPL> static void launch_wta_t(const WtaParams &P, int sm, cudaStream_t st, bool general, bool prune)
 {
     if constexpr (LPL == 1 || LPL == 2 || LPL == 4 || LPL == 8) {
-        if (prune != 0 && !general && P.ndir == kMaxPasses && P.S == nullptr && P.pkr == nullptr) {
-            if (prune == 1) wta_pruned_kernel<LPL><<<sm * 16, kWtaThreads, 0, st>>>(P);
-            else wta_pruned2_kernel<LPL><<<sm * 16, kWtaThreads, 0, st>>>(P);
+        if (prune && !general && P.ndir == kMaxPasses && P.S == nullptr && P.pkr == nullptr) {
+            wta_pruned_kernel<LPL><<<sm * 16, kWtaThreads, 0, st>>>(P);
             return;
         }
     }

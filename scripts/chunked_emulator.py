@@ -22,7 +22,6 @@ if os.environ.get("EMU_WARPS"):          # the configurations of the slabs wider
     STAGE = int(os.environ.get("EMU_STAGE", 2))
     R0 = 2 * STAGE
 FIXED = os.environ.get("EMU_BUGGY") != "1"      # EMU_BUGGY=1 reproduces the first version of the kernel (chunk-edge bug)
-FILL_INF = os.environ.get("EMU_FILL_INF") == "1"   # 1: the variant that writes +INF to the skipped chunks of the global volume
 GENERAL = os.environ.get("EMU_GENERAL") == "1"
 
 
@@ -190,7 +189,7 @@ def run_pass(pd, C, lo_img, hi_img, gmin, DP, tsgm, P1, P2, L, Lmin, W=None):
                 lm = np.full(32, INF, F)
                 wv = wst[k, slot] if W is not None else F(1.0)
                 P1w = F(P1) * wv
-                outv = np.full(DP, INF, F) if FILL_INF else L[w["outpix"]].copy()
+                outv = L[w["outpix"]].copy()
                 for e in range(NC):
                     kk = 32 * e + lane
                     if ea <= e <= eb:
@@ -285,14 +284,11 @@ def main():
     ok = (Ssum == So) | (np.isnan(Ssum) & np.isnan(So)) | (~inr.reshape(npix, DP))
     print("%sDP %d %dx%d tsgm %d (%d warps, %d stages): %d of %d in-range voxels differ" % (
         "general, " if GENERAL else "", DP, w, h, tsgm, W_, STAGE, int((~ok).sum()), int(inr.sum())))
-    # chunks outside every pixel's span must hold +INF in the emulated global volume
+    # chunks outside a pixel's span are never written in the emulated global volume (the chunk-skipping WTA never reads them)
     ea, eb = (lo.reshape(-1) - gmin) >> 5, (hi.reshape(-1) - gmin) >> 5
     e_of = (np.arange(DP) >> 5)[None, :]
     outside = (e_of < ea[:, None]) | (e_of > eb[:, None])
-    if FILL_INF:
-        print("skipped chunks all +INF:", bool(np.all(np.isinf(Ls[0][outside]))))
-    else:
-        print("skipped chunks untouched:", bool(np.all(Ls[0][outside] == np.float32(-1.0))))
+    print("skipped chunks untouched:", bool(np.all(Ls[0][outside] == np.float32(-1.0))))
     if os.environ.get("EMU_WTA", "1") == "1":
         main_wta(DP, h, w, tsgm, seed, Ls, Cf, lo.reshape(-1), hi.reshape(-1), gmin, Wimg, P1, P2)
 

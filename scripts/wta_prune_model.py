@@ -109,7 +109,7 @@ def survivors(C, T):
 
 
 def two_stage(C, T, Ls):
-    """The slots each pass is read on by the two-stage WTA (wta_pruned2_kernel) -> eight [h][w][D] masks.  Pass 0: the
+    """The slots each pass is read on by the two-stage WTA (wta_pruned_kernel) -> eight [h][w][D] masks.  Pass 0: the
     dilated survivors of C.  Passes 1-7: {d : L_0[d] <= T} from what was read of pass 0, dilated (S >= L_0 like S >= C, same
     slack), and {d : C[d] <= L_q[d0]} with d0 the probe slot (first arg-minimum of C): every arg-minimum of L_q lies there."""
     _, d0 = survivors(C, T)

@@ -1,11 +1,10 @@
 #!/usr/bin/env python3
-"""The WTA stage of one C2 tile (1024 x 1024, 128 labels) alone on the device, without pruning, with one-stage and with
-two-stage pruning (DESIGN.md 3.2, 6).
+"""The WTA stage of one C2 tile (1024 x 1024, 128 labels) alone on the device, without and with pruning (DESIGN.md 3.2, 6).
 
 The library records CUDA events around the two WTA launches of a tile (left and right view); this script runs the tile serially,
-nothing else on the device, N times after a warm-up, with S2PB_WTA_PRUNE=0, 1 and 2 in turn, twice (the switch is read when the
-context is created), and sets the bytes the kernel requests -- the sector fractions of scripts/wta_prune_model.py on a strip
-of the same pair -- against the time.  Prints the card's name, power limit and SM clock from the same process.
+nothing else on the device, N times after a warm-up, with S2PB_WTA_PRUNE=0 and unset (the default) in turn, twice (the switch is
+read when the context is created), and sets the bytes the kernel requests -- the sector fractions of scripts/wta_prune_model.py
+on a strip of the same pair -- against the time.  Prints the card's name, power limit and SM clock from the same process.
 
     python scripts/wta_prune_probe.py [--n 20] [--nan-border 0.05]
 """
@@ -36,27 +35,28 @@ def main():
     dmin, dmax = -64, 63
     ref, sec, _ = make_pair(a.size, a.size, dmin, dmax, seed=0, nan_border=a.nan_border)
     npix = a.size * a.size
-    nbytes = {"0": 0.0, "1": 0.0, "2": 0.0}
+    nbytes = {"0": 0.0, "default": 0.0}
     for view in "LR":
         C, S = M.strip_volumes(0, a.size, (300, 396), dmin, dmax, a.nan_border, view)
         DP = C.shape[-1]
         full = npix * (8 * 4 * DP + DP)
         nbytes["0"] += full
         if DP % 32 or DP // 32 not in (1, 2, 4, 8):          # interleaved labels per lane: wta_kernel serves the view
-            nbytes["1"] += full
-            nbytes["2"] += full
+            nbytes["default"] += full
             print("view %s: %d slots, not pruned" % (view, DP))
             continue
-        f2, f1 = M.two_stage_fractions(C, S)
+        f2, _ = M.two_stage_fractions(C, S)
         # sectors asked for, one probe sector per pass, the codes
-        nbytes["1"] += npix * (f1 * 8 * 4 * DP + 8 * 32 + DP)
-        nbytes["2"] += npix * (sum(f2) * 4 * DP + 8 * 32 + DP)
-        print("view %s: %d slots, sector fraction one stage %.3f, two stages %s (mean %.3f)" % (
-            view, DP, f1, " ".join("%.3f" % x for x in f2), np.mean(f2)))
+        nbytes["default"] += npix * (sum(f2) * 4 * DP + 8 * 32 + DP)
+        print("view %s: %d slots, sector fraction per pass %s (mean %.3f)" % (
+            view, DP, " ".join("%.3f" % x for x in f2), np.mean(f2)))
     p = default_params("mgm")
     outs = []
-    for sw in ("0", "1", "2", "0", "1", "2"):
-        os.environ["S2PB_WTA_PRUNE"] = sw
+    for sw in ("0", "default", "0", "default"):
+        if sw == "default":
+            os.environ.pop("S2PB_WTA_PRUNE", None)
+        else:
+            os.environ["S2PB_WTA_PRUNE"] = sw
         eng = Engine(0)
         for _ in range(3):
             out = eng.mgm(ref, sec, dmin, dmax, p, want_right=True)
@@ -68,7 +68,7 @@ def main():
         outs.append(out)
         wta = np.array([x["wta"] for x in t])
         agg = np.array([x["aggregate"] for x in t])
-        print("S2PB_WTA_PRUNE=%s: wta %.3f ms (min %.3f, max %.3f), aggregate %.3f ms, %.2f GB requested -> %.2f TB/s" % (
+        print("S2PB_WTA_PRUNE %s: wta %.3f ms (min %.3f, max %.3f), aggregate %.3f ms, %.2f GB requested -> %.2f TB/s" % (
             sw, wta.mean(), wta.min(), wta.max(), agg.mean(), nbytes[sw] / 1e9, nbytes[sw] / 1e9 / wta.mean()), flush=True)
     same = all(np.array_equal(outs[0][k].view(np.int32), o[k].view(np.int32)) for o in outs[1:] for k in ("disp", "conf", "disp_right"))
     print("outputs identical:", same)

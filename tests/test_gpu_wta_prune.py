@@ -1,6 +1,7 @@
-"""The WTA that reads only the labels that can still win (wta_pruned_kernel, DESIGN.md 3.2) against wta_kernel on the same
-device: disparity, confidence, mask and right disparity bit for bit, NaNs included.  S2PB_WTA_PRUNE is read when a context
-is created, so the two engines of this module differ in nothing else."""
+"""The WTA that reads only the labels that can still win (wta_pruned_kernel, DESIGN.md 3.2: pass 0 read where C <= T,
+passes 1-7 where L_0 <= T or C <= L_q[d0]) against wta_kernel on the same device: disparity, confidence, mask and right
+disparity bit for bit, NaNs included.  S2PB_WTA_PRUNE is read when a context is created: unset selects the pruned kernel,
+0 wta_kernel, so the two engines of this module differ in nothing else."""
 import os
 
 import numpy as np
@@ -17,9 +18,10 @@ def engines():
     old = os.environ.get("S2PB_WTA_PRUNE")
     made = []
     try:
-        for v in ("1", "0"):
-            os.environ["S2PB_WTA_PRUNE"] = v
-            made.append(Engine(0))
+        os.environ.pop("S2PB_WTA_PRUNE", None)
+        made.append(Engine(0))                  # the default: wta_pruned_kernel
+        os.environ["S2PB_WTA_PRUNE"] = "0"
+        made.append(Engine(0))                  # wta_kernel
     finally:
         if old is None:
             os.environ.pop("S2PB_WTA_PRUNE", None)
@@ -86,5 +88,16 @@ def test_pruned_wta_equals_full_wta_in_mgm_multi(engines):
     ref, sec, _ = make_pair(130, 170, -14, 16, seed=5, nan_border=0.06)
     p = default_params("mgm_multi")
     new, old = (e.mgm(ref, sec, -14, 16, p, want_right=True) for e in engines)
+    for k in ("disp", "conf", "disp_right"):
+        assert _same_bits(new[k], old[k]), k
+
+
+def test_pruned_wta_on_a_tile_of_many_warps(engines):
+    """a tile with more pixels than the grid has warps: every warp runs its three-pixel-deep pipeline through several rounds
+    and its tail (the last pixels of a warp, whose successors are past the end)"""
+    from s2p_b200.engine import default_params
+    ref, sec, _ = make_pair(256, 384, -64, 63, seed=11, nan_border=0.03)
+    p = default_params("mgm")
+    new, old = (e.mgm(ref, sec, -64, 63, p, want_right=True) for e in engines)
     for k in ("disp", "conf", "disp_right"):
         assert _same_bits(new[k], old[k]), k

@@ -1,4 +1,4 @@
-"""The claims the two-stage pruned WTA rests on (wta_pruned2_kernel, DESIGN.md 3.2), checked on the CPU: pass 0 read on the
+"""The claims the two-stage pruned WTA rests on (wta_pruned_kernel, DESIGN.md 3.2), checked on the CPU: pass 0 read on the
 dilated survivors {d : C[d] <= S[d0]}, passes 1-7 on {d : L_0[d] <= S[d0]} dilated and {d : C[d] <= L_q[d0]}; from those
 reads alone the winner, the three values of the sub-pixel fit and every pass's last arg-minimum equal those from the full
 vectors.  Census 3x3 and 7x7 (scaled costs) are where the 2^-16 slack of the bound matters."""

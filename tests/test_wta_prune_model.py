@@ -1,6 +1,6 @@
-"""The claims the pruned WTA rests on (DESIGN.md 3.2), checked on the CPU: from the survivors {d : C[d] <= S[d0]} dilated
-by one slot alone, the winner, the three values of the sub-pixel fit and every pass's last arg-minimum equal those from
-the full vectors.  Pass volumes from scripts/wta_prune_model.py's numpy restatement of the scan, pinned to the oracle's S."""
+"""The claims the pruned WTA's pass 0 rests on (wta_pruned_kernel, DESIGN.md 3.2), checked on the CPU: from the survivors
+{d : C[d] <= S[d0]} dilated by one slot alone, the winner, the three values of the sub-pixel fit and every pass's last
+arg-minimum equal those from the full vectors.  Pass volumes from scripts/wta_prune_model.py's numpy restatement of the scan, pinned to the oracle's S."""
 import os
 import sys
 
