@@ -19,7 +19,7 @@ int agg_chunked_configure()
     return 0;
 }
 
-// 0 ok, -1 CUDA error, -2 this shape is not served (the caller then uses the dense kernel)
+// 0 ok, -1 CUDA error, -2 this shape is not served
 int agg_chunked_launch(int tsgm, const ChunkedParams &P, int sm_count, cudaStream_t st)
 {
     if (P.DP < 32 || P.DP > 2048 || (P.DP & 31)) return -2;

@@ -3,8 +3,6 @@
 
 namespace s2pb {
 
-#define S2PB_FOR_EACH_LPL(X) X(1) X(2) X(3) X(4) X(5) X(6) X(8) X(12) X(16)
-
 #define DECL(n) template <> int agg_launch_lpl<n>(int, const AggParams &, int, cudaStream_t, int); template <> int agg_configure_lpl<n>();
 S2PB_FOR_EACH_LPL(DECL)
 #undef DECL

@@ -40,7 +40,8 @@ __global__ void prepare_view_kernel(const float *__restrict__ in, int n, int lo_
     hi[i] = (short)(isn ? sentinel + 1 : hi_all);
 }
 
-// does the image hold a NaN?  (sizes the right view's label hull, see plan_labels in s2pb200.cu)
+// does the image hold a NaN?  (a no-data pixel of the secondary image widens the right view's label hull: mgm_enqueue in
+// s2pb200.cu)
 __global__ void has_nan_kernel(const float *__restrict__ in, int n, int *flag)
 {
     bool f = false;
@@ -482,6 +483,33 @@ __device__ __forceinline__ void parabola3(float v0, float v1, float v2, float &v
     xmin = x;
 }
 
+// The end of every WTA pixel: the sub-pixel fit around the winning slot kbest (V-fit / parabola on sS[kbest-1..kbest+1] when
+// o-1 >= plo and o+2 <= phi, mgm_refine.h:67-84) and the disp / cost / conf stores.  o = gmin + kbest, the winning label;
+// minP = (float)o and minL = S at kbest, formed by the caller as soon as it knows kbest (formed after its S and PKR stores
+// instead, they cost the register-capped WTA kernels stack); confi: the passes whose last arg-minimum is kbest; plo, phi: the
+// pixel's label range.  The closing __syncwarp lets the warp's next pixel reuse sS.
+__device__ __forceinline__ void wta_store(const WtaParams &P, size_t p, int lane, const float *sS, int kbest, int o, float minP,
+                                          float minL, int confi, int plo, int phi)
+{
+    if (P.refine != 0 && lane == 0) {
+        if (o - 1 >= plo && o + 2 <= phi) {
+            const float v0 = sS[kbest - 1], v1 = sS[kbest], v2 = sS[kbest + 1];
+            float dx = 0.f, dxr = 0.f, ml = minL, mlr = minP;
+            if (P.refine == 1) { vfit3(v0, v1, v2, ml, dx); vfit3(v2, v1, v0, mlr, dxr); }
+            else { parabola3(v0, v1, v2, ml, dx); parabola3(v2, v1, v0, mlr, dxr); }
+            minP = (float)o + dx;
+            minL = ml;
+            if (mlr < ml) { minP = (float)o - dxr; minL = mlr; }
+        }
+    }
+    if (lane == 0) {
+        P.disp[p] = __fdiv_rn(minP, P.inv_zoom_div);
+        if (P.cost) P.cost[p] = minL;
+        if (P.conf) P.conf[p] = (float)confi;
+    }
+    __syncwarp();
+}
+
 // One warp per pixel: S = (L0+L1+...+L_{ndir-1}) - (ndir-1) C in pass order (dvec.cc:110-118,
 // mgm_core.cc:1041-1042), first strict minimum over finite S (:1044-1048), consensus (:1054-1057),
 // V-fit / parabola on S[o-1..o+1] when o-1 >= lo and o+2 <= hi (mgm_refine.h:67-84).
@@ -562,23 +590,7 @@ __device__ __forceinline__ void wta_finish(const WtaParams &P, size_t p, int lan
         sec = warp_min_f32(sec);
         if (lane == 0) P.pkr[p] = pkr_ratio(sec, m);
     }
-    if (P.refine != 0 && lane == 0) {
-        if (o - 1 >= plo && o + 2 <= phi) {
-            const float v0 = sSrow[kbest - 1], v1 = sSrow[kbest], v2 = sSrow[kbest + 1];
-            float dx = 0.f, dxr = 0.f, ml = minL, mlr = minP;
-            if (P.refine == 1) { vfit3(v0, v1, v2, ml, dx); vfit3(v2, v1, v0, mlr, dxr); }
-            else { parabola3(v0, v1, v2, ml, dx); parabola3(v2, v1, v0, mlr, dxr); }
-            minP = (float)o + dx;
-            minL = ml;
-            if (mlr < ml) { minP = (float)o - dxr; minL = mlr; }
-        }
-    }
-    if (lane == 0) {
-        P.disp[p] = __fdiv_rn(minP, P.inv_zoom_div);
-        if (P.cost) P.cost[p] = minL;
-        if (P.conf) P.conf[p] = (float)confi;
-    }
-    __syncwarp();
+    wta_store(P, p, lane, sSrow, kbest, o, minP, minL, confi, plo, phi);
 }
 
 // 128-thread CTAs capped at 64 registers for LPL <= 4: one of them still fits on an SM next to the two resident
@@ -705,10 +717,12 @@ __device__ __forceinline__ unsigned wta_range(const WtaParams &P, unsigned p)
 {
     return ((unsigned)(unsigned short)__ldg(P.lo + p)) | ((unsigned)(unsigned short)__ldg(P.hi + p) << 16);
 }
+// the widths wta_pruned_kernel serves (launch_wta in s2pb200.cu picks it): blocked slots, codes held in registers
+__host__ __device__ constexpr bool wta_pruned_width(int LPL) { return LPL == 1 || LPL == 2 || LPL == 4 || LPL == 8; }
 template <int LPL>
 __global__ void __launch_bounds__(kWtaThreads) __maxnreg__((LPL <= 4) ? 64 : 128) wta_pruned_kernel(const WtaParams P)
 {
-    static_assert(!WtaMap<LPL>::interleaved && LPL <= 8, "blocked slots, codes held in registers");
+    static_assert(wta_pruned_width(LPL) && !WtaMap<LPL>::interleaved, "blocked slots, codes held in registers");
     constexpr int DP = 32 * LPL;
     __shared__ float sS[kWtaThreads / 32][DP];
     float *sSrow = sS[threadIdx.x >> 5];
@@ -849,23 +863,7 @@ __global__ void __launch_bounds__(kWtaThreads) wta_chunked_kernel(const WtaParam
             sec = warp_min_f32(sec);
             if (lane == 0) P.pkr[p] = pkr_ratio(sec, m);
         }
-        if (P.refine != 0 && lane == 0) {
-            if (kbest - 1 >= lo && kbest + 2 <= hi) {                 // o - 1 >= lo_label && o + 2 <= hi_label
-                const float v0 = sS[kbest - 1], v1 = sS[kbest], v2 = sS[kbest + 1];
-                float dx = 0.f, dxr = 0.f, ml = minL, mlr = minP;
-                if (P.refine == 1) { vfit3(v0, v1, v2, ml, dx); vfit3(v2, v1, v0, mlr, dxr); }
-                else { parabola3(v0, v1, v2, ml, dx); parabola3(v2, v1, v0, mlr, dxr); }
-                minP = (float)o + dx;
-                minL = ml;
-                if (mlr < ml) { minP = (float)o - dxr; minL = mlr; }
-            }
-        }
-        if (lane == 0) {
-            P.disp[p] = __fdiv_rn(minP, P.inv_zoom_div);
-            if (P.cost) P.cost[p] = minL;
-            if (P.conf) P.conf[p] = (float)confi;
-        }
-        __syncwarp();
+        wta_store(P, p, lane, sS, kbest, o, minP, minL, confi, P.gmin + lo, P.gmin + hi);
     }
 }
 

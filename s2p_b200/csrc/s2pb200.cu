@@ -29,6 +29,7 @@
 #include <cstdlib>
 #include <string>
 #include <thread>
+#include <type_traits>
 #include <vector>
 
 using namespace s2pb;
@@ -184,12 +185,6 @@ private:
     size_t failed_ = 0;       // size of the first request that failed
 };
 
-static int lpl_for(int D)
-{
-    static const int opts[] = {1, 2, 3, 4, 5, 6, 8, 12, 16};
-    for (int o : opts) if (32 * o >= D) return o;
-    return -1;
-}
 // stride of the per-pass progress counters: bands hold kNW scanlines in the register-resident kernel, but as few as 2 in the
 // chunk-skipping kernel on float-cost slabs wider than 1024 slots (agg_chunked.cuh, ck_warps)
 static int max_bands(int w, int h) { return ((w > h ? w : h) + 1) / 2; }
@@ -500,7 +495,7 @@ static bool cost_lut(int win, float lut[64])
 // Label hull of each view (main_mgm.cc:178,207,210-216).  The no-data sentinel range [dmin, dmin+1]
 // always lies inside the left hull; on the right view it only matters when the secondary image
 // really holds no-data pixels, and then it may stick out of [-dmax, -dmin].
-static int plan_labels(int dmin, int dmax, bool sec_has_nodata, int gminv[2], int gmaxv[2])
+static void plan_labels(int dmin, int dmax, bool sec_has_nodata, int gminv[2], int gmaxv[2])
 {
     gminv[0] = dmin; gmaxv[0] = dmax;
     gminv[1] = -dmax; gmaxv[1] = -dmin;
@@ -508,14 +503,19 @@ static int plan_labels(int dmin, int dmax, bool sec_has_nodata, int gminv[2], in
         if (dmin < gminv[1]) gminv[1] = dmin;
         if (dmin + 1 > gmaxv[1]) gmaxv[1] = dmin + 1;
     }
-    int D = 0;
-    for (int vi = 0; vi < 2; vi++) { int d = gmaxv[vi] - gminv[vi] + 1; if (d > D) D = d; }
-    return lpl_for(D);
 }
-// labels per lane of ONE view's slab.  The views may differ: a no-data pixel in the secondary image widens only the right
-// view's hull (by one label when |dmin| > dmax), and each view's kernels run at that view's own width -- the volumes are
-// [H][W][32 LPL_view] inside buffers sized for the wider view.
-static int view_lpl(const int gminv[2], const int gmaxv[2], int vi) { return lpl_for(gmaxv[vi] - gminv[vi] + 1); }
+
+// Labels per lane of a slab of D labels (DP = 32 LPL slots): the narrowest register-resident width up to 512 labels, else
+// ceil(D / 32) 32-slot chunks for the chunk-skipping kernels (wide_slab), up to 2048 labels.
+static int slab_lpl(int D, int *lpl)
+{
+#define FITS(n) if (32 * n >= D) { *lpl = n; return S2PB_OK; }
+    S2PB_FOR_EACH_LPL(FITS)
+#undef FITS
+    if (D > 2048) return fail(S2PB_ERR_UNSUPPORTED, "a slab of %d labels: at most 2048 are supported", D);
+    *lpl = (D + 31) / 32;
+    return S2PB_OK;
+}
 
 static void fill_pass(PassDesc &pd, int pass, int w, int h)
 {
@@ -564,6 +564,7 @@ static int launch_aggregate(s2pb_ctx *ctx, Slot &s, int nviews, int w, int h, in
     P.P1 = P1; P.P2 = P2; P.next_item = counter; P.abort_flag = ctx->abort_flag; P.lut = general ? nullptr : lut;
     P.general = general ? 1 : 0;
     CK(cudaMemsetAsync(counter, 0, 4, st));
+    int r;
     if (wide_slab(LPL)) {
         ChunkedParams Q;
         memset(&Q, 0, sizeof Q);
@@ -572,15 +573,27 @@ static int launch_aggregate(s2pb_ctx *ctx, Slot &s, int nviews, int w, int h, in
         int q = 0;
         for (int vi = first_view; vi < first_view + nviews; vi++)
             for (int p = 0; p < ndir; p++, q++) { Q.lo[q] = s.v[vi].lo; Q.hi[q] = s.v[vi].hi; Q.gmin[q] = gminv[vi]; }
-        int rr = agg_chunked_launch(tsgm, Q, ctx->sm_count, st);
-        if (rr == 0) { ctx->launches++; return S2PB_OK; }
-        if (rr != -2) return fail(S2PB_ERR_CUDA, "chunked aggregation launch failed: %s", cudaGetErrorString(cudaGetLastError()));
+        r = agg_chunked_launch(tsgm, Q, ctx->sm_count, st);
+    } else {
+        r = agg_launch(LPL, tsgm, P, ctx->sm_count, st, ctas_per_sm);
     }
-    int r = agg_launch(LPL, tsgm, P, ctx->sm_count, st, ctas_per_sm);
-    if (r == -2) return fail(S2PB_ERR_UNSUPPORTED, "no aggregation kernel for %d labels per lane", LPL);
+    if (r == -2)
+        return fail(S2PB_ERR_UNSUPPORTED, "no %s aggregation kernel serves a slab of %d slots with TSGM %d%s",
+                    wide_slab(LPL) ? "chunk-skipping" : "register-resident", 32 * LPL, tsgm, general ? " (float costs)" : "");
     if (r != 0) return fail(S2PB_ERR_CUDA, "aggregation launch failed: %s", cudaGetErrorString(cudaGetLastError()));
     ctx->launches++;
     return S2PB_OK;
+}
+
+// f(std::integral_constant<int, LPL>()): the instantiation for a register-resident width LPL
+template <class F> static int with_lpl(int LPL, F &&f)
+{
+    switch (LPL) {
+#define CASE(n) case n: f(std::integral_constant<int, n>()); return S2PB_OK;
+    S2PB_FOR_EACH_LPL(CASE)
+#undef CASE
+    }
+    return fail(S2PB_ERR_UNSUPPORTED, "unsupported labels-per-lane %d", LPL);
 }
 
 // census 3x3 / 5x5 up to 8 labels per lane: the strip-staged kernel; 7x7, the half-pixel pass and 12 / 16 labels per lane: the
@@ -595,62 +608,58 @@ template <int LPL> static void launch_cost_t(const uint64_t *cu, const uint64_t 
     else if constexpr (LPL <= 8) cost_strip_kernel<LPL><<<sm * 16, kCostStripThreads, 0, st>>>(cu, cv, w, h, lo, hi, gmin, C);
     else cost_kernel<LPL, false, true><<<sm * 8, 256, 0, st>>>(cu, cv, cv1, w, h, lo, hi, gmin, C);
 }
-// prune (s2pb_ctx::wta_prune): the census flavour's eight-pass WTA without a dense S or PKR output reads only the labels that
-// can still win
-template <int LPL> static void launch_wta_t(const WtaParams &P, int sm, cudaStream_t st, bool general, bool prune)
+
+// The cost volume of one view into G.C.  general: float costs of G.cost (census through G.lut included); else the 8-bit census
+// codes of G.cu against G.cv0 (G.cv1 at odd labels when G.zoom = 2), read as bytes from G.C, where G.win <= 5 leaves the high
+// word of a code zero.  A wide slab (wide_slab) is written only on the chunks of each pixel's span.
+static int launch_cost(s2pb_ctx *ctx, int LPL, bool general, const CostGenParams &G, cudaStream_t st)
 {
-    if constexpr (LPL == 1 || LPL == 2 || LPL == 4 || LPL == 8) {
-        if (prune && !general && P.ndir == kMaxPasses && P.S == nullptr && P.pkr == nullptr) {
-            wta_pruned_kernel<LPL><<<sm * 16, kWtaThreads, 0, st>>>(P);
-            return;
-        }
+    const int sm = ctx->sm_count;
+    uint8_t *C8 = (uint8_t *)G.C;
+    int rc = S2PB_OK;
+    if (wide_slab(LPL)) {
+        if (general) cost_gen_chunked_kernel<<<sm * 8, 256, 0, st>>>(G, 32 * LPL);
+        else if (G.zoom == 2) cost_chunked_kernel<true><<<sm * 8, 256, 0, st>>>(G.cu, G.cv0, G.cv1, G.w, G.h, G.lo, G.hi, G.gmin, 32 * LPL, C8);
+        else cost_chunked_kernel<false><<<sm * 8, 256, 0, st>>>(G.cu, G.cv0, nullptr, G.w, G.h, G.lo, G.hi, G.gmin, 32 * LPL, C8);
+    } else if (general) {
+        rc = with_lpl(LPL, [&](auto k) { constexpr int K = decltype(k)::value; cost_gen_kernel<K><<<sm * 8, 256, 0, st>>>(G); });
+    } else {
+        rc = with_lpl(LPL, [&](auto k) {
+            constexpr int K = decltype(k)::value;
+            launch_cost_t<K>(G.cu, G.cv0, G.cv1, G.zoom, G.win <= 5, G.w, G.h, G.lo, G.hi, G.gmin, C8, sm, st);
+        });
     }
+    if (rc != S2PB_OK) return rc;
+    CK(cudaGetLastError());
+    ctx->launches++;
+    return S2PB_OK;
+}
+
+template <int LPL> static void launch_wta_t(const WtaParams &P, int sm, cudaStream_t st, bool general, bool pruned)
+{
+    if constexpr (wta_pruned_width(LPL))
+        if (pruned) { wta_pruned_kernel<LPL><<<sm * 16, kWtaThreads, 0, st>>>(P); return; }
     if (general) wta_kernel<LPL, true><<<sm * 16, kWtaThreads, 0, st>>>(P);
     else wta_kernel<LPL, false><<<sm * 16, kWtaThreads, 0, st>>>(P);
 }
-template <int LPL> static void launch_cost_gen_t(const CostGenParams &P, int sm, cudaStream_t st)
-{
-    cost_gen_kernel<LPL><<<sm * 8, 256, 0, st>>>(P);
-}
-#define LPL_SWITCH(LPL, CALL)                                                             \
-    switch (LPL) {                                                                        \
-    case 1: { constexpr int K = 1; CALL; } break;   case 2: { constexpr int K = 2; CALL; } break;   \
-    case 3: { constexpr int K = 3; CALL; } break;   case 4: { constexpr int K = 4; CALL; } break;   \
-    case 5: { constexpr int K = 5; CALL; } break;   case 6: { constexpr int K = 6; CALL; } break;   \
-    case 8: { constexpr int K = 8; CALL; } break;   case 12: { constexpr int K = 12; CALL; } break; \
-    case 16: { constexpr int K = 16; CALL; } break;                                        \
-    default: return fail(S2PB_ERR_UNSUPPORTED, "unsupported labels-per-lane %d", LPL);     \
-    }
-
-// census_win: the census window the codes were made with (3 and 5 leave the high word of a code zero)
-static int launch_cost(s2pb_ctx *ctx, int LPL, int census_win, const uint64_t *cu, const uint64_t *cv, int w, int h, const short *lo, const short *hi,
-                       int gmin, void *C, cudaStream_t st, const uint64_t *cv1 = nullptr, int zoom = 1)
-{
-    const bool narrow = census_win <= 5;
-    LPL_SWITCH(LPL, launch_cost_t<K>(cu, cv, cv1, zoom, narrow, w, h, lo, hi, gmin, (uint8_t *)C, ctx->sm_count, st));
-    CK(cudaGetLastError());
-    ctx->launches++;
-    return S2PB_OK;
-}
-static int launch_cost_gen(s2pb_ctx *ctx, int LPL, const CostGenParams &P, cudaStream_t st)
-{
-    LPL_SWITCH(LPL, launch_cost_gen_t<K>(P, ctx->sm_count, st));
-    CK(cudaGetLastError());
-    ctx->launches++;
-    return S2PB_OK;
-}
+// The WTA of one view.  A wide slab without a dense S: wta_chunked_kernel.  The census flavour's eight-pass WTA without a dense
+// S or PKR output, on the widths wta_pruned_kernel serves: that kernel, which reads only the labels that can still win, unless
+// the context was created with S2PB_WTA_PRUNE=0 (s2pb_ctx::wta_prune).  Everything else: wta_kernel.
 static int launch_wta(s2pb_ctx *ctx, int LPL, const WtaParams &P, cudaStream_t st, bool general = false)
 {
+    const int sm = ctx->sm_count;
+    int rc = S2PB_OK;
     if (P.S == nullptr && wide_slab(LPL)) {
         const int DP = 32 * LPL;
         const size_t smem = (size_t)(kWtaThreads / 32) * DP * sizeof(float);
-        if (general) wta_chunked_kernel<true><<<ctx->sm_count * 16, kWtaThreads, smem, st>>>(P, DP);
-        else wta_chunked_kernel<false><<<ctx->sm_count * 16, kWtaThreads, smem, st>>>(P, DP);
-        CK(cudaGetLastError());
-        ctx->launches++;
-        return S2PB_OK;
+        if (general) wta_chunked_kernel<true><<<sm * 16, kWtaThreads, smem, st>>>(P, DP);
+        else wta_chunked_kernel<false><<<sm * 16, kWtaThreads, smem, st>>>(P, DP);
+    } else {
+        const bool pruned = ctx->wta_prune && !general && P.ndir == kMaxPasses && P.S == nullptr && P.pkr == nullptr &&
+                            wta_pruned_width(LPL);
+        rc = with_lpl(LPL, [&](auto k) { constexpr int K = decltype(k)::value; launch_wta_t<K>(P, sm, st, general, pruned); });
     }
-    LPL_SWITCH(LPL, launch_wta_t<K>(P, ctx->sm_count, st, general, ctx->wta_prune));
+    if (rc != S2PB_OK) return rc;
     CK(cudaGetLastError());
     ctx->launches++;
     return S2PB_OK;
@@ -888,33 +897,15 @@ static int mgm_call(s2pb_ctx *ctx, Slot &s, int w, int h, const float *const img
     // ---- cost volumes: view 0 = left reference, view 1 = right reference (mgm_multiscale.cc:222,270)
     for (int vi = 0; vi < 2; vi++) {
         const ViewWS &v = s.v[vi], &o = s.v[1 - vi];
-        if (general) {
-            CostGenParams G;
-            memset(&G, 0, sizeof G);
-            G.u = img[vi]; G.v0 = o.rt; G.v1 = shf[1 - vi];
-            G.cu = v.census; G.cv0 = o.census_rt; G.cv1 = cen_half[1 - vi];
-            G.su = (const float2 *)G.cu; G.sv0 = (const float2 *)G.cv0; G.sv1 = (const float2 *)G.cv1;
-            G.lut = s.lut; G.lo = lo[vi]; G.hi = hi[vi];
-            G.w = w; G.h = h; G.gmin = gminv[vi]; G.cost = p->cost; G.win = p->census_win; G.zoom = zoom;
-            G.C = (float *)v.C;
-            if (wide_slab(LPLv[vi])) {         // only the chunks of each pixel's span
-                cost_gen_chunked_kernel<<<ctx->sm_count * 8, 256, 0, st>>>(G, 32 * LPLv[vi]);
-                ctx->launches++;
-                rc = cudaGetLastError() == cudaSuccess ? S2PB_OK : fail(S2PB_ERR_CUDA, "cost_gen_chunked_kernel launch failed");
-            } else {
-                rc = launch_cost_gen(ctx, LPLv[vi], G, st);
-            }
-        } else if (wide_slab(LPLv[vi])) {      // only the chunks of each pixel's span
-            if (zoom == 2) cost_chunked_kernel<true><<<ctx->sm_count * 8, 256, 0, st>>>(v.census, o.census_rt, cen_half[1 - vi], w, h,
-                                                                                  lo[vi], hi[vi], gminv[vi], 32 * LPLv[vi], (uint8_t *)v.C);
-            else cost_chunked_kernel<false><<<ctx->sm_count * 8, 256, 0, st>>>(v.census, o.census_rt, nullptr, w, h,
-                                                                               lo[vi], hi[vi], gminv[vi], 32 * LPLv[vi], (uint8_t *)v.C);
-            ctx->launches++;
-            rc = cudaGetLastError() == cudaSuccess ? S2PB_OK : fail(S2PB_ERR_CUDA, "cost_chunked_kernel launch failed");
-        } else {
-            rc = launch_cost(ctx, LPLv[vi], p->census_win, v.census, o.census_rt, w, h, lo[vi], hi[vi], gminv[vi], v.C, st,
-                             cen_half[1 - vi], zoom);
-        }
+        CostGenParams G;
+        memset(&G, 0, sizeof G);
+        G.u = img[vi]; G.v0 = o.rt; G.v1 = shf[1 - vi];
+        G.cu = v.census; G.cv0 = o.census_rt; G.cv1 = cen_half[1 - vi];
+        G.su = (const float2 *)G.cu; G.sv0 = (const float2 *)G.cv0; G.sv1 = (const float2 *)G.cv1;
+        G.lut = s.lut; G.lo = lo[vi]; G.hi = hi[vi];
+        G.w = w; G.h = h; G.gmin = gminv[vi]; G.cost = p->cost; G.win = p->census_win; G.zoom = zoom;
+        G.C = (float *)v.C;
+        rc = launch_cost(ctx, LPLv[vi], general, G, st);
         if (rc != S2PB_OK) return rc;
     }
     if (timed) CK(cudaEventRecord(s.ev[2], st));
@@ -1012,11 +1003,9 @@ static int mgm_call_level(s2pb_ctx *ctx, Slot &s, Level &L, int zoom, const s2pb
         if (gminv[vi] < -16000 || gmaxv[vi] > 16000) return fail(S2PB_ERR_ARG, "label range out of the int16 domain");
         int d = gmaxv[vi] - gminv[vi] + 1; if (d > D) D = d;
     }
-    int LPL = lpl_for(D);
-    if (LPL < 0) {      // hull wider than 512 labels: slab of ceil(D / 32) chunks through the chunk-skipping kernels
-        LPL = (D + 31) / 32;
-        if (LPL > 64) return fail(S2PB_ERR_UNSUPPORTED, "a %dx%d level needs %d labels in its volume; 2048 are supported", w, h, D);
-    }
+    int LPL;
+    rc = slab_lpl(D, &LPL);
+    if (rc != S2PB_OK) return rc;
     rc = slot_ensure(ctx, s, w, h, 32 * LPL, p->ndir, general ? 4 : 1);
     if (rc != S2PB_OK) return rc;
     TRACE(st, "level %dx%d zoom %d: hull L [%d,%d] R [%d,%d] -> LPL %d%s", w, h, zoom, gminv[0], gmaxv[0], gminv[1], gmaxv[1], LPL,
@@ -1182,17 +1171,15 @@ static int mgm_enqueue(s2pb_ctx *ctx, Slot &s, const float *d_im1, const float *
         if (rs != S2PB_OK) return rs;
         nodata_hint = hflag ? 3 : 0;
     }
-    int gminv[2], gmaxv[2];
+    // each view's slab is sized on its own: a no-data pixel in the secondary image widens only the right view's hull (by one
+    // label when |dmin| > dmax), and each view's kernels run at that view's own width -- the volumes are [H][W][32 LPL_view]
+    // inside buffers sized for the wider view
+    int gminv[2], gmaxv[2], LPLv[2], rc;
     plan_labels(dmin, dmax, (nodata_hint & 2) != 0, gminv, gmaxv);
-    int LPLv[2] = {view_lpl(gminv, gmaxv, 0), view_lpl(gminv, gmaxv, 1)};
     for (int vi = 0; vi < 2; vi++)
-        if (LPLv[vi] < 0) {      // more than 512 labels: chunk-skipping kernels on a slab of ceil(D / 32) chunks
-            LPLv[vi] = (gmaxv[vi] - gminv[vi] + 32) / 32;
-            if (LPLv[vi] > 64)
-                return fail(S2PB_ERR_UNSUPPORTED, "disparity range [%d,%d] needs more than the 2048 labels supported", dmin, dmax);
-        }
+        if ((rc = slab_lpl(gmaxv[vi] - gminv[vi] + 1, &LPLv[vi])) != S2PB_OK) return rc;
     const int LPL = LPLv[0] > LPLv[1] ? LPLv[0] : LPLv[1];
-    int rc = slot_ensure(ctx, s, w, h, 32 * LPL, p->ndir, general ? 4 : 1);
+    rc = slot_ensure(ctx, s, w, h, 32 * LPL, p->ndir, general ? 4 : 1);
     if (rc != S2PB_OK) return rc;
     const float *im[2] = {d_im1, d_im2};
     dim3 b2(32, 8);
@@ -1362,10 +1349,10 @@ extern "C" int s2pb_reserve(s2pb_ctx *ctx, int nslots, int w, int h, int nlabels
 {
     if (!ctx || nslots < 1) return fail(S2PB_ERR_ARG, "bad argument");
     CK(cudaSetDevice(ctx->device));
-    int LPL = lpl_for(nlabels);
-    if (LPL < 0) LPL = (nlabels + 31) / 32;
-    if (LPL > 64) return fail(S2PB_ERR_UNSUPPORTED, "too many labels");
-    int rc = ensure_slots(ctx, nslots);
+    int LPL;
+    int rc = slab_lpl(nlabels, &LPL);
+    if (rc != S2PB_OK) return rc;
+    rc = ensure_slots(ctx, nslots);
     if (rc != S2PB_OK) return rc;
     for (int i = 0; i < nslots; i++) {
         rc = slot_ensure(ctx, ctx->slots[i], w, h, 32 * LPL, 8);
@@ -1521,8 +1508,9 @@ static int stage_costvolume(s2pb_ctx *ctx, const float *u, const float *v, int w
     if (win != 3 && win != 5 && win != 7) return fail(S2PB_ERR_ARG, "window must be 3, 5 or 7");
     if (cost < 0 || cost >= S2PB_COST_COUNT) return fail(S2PB_ERR_ARG, "cost must be one of S2PB_COST_*");
     CK(cudaSetDevice(ctx->device));
-    int LPL = lpl_for(D);
-    if (LPL < 0) return fail(S2PB_ERR_UNSUPPORTED, "too many labels");
+    int LPL, rc = slab_lpl(D, &LPL);      // the stage entry points run the register-resident kernels only
+    if (rc == S2PB_OK && wide_slab(LPL)) rc = fail(S2PB_ERR_UNSUPPORTED, "the stage entry points take at most 512 labels, not %d", D);
+    if (rc != S2PB_OK) return rc;
     const int DP = 32 * LPL;
     size_t npix = (size_t)w * h, tot = npix * D;
     cudaStream_t st = ctx->slots[0].stream;
@@ -1533,7 +1521,7 @@ static int stage_costvolume(s2pb_ctx *ctx, const float *u, const float *v, int w
     float *dCf = L.take<float>(tot * 4), *dlut = L.take<float>(256);
     if (!du || !dv || !cu || !cv || !dC || !dCf || !dlut) return L.nomem("the cost volume");
     short *dlo, *dhi;
-    int rc = upload_ranges(L, lo, hi, npix, gmin, D, st, &dlo, &dhi);
+    rc = upload_ranges(L, lo, hi, npix, gmin, D, st, &dlo, &dhi);
     if (rc != S2PB_OK) return rc;
     CK(cudaMemcpyAsync(du, u, npix * 4, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(dv, v, npix * 4, cudaMemcpyHostToDevice, st));
@@ -1554,21 +1542,16 @@ static int stage_costvolume(s2pb_ctx *ctx, const float *u, const float *v, int w
         ncc_stats_kernel<<<grid2d(w, h, b2), b2, 0, st>>>(rt, w, h, win / 2, (float2 *)cv);
         ctx->launches += 2;
     }
-    if (codes) {
-        rc = launch_cost(ctx, LPL, win, cu, cv, w, h, dlo, dhi, gmin, dC, st);
-        if (rc != S2PB_OK) return rc;
-        unpack_cost_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>((uint8_t *)dC, npix, D, DP, scaled ? dlut : nullptr, dCf);
-    } else {
-        CostGenParams G;
-        memset(&G, 0, sizeof G);
-        G.u = du; G.v0 = rt; G.cu = cu; G.cv0 = cv;
-        G.su = (float2 *)cu; G.sv0 = (float2 *)cv;
-        G.lut = dlut; G.lo = dlo; G.hi = dhi;
-        G.w = w; G.h = h; G.gmin = gmin; G.cost = cost; G.win = win; G.zoom = 1; G.C = (float *)dC;
-        rc = launch_cost_gen(ctx, LPL, G, st);
-        if (rc != S2PB_OK) return rc;
-        unpad_cost_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>((float *)dC, npix, D, DP, dCf);
-    }
+    CostGenParams G;
+    memset(&G, 0, sizeof G);
+    G.u = du; G.v0 = rt; G.cu = cu; G.cv0 = cv;
+    G.su = (float2 *)cu; G.sv0 = (float2 *)cv;
+    G.lut = dlut; G.lo = dlo; G.hi = dhi;
+    G.w = w; G.h = h; G.gmin = gmin; G.cost = cost; G.win = win; G.zoom = 1; G.C = (float *)dC;
+    rc = launch_cost(ctx, LPL, !codes, G, st);
+    if (rc != S2PB_OK) return rc;
+    if (codes) unpack_cost_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>((uint8_t *)dC, npix, D, DP, scaled ? dlut : nullptr, dCf);
+    else unpad_cost_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>((float *)dC, npix, D, DP, dCf);
     ctx->launches++;
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync(C, dCf, tot * 4, cudaMemcpyDeviceToHost, st));
@@ -1598,8 +1581,9 @@ static int stage_aggregate(s2pb_ctx *ctx, const float *C, const int32_t *lo, con
     if (ndir != 2 && ndir != 4 && ndir != 8) return fail(S2PB_ERR_ARG, "ndir must be 2, 4 or 8");
     if (tsgm < 1 || tsgm > 4) return fail(S2PB_ERR_ARG, "tsgm must be 1..4");
     CK(cudaSetDevice(ctx->device));
-    int LPL = lpl_for(D);
-    if (LPL < 0) return fail(S2PB_ERR_UNSUPPORTED, "too many labels");
+    int LPL, rc = slab_lpl(D, &LPL);      // the stage entry points run the register-resident kernels only
+    if (rc == S2PB_OK && wide_slab(LPL)) rc = fail(S2PB_ERR_UNSUPPORTED, "the stage entry points take at most 512 labels, not %d", D);
+    if (rc != S2PB_OK) return rc;
     const int DP = 32 * LPL;
     size_t npix = (size_t)w * h, tot = npix * D;
     if (!general) {
@@ -1614,7 +1598,7 @@ static int stage_aggregate(s2pb_ctx *ctx, const float *C, const int32_t *lo, con
     }
     Slot &s = ctx->slots[0];
     cudaStream_t st = s.stream;
-    int rc = slot_ensure(ctx, s, w, h, DP, ndir, general ? 4 : 1);
+    rc = slot_ensure(ctx, s, w, h, DP, ndir, general ? 4 : 1);
     if (rc != S2PB_OK) return rc;
     ScratchLease L(ctx, st);
     float *dCf = L.take<float>(tot * 4);
