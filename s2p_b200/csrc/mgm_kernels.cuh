@@ -660,22 +660,20 @@ __global__ void __launch_bounds__(kWtaThreads) __maxnreg__((LPL <= 4) ? 64 : 128
 }
 
 // The same WTA reading only the labels that can still win (DESIGN.md 3.2).  Census flavour, unit weights: every message of
-// the aggregation is >= 0, so L_p[d] >= C[d] in every pass and S[d] >= C[d].  With T = S[d0] of one probe slot d0 (any slot
-// gives a valid bound; the first slot holding the pixel's smallest cost code is the probe), a slot with C[d] > T is neither
-// the winner, nor a tie for it, nor any pass's arg-minimum (min L_p <= L_p[d0] <= T).  The pixel is read in two stages:
-// - pass 0: a lane requests its LPL slots only when one of them, or a neighbour of one (the sub-pixel fit reads S[k-1],
-//   S[k+1]), has C <= T;
-// - passes 1-7: S[d] >= L_0[d] too, so only where L_0[d] <= T, dilated in the same way, or where C[d] <= L_q[d0]: a pass-q
-//   arg-minimum d* has C[d*] <= L_q[d*] = min L_q <= L_q[d0], so every pass's consensus slot is read.  Lanes 0-7 hold L_q[d0]
-//   from the probe.  L_q >= C holds without rounding (L_q = fl(C + x), x >= 0), so that term needs no slack.
-// The other slots read +INF, which is what the sums, minima and comparisons of wta_finish make of a slot that cannot win.
-// Outputs are those of wta_kernel bit for bit.  Eight passes, blocked slots, no dense S and no PKR image (both read slots
-// that cannot win).
+// the aggregation is >= 0, so L_p[d] >= C[d] in every pass, S[d] >= C[d] and S[d] >= L_0[d].  With T = S[d0] of one probe
+// slot d0 (any slot gives a valid bound; the first slot holding the pixel's smallest cost code is the probe), a slot with
+// L_0[d] > T is neither the winner nor a tie for it.  Pass 0 is read whole.  Passes 1-7 are read only where L_0[d] <= T,
+// dilated by one slot (the sub-pixel fit reads S[k-1], S[k+1]), or where C[d] <= L_q[d0]: a pass-q arg-minimum d* has
+// C[d*] <= L_q[d*] = min L_q <= L_q[d0], so every pass's consensus slot is read.  Lanes 0-7 hold L_q[d0] from the probe.
+// L_q >= C holds without rounding (L_q = fl(C + x), x >= 0), so that term needs no slack.  The other slots of passes 1-7 read
+// +INF, which is what the sums, minima and comparisons of wta_finish make of a slot that cannot win.  Outputs are those of
+// wta_kernel bit for bit.  Eight passes, blocked slots, no dense S and no PKR image (both read slots that cannot win).
 //
-// The probe and pass 0 would each put one more round trip on a pixel's dependent chain (C -> L_p[d0] -> pass 0 -> passes
-// 1-7), so a warp works three pixels deep: pixel p+1's probe and pass 0 are requested while p's passes 1-7 are in flight, and
-// pixel p+2's codes and range one pixel ahead of its probe.  Passes 1-7 are requested together (one round trip; the pruned
-// lanes leave registers for all seven under the 64-register cap), so a pixel waits on one round trip, not two.
+// A pixel's dependent chain is codes -> probe -> passes 1-7.  Pass 0 is requested with the probe: masking it by C <= T would
+// wait on the probe, one more round trip per pixel, to skip about 37 % of its sectors.  A warp works three pixels deep:
+// pixel p+1's probe and whole pass 0 are requested before p's passes 1-7, and pixel p+2's codes and range one pixel ahead of
+// its probe.  Passes 1-7 are requested together (all seven fit in flight under the 64-register cap), so a pixel waits on one
+// round trip.
 template <int LPL> __device__ __forceinline__ unsigned wta_probe_key(const CostPack<LPL> &cp, int lane)
 {   // (smallest code << 9) | first slot holding it
     unsigned key = 0xffffffffu;
@@ -706,13 +704,6 @@ template <int LPL> __device__ __forceinline__ void wta_ld_pass_if(const float *p
     for (int e = 0; e < LPL; e++) v[e] = S2PB_INF;
     if (ld) wta_ld_pass<LPL>(px, lane, v);
 }
-template <int LPL> __device__ __forceinline__ bool wta_lane_reads_c(const WtaParams &P, const CostPack<LPL> &cp, int lane, float T)
-{
-    unsigned m = 0;
-#pragma unroll
-    for (int e = 0; e < LPL; e++) if (cost_value(cost_code(cp, e), P.lut) <= T) m |= 1u << e;
-    return wta_lane_reads<LPL>(m, lane, T);
-}
 __device__ __forceinline__ unsigned wta_range(const WtaParams &P, unsigned p)
 {
     return ((unsigned)(unsigned short)__ldg(P.lo + p)) | ((unsigned)(unsigned short)__ldg(P.hi + p) << 16);
@@ -735,17 +726,14 @@ __global__ void __launch_bounds__(kWtaThreads) __maxnreg__((LPL <= 4) ? 64 : 128
 #pragma unroll
     for (int q = 1; q < kMaxPasses; q++) if (lane == q) probe = P.L[q];
     const uint8_t *codes = reinterpret_cast<const uint8_t *>(P.C) + lane * LPL;
-    // pixel p: range, codes, probe values, bound, pass 0 requested; pixel p1: range and codes requested
+    // pixel p: range, codes, probe values and pass 0 requested; pixel p1: range and codes requested
     unsigned p = warp;
     unsigned range = wta_range(P, p);
     CostPack<LPL> cpk = ld_cost<LPL, true>(codes + (size_t)p * DP);
-    const unsigned key = wta_probe_key<LPL>(cpk, lane);
+    unsigned key = wta_probe_key<LPL>(cpk, lane);
     float pv = lane < kMaxPasses ? __ldcg(probe + (size_t)p * DP + (key & 511u)) : 0.f;
-    // the integer costs of census 5x5 make S >= C exact; the scaled costs of 3x3 / 7x7 round in the eight additions and the
-    // overcount fix, by less than 2^-18 of S in all, so the bound is taken 2^-16 wider
-    float T = wta_probe_sum(P, pv, key) * (1.f + 1.f / 65536.f);
     float v0[LPL];
-    wta_ld_pass_if<LPL>(P.L[0] + (size_t)p * DP, lane, wta_lane_reads_c<LPL>(P, cpk, lane, T), v0);
+    wta_ld_pass<LPL>(P.L[0] + (size_t)p * DP, lane, v0);
     unsigned p1 = p + nwarps;
     unsigned range1 = range;
     CostPack<LPL> cpk1 = cpk;
@@ -756,12 +744,16 @@ __global__ void __launch_bounds__(kWtaThreads) __maxnreg__((LPL <= 4) ? 64 : 128
         unsigned range2 = range1;
         CostPack<LPL> cpk2 = cpk1;
         unsigned key1 = 0;
-        float pv1 = 0.f;
+        float pv1 = 0.f, v01[LPL];
         if (more1) {
             if (p2 < npix) { range2 = wta_range(P, p2); cpk2 = ld_cost<LPL, true>(codes + (size_t)p2 * DP); }
             key1 = wta_probe_key<LPL>(cpk1, lane);
             if (lane < kMaxPasses) pv1 = __ldcg(probe + (size_t)p1 * DP + (key1 & 511u));
+            wta_ld_pass<LPL>(P.L[0] + (size_t)p1 * DP, lane, v01);
         }
+        // the integer costs of census 5x5 make S >= L_0 exact; the scaled costs of 3x3 / 7x7 round in the eight additions and the
+        // overcount fix, by less than 2^-18 of S in all, so the bound is taken 2^-16 wider
+        const float T = wta_probe_sum(P, pv, key) * (1.f + 1.f / 65536.f);
         float s[LPL];
         int am[kMaxPasses];
 #pragma unroll
@@ -782,11 +774,6 @@ __global__ void __launch_bounds__(kWtaThreads) __maxnreg__((LPL <= 4) ? 64 : 128
         float v[kMaxPasses - 1][LPL];
 #pragma unroll
         for (int q = 1; q < kMaxPasses; q++) wta_ld_pass_if<LPL>(P.L[q] + (size_t)p * DP, lane, ld || ((ldq >> q) & 1u), v[q - 1]);
-        float T1 = T;
-        if (more1) {
-            T1 = wta_probe_sum(P, pv1, key1) * (1.f + 1.f / 65536.f);
-            wta_ld_pass_if<LPL>(P.L[0] + (size_t)p1 * DP, lane, wta_lane_reads_c<LPL>(P, cpk1, lane, T1), v0);
-        }
 #pragma unroll
         for (int q = 1; q < kMaxPasses; q++) am[q] = wta_add_pass<LPL>(v[q - 1], lane, s);
         float c[LPL];
@@ -794,7 +781,9 @@ __global__ void __launch_bounds__(kWtaThreads) __maxnreg__((LPL <= 4) ? 64 : 128
         for (int e = 0; e < LPL; e++) c[e] = cost_value(cost_code(cpk, e), P.lut);
         wta_finish<LPL>(P, p, lane, s, am, c, sSrow, (short)(range & 0xffffu), (short)(range >> 16));
         if (!more1) break;
-        p = p1; p1 = p2; range = range1; range1 = range2; cpk = cpk1; cpk1 = cpk2; pv = pv1; T = T1;
+        p = p1; p1 = p2; range = range1; range1 = range2; cpk = cpk1; cpk1 = cpk2; key = key1; pv = pv1;
+#pragma unroll
+        for (int e = 0; e < LPL; e++) v0[e] = v01[e];
     }
 }
 

@@ -9,8 +9,9 @@ pixel's 128-slot pass vector hold a (dilated) survivor, and asserts on every pix
 survivors alone equal those from the full vector.  `check_claims` with pass volumes does the same for the eight pass arg-minima with pass
 volumes from a plain numpy restatement of the scan (small strips only: it is a per-pixel Python loop).
 
-The two-stage mask (`two_stage`) reads pass 0 under that mask and passes 1-7 only where L_0[d] <= S[d0] (dilated) or
-C[d] <= L_q[d0]; `--two-stage` counts it per pass with those pass volumes (slow: minutes per strip and view).
+The two-stage mask (`two_stage`) reads pass 0 whole and passes 1-7 only where L_0[d] <= S[d0] (dilated) or
+C[d] <= L_q[d0]; `--two-stage` counts it per pass with those pass volumes and gives the bytes the kernel requests (slow:
+minutes per strip and view).
 
     python scripts/wta_prune_model.py [--rows 300:396] [--seeds 0,1] [--size 1024] [--views LR] [--two-stage]
 """
@@ -109,14 +110,12 @@ def survivors(C, T):
 
 
 def two_stage(C, T, Ls):
-    """The slots each pass is read on by the two-stage WTA (wta_pruned_kernel) -> eight [h][w][D] masks.  Pass 0: the
-    dilated survivors of C.  Passes 1-7: {d : L_0[d] <= T} from what was read of pass 0, dilated (S >= L_0 like S >= C, same
+    """The slots each pass is read on by the two-stage WTA (wta_pruned_kernel) -> eight [h][w][D] masks.  Pass 0: every
+    slot (the kernel requests it with the probe).  Passes 1-7: {d : L_0[d] <= T}, dilated (S >= L_0 like S >= C, same
     slack), and {d : C[d] <= L_q[d0]} with d0 the probe slot (first arg-minimum of C): every arg-minimum of L_q lies there."""
-    _, d0 = survivors(C, T)
-    L0 = np.where(d0, Ls[0], INF)
-    d1 = dilate(L0 <= (T * np.float32(1 + 2.0 ** -16))[..., None])
+    d1 = dilate(Ls[0] <= (T * np.float32(1 + 2.0 ** -16))[..., None])
     k0 = np.argmin(C, axis=-1)[..., None]
-    return [d0] + [d1 | (C <= np.take_along_axis(L, k0, -1)) for L in Ls[1:]]
+    return [np.ones(C.shape, bool)] + [d1 | (C <= np.take_along_axis(L, k0, -1)) for L in Ls[1:]]
 
 
 def check_claims(C, S, dil, Ls=None):
@@ -182,6 +181,12 @@ def sector_fraction(d):
     return d.reshape(h, w, D // 8, 8).any(-1).mean()
 
 
+def requested_bytes(npix, DP, f):
+    """bytes wta_pruned_kernel requests for a view of npix pixels and DP slots: the 32-byte sectors of the eight passes
+    (fractions f), one probe sector per pass, the codes"""
+    return npix * (sum(f) * 4 * DP + 8 * 32 + DP)
+
+
 def two_stage_fractions(C, S):
     """-> (per-pass 32-byte sector fractions of the two-stage mask, that of the one-stage mask), probes not included; checks
     winner, fit and the eight arg-minima of the two-stage mask on every pixel"""
@@ -204,16 +209,18 @@ def main():
     a = ap.parse_args()
     rows = tuple(int(x) for x in a.rows.split(":"))
     if a.two_stage:
-        print("| tile | view | one stage, every pass | two stages: pass 0 | passes 1-7 | mean of 8 | mean + probes |")
-        print("|---|---|---|---|---|---|---|")
+        # GB: what the kernel requests for the whole size x size view at the strip's fractions
+        print("| tile | view | C <= T, every pass | pass 0 | passes 1-7 | mean of 8 | mean + probes | GB per view |")
+        print("|---|---|---|---|---|---|---|---|")
         for nanb in (0.0, 0.05):
             for seed in (int(s) for s in a.seeds.split(",")):
                 for view in a.views:
                     C, S = strip_volumes(seed, a.size, rows, -64, 63, nanb, view)
                     f, f1 = two_stage_fractions(C, S)
-                    print("| seed %d%s | %s | %.3f | %.3f | %.3f-%.3f | %.3f | %.3f |" % (
+                    print("| seed %d%s | %s | %.3f | %.3f | %.3f-%.3f | %.3f | %.3f | %.2f |" % (
                         seed, " nodata" if nanb else "", view, f1, f[0], min(f[1:]), max(f[1:]), np.mean(f),
-                        np.mean(f) + 1 / (C.shape[-1] // 8)), flush=True)
+                        np.mean(f) + 1 / (C.shape[-1] // 8), requested_bytes(a.size * a.size, C.shape[-1], f) / 1e9),
+                        flush=True)
         return
     # "unpruned pixels": S[d0] >= the largest finite C, recognisable before any mask work -- they read every sector
     print("| tile | view | probe | survivors | 16 B pieces | 32 B sectors | 64 B pairs | unpruned pixels | sectors + probes |")

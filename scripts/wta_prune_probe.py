@@ -46,8 +46,7 @@ def main():
             print("view %s: %d slots, not pruned" % (view, DP))
             continue
         f2, _ = M.two_stage_fractions(C, S)
-        # sectors asked for, one probe sector per pass, the codes
-        nbytes["default"] += npix * (sum(f2) * 4 * DP + 8 * 32 + DP)
+        nbytes["default"] += M.requested_bytes(npix, DP, f2)
         print("view %s: %d slots, sector fraction per pass %s (mean %.3f)" % (
             view, DP, " ".join("%.3f" % x for x in f2), np.mean(f2)))
     p = default_params("mgm")
