@@ -1,0 +1,242 @@
+// host.h -- host-side state and helpers shared by the translation units of the C ABI (not a public header).
+//
+// s2pb200.cu owns the context, the slots, the matcher and the matcher's stage entry points; warp.cu, geometry.cu, sgbm.cu and
+// raster.cu each hold one family of entry points.  Every kernel header that defines a non-template kernel is included by one of
+// those files only, so that its kernels are compiled once; the few launchers another file needs are declared at the end.
+#pragma once
+#include "../../include/s2pb200.h"
+#include "agg_kernel.cuh"          // kMaxPasses
+
+#include <cuda_runtime.h>
+#include <algorithm>
+#include <atomic>
+#include <chrono>
+#include <list>
+#include <mutex>
+#include <string>
+#include <utility>
+#include <vector>
+
+namespace s2pb { struct RtState; }
+using namespace s2pb;            // every file that includes this one launches the kernels of namespace s2pb
+
+// ------------------------------------------------------------------ context
+
+struct ViewWS {
+    float *img;            // NaN-free copy
+    float *rt;             // ... after the reference's DCT round trip (what the OTHER view's cost volume matches against)
+    uint64_t *census_rt;   // census (or NCC window statistics) of rt
+    int *rowlist;          // rows the round trip had to transform
+    float *rowthr;         // per row: pixels with |x| <= rowthr are recomputed (-1: none)
+    RtState *rtstate;
+    short *lo, *hi;        // per-pixel label range
+    uint64_t *census;
+    void *C;               // [H][W][DP] costs: u8 codes (census popcounts, agg_kernel.cuh) or float (general flavour)
+    float *L[kMaxPasses];
+    float *Lmin[kMaxPasses];
+    int *progress;         // [kMaxPasses][maxBands]
+    float *disp, *cost, *conf, *tmp;
+};
+struct Slot {
+    void *base = nullptr;
+    size_t bytes = 0;
+    int w = 0, h = 0, DP = 0, ndir = 0;
+    int cbytes = 1;               // bytes per stored cost: 1 = 8-bit census codes, 4 = float (general flavour)
+    ViewWS v[2];
+    int *next_item = nullptr;
+    float *lut = nullptr;
+    double *Ydct = nullptr;       // [H][W] DCT coefficients of the rows in flight (dct_kernels.cuh)
+    // staging for the host-buffer API
+    float *d_in[2] = {nullptr, nullptr};
+    float *d_w[2] = {nullptr, nullptr};           // -wl / -wr weight images of s2pb_mgm_weighted
+    float *d_disp = nullptr, *d_conf = nullptr, *d_dispR = nullptr;
+    uint8_t *d_mask = nullptr;
+    char *io_base = nullptr;
+    size_t io_pix = 0;
+    float *h_in[2] = {nullptr, nullptr};          // pinned
+    float *h_disp = nullptr, *h_conf = nullptr, *h_dispR = nullptr;
+    uint8_t *h_mask = nullptr;
+    size_t h_pix = 0;
+    // bump arena for the pyramid of mgm_multi (images, range images, per-level results)
+    char *arena = nullptr;
+    size_t arena_cap = 0, arena_off = 0;
+    int *d_small = nullptr;           // 64 words of device memory of this slot's own (hull accumulators of mgm_multi)
+    cudaStream_t stream = nullptr;
+    cudaStream_t stream2 = nullptr;   // the right view's aggregation when the two views' slabs differ in width (runs beside the left one)
+    cudaEvent_t fork = nullptr, join = nullptr;
+    cudaEvent_t ev[S2PB_T_COUNT + 1] = {};
+    cudaEvent_t done = nullptr;
+    bool timed = false;
+    bool direct_out = false;      // the last host-API call wrote its results straight into the caller's pinned buffers
+};
+struct s2pb_ctx {
+    int device = 0;
+    int sm_count = 132;
+    bool wta_prune = true;         // S2PB_WTA_PRUNE (read when the context is created): 0 wta_kernel for every shape, the
+                                   // same-device reference of wta_pruned_kernel (DESIGN.md 3.2); unset or any other value prunes
+    std::vector<Slot> slots;
+    int *abort_flag = nullptr;     // pinned + mapped: the host raises it on timeout
+    int *scratch_flag = nullptr;   // pinned + mapped: device -> host one-word answers
+    int *d_scratch = nullptr;      // 64 words of device memory (hull accumulators of mgm_multi)
+    std::atomic<long long> launches{0};   // (mgm_multi tiles of a batch are enqueued from several host threads)
+    // destination of the PKR images of s2pb_mgm_pkr (device, per view), or null: every mgm_call writes them, the last one stays
+    float *pkr_dst[2] = {nullptr, nullptr};
+    // deadline of the matcher call in flight (timeout_ms counted from the API entry; has_deadline = false: none)
+    std::chrono::steady_clock::time_point deadline;
+    bool has_deadline = false;
+    // DCT coefficient tables of the matched image's round trip, one entry per image width (dct_tables)
+    struct DctTab { int n; double *T10, *T01, *TR01, *mc, *ms; };
+    std::list<DctTab> dct;          // a list: entries stay put while other host threads hold pointers to them
+    std::mutex dct_mu;
+    // scratch pool of the host-buffer entry points: device buffers are kept between calls (a cudaMalloc / cudaFree pair per
+    // call costs more than the merge or the warp itself).  Borrowed through a ScratchLease only.  It has no lock, so nothing
+    // that s2pb_mgm_batch's worker threads run may take from it.
+    struct PoolBuf { void *p; size_t bytes; bool used; };
+    std::vector<PoolBuf> pool;
+};
+
+// nothing declared from here on is part of the library's exported interface
+#pragma GCC visibility push(hidden)
+
+// ------------------------------------------------------------------ errors
+
+extern thread_local std::string g_err;
+int fail(int code, const char *fmt, ...);
+#define CK(call)                                                                                     \
+    do {                                                                                             \
+        cudaError_t e_ = (call);                                                                     \
+        if (e_ != cudaSuccess)                                                                       \
+            return fail(S2PB_ERR_CUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e_), __FILE__, __LINE__); \
+    } while (0)
+
+// ------------------------------------------------------------------ scratch of the host-buffer entry points
+
+inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
+
+// smallest idle pooled buffer that is large enough, else a new allocation; when that fails the idle buffers are given back
+// to the device and the allocation is tried once more (nullptr when out of memory)
+inline void *pool_take(s2pb_ctx *ctx, size_t bytes)
+{
+    int best = -1;
+    for (int i = 0; i < (int)ctx->pool.size(); i++)
+        if (!ctx->pool[i].used && ctx->pool[i].bytes >= bytes && (best < 0 || ctx->pool[i].bytes < ctx->pool[best].bytes)) best = i;
+    if (best >= 0) { ctx->pool[best].used = true; return ctx->pool[best].p; }
+    void *p = nullptr;
+    size_t want = align_up(bytes ? bytes : 1, (size_t)1 << 20);
+    if (cudaMalloc(&p, want) != cudaSuccess) {
+        cudaGetLastError();
+        // an idle buffer is safe to free: the lease that held it waited for its stream before handing it back
+        std::vector<s2pb_ctx::PoolBuf> held;
+        for (auto &b : ctx->pool) if (b.used) held.push_back(b); else cudaFree(b.p);
+        ctx->pool.swap(held);
+        if (cudaMalloc(&p, want) != cudaSuccess) { cudaGetLastError(); return nullptr; }
+    }
+    ctx->pool.push_back({p, want, true});
+    return p;
+}
+
+// The device scratch of one host-buffer call, borrowed from the pool.  `st` is the stream the call runs on.  The destructor
+// waits for that stream, then hands back only the buffers this lease took, on every return path: after any return no kernel
+// or copy still touches the scratch or the caller's buffers, and leases nest.  Success paths still end in a checked
+// cudaStreamSynchronize of their own, which is where an asynchronous error is reported.
+class ScratchLease {
+public:
+    ScratchLease(s2pb_ctx *ctx, cudaStream_t st) : ctx_(ctx), st_(st) {}
+    ScratchLease(const ScratchLease &) = delete;
+    ScratchLease &operator=(const ScratchLease &) = delete;
+    ~ScratchLease()
+    {
+        cudaStreamSynchronize(st_);
+        for (auto &b : ctx_->pool)
+            if (std::find(taken_.begin(), taken_.end(), b.p) != taken_.end()) b.used = false;
+    }
+    // nullptr when the device is out of memory; the caller then returns nomem()
+    template <class T> T *take(size_t bytes)
+    {
+        void *p = pool_take(ctx_, bytes);
+        if (p) taken_.push_back(p);
+        else if (!failed_) failed_ = bytes ? bytes : 1;
+        return (T *)p;
+    }
+    int nomem(const char *what) const { return fail(S2PB_ERR_NOMEM, "cudaMalloc of %zu bytes failed for %s", failed_, what); }
+
+private:
+    s2pb_ctx *ctx_;
+    cudaStream_t st_;
+    std::vector<void *> taken_;
+    size_t failed_ = 0;       // size of the first request that failed
+};
+
+// The protocol of an entry point that works on host buffers: it runs on slot 0's stream of the context's device and borrows
+// its scratch through the lease it is.  take() and upload() (scratch holding a copy of a host buffer) keep the first failure
+// and do nothing after it; the caller returns error() if it is set before its first launch, downloads its results and returns
+// finish(), the checked synchronisation of the stream.
+class HostCall : public ScratchLease {
+public:
+    const cudaStream_t st;
+    // what: the call's scratch, as the message of a failed allocation names it
+    HostCall(s2pb_ctx *ctx, const char *what) : ScratchLease(ctx, ctx->slots[0].stream), st(ctx->slots[0].stream), what_(what)
+    {
+        keep(cudaSetDevice(ctx->device), "cudaSetDevice");
+    }
+    template <class T> T *take(size_t bytes)
+    {
+        T *p = rc_ != S2PB_OK ? nullptr : ScratchLease::take<T>(bytes);
+        if (!p && rc_ == S2PB_OK) rc_ = nomem(what_);
+        return p;
+    }
+    template <class T> T *upload(const T *src, size_t bytes)
+    {
+        T *p = take<T>(bytes);
+        if (p) keep(cudaMemcpyAsync(p, src, bytes, cudaMemcpyHostToDevice, st), "host-to-device copy");
+        return p;
+    }
+    void download(void *dst, const void *src, size_t bytes)
+    {
+        if (rc_ == S2PB_OK) keep(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, st), "device-to-host copy");
+    }
+    int error() const { return rc_; }
+    int finish()
+    {
+        if (rc_ != S2PB_OK) return rc_;
+        CK(cudaStreamSynchronize(st));
+        return S2PB_OK;
+    }
+
+private:
+    void keep(cudaError_t e, const char *what)
+    {
+        if (e != cudaSuccess && rc_ == S2PB_OK) rc_ = fail(S2PB_ERR_CUDA, "%s failed: %s", what, cudaGetErrorString(e));
+    }
+    const char *what_;
+    int rc_ = S2PB_OK;        // the first failure
+};
+
+// ------------------------------------------------------------------ launches
+
+// kernel k<<<grid, block, smem, st>>>(args...), counted in s2pb_kernel_launches
+template <class... P, class... A>
+inline void launch(s2pb_ctx *ctx, void (*k)(P...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, A &&...args)
+{
+    k<<<grid, block, smem, st>>>(std::forward<A>(args)...);
+    ctx->launches++;
+}
+
+inline dim3 grid2d(int w, int h, dim3 b) { return dim3((w + b.x - 1) / b.x, (h + b.y - 1) / b.y); }
+
+// ------------------------------------------------------------------ shared between the translation units
+
+// s2pb200.cu: remove_small_cc and the union-find passes it shares with the 3D filter and sgbm (multiscale_kernels.cuh), and
+// create_rejection_mask (mgm_kernels.cuh)
+int launch_remove_small_cc(s2pb_ctx *ctx, const float *in, float *out, int w, int h, int minarea, float thr, int *lab, int *area,
+                           cudaStream_t st);
+void cc_flatten(s2pb_ctx *ctx, int n, int *lab, cudaStream_t st);
+void cc_area(s2pb_ctx *ctx, int n, const int *lab, int *area, cudaStream_t st);
+void launch_rejection_mask(s2pb_ctx *ctx, const float *disp, const float *im1, const float *im2, int w, int h, uint8_t *mask,
+                           cudaStream_t st);
+// warp.cu
+void invert_homography(const double i[9], double o[9]);
+int warp_host_to_device(s2pb_ctx *ctx, ScratchLease &L, cudaStream_t st, const float *src, int sw, int sh, const double H[9],
+                        float *d_out, int dw, int dh);
+
+#pragma GCC visibility pop

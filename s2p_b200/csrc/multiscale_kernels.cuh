@@ -6,6 +6,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include "union_find.cuh"
 
 namespace s2pb {
 
@@ -111,21 +112,7 @@ __global__ void label_ranges_kernel(const float *__restrict__ dmin, const float 
 
 // ---- remove_small_cc (remove_small_cc.c:9-73): union-find over the 4-neighbour links the reference makes
 // (only from pixels with i < w-1 and j < h-1; |difference| < threshold; NaN never joins), then every
-// component with area <= minarea becomes NaN.  Any union-find yields the same partition.
-__device__ __forceinline__ int uf_find(const int *lab, int a)
-{   // read-only chase: parents only ever move towards smaller roots, so this terminates under concurrent unions
-    while (true) { int p = ((const volatile int *)lab)[a]; if (p == a) return a; a = p; }
-}
-__device__ __forceinline__ void uf_union(int *lab, int a, int b)
-{
-    while (true) {
-        a = uf_find(lab, a); b = uf_find(lab, b);
-        if (a == b) return;
-        if (a < b) { int t = a; a = b; b = t; }                            // a > b: hang the larger root below the smaller
-        int old = atomicCAS(lab + a, a, b);
-        if (old == a) return;
-    }
-}
+// component with area <= minarea becomes NaN.  Any union-find yields the same partition (uf_find / uf_union: union_find.cuh).
 __global__ void cc_init_kernel(const float *__restrict__ in, int n, int *__restrict__ lab, int *__restrict__ area)
 {
     int i = blockIdx.x * blockDim.x + threadIdx.x;

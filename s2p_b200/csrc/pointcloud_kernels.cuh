@@ -10,11 +10,12 @@
 // un-rejecting each rejected point that has a close, non-rejected point in its (2q+1)^2 window.  The distance is
 // symmetric bit for bit and un-rejecting only goes one way, so the sweeps end on an order-free set: a rejected point is
 // saved iff a chain of "close and within the q-window" links through rejected points joins it to a point that was never
-// rejected.  Here that is a connected-components pass over the rejected pixels (union-find of multiscale_kernels.cuh),
-// bounded work where the sweeps need as many passes as the longest chain against the scan order.
+// rejected.  Here that is a connected-components pass over the rejected pixels (union_find.cuh, flattened by
+// remove_small_cc's cc_flatten_kernel), bounded work where the sweeps need as many passes as the longest chain against the
+// scan order.
 #pragma once
 #include <cuda_runtime.h>
-#include "multiscale_kernels.cuh"
+#include "union_find.cuh"
 
 namespace s2pb {
 

@@ -1,46 +1,29 @@
-// s2pb200.cu -- context, workspace and the C ABI declared in include/s2pb200.h.
+// s2pb200.cu -- context, workspace, the matcher and its stage entry points of the C ABI declared in include/s2pb200.h.
 //
 // Host-side orchestration of the kernels in mgm_kernels.cuh.  The sequence of stages mirrors
 // what one `mgm` process does for one tile (main_mgm.cc:167-262 -> mgm_call,
 // mgm_multiscale.cc:161-335 in the reference) followed by create_rejection_mask
-// (s2p/block_matching.py:18-32).  There is no CPU fallback in this file.
-#include "../../include/s2pb200.h"
+// (s2p/block_matching.py:18-32).  There is no CPU fallback in this file.  The other entry points are in warp.cu,
+// geometry.cu, sgbm.cu and raster.cu; host.h holds what they share with this file.
+#include "host.h"
 #include "mgm_kernels.cuh"
 #include "multiscale_kernels.cuh"
 #include "dct_kernels.cuh"
-#include "homography_kernels.cuh"
-#include "fusion_kernels.cuh"
-#include "triangulation_kernels.cuh"
-#include "pointcloud_kernels.cuh"
-#include "heightmap_kernels.cuh"
-#include "sgbm_kernels.cuh"
-#include "dsm_kernels.cuh"
 #include "agg_dispatch.h"
 #include "agg_chunked.cuh"
 
-#include <cub/device/device_radix_sort.cuh>
-
-#include <algorithm>
-#include <atomic>
-#include <chrono>
-#include <list>
-#include <mutex>
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
 #include <cstdlib>
-#include <string>
 #include <thread>
 #include <type_traits>
-#include <vector>
-
-using namespace s2pb;
 
 // ------------------------------------------------------------------ errors
 
-static thread_local std::string g_err;
-static int fail(int code, const char *fmt, ...)
+thread_local std::string g_err;
+int fail(int code, const char *fmt, ...)
 {
     char buf[512];
     va_list ap;
@@ -50,143 +33,8 @@ static int fail(int code, const char *fmt, ...)
     g_err = buf;
     return code;
 }
-#define CK(call)                                                                                     \
-    do {                                                                                             \
-        cudaError_t e_ = (call);                                                                     \
-        if (e_ != cudaSuccess)                                                                       \
-            return fail(S2PB_ERR_CUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e_), __FILE__, __LINE__); \
-    } while (0)
 
 // ------------------------------------------------------------------ context
-
-struct ViewWS {
-    float *img;            // NaN-free copy
-    float *rt;             // ... after the reference's DCT round trip (what the OTHER view's cost volume matches against)
-    uint64_t *census_rt;   // census (or NCC window statistics) of rt
-    int *rowlist;          // rows the round trip had to transform
-    float *rowthr;         // per row: pixels with |x| <= rowthr are recomputed (-1: none)
-    RtState *rtstate;
-    short *lo, *hi;        // per-pixel label range
-    uint64_t *census;
-    void *C;               // [H][W][DP] costs: u8 codes (census popcounts, agg_kernel.cuh) or float (general flavour)
-    float *L[kMaxPasses];
-    float *Lmin[kMaxPasses];
-    int *progress;         // [kMaxPasses][maxBands]
-    float *disp, *cost, *conf, *tmp;
-};
-struct Slot {
-    void *base = nullptr;
-    size_t bytes = 0;
-    int w = 0, h = 0, DP = 0, ndir = 0;
-    int cbytes = 1;               // bytes per stored cost: 1 = 8-bit census codes, 4 = float (general flavour)
-    ViewWS v[2];
-    int *next_item = nullptr;
-    float *lut = nullptr;
-    double *Ydct = nullptr;       // [H][W] DCT coefficients of the rows in flight (dct_kernels.cuh)
-    // staging for the host-buffer API
-    float *d_in[2] = {nullptr, nullptr};
-    float *d_w[2] = {nullptr, nullptr};           // -wl / -wr weight images of s2pb_mgm_weighted
-    float *d_disp = nullptr, *d_conf = nullptr, *d_dispR = nullptr;
-    uint8_t *d_mask = nullptr;
-    char *io_base = nullptr;
-    size_t io_pix = 0;
-    float *h_in[2] = {nullptr, nullptr};          // pinned
-    float *h_disp = nullptr, *h_conf = nullptr, *h_dispR = nullptr;
-    uint8_t *h_mask = nullptr;
-    size_t h_pix = 0;
-    // bump arena for the pyramid of mgm_multi (images, range images, per-level results)
-    char *arena = nullptr;
-    size_t arena_cap = 0, arena_off = 0;
-    int *d_small = nullptr;           // 64 words of device memory of this slot's own (hull accumulators of mgm_multi)
-    cudaStream_t stream = nullptr;
-    cudaStream_t stream2 = nullptr;   // the right view's aggregation when the two views' slabs differ in width (runs beside the left one)
-    cudaEvent_t fork = nullptr, join = nullptr;
-    cudaEvent_t ev[S2PB_T_COUNT + 1] = {};
-    cudaEvent_t done = nullptr;
-    bool timed = false;
-    bool direct_out = false;      // the last host-API call wrote its results straight into the caller's pinned buffers
-};
-struct s2pb_ctx {
-    int device = 0;
-    int sm_count = 132;
-    bool wta_prune = true;         // S2PB_WTA_PRUNE (read when the context is created): 0 wta_kernel for every shape, the
-                                   // same-device reference of wta_pruned_kernel (DESIGN.md 3.2); unset or any other value prunes
-    std::vector<Slot> slots;
-    int *abort_flag = nullptr;     // pinned + mapped: the host raises it on timeout
-    int *scratch_flag = nullptr;   // pinned + mapped: device -> host one-word answers
-    int *d_scratch = nullptr;      // 64 words of device memory (hull accumulators of mgm_multi)
-    std::atomic<long long> launches{0};   // (mgm_multi tiles of a batch are enqueued from several host threads)
-    // destination of the PKR images of s2pb_mgm_pkr (device, per view), or null: every mgm_call writes them, the last one stays
-    float *pkr_dst[2] = {nullptr, nullptr};
-    // deadline of the matcher call in flight (timeout_ms counted from the API entry; has_deadline = false: none)
-    std::chrono::steady_clock::time_point deadline;
-    bool has_deadline = false;
-    // DCT coefficient tables of the matched image's round trip, one entry per image width (dct_tables)
-    struct DctTab { int n; double *T10, *T01, *TR01, *mc, *ms; };
-    std::list<DctTab> dct;          // a list: entries stay put while other host threads hold pointers to them
-    std::mutex dct_mu;
-    // scratch pool of the host-buffer entry points: device buffers are kept between calls (a cudaMalloc / cudaFree pair per
-    // call costs more than the merge or the warp itself).  Borrowed through a ScratchLease only.  It has no lock, so nothing
-    // that s2pb_mgm_batch's worker threads run may take from it.
-    struct PoolBuf { void *p; size_t bytes; bool used; };
-    std::vector<PoolBuf> pool;
-};
-
-static size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
-
-// smallest idle pooled buffer that is large enough, else a new allocation; when that fails the idle buffers are given back
-// to the device and the allocation is tried once more (nullptr when out of memory)
-static void *pool_take(s2pb_ctx *ctx, size_t bytes)
-{
-    int best = -1;
-    for (int i = 0; i < (int)ctx->pool.size(); i++)
-        if (!ctx->pool[i].used && ctx->pool[i].bytes >= bytes && (best < 0 || ctx->pool[i].bytes < ctx->pool[best].bytes)) best = i;
-    if (best >= 0) { ctx->pool[best].used = true; return ctx->pool[best].p; }
-    void *p = nullptr;
-    size_t want = align_up(bytes ? bytes : 1, (size_t)1 << 20);
-    if (cudaMalloc(&p, want) != cudaSuccess) {
-        cudaGetLastError();
-        // an idle buffer is safe to free: the lease that held it waited for its stream before handing it back
-        std::vector<s2pb_ctx::PoolBuf> held;
-        for (auto &b : ctx->pool) if (b.used) held.push_back(b); else cudaFree(b.p);
-        ctx->pool.swap(held);
-        if (cudaMalloc(&p, want) != cudaSuccess) { cudaGetLastError(); return nullptr; }
-    }
-    ctx->pool.push_back({p, want, true});
-    return p;
-}
-
-// The device scratch of one host-buffer call, borrowed from the pool.  `st` is the stream the call runs on.  The destructor
-// waits for that stream, then hands back only the buffers this lease took, on every return path: after any return no kernel
-// or copy still touches the scratch or the caller's buffers, and leases nest.  Success paths still end in a checked
-// cudaStreamSynchronize of their own, which is where an asynchronous error is reported.
-class ScratchLease {
-public:
-    ScratchLease(s2pb_ctx *ctx, cudaStream_t st) : ctx_(ctx), st_(st) {}
-    ScratchLease(const ScratchLease &) = delete;
-    ScratchLease &operator=(const ScratchLease &) = delete;
-    ~ScratchLease()
-    {
-        cudaStreamSynchronize(st_);
-        for (auto &b : ctx_->pool)
-            if (std::find(taken_.begin(), taken_.end(), b.p) != taken_.end()) b.used = false;
-    }
-    // nullptr when the device is out of memory; the caller then returns nomem()
-    template <class T> T *take(size_t bytes)
-    {
-        void *p = pool_take(ctx_, bytes);
-        if (p) taken_.push_back(p);
-        else if (!failed_) failed_ = bytes ? bytes : 1;
-        return (T *)p;
-    }
-    int nomem(const char *what) const { return fail(S2PB_ERR_NOMEM, "cudaMalloc of %zu bytes failed for %s", failed_, what); }
-
-private:
-    s2pb_ctx *ctx_;
-    cudaStream_t st_;
-    std::vector<void *> taken_;
-    size_t failed_ = 0;       // size of the first request that failed
-};
 
 // stride of the per-pass progress counters: bands hold kNW scanlines in the register-resident kernel, but as few as 2 in the
 // chunk-skipping kernel on float-cost slabs wider than 1024 slots (agg_chunked.cuh, ck_warps)
@@ -458,8 +306,6 @@ static bool other_aggregation_pending(s2pb_ctx *ctx, const Slot &me)
 
 // ------------------------------------------------------------------ stage launchers
 
-static dim3 grid2d(int w, int h, dim3 b) { return dim3((w + b.x - 1) / b.x, (h + b.y - 1) / b.y); }
-
 static int check_params(const s2pb_mgm_params *p, int w, int h, int dmin, int dmax)
 {
     if (!p) return fail(S2PB_ERR_ARG, "null params");
@@ -601,15 +447,16 @@ template <class F> static int with_lpl(int LPL, F &&f)
 
 // census 3x3 / 5x5 up to 8 labels per lane: the strip-staged kernel; 7x7, the half-pixel pass and 12 / 16 labels per lane: the
 // per-pixel one
-template <int LPL> static void launch_cost_t(const uint64_t *cu, const uint64_t *cv, const uint64_t *cv1, int zoom, bool narrow, int w, int h,
-                                             const short *lo, const short *hi, int gmin, uint8_t *C, int sm, cudaStream_t st)
+template <int LPL> static void launch_cost_t(s2pb_ctx *ctx, const uint64_t *cu, const uint64_t *cv, const uint64_t *cv1, int zoom, bool narrow,
+                                             int w, int h, const short *lo, const short *hi, int gmin, uint8_t *C, cudaStream_t st)
 {
+    const int sm = ctx->sm_count;
     if (zoom == 2) {
-        if (narrow) cost_kernel<LPL, true, true><<<sm * 8, 256, 0, st>>>(cu, cv, cv1, w, h, lo, hi, gmin, C);
-        else cost_kernel<LPL, true, false><<<sm * 8, 256, 0, st>>>(cu, cv, cv1, w, h, lo, hi, gmin, C);
-    } else if (!narrow) cost_kernel<LPL, false, false><<<sm * 8, 256, 0, st>>>(cu, cv, cv1, w, h, lo, hi, gmin, C);
-    else if constexpr (LPL <= 8) cost_strip_kernel<LPL><<<sm * 16, kCostStripThreads, 0, st>>>(cu, cv, w, h, lo, hi, gmin, C);
-    else cost_kernel<LPL, false, true><<<sm * 8, 256, 0, st>>>(cu, cv, cv1, w, h, lo, hi, gmin, C);
+        if (narrow) launch(ctx, cost_kernel<LPL, true, true>, sm * 8, 256, 0, st, cu, cv, cv1, w, h, lo, hi, gmin, C);
+        else launch(ctx, cost_kernel<LPL, true, false>, sm * 8, 256, 0, st, cu, cv, cv1, w, h, lo, hi, gmin, C);
+    } else if (!narrow) launch(ctx, cost_kernel<LPL, false, false>, sm * 8, 256, 0, st, cu, cv, cv1, w, h, lo, hi, gmin, C);
+    else if constexpr (LPL <= 8) launch(ctx, cost_strip_kernel<LPL>, sm * 16, kCostStripThreads, 0, st, cu, cv, w, h, lo, hi, gmin, C);
+    else launch(ctx, cost_kernel<LPL, false, true>, sm * 8, 256, 0, st, cu, cv, cv1, w, h, lo, hi, gmin, C);
 }
 
 // The cost volume of one view into G.C.  general: float costs of G.cost (census through G.lut included); else the 8-bit census
@@ -621,29 +468,29 @@ static int launch_cost(s2pb_ctx *ctx, int LPL, bool general, const CostGenParams
     uint8_t *C8 = (uint8_t *)G.C;
     int rc = S2PB_OK;
     if (wide_slab(LPL)) {
-        if (general) cost_gen_chunked_kernel<<<sm * 8, 256, 0, st>>>(G, 32 * LPL);
-        else if (G.zoom == 2) cost_chunked_kernel<true><<<sm * 8, 256, 0, st>>>(G.cu, G.cv0, G.cv1, G.w, G.h, G.lo, G.hi, G.gmin, 32 * LPL, C8);
-        else cost_chunked_kernel<false><<<sm * 8, 256, 0, st>>>(G.cu, G.cv0, nullptr, G.w, G.h, G.lo, G.hi, G.gmin, 32 * LPL, C8);
+        if (general) launch(ctx, cost_gen_chunked_kernel, sm * 8, 256, 0, st, G, 32 * LPL);
+        else if (G.zoom == 2) launch(ctx, cost_chunked_kernel<true>, sm * 8, 256, 0, st, G.cu, G.cv0, G.cv1, G.w, G.h, G.lo, G.hi, G.gmin, 32 * LPL, C8);
+        else launch(ctx, cost_chunked_kernel<false>, sm * 8, 256, 0, st, G.cu, G.cv0, nullptr, G.w, G.h, G.lo, G.hi, G.gmin, 32 * LPL, C8);
     } else if (general) {
-        rc = with_lpl(LPL, [&](auto k) { constexpr int K = decltype(k)::value; cost_gen_kernel<K><<<sm * 8, 256, 0, st>>>(G); });
+        rc = with_lpl(LPL, [&](auto k) { constexpr int K = decltype(k)::value; launch(ctx, cost_gen_kernel<K>, sm * 8, 256, 0, st, G); });
     } else {
         rc = with_lpl(LPL, [&](auto k) {
             constexpr int K = decltype(k)::value;
-            launch_cost_t<K>(G.cu, G.cv0, G.cv1, G.zoom, G.win <= 5, G.w, G.h, G.lo, G.hi, G.gmin, C8, sm, st);
+            launch_cost_t<K>(ctx, G.cu, G.cv0, G.cv1, G.zoom, G.win <= 5, G.w, G.h, G.lo, G.hi, G.gmin, C8, st);
         });
     }
     if (rc != S2PB_OK) return rc;
     CK(cudaGetLastError());
-    ctx->launches++;
     return S2PB_OK;
 }
 
-template <int LPL> static void launch_wta_t(const WtaParams &P, int sm, cudaStream_t st, bool general, bool pruned)
+template <int LPL> static void launch_wta_t(s2pb_ctx *ctx, const WtaParams &P, cudaStream_t st, bool general, bool pruned)
 {
+    const int sm = ctx->sm_count;
     if constexpr (wta_pruned_width(LPL))
-        if (pruned) { wta_pruned_kernel<LPL><<<sm * 16, kWtaThreads, 0, st>>>(P); return; }
-    if (general) wta_kernel<LPL, true><<<sm * 16, kWtaThreads, 0, st>>>(P);
-    else wta_kernel<LPL, false><<<sm * 16, kWtaThreads, 0, st>>>(P);
+        if (pruned) { launch(ctx, wta_pruned_kernel<LPL>, sm * 16, kWtaThreads, 0, st, P); return; }
+    if (general) launch(ctx, wta_kernel<LPL, true>, sm * 16, kWtaThreads, 0, st, P);
+    else launch(ctx, wta_kernel<LPL, false>, sm * 16, kWtaThreads, 0, st, P);
 }
 // The WTA of one view.  A wide slab without a dense S: wta_chunked_kernel.  The census flavour's eight-pass WTA without a dense
 // S or PKR output, on the widths wta_pruned_kernel serves: that kernel, which reads only the labels that can still win, unless
@@ -655,16 +502,15 @@ static int launch_wta(s2pb_ctx *ctx, int LPL, const WtaParams &P, cudaStream_t s
     if (P.S == nullptr && wide_slab(LPL)) {
         const int DP = 32 * LPL;
         const size_t smem = (size_t)(kWtaThreads / 32) * DP * sizeof(float);
-        if (general) wta_chunked_kernel<true><<<sm * 16, kWtaThreads, smem, st>>>(P, DP);
-        else wta_chunked_kernel<false><<<sm * 16, kWtaThreads, smem, st>>>(P, DP);
+        if (general) launch(ctx, wta_chunked_kernel<true>, sm * 16, kWtaThreads, smem, st, P, DP);
+        else launch(ctx, wta_chunked_kernel<false>, sm * 16, kWtaThreads, smem, st, P, DP);
     } else {
         const bool pruned = ctx->wta_prune && !general && P.ndir == kMaxPasses && P.S == nullptr && P.pkr == nullptr &&
                             wta_pruned_width(LPL);
-        rc = with_lpl(LPL, [&](auto k) { constexpr int K = decltype(k)::value; launch_wta_t<K>(P, sm, st, general, pruned); });
+        rc = with_lpl(LPL, [&](auto k) { constexpr int K = decltype(k)::value; launch_wta_t<K>(ctx, P, st, general, pruned); });
     }
     if (rc != S2PB_OK) return rc;
     CK(cudaGetLastError());
-    ctx->launches++;
     return S2PB_OK;
 }
 
@@ -746,11 +592,10 @@ static int round_trip_zero(s2pb_ctx *ctx, const float *img, int w, int h, float 
     if (rc != S2PB_OK) return rc;
     CK(cudaMemsetAsync(state, 0, sizeof(RtState), st));
     CK(cudaMemsetAsync(colflag, 0, (size_t)w, st));
-    rt_flag_kernel<<<h, 256, 0, st>>>(img, w, h, rt, state, rowlist, rowthr, colflag);
-    rt_collist_kernel<<<1, 1024, 0, st>>>(colflag, w, state, collist);
-    dct_gemm_kernel<float, true><<<ctx->sm_count * 4, kGemmThreads, 0, st>>>(t->T10, img, w, h, state, rowlist, Y, nullptr, nullptr, nullptr);
-    rt_inverse_gemm_kernel<<<ctx->sm_count * 4, kGemmThreads, 0, st>>>(t->T01, Y, w, state, rowlist, collist, rowthr, img, rt);
-    ctx->launches += 4;
+    launch(ctx, rt_flag_kernel, h, 256, 0, st, img, w, h, rt, state, rowlist, rowthr, colflag);
+    launch(ctx, rt_collist_kernel, 1, 1024, 0, st, colflag, w, state, collist);
+    launch(ctx, dct_gemm_kernel<float, true>, ctx->sm_count * 4, kGemmThreads, 0, st, t->T10, img, w, h, state, rowlist, Y, nullptr, nullptr, nullptr);
+    launch(ctx, rt_inverse_gemm_kernel, ctx->sm_count * 4, kGemmThreads, 0, st, t->T01, Y, w, state, rowlist, collist, rowthr, img, rt);
     CK(cudaGetLastError());
     return S2PB_OK;
 }
@@ -764,11 +609,10 @@ static int shift_half(s2pb_ctx *ctx, const float *img, int w, int h, float *out,
     const size_t npix = (size_t)w * h;
     double *ck = scratch, *sk = scratch + npix, *sym = scratch + 2 * npix, *anti = scratch + 3 * npix;
     const int g = ctx->sm_count * 4;
-    dct_gemm_kernel<float, true><<<g, kGemmThreads, 0, st>>>(t->T10, img, w, h, nullptr, nullptr, ck, t->mc, t->ms, sk);
-    dct_gemm_kernel<double, false><<<g, kGemmThreads, 0, st>>>(t->T01, ck, w, h, nullptr, nullptr, sym, nullptr, nullptr, nullptr);
-    dct_gemm_kernel<double, false><<<g, kGemmThreads, 0, st>>>(t->TR01, sk, w, h, nullptr, nullptr, anti, nullptr, nullptr, nullptr);
-    dct_combine_kernel<<<(unsigned)((npix + 255) / 256), 256, 0, st>>>(sym, anti, npix, out);
-    ctx->launches += 4;
+    launch(ctx, dct_gemm_kernel<float, true>, g, kGemmThreads, 0, st, t->T10, img, w, h, nullptr, nullptr, ck, t->mc, t->ms, sk);
+    launch(ctx, dct_gemm_kernel<double, false>, g, kGemmThreads, 0, st, t->T01, ck, w, h, nullptr, nullptr, sym, nullptr, nullptr, nullptr);
+    launch(ctx, dct_gemm_kernel<double, false>, g, kGemmThreads, 0, st, t->TR01, sk, w, h, nullptr, nullptr, anti, nullptr, nullptr, nullptr);
+    launch(ctx, dct_combine_kernel, (unsigned)((npix + 255) / 256), 256, 0, st, sym, anti, npix, out);
     CK(cudaGetLastError());
     return S2PB_OK;
 }
@@ -816,20 +660,28 @@ static GaussTaps gauss_taps(float sigma)
 }
 
 // remove_small_cc on a device image (in -> out), scratch: two int images; thr: the intensity threshold of a link
-static int launch_remove_small_cc(s2pb_ctx *ctx, const float *in, float *out, int w, int h, int minarea, float thr, int *lab, int *area,
-                                  cudaStream_t st)
+int launch_remove_small_cc(s2pb_ctx *ctx, const float *in, float *out, int w, int h, int minarea, float thr, int *lab, int *area,
+                           cudaStream_t st)
 {
     int n = w * h;
     dim3 b2(32, 8);
-    cc_init_kernel<<<(n + 255) / 256, 256, 0, st>>>(in, n, lab, area);
-    cc_rows_kernel<<<(h + 3) / 4, 128, 0, st>>>(in, w, h, thr, lab);                 // one warp per row
-    cc_link_kernel<<<grid2d(w, h, b2), b2, 0, st>>>(in, w, h, thr, lab);
-    cc_flatten_kernel<<<(n + 255) / 256, 256, 0, st>>>(n, lab);
-    cc_area_kernel<<<(n + 255) / 256, 256, 0, st>>>(n, lab, area);
-    cc_filter_kernel<<<(n + 255) / 256, 256, 0, st>>>(in, n, lab, area, minarea, out);
-    ctx->launches += 6;
+    launch(ctx, cc_init_kernel, (n + 255) / 256, 256, 0, st, in, n, lab, area);
+    launch(ctx, cc_rows_kernel, (h + 3) / 4, 128, 0, st, in, w, h, thr, lab);                 // one warp per row
+    launch(ctx, cc_link_kernel, grid2d(w, h, b2), b2, 0, st, in, w, h, thr, lab);
+    launch(ctx, cc_flatten_kernel, (n + 255) / 256, 256, 0, st, n, lab);
+    launch(ctx, cc_area_kernel, (n + 255) / 256, 256, 0, st, n, lab, area);
+    launch(ctx, cc_filter_kernel, (n + 255) / 256, 256, 0, st, in, n, lab, area, minarea, out);
     CK(cudaGetLastError());
     return S2PB_OK;
+}
+// its union-find passes over n labels, for the 3D filter and sgbm
+void cc_flatten(s2pb_ctx *ctx, int n, int *lab, cudaStream_t st)
+{
+    launch(ctx, cc_flatten_kernel, (unsigned)(((size_t)n + 255) / 256), 256, 0, st, n, lab);
+}
+void cc_area(s2pb_ctx *ctx, int n, const int *lab, int *area, cudaStream_t st)
+{
+    launch(ctx, cc_area_kernel, (unsigned)(((size_t)n + 255) / 256), 256, 0, st, n, lab, area);
 }
 
 // S2PB_TRACE=1: synchronise and report after every stage of mgm_call; 2: report only (debugging aid)
@@ -871,14 +723,10 @@ static int mgm_call(s2pb_ctx *ctx, Slot &s, int w, int h, const float *const img
         // v.rt = shift(img[vi], 0): the reference's DCT round trip (mgm_costvolume.cc:50-60)
         rc = round_trip_zero(ctx, img[vi], w, h, v.rt, v.rtstate, v.rowlist, v.rowthr, s.Ydct, st);
         if (rc != S2PB_OK) return rc;
-        if (census) {
-            census_pair_kernel<<<grid2d(w, h, b2), b2, 0, st>>>(img[vi], v.rt, v.rtstate, w, h, p->census_win / 2, v.census, v.census_rt);
-            ctx->launches++;
-        }
+        if (census) launch(ctx, census_pair_kernel, grid2d(w, h, b2), b2, 0, st, img[vi], v.rt, v.rtstate, w, h, p->census_win / 2, v.census, v.census_rt);
         if (ncc) {     // window statistics in the (then unused) census buffers: 8 B / pixel
-            ncc_stats_kernel<<<grid2d(w, h, b2), b2, 0, st>>>(img[vi], w, h, p->census_win / 2, (float2 *)v.census);
-            ncc_stats_kernel<<<grid2d(w, h, b2), b2, 0, st>>>(v.rt, w, h, p->census_win / 2, (float2 *)v.census_rt);
-            ctx->launches += 2;
+            launch(ctx, ncc_stats_kernel, grid2d(w, h, b2), b2, 0, st, img[vi], w, h, p->census_win / 2, (float2 *)v.census);
+            launch(ctx, ncc_stats_kernel, grid2d(w, h, b2), b2, 0, st, v.rt, w, h, p->census_win / 2, (float2 *)v.census_rt);
         }
     }
     // ZOOMFACTOR 2: shf[vi] = shift(img[vi], 1/2) (kept for the image-domain distances) and its census, in the pyramid arena
@@ -891,8 +739,8 @@ static int mgm_call(s2pb_ctx *ctx, Slot &s, int w, int h, const float *const img
         for (int vi = 0; vi < 2; vi++) {
             rc = shift_half(ctx, img[vi], w, h, shf[vi], scratch, st);
             if (rc != S2PB_OK) return rc;
-            if (census) { census_kernel<<<grid2d(w, h, b2), b2, 0, st>>>(shf[vi], w, h, p->census_win / 2, cen_half[vi]); ctx->launches++; }
-            if (ncc) { ncc_stats_kernel<<<grid2d(w, h, b2), b2, 0, st>>>(shf[vi], w, h, p->census_win / 2, (float2 *)cen_half[vi]); ctx->launches++; }
+            if (census) launch(ctx, census_kernel, grid2d(w, h, b2), b2, 0, st, shf[vi], w, h, p->census_win / 2, cen_half[vi]);
+            if (ncc) launch(ctx, ncc_stats_kernel, grid2d(w, h, b2), b2, 0, st, shf[vi], w, h, p->census_win / 2, (float2 *)cen_half[vi]);
         }
     }
     CK(cudaGetLastError());
@@ -950,21 +798,18 @@ static int mgm_call(s2pb_ctx *ctx, Slot &s, int w, int h, const float *const img
     // ---- post filters (mgm_multiscale.cc:310-334)
     float *dl = s.v[0].disp, *dr = s.v[1].disp, *xl = s.v[0].tmp, *xr = s.v[1].tmp;
     if (p->median > 0) {
-        median_kernel<<<grid2d(w, h, b2), b2, 0, st>>>(dl, xl, w, h, p->median);
-        median_kernel<<<grid2d(w, h, b2), b2, 0, st>>>(dr, xr, w, h, p->median);
-        ctx->launches += 2;
+        launch(ctx, median_kernel, grid2d(w, h, b2), b2, 0, st, dl, xl, w, h, p->median);
+        launch(ctx, median_kernel, grid2d(w, h, b2), b2, 0, st, dr, xr, w, h, p->median);
         float *t = dl; dl = xl; xl = t; t = dr; dr = xr; xr = t;
     }
     if (p->mindiff >= 0) {      // mgm_multiscale.cc:318-319: only the left map, against the right view's cost image
-        mindiff_kernel<<<grid2d(w, h, b2), b2, 0, st>>>(dl, s.v[1].cost, xl, w, h, p->census_win, p->mindiff);
-        ctx->launches++;
+        launch(ctx, mindiff_kernel, grid2d(w, h, b2), b2, 0, st, dl, s.v[1].cost, xl, w, h, p->census_win, p->mindiff);
         float *t = dl; dl = xl; xl = t;
     }
     if (!outR) outR = xr;
     if (p->lr_mode == 1) {
-        lrcheck_kernel<<<grid2d(w, h, b2), b2, 0, st>>>(dr, dl, outR, w, h, p->lr_tau);
-        lrcheck_kernel<<<grid2d(w, h, b2), b2, 0, st>>>(dl, dr, outL, w, h, p->lr_tau);
-        ctx->launches += 2;
+        launch(ctx, lrcheck_kernel, grid2d(w, h, b2), b2, 0, st, dr, dl, outR, w, h, p->lr_tau);
+        launch(ctx, lrcheck_kernel, grid2d(w, h, b2), b2, 0, st, dl, dr, outL, w, h, p->lr_tau);
     } else {
         CK(cudaMemcpyAsync(outL, dl, npix * 4, cudaMemcpyDeviceToDevice, st));
         CK(cudaMemcpyAsync(outR, dr, npix * 4, cudaMemcpyDeviceToDevice, st));
@@ -992,9 +837,8 @@ static int mgm_call_level(s2pb_ctx *ctx, Slot &s, Level &L, int zoom, const s2pb
     int *d_hull = s.d_small;
     const int hull_init[4] = {0x7fffffff, (int)0x80000000, 0x7fffffff, (int)0x80000000};
     CK(cudaMemcpyAsync(d_hull, hull_init, sizeof hull_init, cudaMemcpyHostToDevice, st));
-    label_ranges_kernel<<<(n + 255) / 256, 256, 0, st>>>(L.dminL, L.dmaxL, n, (float)zoom, lo[0], hi[0], d_hull);
-    label_ranges_kernel<<<(n + 255) / 256, 256, 0, st>>>(L.dminR, L.dmaxR, n, (float)zoom, lo[1], hi[1], d_hull + 2);
-    ctx->launches += 2;
+    launch(ctx, label_ranges_kernel, (n + 255) / 256, 256, 0, st, L.dminL, L.dmaxL, n, (float)zoom, lo[0], hi[0], d_hull);
+    launch(ctx, label_ranges_kernel, (n + 255) / 256, 256, 0, st, L.dminR, L.dmaxR, n, (float)zoom, lo[1], hi[1], d_hull + 2);
     CK(cudaGetLastError());
     int hull[4];
     CK(cudaMemcpyAsync(hull, d_hull, sizeof hull, cudaMemcpyDeviceToHost, st));
@@ -1071,25 +915,22 @@ static int mgm_multi_enqueue(s2pb_ctx *ctx, Slot &s, const float *d_im1, const f
     }
     s.timed = false;
     // level 0: NaN -> 0, initial bounds (main_mgm_multi.cc:160-196; the sentinel for no-data is dmin in both views)
-    init_ranges_kernel<<<(n + 255) / 256, 256, 0, st>>>(d_im1, n, (float)dmin, (float)dmax, (float)dmin, lv[0].u, lv[0].dminL, lv[0].dmaxL);
-    init_ranges_kernel<<<(n + 255) / 256, 256, 0, st>>>(d_im2, n, (float)-dmax, (float)-dmin, (float)dmin, lv[0].v, lv[0].dminR, lv[0].dmaxR);
-    ctx->launches += 2;
+    launch(ctx, init_ranges_kernel, (n + 255) / 256, 256, 0, st, d_im1, n, (float)dmin, (float)dmax, (float)dmin, lv[0].u, lv[0].dminL, lv[0].dmaxL);
+    launch(ctx, init_ranges_kernel, (n + 255) / 256, 256, 0, st, d_im2, n, (float)-dmax, (float)-dmin, (float)dmin, lv[0].v, lv[0].dminR, lv[0].dmaxR);
     const GaussTaps T = gauss_taps(0.8f);
     for (size_t l = 0; l + 1 < lv.size(); l++) {
         Level &a = lv[l], &b = lv[l + 1];
         dim3 g = grid2d(b.w, b.h, b2);
-        downsample2x_kernel<<<g, b2, 0, st>>>(a.u, a.w, a.h, T, b.u, b.w, b.h);
-        downsample2x_kernel<<<g, b2, 0, st>>>(a.v, a.w, a.h, T, b.v, b.w, b.h);
+        launch(ctx, downsample2x_kernel, g, b2, 0, st, a.u, a.w, a.h, T, b.u, b.w, b.h);
+        launch(ctx, downsample2x_kernel, g, b2, 0, st, a.v, a.w, a.h, T, b.v, b.w, b.h);
         if (weighted) {                        // the weight maps follow the pyramid, mgm_multiscale.cc:375-378
-            downsample2x_kernel<<<g, b2, 0, st>>>(a.wl, a.w, a.h, T, b.wl, b.w, b.h);
-            downsample2x_kernel<<<g, b2, 0, st>>>(a.wr, a.w, a.h, T, b.wr, b.w, b.h);
-            ctx->launches += 2;
+            launch(ctx, downsample2x_kernel, g, b2, 0, st, a.wl, a.w, a.h, T, b.wl, b.w, b.h);
+            launch(ctx, downsample2x_kernel, g, b2, 0, st, a.wr, a.w, a.h, T, b.wr, b.w, b.h);
         }
-        downsample2x_disp_kernel<<<g, b2, 0, st>>>(a.dminL, a.w, a.h, 0, b.dminL, b.w, b.h);
-        downsample2x_disp_kernel<<<g, b2, 0, st>>>(a.dmaxL, a.w, a.h, 1, b.dmaxL, b.w, b.h);
-        downsample2x_disp_kernel<<<g, b2, 0, st>>>(a.dminR, a.w, a.h, 0, b.dminR, b.w, b.h);
-        downsample2x_disp_kernel<<<g, b2, 0, st>>>(a.dmaxR, a.w, a.h, 1, b.dmaxR, b.w, b.h);
-        ctx->launches += 6;
+        launch(ctx, downsample2x_disp_kernel, g, b2, 0, st, a.dminL, a.w, a.h, 0, b.dminL, b.w, b.h);
+        launch(ctx, downsample2x_disp_kernel, g, b2, 0, st, a.dmaxL, a.w, a.h, 1, b.dmaxL, b.w, b.h);
+        launch(ctx, downsample2x_disp_kernel, g, b2, 0, st, a.dminR, a.w, a.h, 0, b.dminR, b.w, b.h);
+        launch(ctx, downsample2x_disp_kernel, g, b2, 0, st, a.dmaxR, a.w, a.h, 1, b.dmaxR, b.w, b.h);
     }
     CK(cudaGetLastError());
     const size_t arena_mark = s.arena_off;
@@ -1103,11 +944,10 @@ static int mgm_multi_enqueue(s2pb_ctx *ctx, Slot &s, const float *d_im1, const f
             const float *disp2[2] = {c.dl, c.dr};
             float *fmin[2] = {L.dminL, L.dminR}, *fmax[2] = {L.dmaxL, L.dmaxR};
             for (int vi = 0; vi < 2; vi++) {
-                update_ranges_kernel<<<grid2d(c.w, c.h, b2), b2, 0, st>>>(disp2[vi], 2.f, c.w, c.h, nullptr, nullptr, fmin[vi], fmax[vi],
+                launch(ctx, update_ranges_kernel, grid2d(c.w, c.h, b2), b2, 0, st, disp2[vi], 2.f, c.w, c.h, nullptr, nullptr, fmin[vi], fmax[vi],
                                                                        L.w, L.h, 8.f, 4, omin, omax);
-                zoom2_kernel<<<grid2d(L.w, L.h, b2), b2, 0, st>>>(omin, c.w, fmin[vi], L.w, L.h);
-                zoom2_kernel<<<grid2d(L.w, L.h, b2), b2, 0, st>>>(omax, c.w, fmax[vi], L.w, L.h);
-                ctx->launches += 3;
+                launch(ctx, zoom2_kernel, grid2d(L.w, L.h, b2), b2, 0, st, omin, c.w, fmin[vi], L.w, L.h);
+                launch(ctx, zoom2_kernel, grid2d(L.w, L.h, b2), b2, 0, st, omax, c.w, fmax[vi], L.w, L.h);
             }
             CK(cudaGetLastError());
         }
@@ -1121,9 +961,8 @@ static int mgm_multi_enqueue(s2pb_ctx *ctx, Slot &s, const float *d_im1, const f
         s.arena_off = arena_mark;
         float *a = arena_take<float>(s, n), *b = arena_take<float>(s, n), *c = arena_take<float>(s, n), *d = arena_take<float>(s, n);
         const size_t mark2 = s.arena_off;
-        update_ranges_kernel<<<grid2d(w, h, b2), b2, 0, st>>>(L0.dl, 1.f, w, h, L0.dminL, L0.dmaxL, L0.dminL, L0.dmaxL, w, h, 2.f, 4, a, b);
-        update_ranges_kernel<<<grid2d(w, h, b2), b2, 0, st>>>(L0.dr, 1.f, w, h, L0.dminR, L0.dmaxR, L0.dminR, L0.dmaxR, w, h, 2.f, 4, c, d);
-        ctx->launches += 2;
+        launch(ctx, update_ranges_kernel, grid2d(w, h, b2), b2, 0, st, L0.dl, 1.f, w, h, L0.dminL, L0.dmaxL, L0.dminL, L0.dmaxL, w, h, 2.f, 4, a, b);
+        launch(ctx, update_ranges_kernel, grid2d(w, h, b2), b2, 0, st, L0.dr, 1.f, w, h, L0.dminR, L0.dmaxR, L0.dminR, L0.dmaxR, w, h, 2.f, 4, c, d);
         L0.dminL = a; L0.dmaxL = b; L0.dminR = c; L0.dmaxR = d;
         s.arena_off = mark2;
         float *keep[2] = {ctx->pkr_dst[0], ctx->pkr_dst[1]};          // ... and with its own img_dict: the PKR images written are the ZOOM = 1 call's
@@ -1136,18 +975,16 @@ static int mgm_multi_enqueue(s2pb_ctx *ctx, Slot &s, const float *d_im1, const f
     if (p->lr_mode == 2) {                     // main_mgm_multi.cc:212-217
         s.arena_off = arena_mark;
         float *tr = arena_take<float>(s, n);
-        lrcheck_kernel<<<grid2d(w, h, b2), b2, 0, st>>>(L0.dr, L0.dl, tr, w, h, p->lr_tau);
-        lrcheck_kernel<<<grid2d(w, h, b2), b2, 0, st>>>(L0.dl, L0.dr, outL, w, h, p->lr_tau);
-        ctx->launches += 2;
+        launch(ctx, lrcheck_kernel, grid2d(w, h, b2), b2, 0, st, L0.dr, L0.dl, tr, w, h, p->lr_tau);
+        launch(ctx, lrcheck_kernel, grid2d(w, h, b2), b2, 0, st, L0.dl, L0.dr, outL, w, h, p->lr_tau);
         if (d_dispR) CK(cudaMemcpyAsync(d_dispR, tr, (size_t)n * 4, cudaMemcpyDeviceToDevice, st));
     } else {
         CK(cudaMemcpyAsync(outL, L0.dl, (size_t)n * 4, cudaMemcpyDeviceToDevice, st));
         if (d_dispR) CK(cudaMemcpyAsync(d_dispR, L0.dr, (size_t)n * 4, cudaMemcpyDeviceToDevice, st));
     }
-    nan_restore_kernel<<<(n + 255) / 256, 256, 0, st>>>(outL, d_im1, n);
-    ctx->launches++;
-    if (d_dispR) { nan_restore_kernel<<<(n + 255) / 256, 256, 0, st>>>(d_dispR, d_im2, n); ctx->launches++; }
-    if (d_mask) { rejection_mask_kernel<<<grid2d(w, h, b2), b2, 0, st>>>(outL, d_im1, d_im2, w, h, d_mask); ctx->launches++; }
+    launch(ctx, nan_restore_kernel, (n + 255) / 256, 256, 0, st, outL, d_im1, n);
+    if (d_dispR) launch(ctx, nan_restore_kernel, (n + 255) / 256, 256, 0, st, d_dispR, d_im2, n);
+    if (d_mask) launch_rejection_mask(ctx, outL, d_im1, d_im2, w, h, d_mask, st);
     CK(cudaGetLastError());
     return S2PB_OK;
 }
@@ -1166,8 +1003,7 @@ static int mgm_enqueue(s2pb_ctx *ctx, Slot &s, const float *d_im1, const float *
     if (nodata_hint < 0) {     // unknown: look (costs one stream synchronisation)
         int *flag = s.d_small + 16;      // this slot's own word (several slots may ask at once)
         CK(cudaMemsetAsync(flag, 0, 4, st));
-        has_nan_kernel<<<ctx->sm_count * 4, 256, 0, st>>>(d_im2, n, flag);
-        ctx->launches++;
+        launch(ctx, has_nan_kernel, ctx->sm_count * 4, 256, 0, st, d_im2, n, flag);
         int hflag = 0;
         CK(cudaMemcpyAsync(&hflag, flag, 4, cudaMemcpyDeviceToHost, st));
         int rs = sync_or_timeout(ctx, st);
@@ -1185,14 +1021,12 @@ static int mgm_enqueue(s2pb_ctx *ctx, Slot &s, const float *d_im1, const float *
     rc = slot_ensure(ctx, s, w, h, 32 * LPL, p->ndir, general ? 4 : 1);
     if (rc != S2PB_OK) return rc;
     const float *im[2] = {d_im1, d_im2};
-    dim3 b2(32, 8);
     s.timed = true;
     CK(cudaEventRecord(s.ev[0], st));
     // ---- NaN-free copies of both images and their label ranges
     for (int vi = 0; vi < 2; vi++) {
         int lo_all = vi == 0 ? dmin : -dmax, hi_all = vi == 0 ? dmax : -dmin;
-        prepare_view_kernel<<<(n + 255) / 256, 256, 0, st>>>(im[vi], n, lo_all, hi_all, dmin, s.v[vi].img, s.v[vi].lo, s.v[vi].hi);
-        ctx->launches++;
+        launch(ctx, prepare_view_kernel, (n + 255) / 256, 256, 0, st, im[vi], n, lo_all, hi_all, dmin, s.v[vi].img, s.v[vi].lo, s.v[vi].hi);
     }
     const float *img[2] = {s.v[0].img, s.v[1].img};
     short *lo[2] = {s.v[0].lo, s.v[1].lo}, *hi[2] = {s.v[0].hi, s.v[1].hi};
@@ -1200,14 +1034,10 @@ static int mgm_enqueue(s2pb_ctx *ctx, Slot &s, const float *d_im1, const float *
     rc = mgm_call(ctx, s, w, h, img, lo, hi, gminv, LPLv, 1, wgt, p, outL, outR, st, true);
     if (rc != S2PB_OK) return rc;
     // ---- no-data restore (main_mgm.cc:231-236), mask
-    nan_restore_kernel<<<(n + 255) / 256, 256, 0, st>>>(outL, d_im1, n);
-    nan_restore_kernel<<<(n + 255) / 256, 256, 0, st>>>(outR, d_im2, n);
-    ctx->launches += 2;
+    launch(ctx, nan_restore_kernel, (n + 255) / 256, 256, 0, st, outL, d_im1, n);
+    launch(ctx, nan_restore_kernel, (n + 255) / 256, 256, 0, st, outR, d_im2, n);
     if (d_conf) CK(cudaMemcpyAsync(d_conf, s.v[0].conf, npix * 4, cudaMemcpyDeviceToDevice, st));
-    if (d_mask) {
-        rejection_mask_kernel<<<grid2d(w, h, b2), b2, 0, st>>>(outL, d_im1, d_im2, w, h, d_mask);
-        ctx->launches++;
-    }
+    if (d_mask) launch_rejection_mask(ctx, outL, d_im1, d_im2, w, h, d_mask, st);
     CK(cudaGetLastError());
     CK(cudaEventRecord(s.ev[5], st));
     return S2PB_OK;
@@ -1330,22 +1160,17 @@ extern "C" int s2pb_mgm_pkr(s2pb_ctx *ctx, const float *im1, const float *im2, i
                             float *pkr_left, float *pkr_right)
 {
     if (!ctx || !pkr_left || !pkr_right) return fail(S2PB_ERR_ARG, "null argument");
-    CK(cudaSetDevice(ctx->device));
     const size_t npix = (size_t)w * h;
-    cudaStream_t st = ctx->slots[0].stream;
-    ScratchLease L(ctx, st);
+    HostCall L(ctx, "the PKR images");
     float *d0 = L.take<float>(npix * 4), *d1 = L.take<float>(npix * 4);
-    if (!d0 || !d1) return L.nomem("the PKR images");
+    if (int rc = L.error()) return rc;
     ctx->pkr_dst[0] = d0; ctx->pkr_dst[1] = d1;
     int rc = s2pb_mgm_weighted(ctx, im1, im2, w, h, dmin, dmax, p, nullptr, nullptr, disp, conf, mask, disp_right);
     ctx->pkr_dst[0] = ctx->pkr_dst[1] = nullptr;
-    if (rc == S2PB_OK) {
-        cudaError_t e = cudaMemcpyAsync(pkr_left, d0, npix * 4, cudaMemcpyDeviceToHost, st);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(pkr_right, d1, npix * 4, cudaMemcpyDeviceToHost, st);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-        if (e != cudaSuccess) rc = fail(S2PB_ERR_CUDA, "copy of the PKR images failed: %s", cudaGetErrorString(e));
-    }
-    return rc;
+    if (rc != S2PB_OK) return rc;
+    L.download(pkr_left, d0, npix * 4);
+    L.download(pkr_right, d1, npix * 4);
+    return L.finish();
 }
 
 extern "C" int s2pb_reserve(s2pb_ctx *ctx, int nslots, int w, int h, int nlabels)
@@ -1468,37 +1293,29 @@ extern "C" int s2pb_census(s2pb_ctx *ctx, const float *img, int w, int h, int wi
 {
     if (!ctx || !img || !codes || w < 1 || h < 1) return fail(S2PB_ERR_ARG, "bad argument");
     if (win != 3 && win != 5 && win != 7) return fail(S2PB_ERR_ARG, "census window must be 3, 5 or 7");
-    CK(cudaSetDevice(ctx->device));
     size_t npix = (size_t)w * h;
-    cudaStream_t st = ctx->slots[0].stream;
-    ScratchLease L(ctx, st);
-    float *a = L.take<float>(npix * 4);
+    HostCall L(ctx, "the census");
+    float *a = L.upload(img, npix * 4);
     uint64_t *b = L.take<uint64_t>(npix * 8);
-    if (!a || !b) return L.nomem("the census");
-    CK(cudaMemcpyAsync(a, img, npix * 4, cudaMemcpyHostToDevice, st));
+    if (int rc = L.error()) return rc;
     dim3 b2(32, 8);
-    census_kernel<<<grid2d(w, h, b2), b2, 0, st>>>(a, w, h, win / 2, b);
-    ctx->launches++;
+    launch(ctx, census_kernel, grid2d(w, h, b2), b2, 0, L.st, a, w, h, win / 2, b);
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(codes, b, npix * 8, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    return S2PB_OK;
+    L.download(codes, b, npix * 8);
+    return L.finish();
 }
 
-static int upload_ranges(ScratchLease &L, const int32_t *lo, const int32_t *hi, size_t npix, int gmin, int D, cudaStream_t st,
-                         short **dlo, short **dhi)
+// the int16 label ranges of a host-buffer call, uploaded through its protocol: the caller checks L.error() after this
+static int upload_ranges(HostCall &L, const int32_t *lo, const int32_t *hi, size_t npix, int gmin, int D, short **dlo, short **dhi)
 {
     std::vector<short> a(npix), b(npix);
     for (size_t i = 0; i < npix; i++) {
         if (lo[i] < gmin || hi[i] > gmin + D - 1 || lo[i] > hi[i]) return fail(S2PB_ERR_ARG, "range of pixel %zu outside the volume", i);
         a[i] = (short)lo[i]; b[i] = (short)hi[i];
     }
-    *dlo = L.take<short>(npix * 2);
-    *dhi = L.take<short>(npix * 2);
-    if (!*dlo || !*dhi) return L.nomem("the label ranges");
-    CK(cudaMemcpyAsync(*dlo, a.data(), npix * 2, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(*dhi, b.data(), npix * 2, cudaMemcpyHostToDevice, st));
-    CK(cudaStreamSynchronize(st));
+    *dlo = L.upload(a.data(), npix * 2);
+    *dhi = L.upload(b.data(), npix * 2);
+    CK(cudaStreamSynchronize(L.st));         // a and b go on return
     return S2PB_OK;
 }
 
@@ -1510,40 +1327,33 @@ static int stage_costvolume(s2pb_ctx *ctx, const float *u, const float *v, int w
     if (!ctx || !u || !v || !lo || !hi || !C || w < 1 || h < 1 || D < 1) return fail(S2PB_ERR_ARG, "bad argument");
     if (win != 3 && win != 5 && win != 7) return fail(S2PB_ERR_ARG, "window must be 3, 5 or 7");
     if (cost < 0 || cost >= S2PB_COST_COUNT) return fail(S2PB_ERR_ARG, "cost must be one of S2PB_COST_*");
-    CK(cudaSetDevice(ctx->device));
     int LPL, rc = slab_lpl(D, &LPL);      // the stage entry points run the register-resident kernels only
     if (rc == S2PB_OK && wide_slab(LPL)) rc = fail(S2PB_ERR_UNSUPPORTED, "the stage entry points take at most 512 labels, not %d", D);
     if (rc != S2PB_OK) return rc;
     const int DP = 32 * LPL;
     size_t npix = (size_t)w * h, tot = npix * D;
-    cudaStream_t st = ctx->slots[0].stream;
-    ScratchLease L(ctx, st);
-    float *du = L.take<float>(npix * 4), *dv = L.take<float>(npix * 4);
-    uint64_t *cu = L.take<uint64_t>(npix * 8), *cv = L.take<uint64_t>(npix * 8);      // census codes or NCC window statistics
-    void *dC = L.take<void>(npix * DP * (codes ? 1 : 4));
-    float *dCf = L.take<float>(tot * 4), *dlut = L.take<float>(256);
-    if (!du || !dv || !cu || !cv || !dC || !dCf || !dlut) return L.nomem("the cost volume");
-    short *dlo, *dhi;
-    rc = upload_ranges(L, lo, hi, npix, gmin, D, st, &dlo, &dhi);
-    if (rc != S2PB_OK) return rc;
-    CK(cudaMemcpyAsync(du, u, npix * 4, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(dv, v, npix * 4, cudaMemcpyHostToDevice, st));
-    float *rt = nullptr;
-    rc = stage_round_trip(ctx, L, dv, w, h, st, &rt);
-    if (rc != S2PB_OK) return rc;
     float lut_h[64];
     const bool scaled = cost_lut(win, lut_h);
-    CK(cudaMemcpyAsync(dlut, lut_h, 256, cudaMemcpyHostToDevice, st));
+    HostCall L(ctx, "the cost volume");
+    float *du = L.upload(u, npix * 4), *dv = L.upload(v, npix * 4);
+    uint64_t *cu = L.take<uint64_t>(npix * 8), *cv = L.take<uint64_t>(npix * 8);      // census codes or NCC window statistics
+    void *dC = L.take<void>(npix * DP * (codes ? 1 : 4));
+    float *dCf = L.take<float>(tot * 4), *dlut = L.upload(lut_h, 256);
+    short *dlo, *dhi;
+    rc = upload_ranges(L, lo, hi, npix, gmin, D, &dlo, &dhi);
+    if (rc == S2PB_OK) rc = L.error();
+    if (rc != S2PB_OK) return rc;
+    float *rt = nullptr;
+    rc = stage_round_trip(ctx, L, dv, w, h, L.st, &rt);
+    if (rc != S2PB_OK) return rc;
     dim3 b2(32, 8);
     if (cost == S2PB_COST_CENSUS) {
-        census_kernel<<<grid2d(w, h, b2), b2, 0, st>>>(du, w, h, win / 2, cu);
-        census_kernel<<<grid2d(w, h, b2), b2, 0, st>>>(rt, w, h, win / 2, cv);
-        ctx->launches += 2;
+        launch(ctx, census_kernel, grid2d(w, h, b2), b2, 0, L.st, du, w, h, win / 2, cu);
+        launch(ctx, census_kernel, grid2d(w, h, b2), b2, 0, L.st, rt, w, h, win / 2, cv);
     }
     if (cost == S2PB_COST_NCC) {
-        ncc_stats_kernel<<<grid2d(w, h, b2), b2, 0, st>>>(du, w, h, win / 2, (float2 *)cu);
-        ncc_stats_kernel<<<grid2d(w, h, b2), b2, 0, st>>>(rt, w, h, win / 2, (float2 *)cv);
-        ctx->launches += 2;
+        launch(ctx, ncc_stats_kernel, grid2d(w, h, b2), b2, 0, L.st, du, w, h, win / 2, (float2 *)cu);
+        launch(ctx, ncc_stats_kernel, grid2d(w, h, b2), b2, 0, L.st, rt, w, h, win / 2, (float2 *)cv);
     }
     CostGenParams G;
     memset(&G, 0, sizeof G);
@@ -1551,15 +1361,13 @@ static int stage_costvolume(s2pb_ctx *ctx, const float *u, const float *v, int w
     G.su = (float2 *)cu; G.sv0 = (float2 *)cv;
     G.lut = dlut; G.lo = dlo; G.hi = dhi;
     G.w = w; G.h = h; G.gmin = gmin; G.cost = cost; G.win = win; G.zoom = 1; G.C = (float *)dC;
-    rc = launch_cost(ctx, LPL, !codes, G, st);
+    rc = launch_cost(ctx, LPL, !codes, G, L.st);
     if (rc != S2PB_OK) return rc;
-    if (codes) unpack_cost_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>((uint8_t *)dC, npix, D, DP, scaled ? dlut : nullptr, dCf);
-    else unpad_cost_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>((float *)dC, npix, D, DP, dCf);
-    ctx->launches++;
+    if (codes) launch(ctx, unpack_cost_kernel, (unsigned)((tot + 255) / 256), 256, 0, L.st, (uint8_t *)dC, npix, D, DP, scaled ? dlut : nullptr, dCf);
+    else launch(ctx, unpad_cost_kernel, (unsigned)((tot + 255) / 256), 256, 0, L.st, (float *)dC, npix, D, DP, dCf);
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(C, dCf, tot * 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    return S2PB_OK;
+    L.download(C, dCf, tot * 4);
+    return L.finish();
 }
 
 extern "C" int s2pb_costvolume(s2pb_ctx *ctx, const float *u, const float *v, int w, int h, const int32_t *lo, const int32_t *hi,
@@ -1583,7 +1391,6 @@ static int stage_aggregate(s2pb_ctx *ctx, const float *C, const int32_t *lo, con
     if (!ctx || !C || !lo || !hi || !disp || w < 2 || h < 2 || D < 1) return fail(S2PB_ERR_ARG, "bad argument");
     if (ndir != 2 && ndir != 4 && ndir != 8) return fail(S2PB_ERR_ARG, "ndir must be 2, 4 or 8");
     if (tsgm < 1 || tsgm > 4) return fail(S2PB_ERR_ARG, "tsgm must be 1..4");
-    CK(cudaSetDevice(ctx->device));
     int LPL, rc = slab_lpl(D, &LPL);      // the stage entry points run the register-resident kernels only
     if (rc == S2PB_OK && wide_slab(LPL)) rc = fail(S2PB_ERR_UNSUPPORTED, "the stage entry points take at most 512 labels, not %d", D);
     if (rc != S2PB_OK) return rc;
@@ -1599,27 +1406,23 @@ static int stage_aggregate(s2pb_ctx *ctx, const float *C, const int32_t *lo, con
             if (c > (float)kCostMaxCode && c != INFINITY) general = true;
         }
     }
-    Slot &s = ctx->slots[0];
-    cudaStream_t st = s.stream;
+    HostCall L(ctx, "the aggregation");
+    float *dCf = L.upload(C, tot * 4);
+    float *dS = S ? L.take<float>(tot * 4) : nullptr;
+    float *dW = weights ? L.upload(weights, npix * 4) : nullptr;
+    short *dlo, *dhi;
+    rc = upload_ranges(L, lo, hi, npix, gmin, D, &dlo, &dhi);
+    if (rc == S2PB_OK) rc = L.error();
+    if (rc != S2PB_OK) return rc;
+    Slot &s = ctx->slots[0];          // the workspace of slot 0 holds the slab
     rc = slot_ensure(ctx, s, w, h, DP, ndir, general ? 4 : 1);
     if (rc != S2PB_OK) return rc;
-    ScratchLease L(ctx, st);
-    float *dCf = L.take<float>(tot * 4);
-    float *dS = S ? L.take<float>(tot * 4) : nullptr;
-    float *dW = weights ? L.take<float>(npix * 4) : nullptr;
-    if (!dCf || (S && !dS) || (weights && !dW)) return L.nomem("the aggregation");
-    if (weights) CK(cudaMemcpyAsync(dW, weights, npix * 4, cudaMemcpyHostToDevice, st));
-    short *dlo, *dhi;
-    rc = upload_ranges(L, lo, hi, npix, gmin, D, st, &dlo, &dhi);
-    if (rc != S2PB_OK) return rc;
-    CK(cudaMemcpyAsync(dCf, C, tot * 4, cudaMemcpyHostToDevice, st));
     size_t totp = npix * DP;
-    if (general) pad_cost_kernel<<<(unsigned)((totp + 255) / 256), 256, 0, st>>>(dCf, npix, D, DP, (float *)s.v[0].C);
-    else pack_cost_kernel<<<(unsigned)((totp + 255) / 256), 256, 0, st>>>(dCf, npix, D, DP, (uint8_t *)s.v[0].C);
-    ctx->launches++;
+    if (general) launch(ctx, pad_cost_kernel, (unsigned)((totp + 255) / 256), 256, 0, L.st, dCf, npix, D, DP, (float *)s.v[0].C);
+    else launch(ctx, pack_cost_kernel, (unsigned)((totp + 255) / 256), 256, 0, L.st, dCf, npix, D, DP, (uint8_t *)s.v[0].C);
     CK(cudaGetLastError());
     const float *wgt[2] = {dW, nullptr};
-    rc = launch_aggregate(ctx, s, 1, w, h, LPL, P1, P2, ndir, tsgm, nullptr, st, general, wgt);
+    rc = launch_aggregate(ctx, s, 1, w, h, LPL, P1, P2, ndir, tsgm, nullptr, L.st, general, wgt);
     if (rc != S2PB_OK) return rc;
     s2pb_mgm_params prm;
     s2pb_default_params("mgm", &prm);
@@ -1628,14 +1431,13 @@ static int stage_aggregate(s2pb_ctx *ctx, const float *C, const int32_t *lo, con
     fill_wta(W, s.v[0], ndir, gmin, &prm, nullptr, npix);
     W.lo = dlo; W.hi = dhi;
     W.S = dS; W.Dout = D;
-    rc = launch_wta(ctx, LPL, W, st, general);
+    rc = launch_wta(ctx, LPL, W, L.st, general);
     if (rc != S2PB_OK) return rc;
-    CK(cudaMemcpyAsync(disp, s.v[0].disp, npix * 4, cudaMemcpyDeviceToHost, st));
-    if (cost) CK(cudaMemcpyAsync(cost, s.v[0].cost, npix * 4, cudaMemcpyDeviceToHost, st));
-    if (conf) CK(cudaMemcpyAsync(conf, s.v[0].conf, npix * 4, cudaMemcpyDeviceToHost, st));
-    if (S) CK(cudaMemcpyAsync(S, dS, tot * 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    return S2PB_OK;
+    L.download(disp, s.v[0].disp, npix * 4);
+    if (cost) L.download(cost, s.v[0].cost, npix * 4);
+    if (conf) L.download(conf, s.v[0].conf, npix * 4);
+    if (S) L.download(S, dS, tot * 4);
+    return L.finish();
 }
 
 extern "C" int s2pb_aggregate_w(s2pb_ctx *ctx, const float *C, const int32_t *lo, const int32_t *hi, int w, int h, int gmin, int D,
@@ -1654,248 +1456,69 @@ extern "C" int s2pb_aggregate(s2pb_ctx *ctx, const float *C, const int32_t *lo, 
 extern "C" int s2pb_median(s2pb_ctx *ctx, const float *in, float *out, int w, int h, int radius)
 {
     if (!ctx || !in || !out || w < 1 || h < 1 || radius < 0 || radius > 2) return fail(S2PB_ERR_ARG, "bad argument");
-    CK(cudaSetDevice(ctx->device));
     size_t npix = (size_t)w * h;
-    cudaStream_t st = ctx->slots[0].stream;
-    ScratchLease L(ctx, st);
-    float *a = L.take<float>(npix * 4), *b = L.take<float>(npix * 4);
-    if (!a || !b) return L.nomem("the median");
-    CK(cudaMemcpyAsync(a, in, npix * 4, cudaMemcpyHostToDevice, st));
+    HostCall L(ctx, "the median");
+    float *a = L.upload(in, npix * 4), *b = L.take<float>(npix * 4);
+    if (int rc = L.error()) return rc;
     dim3 b2(32, 8);
-    median_kernel<<<grid2d(w, h, b2), b2, 0, st>>>(a, b, w, h, radius);
-    ctx->launches++;
+    launch(ctx, median_kernel, grid2d(w, h, b2), b2, 0, L.st, a, b, w, h, radius);
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(out, b, npix * 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    return S2PB_OK;
+    L.download(out, b, npix * 4);
+    return L.finish();
 }
 
 extern "C" int s2pb_remove_small_cc(s2pb_ctx *ctx, const float *in, float *out, int w, int h, int minarea)
 {
     if (!ctx || !in || !out || w < 2 || h < 2) return fail(S2PB_ERR_ARG, "bad argument");
-    CK(cudaSetDevice(ctx->device));
     size_t npix = (size_t)w * h;
-    cudaStream_t st = ctx->slots[0].stream;
-    ScratchLease L(ctx, st);
-    float *a = L.take<float>(npix * 4), *b = L.take<float>(npix * 4);
+    HostCall L(ctx, "remove_small_cc");
+    float *a = L.upload(in, npix * 4), *b = L.take<float>(npix * 4);
     int *lab = L.take<int>(npix * 4), *area = L.take<int>(npix * 4);
-    if (!a || !b || !lab || !area) return L.nomem("remove_small_cc");
-    CK(cudaMemcpyAsync(a, in, npix * 4, cudaMemcpyHostToDevice, st));
-    int rc = launch_remove_small_cc(ctx, a, b, w, h, minarea, 5.f, lab, area, st);
+    if (int rc = L.error()) return rc;
+    int rc = launch_remove_small_cc(ctx, a, b, w, h, minarea, 5.f, lab, area, L.st);
     if (rc != S2PB_OK) return rc;
-    CK(cudaMemcpyAsync(out, b, npix * 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    return S2PB_OK;
+    L.download(out, b, npix * 4);
+    return L.finish();
 }
 
 extern "C" int s2pb_erode_mask(s2pb_ctx *ctx, const uint8_t *in, uint8_t *out, int w, int h, float radius)
 {
     if (!ctx || !in || !out || w < 1 || h < 1) return fail(S2PB_ERR_ARG, "bad argument");
     if (!(radius > 1.f) || radius > 64.f) return fail(S2PB_ERR_ARG, "disk radius must be in (1, 64]");   // build_disk, c/morsi.c:282
-    CK(cudaSetDevice(ctx->device));
     size_t npix = (size_t)w * h;
-    cudaStream_t st = ctx->slots[0].stream;
-    ScratchLease L(ctx, st);
-    uint8_t *a = L.take<uint8_t>(npix), *b = L.take<uint8_t>(npix);
-    if (!a || !b) return L.nomem("the mask erosion");
-    CK(cudaMemcpyAsync(a, in, npix, cudaMemcpyHostToDevice, st));
+    HostCall L(ctx, "the mask erosion");
+    uint8_t *a = L.upload(in, npix), *b = L.take<uint8_t>(npix);
+    if (int rc = L.error()) return rc;
     dim3 b2(32, 8);
-    erode_mask_kernel<<<grid2d(w, h, b2), b2, 0, st>>>(a, b, w, h, radius);
-    ctx->launches++;
+    launch(ctx, erode_mask_kernel, grid2d(w, h, b2), b2, 0, L.st, a, b, w, h, radius);
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(out, b, npix, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    return S2PB_OK;
+    L.download(out, b, npix);
+    return L.finish();
+}
+
+// create_rejection_mask (s2p/block_matching.py:18-32) of a device disparity map
+void launch_rejection_mask(s2pb_ctx *ctx, const float *disp, const float *im1, const float *im2, int w, int h, uint8_t *mask,
+                           cudaStream_t st)
+{
+    dim3 b2(32, 8);
+    launch(ctx, rejection_mask_kernel, grid2d(w, h, b2), b2, 0, st, disp, im1, im2, w, h, mask);
 }
 
 extern "C" int s2pb_rejection_mask(s2pb_ctx *ctx, const float *disp, const float *im1, const float *im2, int w, int h, uint8_t *mask)
 {
     if (!ctx || !disp || !im1 || !im2 || !mask || w < 1 || h < 1) return fail(S2PB_ERR_ARG, "bad argument");
-    CK(cudaSetDevice(ctx->device));
     size_t npix = (size_t)w * h;
-    cudaStream_t st = ctx->slots[0].stream;
-    ScratchLease L(ctx, st);
-    float *a = L.take<float>(npix * 4), *b = L.take<float>(npix * 4), *c = L.take<float>(npix * 4);
+    HostCall L(ctx, "the rejection mask");
+    float *a = L.upload(disp, npix * 4), *b = L.upload(im1, npix * 4), *c = L.upload(im2, npix * 4);
     uint8_t *m = L.take<uint8_t>(npix);
-    if (!a || !b || !c || !m) return L.nomem("the rejection mask");
-    CK(cudaMemcpyAsync(a, disp, npix * 4, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(b, im1, npix * 4, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(c, im2, npix * 4, cudaMemcpyHostToDevice, st));
-    dim3 b2(32, 8);
-    rejection_mask_kernel<<<grid2d(w, h, b2), b2, 0, st>>>(a, b, c, w, h, m);
-    ctx->launches++;
+    if (int rc = L.error()) return rc;
+    launch_rejection_mask(ctx, a, b, c, w, h, m, L.st);
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(mask, m, npix, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    return S2PB_OK;
+    L.download(mask, m, npix);
+    return L.finish();
 }
 
-// ------------------------------------------------------------------ rectification warp
-
-static void invert33(const double m[9], double o[9])
-{   // Homography.cpp:281-303
-    const double det = 1.0 / (m[0] * m[4] * m[8] - m[0] * m[5] * m[7] - m[1] * m[3] * m[8] + m[1] * m[5] * m[6] + m[2] * m[3] * m[7] -
-                              m[2] * m[4] * m[6]);
-    o[0] = det * (m[4] * m[8] - m[5] * m[7]); o[1] = det * (m[2] * m[7] - m[1] * m[8]); o[2] = det * (m[1] * m[5] - m[2] * m[4]);
-    o[3] = det * (m[5] * m[6] - m[3] * m[8]); o[4] = det * (m[0] * m[8] - m[2] * m[6]); o[5] = det * (m[2] * m[3] - m[0] * m[5]);
-    o[6] = det * (m[3] * m[7] - m[4] * m[6]); o[7] = det * (m[1] * m[6] - m[0] * m[7]); o[8] = det * (m[0] * m[4] - m[1] * m[3]);
-}
-// adjugate over determinant: invert_homography of c/disp_to_h.c:26-42, also the ROI inverse of 3rdparty/homography/main.cpp.
-// It rounds differently from invert33, which multiplies by 1/det as Homography.cpp does.
-static void invert_homography(const double i[9], double o[9])
-{
-    const double det = i[0] * i[4] * i[8] + i[2] * i[3] * i[7] + i[1] * i[5] * i[6] - i[2] * i[4] * i[6] - i[1] * i[3] * i[8] - i[0] * i[5] * i[7];
-    o[0] = (i[4] * i[8] - i[5] * i[7]) / det; o[1] = (i[2] * i[7] - i[1] * i[8]) / det; o[2] = (i[1] * i[5] - i[2] * i[4]) / det;
-    o[3] = (i[5] * i[6] - i[3] * i[8]) / det; o[4] = (i[0] * i[8] - i[2] * i[6]) / det; o[5] = (i[2] * i[3] - i[0] * i[5]) / det;
-    o[6] = (i[3] * i[7] - i[4] * i[6]) / det; o[7] = (i[1] * i[6] - i[0] * i[7]) / det; o[8] = (i[0] * i[4] - i[1] * i[3]) / det;
-}
-static float min_sv_jacobian(const double m[9], double px, double py)
-{   // getMinSVJacob, Homography.cpp:174-198
-    const double X[3] = {m[0] * px + m[1] * py + m[2], m[3] * px + m[4] * py + m[5], m[6] * px + m[7] * py + m[8]};
-    const double z = 1.0 / X[2], x = z * X[0], y = z * X[1];
-    const double a = z * (m[0] - m[6] * x), b = z * (m[1] - m[7] * x), c = z * (m[3] - m[6] * y), d = z * (m[4] - m[7] * y);
-    return (float)sqrt(0.5 * (a * a + b * b + c * c + d * d -
-                              sqrt((a * a + b * b - c * c - d * d) * (a * a + b * b - c * c - d * d) + 4.0 * (a * c + b * d) * (a * c + b * d))));
-}
-static float min_zoom_out(const double m[9], size_t w, size_t h)
-{   // getMinZoomOut, Homography.cpp:203-212
-    float r = std::fmin(min_sv_jacobian(m, 0, (double)h), min_sv_jacobian(m, (double)w, (double)h));
-    r = std::fmin(min_sv_jacobian(m, (double)w, 0), r);
-    r = std::fmin(min_sv_jacobian(m, 0, 0), r);
-    return std::fmin(1.f, r);
-}
-
-// mapImage (Homography.cpp:50-168) on device images; recursive through the anti-aliasing branch.
-static int map_image(s2pb_ctx *ctx, ScratchLease &L, cudaStream_t st, const float *d_src, int w, int h, const double M[9],
-                     float *d_out, int ow, int oh, bool use_aa, int depth)
-{
-    if (depth > 6) return fail(S2PB_ERR_ARG, "homography: anti-aliasing recursion does not settle");
-    dim3 b2(32, 8);
-    const float zoomOut = use_aa ? min_zoom_out(M, (size_t)w, (size_t)h) : 1.f;
-    const bool useZ = zoomOut < 1.f;
-    double matZ[9] = {0};
-    float *tmp, *scratch;
-    int tw = w, th = h;
-    if (useZ) {
-        const float zoomIn = 1.0f / zoomOut;
-        tw = (int)std::ceil((size_t)ow * zoomIn * 1.5);
-        th = (int)std::ceil((size_t)oh * zoomIn * 1.5);
-        if (tw < 1 || th < 1 || (size_t)tw * th > ((size_t)1 << 31)) return fail(S2PB_ERR_ARG, "homography: degenerate zoom %g", (double)zoomIn);
-        for (int k = 0; k < 6; k++) matZ[k] = zoomIn * M[k];
-        for (int k = 6; k < 9; k++) matZ[k] = M[k];
-        tmp = L.take<float>((size_t)tw * th * 4);
-        scratch = L.take<float>((size_t)tw * th * 4);
-        if (!tmp || !scratch) return L.nomem("the warp");
-        int rc = map_image(ctx, L, st, d_src, w, h, matZ, tmp, tw, th, true, depth + 1);
-        if (rc != S2PB_OK) return rc;
-        // Gaussian of sigma = 0.8 sqrt(zoomIn^2 - 1) (Homography.cpp:101-102, LibImages.cpp:506-687)
-        const float sigma = 0.8f * std::sqrt(zoomIn * zoomIn - 1.f);
-        GaussKernel K;
-        int ks = (int)(8.f * sigma + 1.f);
-        ks = ks > 3 ? ks + 1 - ks % 2 : 3;
-        if (ks > 64) return fail(S2PB_ERR_UNSUPPORTED, "homography: zoom-out of %g needs a %d-tap anti-aliasing filter (64 supported)", (double)zoomIn, ks);
-        K.size = ks;
-        float sum = 0.f;
-        for (int i = 0; i < ks; i++) { const float x = (float)(i - ks / 2); K.k[i] = std::exp(-x * x / (2.f * sigma * sigma)); sum += K.k[i]; }
-        for (int i = 0; i < ks; i++) K.k[i] /= sum;
-        int jlim = 0;
-        while (jlim < tw - 4) jlim += 4;       // first column of the reference's scalar tail
-        gauss_rows_kernel<<<grid2d(tw, th, b2), b2, 0, st>>>(tmp, scratch, tw, th, K);
-        gauss_cols_kernel<<<grid2d(tw, th, b2), b2, 0, st>>>(scratch, tmp, tw, th, K, jlim);
-        ctx->launches += 2;
-        matZ[0] = zoomOut; matZ[1] = 0; matZ[2] = 0; matZ[3] = 0; matZ[4] = zoomOut; matZ[5] = 0; matZ[6] = 0; matZ[7] = 0; matZ[8] = 1;
-    } else {
-        tmp = L.take<float>((size_t)w * h * 4);
-        scratch = L.take<float>((size_t)w * h * 4);
-        if (!tmp || !scratch) return L.nomem("the warp");
-        CK(cudaMemcpyAsync(tmp, d_src, (size_t)w * h * 4, cudaMemcpyDeviceToDevice, st));
-    }
-    // prepareSpline (Splines.cpp:26-121): NaN -> 0, 2-pole prefilter along rows, then along columns
-    const size_t n = (size_t)tw * th;
-    const float lambda = (float)(1.430575 * (1.0 + 1.0 / 0.430575) * 1.0430963 * (1.0 + 1.0 / 0.0430963));
-    const double z0 = -0.430575, z1 = -0.0430963;
-    nan_to_zero_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(tmp, n);
-    dim3 bt(32, 8);
-    // prefilter along x (on the transposed image) then along y; `a` holds the data, `b` is the other buffer
-    auto prefilter = [&](float *a, float *b, int lw, int lh) {      // columns of an lw x lh image, result back in a
-        if (lh >= 2 * kSplineSeg) {
-            dim3 g((lw + 127) / 128, (lh + kSplineSeg - 1) / kSplineSeg);
-            spline_segments_kernel<<<g, 128, 0, st>>>(a, b, lw, lh, lambda, z0);
-            spline_segments_kernel<<<g, 128, 0, st>>>(b, a, lw, lh, 1.f, z1);
-            ctx->launches += 2;
-        } else {
-            spline_columns_kernel<<<(lw + 31) / 32, 32, 0, st>>>(a, lw, lh, lambda, z0, z1);
-            ctx->launches++;
-        }
-    };
-    transpose_kernel<<<dim3((tw + 31) / 32, (th + 31) / 32), bt, 0, st>>>(tmp, tw, th, scratch);
-    prefilter(scratch, tmp, th, tw);                                                // rows of the image
-    transpose_kernel<<<dim3((th + 31) / 32, (tw + 31) / 32), bt, 0, st>>>(scratch, th, tw, tmp);
-    prefilter(tmp, scratch, tw, th);
-    Mat9 Hi;
-    invert33(useZ ? matZ : M, Hi.m);
-    spline_warp_kernel<<<grid2d(ow, oh, b2), b2, 0, st>>>(tmp, tw, th, Hi, d_out, ow, oh);
-    ctx->launches += 4;
-    if (useZ) {
-        Mat9 Ht;
-        invert33(M, Ht.m);
-        warp_mask_kernel<<<grid2d(ow, oh, b2), b2, 0, st>>>(d_out, ow, oh, Ht, w, h);
-        ctx->launches++;
-    }
-    CK(cudaGetLastError());
-    return S2PB_OK;
-}
-
-// The part of `homography im -h "..." out w h` (3rdparty/homography/main.cpp:65-177) between reading and writing: needed
-// region of the host image `src`, upload of that region only, crop compensation of H, warp into the DEVICE image d_out.
-// Asynchronous on `st`; its scratch comes from the caller's lease.
-static int warp_host_to_device(s2pb_ctx *ctx, ScratchLease &L, cudaStream_t st, const float *src, int sw, int sh, const double H[9],
-                               float *d_out, int dw, int dh)
-{
-    // needed ROI of the source: pre-image of the output corners, integer bounding box, clipped (main.cpp:29-55,94-127)
-    double Hi[9];
-    invert_homography(H, Hi);
-    const double cx[4] = {0, (double)dw, (double)dw, 0}, cy[4] = {0, 0, (double)dh, (double)dh};
-    double px[4], py[4];
-    for (int k = 0; k < 4; k++) {
-        double z = Hi[6] * cx[k] + Hi[7] * cy[k] + Hi[8];
-        px[k] = (Hi[0] * cx[k] + Hi[1] * cy[k] + Hi[2]) / z;
-        py[k] = (Hi[3] * cx[k] + Hi[4] * cy[k] + Hi[5]) / z;
-    }
-    double mnx = px[0], mxx = px[0], mny = py[0], mxy = py[0];
-    for (int k = 1; k < 4; k++) { if (px[k] < mnx) mnx = px[k]; if (px[k] > mxx) mxx = px[k]; if (py[k] < mny) mny = py[k]; if (py[k] > mxy) mxy = py[k]; }
-    if (!(std::isfinite(mnx) && std::isfinite(mxx) && std::isfinite(mny) && std::isfinite(mxy))) return fail(S2PB_ERR_ARG, "homography: degenerate matrix");
-    if (mnx < -1e9 || mny < -1e9 || mxx > 1e9 || mxy > 1e9) return fail(S2PB_ERR_ARG, "homography: region of interest out of range");
-    int x = (int)std::floor(mnx), y = (int)std::floor(mny), w = (int)std::ceil(mxx - x), h = (int)std::ceil(mxy - y);
-    if (x < 0) { w += x; x = 0; }
-    if (y < 0) { h += y; y = 0; }
-    if (x + w > sw) w = sw - x;
-    if (y + h > sh) h = sh - y;
-    if (w <= 0 || h <= 0) return fail(S2PB_ERR_ARG, "ERROR: empty roi");
-    const double T[9] = {1, 0, (double)x, 0, 1, (double)y, 0, 0, 1};
-    double Hc[9];
-    for (int r = 0; r < 3; r++) for (int q = 0; q < 3; q++) Hc[3 * r + q] = H[3 * r] * T[q] + H[3 * r + 1] * T[3 + q] + H[3 * r + 2] * T[6 + q];
-    float *roi = L.take<float>((size_t)w * h * 4);
-    if (!roi) return L.nomem("the warp");
-    CK(cudaMemcpy2DAsync(roi, (size_t)w * 4, src + (size_t)y * sw + x, (size_t)sw * 4, (size_t)w * 4, (size_t)h, cudaMemcpyHostToDevice, st));
-    return map_image(ctx, L, st, roi, w, h, Hc, d_out, dw, dh, true, 0);
-}
-
-// `homography im -h "..." out w h` (3rdparty/homography/main.cpp:65-177) from memory to memory
-extern "C" int s2pb_homography(s2pb_ctx *ctx, const float *src, int sw, int sh, const double H[9], float *dst, int dw, int dh)
-{
-    if (!ctx || !src || !H || !dst || sw < 1 || sh < 1 || dw < 1 || dh < 1) return fail(S2PB_ERR_ARG, "bad argument");
-    CK(cudaSetDevice(ctx->device));
-    cudaStream_t st = ctx->slots[0].stream;
-    ScratchLease L(ctx, st);
-    float *out = L.take<float>((size_t)dw * dh * 4);
-    if (!out) return L.nomem("the warp");
-    int rc = warp_host_to_device(ctx, L, st, src, sw, sh, H, out, dw, dh);
-    if (rc != S2PB_OK) return rc;
-    CK(cudaMemcpyAsync(dst, out, (size_t)dw * dh * 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    return S2PB_OK;
-}
+// ------------------------------------------------------------------ warp (warp.cu) and match
 
 // Steps 3 and 4 of a tile in one call (s2p/__init__.py:147-155 rectify_pair's two warps, :184-190 compute_disparity_map): both
 // images are warped straight into the matcher's device inputs and matched there; the rectified pair never travels through
@@ -1929,501 +1552,4 @@ extern "C" int s2pb_rectify_match(s2pb_ctx *ctx, const float *src1, int sw1, int
     if (mask) CK(cudaMemcpyAsync(mask, s.d_mask, npix, cudaMemcpyDeviceToHost, st));
     if (disp_right) CK(cudaMemcpyAsync(disp_right, s.d_dispR, npix * 4, cudaMemcpyDeviceToHost, st));
     return sync_or_timeout(ctx, st);
-}
-
-// ------------------------------------------------------------------ n-view merge (section 8f)
-
-extern "C" int s2pb_merge_n(s2pb_ctx *ctx, const float *const *inputs, const double *offsets, int n, int w, int h, int op,
-                            double threshold, float *out)
-{
-    if (!ctx || !inputs || !offsets || !out || n < 1 || w < 1 || h < 1) return fail(S2PB_ERR_ARG, "bad argument");
-    if (n > kMaxFusion) return fail(S2PB_ERR_UNSUPPORTED, "at most %d rasters can be merged", kMaxFusion);
-    const int sub_f32 = (op & S2PB_FUSE_SUB_F32) ? 1 : 0;
-    op &= ~S2PB_FUSE_SUB_F32;
-    if (op < FUSE_AVERAGE_IF_CLOSE || op >= FUSE_OP_COUNT) return fail(S2PB_ERR_ARG, "unknown averaging operator %d", op);
-    CK(cudaSetDevice(ctx->device));
-    const size_t npix = (size_t)w * h;
-    cudaStream_t st = ctx->slots[0].stream;
-    ScratchLease L(ctx, st);
-    float *in = L.take<float>(npix * 4 * n), *o = L.take<float>(npix * 4);
-    if (!in || !o) return L.nomem("the merge");
-    FusionParams P;
-    memset(&P, 0, sizeof P);
-    double s = 0;
-    for (int k = 0; k < n; k++) {
-        if (!inputs[k]) return fail(S2PB_ERR_ARG, "null raster %d", k);
-        P.in[k] = in + npix * k;
-        CK(cudaMemcpyAsync((void *)P.in[k], inputs[k], npix * 4, cudaMemcpyHostToDevice, st));
-        P.offset[k] = offsets[k];
-        s += offsets[k];                     // np.mean of a short list: plain left-to-right sum / n
-    }
-    P.n = n; P.op = op; P.sub_f32 = sub_f32; P.threshold = threshold; P.mean_offset = s / n; P.npix = npix; P.out = o;
-    fusion_kernel<<<(unsigned)((npix + 255) / 256), 256, 0, st>>>(P);
-    ctx->launches++;
-    CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(out, o, npix * 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    return S2PB_OK;
-}
-
-// ------------------------------------------------------------------ triangulation (section 8f)
-
-static_assert(sizeof(s2pb_rpc) == sizeof(RpcModel), "s2pb_rpc must have the layout of the reference's struct rpc");
-
-// disp_to_lonlatalt (c/disp_to_h.c:70-141) on device buffers: lonlatalt nx*ny*3 doubles, err nx*ny floats
-static int triangulate_enqueue(s2pb_ctx *ctx, cudaStream_t st, const float *d_dx, const float *d_dy, const float *d_m, int nx, int ny,
-                               const float *d_mo, int w, int h, const double ha[9], const double hb[9], const s2pb_rpc *rpca,
-                               const s2pb_rpc *rpcb, const float bbox[4], double *d_out, float *d_err)
-{
-    TriParams P;
-    memset(&P, 0, sizeof P);
-    P.dispx = d_dx; P.dispy = d_dy; P.msk = d_m; P.msk_orig = d_mo;
-    P.nx = nx; P.ny = ny; P.w = w; P.h = h;
-    invert_homography(ha, P.ha_inv);
-    invert_homography(hb, P.hb_inv);
-    memcpy(&P.rpca, rpca, sizeof(RpcModel)); memcpy(&P.rpcb, rpcb, sizeof(RpcModel));      // kernel parameters: constant bank
-    P.col_min = bbox[0]; P.col_max = bbox[1]; P.row_min = bbox[2]; P.row_max = bbox[3];
-    P.lonlatalt = d_out; P.err = d_err;
-    dim3 b2(32, 4);
-    triangulate_kernel<<<grid2d(nx, ny, b2), b2, 0, st>>>(P);
-    ctx->launches++;
-    CK(cudaGetLastError());
-    return S2PB_OK;
-}
-
-// Same argument list as the reference's ctypes entry point disp_to_lonlatalt (c/disp_to_h.c:70-76), plus the context.
-extern "C" int s2pb_disp_to_lonlatalt(s2pb_ctx *ctx, double *lonlatalt, float *err, const float *dispx, const float *dispy,
-                                      const float *msk, int nx, int ny, const float *msk_orig, int w, int h, const double ha[9],
-                                      const double hb[9], const s2pb_rpc *rpca, const s2pb_rpc *rpcb, const float bbox[4])
-{
-    if (!ctx || !lonlatalt || !err || !dispx || !dispy || !msk || !msk_orig || !ha || !hb || !rpca || !rpcb || !bbox || nx < 1 ||
-        ny < 1 || w < 1 || h < 1)
-        return fail(S2PB_ERR_ARG, "bad argument");
-    CK(cudaSetDevice(ctx->device));
-    const size_t npix = (size_t)nx * ny, nm = (size_t)w * h;
-    cudaStream_t st = ctx->slots[0].stream;
-    ScratchLease L(ctx, st);
-    float *d_dx = L.take<float>(npix * 4), *d_dy = L.take<float>(npix * 4), *d_m = L.take<float>(npix * 4), *d_mo = L.take<float>(nm * 4);
-    double *d_out = L.take<double>(npix * 24);
-    float *d_err = L.take<float>(npix * 4);
-    if (!d_dx || !d_dy || !d_m || !d_mo || !d_out || !d_err) return L.nomem("the triangulation");
-    CK(cudaMemcpyAsync(d_dx, dispx, npix * 4, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d_dy, dispy, npix * 4, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d_m, msk, npix * 4, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d_mo, msk_orig, nm * 4, cudaMemcpyHostToDevice, st));
-    int rc = triangulate_enqueue(ctx, st, d_dx, d_dy, d_m, nx, ny, d_mo, w, h, ha, hb, rpca, rpcb, bbox, d_out, d_err);
-    if (rc != S2PB_OK) return rc;
-    CK(cudaMemcpyAsync(lonlatalt, d_out, npix * 24, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(err, d_err, npix * 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    return S2PB_OK;
-}
-
-// ------------------------------------------------------------------ tri-stereo height maps (section 8f)
-
-// affine_transform(nan_to_num(z).T, H, output_shape=(w, h), order=1).T with the NaN restoration of height_map
-// (heightmap_kernels.cuh), z on the device with `zstride` doubles per pixel
-static int resample_heights_enqueue(s2pb_ctx *ctx, cudaStream_t st, const double *z, int zstride, int zw, int zh, const double H[9],
-                                    double *out, int w, int h)
-{
-    ResampleParams P;
-    memset(&P, 0, sizeof P);
-    P.z = z; P.zstride = zstride; P.zw = zw; P.zh = zh;
-    for (int k = 0; k < 6; k++) P.H[k] = H[k];
-    P.w = w; P.h = h; P.out = out;
-    const dim3 b2(32, 8);
-    heightmap_resample_kernel<<<grid2d(w, h, b2), b2, 0, st>>>(P);
-    ctx->launches++;
-    CK(cudaGetLastError());
-    return S2PB_OK;
-}
-
-// scipy.ndimage.affine_transform refuses a homogeneous matrix whose last row is not exactly (0, 0, 1)
-static bool affine_last_row(const double H[9]) { return H[6] == 0.0 && H[7] == 0.0 && H[8] == 1.0; }
-
-extern "C" int s2pb_resample_heights(s2pb_ctx *ctx, const double *z, int zw, int zh, const double H[9], double *out, int w, int h)
-{
-    if (!ctx || !z || !H || !out || zw < 1 || zh < 1 || w < 1 || h < 1) return fail(S2PB_ERR_ARG, "bad argument");
-    if (!affine_last_row(H)) return fail(S2PB_ERR_ARG, "the last row of the matrix is not (0, 0, 1)");
-    CK(cudaSetDevice(ctx->device));
-    const size_t nz = (size_t)zw * zh, npix = (size_t)w * h;
-    cudaStream_t st = ctx->slots[0].stream;
-    ScratchLease L(ctx, st);
-    double *d_z = L.take<double>(nz * 8), *d_out = L.take<double>(npix * 8);
-    if (!d_z || !d_out) return L.nomem("the height resampling");
-    CK(cudaMemcpyAsync(d_z, z, nz * 8, cudaMemcpyHostToDevice, st));
-    int rc = resample_heights_enqueue(ctx, st, d_z, 1, zw, zh, H, d_out, w, h);
-    if (rc != S2PB_OK) return rc;
-    CK(cudaMemcpyAsync(out, d_out, npix * 8, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    return S2PB_OK;
-}
-
-// s2p.triangulation.height_map (s2p/triangulation.py:346-389) with p = 1: triangulate inside the bounding box
-// float32(x-1, x+w+2, y-1, y+h+2) against mask_orig padded by one row / column of ones, keep the altitude on the device
-// and resample it onto the tile grid through H1 * T(x, y).
-extern "C" int s2pb_height_map(s2pb_ctx *ctx, double *out, const float *disp, const float *msk, int nx, int ny,
-                               const float *mask_orig, int mw, int mh, int x, int y, int w, int h, const double H1[9],
-                               const double H2[9], const double *A, const s2pb_rpc *rpc1, const s2pb_rpc *rpc2)
-{
-    if (!ctx || !out || !disp || !msk || !mask_orig || !H1 || !H2 || !rpc1 || !rpc2 || nx < 1 || ny < 1 || mw < 1 || mh < 1 ||
-        w < 1 || h < 1)
-        return fail(S2PB_ERR_ARG, "bad argument");
-    if (nx < 2 || ny < 2) return fail(S2PB_ERR_UNSUPPORTED, "a %dx%d rectified map (the reference squeezes it to 1-D)", nx, ny);
-    double Hb[9];
-    if (A) {                                        // H2 * A^-1 (s2p/triangulation.py:114-115)
-        double Ai[9];
-        invert_homography(A, Ai);
-        for (int r = 0; r < 3; r++)
-            for (int q = 0; q < 3; q++) Hb[3 * r + q] = H2[3 * r] * Ai[q] + H2[3 * r + 1] * Ai[3 + q] + H2[3 * r + 2] * Ai[6 + q];
-    } else {
-        memcpy(Hb, H2, sizeof Hb);
-    }
-    // H1 * T(x, y): the first two columns are H1's, the third H1 (x, y, 1)^T summed left to right
-    double H[9];
-    memcpy(H, H1, sizeof H);
-    for (int r = 0; r < 3; r++) H[3 * r + 2] = H1[3 * r] * x + H1[3 * r + 1] * y + H1[3 * r + 2];
-    if (!affine_last_row(H)) return fail(S2PB_ERR_ARG, "the last row of H1 * T(x, y) is not (0, 0, 1)");
-    const float bbox[4] = {(float)(x - 1), (float)(x + w + 2), (float)(y - 1), (float)(y + h + 2)};
-    CK(cudaSetDevice(ctx->device));
-    const size_t npix = (size_t)nx * ny, pw = (size_t)mw + 2, ph = (size_t)mh + 2;
-    cudaStream_t st = ctx->slots[0].stream;
-    ScratchLease L(ctx, st);
-    float *d_dx = L.take<float>(npix * 4), *d_dy = L.take<float>(npix * 4), *d_m = L.take<float>(npix * 4);
-    float *d_mo0 = L.take<float>((size_t)mw * mh * 4), *d_mo = L.take<float>(pw * ph * 4), *d_err = L.take<float>(npix * 4);
-    double *d_xyz = L.take<double>(npix * 24), *d_out = L.take<double>((size_t)w * h * 8);
-    if (!d_dx || !d_dy || !d_m || !d_mo0 || !d_mo || !d_err || !d_xyz || !d_out) return L.nomem("the height map");
-    CK(cudaMemcpyAsync(d_dx, disp, npix * 4, cudaMemcpyHostToDevice, st));
-    CK(cudaMemsetAsync(d_dy, 0, npix * 4, st));
-    CK(cudaMemcpyAsync(d_m, msk, npix * 4, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d_mo0, mask_orig, (size_t)mw * mh * 4, cudaMemcpyHostToDevice, st));
-    const dim3 b2(32, 8);
-    pad_ones_kernel<<<grid2d((int)pw, (int)ph, b2), b2, 0, st>>>(d_mo0, mw, mh, d_mo);
-    ctx->launches++;
-    int rc = triangulate_enqueue(ctx, st, d_dx, d_dy, d_m, nx, ny, d_mo, (int)pw, (int)ph, H1, Hb, rpc1, rpc2, bbox, d_xyz, d_err);
-    if (rc == S2PB_OK) rc = resample_heights_enqueue(ctx, st, d_xyz + 2, 3, nx, ny, H, d_out, w, h);
-    if (rc != S2PB_OK) return rc;
-    CK(cudaMemcpyAsync(out, d_out, (size_t)w * h * 8, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    return S2PB_OK;
-}
-
-// s2p.common.cargarse_basura (s2p/common.py:251-262) on the float32 image its tools read: 5x5 min / max and plambda in one
-// kernel, then remove_small_cc(200, 5)
-extern "C" int s2pb_cargarse_basura(s2pb_ctx *ctx, const float *in, float *out, int w, int h)
-{
-    if (!ctx || !in || !out || w < 1 || h < 1) return fail(S2PB_ERR_ARG, "bad argument");
-    if (w < 2 || h < 2) return fail(S2PB_ERR_UNSUPPORTED, "a %dx%d image: the reference's morphoop reads outside it", w, h);
-    CK(cudaSetDevice(ctx->device));
-    const size_t npix = (size_t)w * h;
-    if (npix > INT32_MAX) return fail(S2PB_ERR_UNSUPPORTED, "at most 2^31 - 1 pixels");
-    cudaStream_t st = ctx->slots[0].stream;
-    ScratchLease L(ctx, st);
-    float *a = L.take<float>(npix * 4), *m = L.take<float>(npix * 4), *b = L.take<float>(npix * 4);
-    int *lab = L.take<int>(npix * 4), *area = L.take<int>(npix * 4);
-    if (!a || !m || !b || !lab || !area) return L.nomem("cargarse_basura");
-    CK(cudaMemcpyAsync(a, in, npix * 4, cudaMemcpyHostToDevice, st));
-    const dim3 bb(kBasuraTx, kBasuraTy);
-    basura_minmax_kernel<<<grid2d(w, h, bb), bb, 0, st>>>(a, w, h, m);
-    ctx->launches++;
-    CK(cudaGetLastError());
-    int rc = launch_remove_small_cc(ctx, m, b, w, h, 200, 5.f, lab, area, st);
-    if (rc != S2PB_OK) return rc;
-    CK(cudaMemcpyAsync(out, b, npix * 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    return S2PB_OK;
-}
-
-// ------------------------------------------------------------------ 3D outlier filter of triangulation (section 8f)
-
-// count_3d_neighbors (c/disp_to_h.c:152-174) of a device cloud into a device count image
-static int pc_count_enqueue(s2pb_ctx *ctx, cudaStream_t st, const double *xyz, int nx, int ny, float r, int p, int *count)
-{
-    if (p < 0) { CK(cudaMemsetAsync(count, 0, (size_t)nx * ny * 4, st)); return S2PB_OK; }     // empty windows
-    p = std::min(p, std::max(nx, ny));                                  // a wider window is the whole image
-    const long long side = kPcTile + 2LL * p;
-    const size_t smem = (size_t)std::min<long long>(side, nx) * std::min<long long>(side, ny) * 24;    // one CTA's clipped footprint
-    int optin = 0;
-    CK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx->device));
-    const dim3 b(kPcTile, kPcTile), g = grid2d(nx, ny, b);
-    if (smem <= (size_t)optin) {
-        CK(cudaFuncSetAttribute(pc_count_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        pc_count_kernel<true><<<g, b, smem, st>>>(xyz, nx, ny, r, p, count);
-    } else {
-        pc_count_kernel<false><<<g, b, 0, st>>>(xyz, nx, ny, r, p, count);
-    }
-    ctx->launches++;
-    CK(cudaGetLastError());
-    return S2PB_OK;
-}
-
-// Same argument list as the reference's count_3d_neighbors (c/disp_to_h.c:152), plus the context.
-extern "C" int s2pb_count_3d_neighbors(s2pb_ctx *ctx, int32_t *count, const double *xyz, int nx, int ny, float r, int p)
-{
-    if (!ctx || !count || !xyz || nx < 1 || ny < 1) return fail(S2PB_ERR_ARG, "bad argument");
-    const size_t npix = (size_t)nx * ny;
-    if (npix > INT32_MAX) return fail(S2PB_ERR_UNSUPPORTED, "at most 2^31 - 1 points");
-    CK(cudaSetDevice(ctx->device));
-    cudaStream_t st = ctx->slots[0].stream;
-    ScratchLease L(ctx, st);
-    double *d_xyz = L.take<double>(npix * 24);
-    int *d_count = L.take<int>(npix * 4);
-    if (!d_xyz || !d_count) return L.nomem("the point cloud");
-    CK(cudaMemcpyAsync(d_xyz, xyz, npix * 24, cudaMemcpyHostToDevice, st));
-    int rc = pc_count_enqueue(ctx, st, d_xyz, nx, ny, r, p, d_count);
-    if (rc != S2PB_OK) return rc;
-    CK(cudaMemcpyAsync(count, d_count, npix * 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    return S2PB_OK;
-}
-
-// Same argument list as the reference's remove_isolated_3d_points (c/disp_to_h.c:177-184), plus the context; in place on
-// the host cloud.  Rejection by count, then the closure of the reference's "mercy" sweeps as connected components
-// (pointcloud_kernels.cuh): label, link, flatten, mark the saved components, NaN the rest.
-extern "C" int s2pb_remove_isolated_3d_points(s2pb_ctx *ctx, double *xyz, int nx, int ny, float r, int p, int n, int q)
-{
-    if (!ctx || !xyz || nx < 1 || ny < 1) return fail(S2PB_ERR_ARG, "bad argument");
-    const size_t npix = (size_t)nx * ny;
-    if (npix > INT32_MAX) return fail(S2PB_ERR_UNSUPPORTED, "at most 2^31 - 1 points");
-    if (n <= 0) return S2PB_OK;                                         // a count is never negative: nothing is rejected
-    CK(cudaSetDevice(ctx->device));
-    cudaStream_t st = ctx->slots[0].stream;
-    ScratchLease L(ctx, st);
-    double *d_xyz = L.take<double>(npix * 24);
-    int *d_count = L.take<int>(npix * 4), *d_lab = L.take<int>(npix * 4), *d_saved = L.take<int>(npix * 4);
-    if (!d_xyz || !d_count || !d_lab || !d_saved) return L.nomem("the point cloud");
-    CK(cudaMemcpyAsync(d_xyz, xyz, npix * 24, cudaMemcpyHostToDevice, st));
-    int rc = pc_count_enqueue(ctx, st, d_xyz, nx, ny, r, p, d_count);
-    if (rc != S2PB_OK) return rc;
-    const unsigned g1 = (unsigned)((npix + 255) / 256);
-    const dim3 b2(32, 8), g2 = grid2d(nx, ny, b2);
-    pc_label_kernel<<<g1, 256, 0, st>>>(d_count, (int)npix, n, d_lab, d_saved);
-    ctx->launches++;
-    if (q >= 0) {                                                       // q < 0: empty windows, nothing is saved
-        q = std::min(q, std::max(nx, ny));
-        pc_link_kernel<<<g2, b2, 0, st>>>(d_xyz, nx, ny, r, q, d_lab);
-        cc_flatten_kernel<<<g1, 256, 0, st>>>((int)npix, d_lab);
-        pc_mark_kernel<<<g2, b2, 0, st>>>(d_xyz, nx, ny, r, q, d_lab, d_saved);
-        ctx->launches += 3;
-    }
-    pc_reject_kernel<<<g1, 256, 0, st>>>((int)npix, d_lab, d_saved, d_xyz);
-    ctx->launches++;
-    CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(xyz, d_xyz, npix * 24, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    return S2PB_OK;
-}
-
-// ------------------------------------------------------------------ sgbm (3rdparty/sgbm, sgbm_kernels.cuh)
-
-extern "C" int s2pb_sgbm_default_params(s2pb_sgbm_params *p)
-{
-    if (!p) return fail(S2PB_ERR_ARG, "null params");
-    p->win = 3; p->P1 = 8; p->P2 = 32; p->lr_diff = 1;       // what s2p passes: s2p/block_matching.py:116-134
-    return S2PB_OK;
-}
-
-// The whole `sgbm im1 im2 disp cost dmin dmax win P1 P2 lr` run followed by create_rejection_mask, enqueued on `st`.
-// d_im1 / d_im2 / d_disp: w*h float32, d_mask: w*h uint8 or null.  Its scratch comes from the caller's lease.
-static int sgbm_enqueue(s2pb_ctx *ctx, ScratchLease &L, cudaStream_t st, const float *d_im1, const float *d_im2, int w, int h, int dmin,
-                        int dmax, const s2pb_sgbm_params *p, float *d_disp, uint8_t *d_mask)
-{
-    // sgbm.cpp:166-192: OpenCV's convention is the opposite of s2p's; the label count is rounded up to a multiple of 16
-    const int mindisp = -dmax, maxdisp = -dmin;
-    const int ND = (maxdisp - mindisp + 15) / 16 * 16;
-    SgbmGeom g;
-    g.minD = mindisp; g.D = ND;
-    const int maxD = g.minD + ND;
-    g.wp = w + std::max(-mindisp, 0) + std::max(maxdisp, 0);         // the crop trick, sgbm.cpp:204-207
-    g.h = h;
-    const int off = std::max(maxdisp, 0);
-    g.minX1 = std::max(-maxD, 0);
-    const int maxX1 = g.wp + std::min(g.minD, 0);
-    g.w1 = maxX1 - g.minX1;
-    g.minX2 = std::max(g.minX1 - maxD, 0);
-    g.w2 = std::min(maxX1 - g.minD, g.wp) - g.minX2;
-    g.SW2 = g.SH2 = p->win / 2;
-    g.P1 = p->P1 > 0 ? p->P1 : 2;                                      // stereosgbm.cpp:333-334
-    g.P2 = std::max(p->P2 > 0 ? p->P2 : 5, g.P1 + 1);
-    const int lr = p->lr_diff > 0 ? p->lr_diff : 1;
-    const int invalid = (g.minD - 1) * 16;
-
-    if ((long long)invalid < -32768 || (long long)maxD * 16 > 32767)
-        return fail(S2PB_ERR_UNSUPPORTED, "disparity range [%d,%d] does not fit the reference's int16 disparities (x16)", dmin, dmax);
-    // every L is in [C - P2, C]: min L + P2 must stay an int16, and 8 L of a zero-cost pixel must not reach -32768
-    // (DESIGN.md section 3.5)
-    if ((long long)p->win * p->win * kSgbmPixMax + 2LL * g.P2 > kSgbmMaxCost || g.P2 > 4096)
-        return fail(S2PB_ERR_UNSUPPORTED, "win %d with P2 %d can overflow the reference's int16 path costs "
-                    "(needs win^2 * %d + 2 * P2 <= 32767 and P2 <= 4096)", p->win, g.P2, kSgbmPixMax);
-    const bool any = g.w1 > 0;                                         // else every pixel is invalid (stereosgbm.cpp:347-351)
-    size_t pix_smem = 4 * (size_t)g.wp + 4 * (size_t)std::max(g.w2, 0);
-    const size_t path_smem = 4 * 2 * ((size_t)ND + 2) * sizeof(int);
-    if (any) {
-        if (g.w1 <= g.SW2) return fail(S2PB_ERR_UNSUPPORTED, "a %d px wide cost volume is narrower than the half window %d", g.w1, g.SW2);
-        // bytes calcPixelCostBT reads around its row buffer: at most 4 * width before it (disp2ptr, disp2cost, zero while
-        // the costs are computed) and below 16 * width after it (its own never-written tail)
-        const long long jmin = (long long)g.wp - maxX1 + g.minD, jmax = (long long)g.wp - 1 - g.minX1 + maxD - 1;
-        if (jmin - g.minX2 < -4LL * g.wp || 2LL * g.w2 + 3LL * g.wp + jmax >= 16LL * g.wp)
-            return fail(S2PB_ERR_UNSUPPORTED, "disparity range [%d,%d] reads outside the reference's row buffers", dmin, dmax);
-        if (pix_smem > 227 * 1024 || path_smem > 227 * 1024)
-            return fail(S2PB_ERR_UNSUPPORTED, "a %d px wide, %d label tile needs more shared memory than an SM has", g.wp, ND);
-    }
-    const size_t npix = (size_t)w * h, ppix = (size_t)g.wp * h;
-    if (ppix > INT32_MAX) return fail(S2PB_ERR_UNSUPPORTED, "at most 2^31 - 1 padded pixels");
-    const size_t vol = any ? (size_t)h * g.w1 * ND : 0;
-
-    SgbmState *d_st = L.take<SgbmState>(sizeof(SgbmState) + 512 * 4);
-    unsigned *d_hist = (unsigned *)(d_st + 1);
-    uint8_t *q1 = L.take<uint8_t>(ppix), *q2 = L.take<uint8_t>(ppix);
-    short *pix = any ? L.take<short>(vol * 2) : nullptr, *C = any ? L.take<short>(vol * 2) : nullptr;
-    short *disp1 = L.take<short>(ppix * 2), *dmed = L.take<short>(ppix * 2);
-    unsigned long long *d2key = L.take<unsigned long long>(ppix * 8);
-    int *lab = L.take<int>(ppix * 4), *area = L.take<int>(ppix * 4);
-    if (!d_st || !q1 || !q2 || (any && (!pix || !C)) || !disp1 || !dmed || !d2key || !lab || !area) return L.nomem("the sgbm volumes");
-
-    // qauto thresholds: four radix digits of both order statistics
-    CK(cudaMemsetAsync(d_st, 0, sizeof(SgbmState) + 512 * 4, st));
-    const int hblocks = (int)std::min<size_t>((npix + 255) / 256, (size_t)ctx->sm_count * 4);
-    for (int digit = 3; digit >= 0; digit--) {
-        sgbm_hist_kernel<<<hblocks, 256, 0, st>>>(d_im1, (int)npix, digit, d_st, d_hist);
-        sgbm_select_kernel<<<1, 32, 0, st>>>(digit, d_st, d_hist);
-        ctx->launches += 2;
-    }
-    sgbm_quantize_kernel<<<dim3((g.wp + 255) / 256, h), 256, 0, st>>>(d_im1, d_im2, w, h, off, g.wp, d_st, q1, q2);
-    sgbm_fill_kernel<<<std::max(1, (int)std::min<size_t>((ppix + 255) / 256, 4096)), 256, 0, st>>>(disp1, ppix, (short)invalid);
-    ctx->launches += 2;
-    if (any) {
-        CK(cudaFuncSetAttribute(sgbm_pixcost_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pix_smem));
-        CK(cudaFuncSetAttribute(sgbm_path_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)path_smem));
-        sgbm_pixcost_kernel<<<h, 256, pix_smem, st>>>(q1, q2, g, pix);
-        const size_t rowel = (size_t)g.w1 * ND;
-        sgbm_window_kernel<<<dim3((unsigned)std::min<size_t>((rowel + 255) / 256, 1024), h), 256, 0, st>>>(pix, g, C);
-        short *S = pix;                                                  // the pixel costs are dead once C is formed
-        CK(cudaMemsetAsync(S, 0, vol * 2, st));
-        ctx->launches += 2;
-        // pass 1 (top-down: predecessors left, up-left, up, up-right) and pass 2 (bottom-up, the mirrored four)
-        static const int steps[8][2] = {{1, 0}, {1, 1}, {0, 1}, {-1, 1}, {-1, 0}, {1, -1}, {0, -1}, {-1, -1}};
-        for (auto &s : steps) {
-            const int nlines = s[1] == 0 ? h : s[0] == 0 ? g.w1 : g.w1 + h - 1;
-            sgbm_path_kernel<<<(nlines + 3) / 4, 128, path_smem, st>>>(C, g, s[0], s[1], S);
-            ctx->launches++;
-        }
-        CK(cudaMemsetAsync(d2key, 0xff, ppix * 8, st));
-        const size_t nw = (size_t)g.w1 * h;
-        sgbm_wta_kernel<<<(unsigned)((nw + 7) / 8), 256, 0, st>>>(S, g, disp1, d2key);
-        sgbm_lr_kernel<<<dim3((g.w1 + 255) / 256, h), 256, 0, st>>>(disp1, d2key, g, lr);
-        ctx->launches += 2;
-    }
-    const dim3 b2(32, 8);
-    const unsigned g1 = (unsigned)((ppix + 255) / 256);
-    sgbm_median_kernel<<<grid2d(g.wp, h, b2), b2, 0, st>>>(disp1, g.wp, h, dmed);
-    sgbm_speckle_init_kernel<<<g1, 256, 0, st>>>(dmed, (int)ppix, invalid, lab, area);
-    sgbm_speckle_link_kernel<<<grid2d(g.wp, h, b2), b2, 0, st>>>(dmed, g.wp, h, invalid, lab);
-    cc_flatten_kernel<<<g1, 256, 0, st>>>((int)ppix, lab);
-    cc_area_kernel<<<g1, 256, 0, st>>>((int)ppix, lab, area);
-    sgbm_output_kernel<<<grid2d(w, h, b2), b2, 0, st>>>(dmed, lab, area, g.wp, off, w, h, invalid, d_st, d_disp);
-    ctx->launches += 6;
-    if (d_mask) { rejection_mask_kernel<<<grid2d(w, h, b2), b2, 0, st>>>(d_disp, d_im1, d_im2, w, h, d_mask); ctx->launches++; }
-    CK(cudaGetLastError());
-    return S2PB_OK;
-}
-
-// `sgbm im1 im2 disp cost dmin dmax win P1 P2 lr` + create_rejection_mask from host buffers (pageable or page-locked)
-extern "C" int s2pb_sgbm(s2pb_ctx *ctx, const float *im1, const float *im2, int w, int h, int dmin, int dmax,
-                         const s2pb_sgbm_params *p, float *disp, uint8_t *mask)
-{
-    if (!ctx || !im1 || !im2 || !p || !disp || w < 1 || h < 1) return fail(S2PB_ERR_ARG, "bad argument");
-    if (dmin >= dmax) return fail(S2PB_ERR_ARG, "mindisp(%d) > maxdisp(%d)", -dmax, -dmin);     // sgbm.cpp:174-177
-    if (p->win < 1 || p->win % 2 == 0) return fail(S2PB_ERR_ARG, "SADWindowSize must be odd and positive (got %d)", p->win);
-    const size_t npix = (size_t)w * h;
-    CK(cudaSetDevice(ctx->device));
-    cudaStream_t st = ctx->slots[0].stream;
-    ScratchLease L(ctx, st);
-    float *d_im1 = L.take<float>(npix * 4), *d_im2 = L.take<float>(npix * 4), *d_disp = L.take<float>(npix * 4);
-    uint8_t *d_mask = mask ? L.take<uint8_t>(npix) : nullptr;
-    if (!d_im1 || !d_im2 || !d_disp || (mask && !d_mask)) return L.nomem("the sgbm images");
-    CK(cudaMemcpyAsync(d_im1, im1, npix * 4, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d_im2, im2, npix * 4, cudaMemcpyHostToDevice, st));
-    int rc = sgbm_enqueue(ctx, L, st, d_im1, d_im2, w, h, dmin, dmax, p, d_disp, d_mask);
-    if (rc != S2PB_OK) return rc;
-    CK(cudaMemcpyAsync(disp, d_disp, npix * 4, cudaMemcpyDeviceToHost, st));
-    if (mask) CK(cudaMemcpyAsync(mask, d_mask, npix, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    return S2PB_OK;
-}
-
-// ------------------------------------------------------------------ DSM rasterisation (plys_to_dsm)
-
-// bits of the largest key, ncells: the radix sort looks at no more
-static int key_bits(uint32_t ncells) { int b = 1; while (b < 32 && (ncells >> b)) b++; return b; }
-
-// plyflatten with radius 0 and no sigma (dsm_kernels.cuh): upload the clouds' records back to back, key each point by its
-// cell, stable radix sort by key, fold each cell's run in point order into the NaN-filled raster.
-extern "C" int s2pb_plyflatten(s2pb_ctx *ctx, int nclouds, const void *const *records, const int64_t *npoints, int record_bytes,
-                               const s2pb_ply_column *cols, int ncols, double xoff, double yoff, double resolution, int xsize,
-                               int ysize, float *raster)
-{
-    if (!ctx || nclouds < 0 || (nclouds > 0 && (!records || !npoints)) || !cols || !raster || record_bytes < 1 || ncols < 3 ||
-        !(resolution > 0.0) || !std::isfinite(resolution) || xsize < 1 || ysize < 1)
-        return fail(S2PB_ERR_ARG, "bad argument");
-    if (ncols > kDsmMaxCols) return fail(S2PB_ERR_UNSUPPORTED, "at most %d PLY properties, got %d", kDsmMaxCols, ncols);
-    DsmParams P;
-    memset(&P, 0, sizeof P);
-    for (int c = 0; c < ncols; c++) {
-        const int size = cols[c].type == S2PB_PLY_F64 ? 8 : cols[c].type == S2PB_PLY_F32 ? 4 : cols[c].type == S2PB_PLY_U8 ? 1 : 0;
-        if (!size) return fail(S2PB_ERR_ARG, "column %d: unknown type %d", c, cols[c].type);
-        if (cols[c].offset < 0 || cols[c].offset + size > record_bytes)
-            return fail(S2PB_ERR_ARG, "column %d: bytes [%d, %d) outside a %d-byte record", c, cols[c].offset, cols[c].offset + size,
-                        record_bytes);
-        P.off[c] = cols[c].offset;
-        P.type[c] = cols[c].type;
-    }
-    int64_t n = 0;
-    for (int k = 0; k < nclouds; k++) {
-        if (npoints[k] < 0 || (npoints[k] > 0 && !records[k])) return fail(S2PB_ERR_ARG, "cloud %d: bad records or count", k);
-        n += npoints[k];
-        if (n > INT32_MAX) return fail(S2PB_ERR_UNSUPPORTED, "at most 2^31 - 1 points in all");
-    }
-    const uint64_t ncells = (uint64_t)xsize * (uint64_t)ysize;
-    if (ncells >= 0xFFFFFFFFull) return fail(S2PB_ERR_UNSUPPORTED, "a %dx%d raster: at most 2^32 - 2 cells", xsize, ysize);
-    const int nch = ncols - 2;
-    P.n = (uint32_t)n; P.rb = record_bytes; P.ncols = ncols;
-    P.xoff = xoff; P.yoff = yoff; P.r = resolution; P.xsize = xsize; P.ysize = ysize; P.ncells = (uint32_t)ncells;
-    CK(cudaSetDevice(ctx->device));
-    cudaStream_t st = ctx->slots[0].stream;
-    ScratchLease L(ctx, st);
-    const size_t out_bytes = (size_t)ncells * nch * 4;
-    float *d_raster = L.take<float>(out_bytes);
-    if (!d_raster) return L.nomem("the DSM raster");
-    dsm_fill_nan_kernel<<<(unsigned)std::min<size_t>((out_bytes / 4 + 255) / 256, 65536), 256, 0, st>>>(d_raster, out_bytes / 4);
-    ctx->launches++;
-    CK(cudaGetLastError());
-    if (n > 0) {
-        const int bits = key_bits(P.ncells);
-        size_t sort_bytes = 0;
-        CK(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (const uint32_t *)nullptr, (uint32_t *)nullptr,
-                                           (const uint32_t *)nullptr, (uint32_t *)nullptr, (int)n, 0, bits, st));
-        uint8_t *d_rec = L.take<uint8_t>((size_t)n * record_bytes);
-        uint32_t *key = L.take<uint32_t>((size_t)n * 4), *idx = L.take<uint32_t>((size_t)n * 4);
-        uint32_t *key_s = L.take<uint32_t>((size_t)n * 4), *idx_s = L.take<uint32_t>((size_t)n * 4);
-        void *sort_tmp = L.take<void>(sort_bytes);
-        if (!d_rec || !key || !idx || !key_s || !idx_s || !sort_tmp) return L.nomem("the DSM rasterisation");
-        size_t at = 0;
-        for (int k = 0; k < nclouds; k++) {               // host (pageable or page-locked) or device records, by unified addressing
-            const size_t bytes = (size_t)npoints[k] * record_bytes;
-            if (bytes) CK(cudaMemcpyAsync(d_rec + at, records[k], bytes, cudaMemcpyDefault, st));
-            at += bytes;
-        }
-        P.rec = d_rec;
-        const unsigned g = (unsigned)((n + 255) / 256);
-        dsm_key_kernel<<<g, 256, 0, st>>>(P, key, idx);
-        CK(cudaGetLastError());
-        CK(cub::DeviceRadixSort::SortPairs(sort_tmp, sort_bytes, key, key_s, idx, idx_s, (int)n, 0, bits, st));
-        dsm_fold_kernel<<<g, 256, 0, st>>>(P, key_s, idx_s, d_raster);
-        ctx->launches += 3;
-        CK(cudaGetLastError());
-    }
-    CK(cudaMemcpyAsync(raster, d_raster, out_bytes, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    return S2PB_OK;
 }

@@ -10,7 +10,9 @@
 //   post-filters      -> 3x3 median (replicated border), speckle filter by union-find, crop and -d/16
 // Coordinates: X = column of the padded images (width `wp`), x = X - minX1 = column of the cost volume (width `w1`).
 #pragma once
-#include "multiscale_kernels.cuh"
+#include <cuda_runtime.h>
+#include <stdint.h>
+#include "union_find.cuh"
 
 namespace s2pb {
 
