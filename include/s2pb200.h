@@ -20,6 +20,8 @@
  *                        parallel.launch_calls (s2p/__init__.py:166-196,586-591)
  *   s2pb_cargarse_basura() the morphoop / plambda / remove_small_cc subprocesses of
  *                        common.cargarse_basura (s2p/common.py:251-262)
+ *   s2pb_disp_to_xyz()   s2p.triangulation.disp_to_xyz with a WGS84 / UTM output CRS: the lib/disp_to_h.so call and the
+ *                        pyproj change of coordinates (s2p/triangulation.py:85-162)
  *   s2pb_plyflatten()    plyflatten_from_plyfiles_list with radius 0 (the external plyflatten package) in plys_to_dsm
  *                        (s2p/__init__.py:432-476)
  *   s2pb_sgbm()          the `sgbm` subprocess (OpenCV 2's StereoSGBM, 3rdparty/sgbm) + create_rejection_mask
@@ -211,6 +213,21 @@ int s2pb_disp_to_lonlatalt(s2pb_ctx *ctx, double *lonlatalt, float *err, const f
                            const float *msk, int nx, int ny, const float *msk_orig, int w, int h,
                            const double ha[9], const double hb[9], const s2pb_rpc *rpca, const s2pb_rpc *rpcb,
                            const float orig_img_bounding_box[4]);
+/* s2p.triangulation.disp_to_xyz (s2p/triangulation.py:85-162) for an output CRS of WGS84 / UTM (EPSG 32601-32660 north,
+ * 32701-32760 south) in one call: s2pb_disp_to_lonlatalt's argument list, then the UTM zone (1..60, or 0: the output is
+ * lon, lat, alt as they are) and south (non-zero: false northing 10 000 000 m).  The cloud is triangulated and projected as
+ * s2pb_lonlat_to_utm projects it on the device; xyz (nx*ny*3 float64) and err (nx*ny float32) come back.
+ * S2PB_ERR_ARG: a null pointer, a size below 1, a zone outside 0..60. */
+int s2pb_disp_to_xyz(s2pb_ctx *ctx, double *xyz, float *err, const float *dispx, const float *dispy, const float *msk, int nx,
+                     int ny, const float *msk_orig, int w, int h, const double ha[9], const double hb[9], const s2pb_rpc *rpca,
+                     const s2pb_rpc *rpcb, const float orig_img_bounding_box[4], int zone, int south);
+/* EPSG:4979 -> UTM zone `zone` (1..60) of WGS84, north (EPSG 326zz) or south (south != 0, EPSG 327zz), for n points of
+ * three float64 (lon and lat in degrees, alt), host buffers (xyz may be lonlatalt).  The exact transverse Mercator that PROJ
+ * runs for +proj=utm (Poder / Engsager, Krueger's series to order n^6; Karney 2011), k0 = 0.9996, central meridian
+ * 6 zone - 183, false easting 500 000 m.  The altitude passes through.  A point with a NaN coordinate becomes NaN in all
+ * three; a point outside the projection's domain (|lat| > 90, or too far from the central meridian) +inf in all three.
+ * Within 1e-6 m of the exact map.  S2PB_ERR_ARG: a null pointer with n > 0, n < 0, a zone outside 1..60. */
+int s2pb_lonlat_to_utm(s2pb_ctx *ctx, double *xyz, const double *lonlatalt, int64_t n, int zone, int south);
 
 /* ---- tri-stereo height maps (s2p/__init__.py disparity_to_height and heights_fusion) ---- */
 /* s2p.triangulation.height_map (s2p/triangulation.py:346-389) in one call.  disp, msk: the rectified disparity and mask,

@@ -52,6 +52,31 @@ extern "C" int s2pb_disp_to_lonlatalt(s2pb_ctx *ctx, double *lonlatalt, float *e
     return L.finish();
 }
 
+// s2p.triangulation.disp_to_xyz (s2p/triangulation.py:85-162) with a UTM (or no) output CRS: disp_to_lonlatalt, then the
+// projection (projection.cu) in place on the device cloud; only the projected cloud and the error come back.
+extern "C" int s2pb_disp_to_xyz(s2pb_ctx *ctx, double *xyz, float *err, const float *dispx, const float *dispy, const float *msk,
+                                int nx, int ny, const float *msk_orig, int w, int h, const double ha[9], const double hb[9],
+                                const s2pb_rpc *rpca, const s2pb_rpc *rpcb, const float bbox[4], int zone, int south)
+{
+    if (!ctx || !xyz || !err || !dispx || !dispy || !msk || !msk_orig || !ha || !hb || !rpca || !rpcb || !bbox || nx < 1 ||
+        ny < 1 || w < 1 || h < 1)
+        return fail(S2PB_ERR_ARG, "bad argument");
+    if (zone < 0 || zone > 60) return fail(S2PB_ERR_ARG, "UTM zone %d (1 to 60, or 0 for lon, lat, alt)", zone);
+    const size_t npix = (size_t)nx * ny, nm = (size_t)w * h;
+    HostCall L(ctx, "the triangulation");
+    float *d_dx = L.upload(dispx, npix * 4), *d_dy = L.upload(dispy, npix * 4), *d_m = L.upload(msk, npix * 4);
+    float *d_mo = L.upload(msk_orig, nm * 4);
+    double *d_out = L.take<double>(npix * 24);
+    float *d_err = L.take<float>(npix * 4);
+    if (int rc = L.error()) return rc;
+    int rc = triangulate_enqueue(ctx, L.st, d_dx, d_dy, d_m, nx, ny, d_mo, w, h, ha, hb, rpca, rpcb, bbox, d_out, d_err);
+    if (rc == S2PB_OK && zone) rc = launch_utm_project(ctx, L.st, zone, south != 0, d_out, d_out, npix);
+    if (rc != S2PB_OK) return rc;
+    L.download(xyz, d_out, npix * 24);
+    L.download(err, d_err, npix * 4);
+    return L.finish();
+}
+
 // ------------------------------------------------------------------ tri-stereo height maps (section 8f)
 
 // affine_transform(nan_to_num(z).T, H, output_shape=(w, h), order=1).T with the NaN restoration of height_map

@@ -1,7 +1,7 @@
 // host.h -- host-side state and helpers shared by the translation units of the C ABI (not a public header).
 //
-// s2pb200.cu owns the context, the slots, the matcher and the matcher's stage entry points; warp.cu, geometry.cu, sgbm.cu and
-// raster.cu each hold one family of entry points.  Every kernel header that defines a non-template kernel is included by one of
+// s2pb200.cu owns the context, the slots, the matcher and the matcher's stage entry points; warp.cu, geometry.cu, projection.cu,
+// sgbm.cu and raster.cu each hold one family of entry points.  Every kernel header that defines a non-template kernel is included by one of
 // those files only, so that its kernels are compiled once; the few launchers another file needs are declared at the end.
 #pragma once
 #include "../../include/s2pb200.h"
@@ -234,6 +234,8 @@ void cc_flatten(s2pb_ctx *ctx, int n, int *lab, cudaStream_t st);
 void cc_area(s2pb_ctx *ctx, int n, const int *lab, int *area, cudaStream_t st);
 void launch_rejection_mask(s2pb_ctx *ctx, const float *disp, const float *im1, const float *im2, int w, int h, uint8_t *mask,
                            cudaStream_t st);
+// projection.cu: (lon, lat, alt) -> UTM zone `zone` (1..60) of n device points, in place when d_in == d_out
+int launch_utm_project(s2pb_ctx *ctx, cudaStream_t st, int zone, bool south, const double *d_in, double *d_out, size_t n);
 // warp.cu
 void invert_homography(const double i[9], double o[9]);
 int warp_host_to_device(s2pb_ctx *ctx, ScratchLease &L, cudaStream_t st, const float *src, int sw, int sh, const double H[9],

@@ -295,6 +295,41 @@ class Engine:
                                                                float(r), operator.index(p), operator.index(n), operator.index(q)))
         return a
 
+    # ------------------------------------------------------------------ triangulation into output coordinates
+    def disp_to_xyz(self, disp, mask_rect, mask_orig, H1, H2, rpc1, rpc2, img_bbx, zone=0, south=False, dispy=None):
+        """disp_to_lonlatalt and the projection to UTM zone `zone` (1..60; 0: lon, lat, alt as they are) in one device call
+        -> (xyz (h, w, 3) float64, err (h, w) float32).  rpc1 / rpc2: ctypes structures with the layout of
+        ``triangulation.RPCStruct``; H2 already carries the pointing correction."""
+        dispx, msk, mo = _f32(disp), _f32(mask_rect), _f32(mask_orig)
+        if dispx.ndim != 2 or msk.shape != dispx.shape or mo.ndim != 2:
+            raise ValueError("disp and mask_rect must be 2-D arrays of the same shape, and mask_orig a 2-D array")
+        h, w = dispx.shape
+        dy = np.zeros((h, w), np.float32) if dispy is None else _f32(dispy)
+        if dy.shape != dispx.shape:
+            raise ValueError("dispy must have the shape of disp")
+        dp = lambda a: a.ctypes.data_as(ctypes.POINTER(ctypes.c_double))
+        Ha = np.ascontiguousarray(np.asarray(H1, np.float64).reshape(9))
+        Hb = np.ascontiguousarray(np.asarray(H2, np.float64).reshape(9))
+        bb = np.ascontiguousarray(np.asarray(img_bbx, np.float32).reshape(4))
+        xyz = np.empty((h, w, 3), np.float64)
+        err = np.empty((h, w), np.float32)
+        _lib.check(self._L.s2pb_disp_to_xyz(self._ctx, dp(xyz), _fp(err), _fp(dispx), _fp(dy), _fp(msk), w, h, _fp(mo),
+                                            mo.shape[1], mo.shape[0], dp(Ha), dp(Hb),
+                                            ctypes.cast(ctypes.pointer(rpc1), ctypes.c_void_p),
+                                            ctypes.cast(ctypes.pointer(rpc2), ctypes.c_void_p), _fp(bb), int(zone), int(bool(south))))
+        return xyz, err
+
+    def lonlat_to_utm(self, lonlatalt, zone, south=False):
+        """(..., 3) float64 (lon, lat in degrees, alt) -> (..., 3) float64 (easting, northing, alt) in UTM zone `zone` (1..60)
+        of WGS84, north or south (EPSG 326zz / 327zz).  NaN in any coordinate gives NaN in all three."""
+        a = np.ascontiguousarray(lonlatalt, np.float64)
+        if a.ndim < 1 or a.shape[-1] != 3:
+            raise ValueError("expecting points of three coordinates, got shape %s" % (a.shape,))
+        out = np.empty_like(a)
+        dp = lambda v: v.ctypes.data_as(ctypes.POINTER(ctypes.c_double))
+        _lib.check(self._L.s2pb_lonlat_to_utm(self._ctx, dp(out), dp(a), a.size // 3, int(zone), int(bool(south))))
+        return out
+
     # ------------------------------------------------------------------ DSM rasterisation
     def plyflatten(self, clouds, record_bytes, columns, xoff, yoff, resolution, xsize, ysize):
         """plyflatten with radius 0 and no sigma on the roi (xoff, yoff, xsize, ysize) -> (ysize, xsize, len(columns) - 2)

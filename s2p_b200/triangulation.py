@@ -9,6 +9,10 @@ library handle of an importable ``s2p.triangulation`` for an adapter that forwar
 The 3D outlier filter of the same library, ``count_3d_neighbors`` and ``remove_isolated_3d_points`` (c/disp_to_h.c:143-230),
 which ``filter_xyz`` runs on the cloud of a tile (s2p/triangulation.py:275-343), goes through the adapter too.
 
+``disp_to_xyz`` (s2p/triangulation.py:85-162) triangulates and projects the cloud to its output CRS in one device call
+(``s2pb_disp_to_xyz``) when that CRS is WGS84 or one of its UTM zones (``projection``); ``install()`` replaces the reference's
+function with it.
+
 ``height_map`` (s2p/triangulation.py:346-389), the tri-stereo step that triangulates a pair and resamples the altitude onto the
 tile grid, runs as one device call (``s2pb_height_map``); ``install()`` replaces the reference's function with it.
 """
@@ -17,7 +21,7 @@ from ctypes import c_double
 
 import numpy as np
 
-from . import _lib
+from . import _lib, projection
 from .engine import get_engine
 
 
@@ -73,6 +77,22 @@ def disp_to_lonlatalt(disp, mask_rect, mask_orig, H1, H2, rpc1, rpc2, img_bbx, d
                                         dp(Ha), dp(Hb), ctypes.cast(ctypes.pointer(rpc1), ctypes.c_void_p),
                                         ctypes.cast(ctypes.pointer(rpc2), ctypes.c_void_p), fp(bb)))
     return out, err
+
+
+def disp_to_xyz(rpc1, rpc2, H1, H2, disp, mask_rect, img_bbx, mask_orig, A=None, out_crs=None, engine=None):
+    """s2p.triangulation.disp_to_xyz (s2p/triangulation.py:85-162): -> (xyz (h, w, 3) float64 in the coordinates of
+    out_crs, err (h, w) float32).  rpc1 / rpc2 are wrapped as the reference wraps them (``RPCStruct(rpc)``); ctypes
+    structures pass as they are.  No out_crs, EPSG 4979 / 4326 and the UTM zones of WGS84 run on the device in one call;
+    any other out_crs is triangulated on the device and projected by the reference's pyproj code (``projection``)."""
+    r1, r2 = _rpc_struct(rpc1), _rpc_struct(rpc2)
+    if A is not None:                                       # pointing correction (s2p/triangulation.py:114-115)
+        H2 = np.dot(H2, np.linalg.inv(A))
+    eng = engine or get_engine()
+    target = projection.utm_target(out_crs)
+    if target is None:
+        lla, err = disp_to_lonlatalt(disp, mask_rect, mask_orig, H1, H2, r1, r2, img_bbx, engine=eng)
+        return projection.pyproj_original(lla, out_crs), err
+    return eng.disp_to_xyz(disp, mask_rect, mask_orig, H1, H2, r1, r2, img_bbx, *target)
 
 
 def height_map(x, y, w, h, rpc1, rpc2, H1, H2, disp, mask, mask_orig, A=None, engine=None):
@@ -149,6 +169,10 @@ def install():
     import s2p.triangulation as original
     if not isinstance(original.lib, _LibAdapter):
         original.lib = _LibAdapter(original.lib)
+    if hasattr(original, "disp_to_xyz"):
+        if not hasattr(original, "_s2pb_original_disp_to_xyz"):
+            original._s2pb_original_disp_to_xyz = original.disp_to_xyz
+        original.disp_to_xyz = disp_to_xyz
     if hasattr(original, "height_map"):
         if not hasattr(original, "_s2pb_original_height_map"):
             original._s2pb_original_height_map = original.height_map
