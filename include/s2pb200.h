@@ -22,6 +22,9 @@
  *                        common.cargarse_basura (s2p/common.py:251-262)
  *   s2pb_disp_to_xyz()   s2p.triangulation.disp_to_xyz with a WGS84 / UTM output CRS: the lib/disp_to_h.so call and the
  *                        pyproj change of coordinates (s2p/triangulation.py:85-162)
+ *   s2pb_height_map_to_xyz() s2p.triangulation.height_map_to_xyz with a WGS84 / UTM output CRS: rpcm's localisation
+ *                        of every pixel of the merged height map and the pyproj change of coordinates
+ *                        (s2p/triangulation.py:165-217)
  *   s2pb_plyflatten()    plyflatten_from_plyfiles_list with radius 0 (the external plyflatten package) in plys_to_dsm
  *                        (s2p/__init__.py:432-476)
  *   s2pb_sgbm()          the `sgbm` subprocess (OpenCV 2's StereoSGBM, 3rdparty/sgbm) + create_rejection_mask
@@ -253,6 +256,18 @@ int s2pb_resample_heights(s2pb_ctx *ctx, const double *z, int zw, int zh, const 
  * threshold 5 (components of area <= 200 become NaN).  Bit for bit the output of the reference's six commands.
  * S2PB_ERR_UNSUPPORTED: w or h below 2 (the reference's morphoop reads outside the image). */
 int s2pb_cargarse_basura(s2pb_ctx *ctx, const float *in, float *out, int w, int h);
+/* s2p.triangulation.height_map_to_xyz (s2p/triangulation.py:165-217), which heights_to_ply runs on the merged height map,
+ * for an output CRS of WGS84 / UTM in one call.  heights: w*h float64, row-major (a float32 map converts exactly); rpc: the
+ * camera of the reference image; (off_x, off_y): where the map's origin lies in that image.  Pixel (i, j) with height z
+ * becomes the ground point of image pixel (j + off_x, i + off_y) at height z (rpc_localization, c/rpc.c:469: the direct
+ * polynomials when the model has them, the iteration of c/rpc.c:378-411 otherwise), then UTM zone `zone` (1..60; 0: lon,
+ * lat, alt as they are) north or south (south != 0) as s2pb_lonlat_to_utm projects it; xyz (w*h*3 float64) comes back.
+ * The third coordinate is z bit for bit.  A NaN height gives NaN in all three (the reference leaves lon and lat undefined
+ * there); an iteration whose residual turns NaN stops, as the reference's does, with a NaN lon and lat.
+ * S2PB_ERR_ARG: a null pointer, a size below 1, a zone outside 0..60, or pixels whose iteration did not meet the
+ * reference's stopping test within 1000 steps (the reference would not return; the message gives their number). */
+int s2pb_height_map_to_xyz(s2pb_ctx *ctx, double *xyz, const double *heights, int w, int h, const s2pb_rpc *rpc, double off_x,
+                           double off_y, int zone, int south);
 
 /* The 3D outlier filter of s2p.triangulation.filter_xyz (s2p/triangulation.py:275-343): same argument lists as
  * lib/disp_to_h.so's count_3d_neighbors and remove_isolated_3d_points (c/disp_to_h.c:152-230), plus the context.

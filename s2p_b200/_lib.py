@@ -79,6 +79,8 @@ _SIGNATURES = {
     "s2pb_disp_to_xyz": (c_int, [c_void_p, POINTER(c_double), _f, _f, _f, _f, c_int, c_int, _f, c_int, c_int,
                                  POINTER(c_double), POINTER(c_double), c_void_p, c_void_p, _f, c_int, c_int]),
     "s2pb_lonlat_to_utm": (c_int, [c_void_p, POINTER(c_double), POINTER(c_double), c_int64, c_int, c_int]),
+    "s2pb_height_map_to_xyz": (c_int, [c_void_p, POINTER(c_double), POINTER(c_double), c_int, c_int, c_void_p, c_double, c_double,
+                                       c_int, c_int]),
     "s2pb_height_map": (c_int, [c_void_p, POINTER(c_double), _f, _f, c_int, c_int, _f, c_int, c_int, c_int, c_int, c_int, c_int,
                                 POINTER(c_double), POINTER(c_double), POINTER(c_double), c_void_p, c_void_p]),
     "s2pb_resample_heights": (c_int, [c_void_p, POINTER(c_double), c_int, c_int, POINTER(c_double), POINTER(c_double), c_int, c_int]),

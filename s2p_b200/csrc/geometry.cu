@@ -77,6 +77,38 @@ extern "C" int s2pb_disp_to_xyz(s2pb_ctx *ctx, double *xyz, float *err, const fl
     return L.finish();
 }
 
+// s2p.triangulation.height_map_to_xyz (s2p/triangulation.py:165-217) with a UTM (or no) output CRS: every pixel of the height
+// map localised by the camera, then the projection (projection.cu) in place on the device cloud.
+extern "C" int s2pb_height_map_to_xyz(s2pb_ctx *ctx, double *xyz, const double *heights, int w, int h, const s2pb_rpc *rpc,
+                                      double off_x, double off_y, int zone, int south)
+{
+    if (!ctx || !xyz || !heights || !rpc || w < 1 || h < 1) return fail(S2PB_ERR_ARG, "bad argument");
+    if (zone < 0 || zone > 60) return fail(S2PB_ERR_ARG, "UTM zone %d (1 to 60, or 0 for lon, lat, alt)", zone);
+    const size_t npix = (size_t)w * h;
+    HostCall L(ctx, "the localisation");
+    double *d_z = L.upload(heights, npix * 8), *d_out = L.take<double>(npix * 24);
+    int *d_capped = L.take<int>(4);
+    if (int rc = L.error()) return rc;
+    CK(cudaMemsetAsync(d_capped, 0, 4, L.st));
+    HeightMapParams P;
+    memset(&P, 0, sizeof P);
+    P.heights = d_z; P.w = w; P.h = h; P.off_x = off_x; P.off_y = off_y;
+    memcpy(&P.rpc, rpc, sizeof(RpcModel));
+    P.xyz = d_out; P.capped = d_capped;
+    const dim3 b2(32, 4);
+    launch(ctx, height_map_to_xyz_kernel, grid2d(w, h, b2), b2, 0, L.st, P);
+    CK(cudaGetLastError());
+    if (zone) {
+        if (int rc = launch_utm_project(ctx, L.st, zone, south != 0, d_out, d_out, npix)) return rc;
+    }
+    int capped = 0;
+    L.download(xyz, d_out, npix * 24);
+    L.download(&capped, d_capped, 4);
+    if (int rc = L.finish()) return rc;
+    if (capped) return fail(S2PB_ERR_ARG, "the localisation of %d pixel(s) did not converge in 1000 steps", capped);
+    return S2PB_OK;
+}
+
 // ------------------------------------------------------------------ tri-stereo height maps (section 8f)
 
 // affine_transform(nan_to_num(z).T, H, output_shape=(w, h), order=1).T with the NaN restoration of height_map

@@ -88,11 +88,13 @@ __device__ __forceinline__ PixelRay make_ray(const RpcModel &a, double x, double
     if (r.direct) { zform(a.numx, r.xn, r.yn, r.zx); zform(a.denx, r.xn, r.yn, r.zdx); zform(a.numy, r.xn, r.yn, r.zy); zform(a.deny, r.xn, r.yn, r.zdy); }
     return r;
 }
-// ground point (lon, lat) of the pixel at height z
-__device__ void ray_at(const RpcModel &a, const PixelRay &r, double z, double &lon, double &lat)
+// ground point (lon, lat) of the pixel at height z.  -> false when the iteration stopped at its cap of 1000 steps without
+// meeting the reference's stopping test (the reference would loop on); a NaN residual leaves the loop as in c/rpc.c.
+__device__ bool ray_at(const RpcModel &a, const PixelRay &r, double z, double &lon, double &lat)
 {
     const double w = (z - a.offset[2]) / a.scale[2];
     double ln, lt;
+    bool converged = true;
     if (r.direct) {
         ln = horner3(r.zx, w) / horner3(r.zdx, w);
         lt = horner3(r.zy, w) / horner3(r.zdy, w);
@@ -106,7 +108,8 @@ __device__ void ray_at(const RpcModel &a, const PixelRay &r, double z, double &l
         ratio_pair(a.inumx, a.idenx, a.inumy, a.ideny, ln, lt, w, x0, y0);
         ratio_pair(a.inumx, a.idenx, a.inumy, a.ideny, ln + eps, lt, w, x1, y1);
         ratio_pair(a.inumx, a.idenx, a.inumy, a.ideny, ln, lt + eps, w, x2, y2);
-        for (int it = 0; it < 1000; it++) {       // (the reference loops until convergence; it takes a handful of steps)
+        int it = 0;
+        for (; it < 1000; it++) {                 // (the reference loops until convergence; it takes a handful of steps)
             const double ux = r.xn - x0, uy = r.yn - y0;
             if (!(ux * ux + uy * uy > 1e-18)) break;
             const double e1x = x1 - x0, e1y = y1 - y0, e2x = x2 - x0, e2y = y2 - y0;
@@ -118,9 +121,14 @@ __device__ void ray_at(const RpcModel &a, const PixelRay &r, double z, double &l
             ratio_pair(a.inumx, a.idenx, a.inumy, a.ideny, ln + eps, lt, w, x1, y1);
             ratio_pair(a.inumx, a.idenx, a.inumy, a.ideny, ln, lt + eps, w, x2, y2);
         }
+        if (it == 1000) {                         // at the cap: the point of the last step has not been tested yet
+            const double ux = r.xn - x0, uy = r.yn - y0;
+            converged = !(ux * ux + uy * uy > 1e-18);
+        }
     }
     lon = ln * a.iscale[0] + a.ioffset[0];
     lat = lt * a.iscale[1] + a.ioffset[1];
+    return converged;
 }
 // ground point -> pixel of image b
 __device__ __forceinline__ void project(const RpcModel &b, double lon, double lat, double z, double &x, double &y)
@@ -191,6 +199,33 @@ __global__ void __maxnreg__(120) triangulate_kernel(const __grid_constant__ TriP
     P.lonlatalt[3 * pix + 1] = o1;
     P.lonlatalt[3 * pix + 2] = o2;
     P.err[pix] = oe;
+}
+
+// Localisation of a height map (s2p.triangulation.height_map_to_xyz, s2p/triangulation.py:165-217): pixel (i, j) of a w x h
+// map with height z is the ground point of image pixel (j + off_x, i + off_y) at height z (rpc_localization, c/rpc.c:469),
+// written as (lon, lat, z).  A NaN height gives NaN in all three; a pixel whose iteration hits its cap is counted in *capped.
+struct HeightMapParams {
+    const double *heights;
+    int w, h;
+    double off_x, off_y;
+    RpcModel rpc;                             // by value: the constant bank
+    double *xyz;
+    int *capped;
+};
+__global__ void height_map_to_xyz_kernel(const __grid_constant__ HeightMapParams P)
+{
+    const int col = blockIdx.x * blockDim.x + threadIdx.x, row = blockIdx.y * blockDim.y + threadIdx.y;
+    if (col >= P.w || row >= P.h) return;
+    const size_t pix = (size_t)row * P.w + col;
+    const double z = P.heights[pix];
+    double lon = z, lat = z;                  // NaN stays NaN
+    if (!isnan(z)) {
+        const PixelRay ray = make_ray(P.rpc, (double)col + P.off_x, (double)row + P.off_y);
+        if (!ray_at(P.rpc, ray, z, lon, lat)) atomicAdd(P.capped, 1);
+    }
+    P.xyz[3 * pix + 0] = lon;
+    P.xyz[3 * pix + 1] = lat;
+    P.xyz[3 * pix + 2] = z;
 }
 
 }  // namespace s2pb

@@ -330,6 +330,22 @@ class Engine:
         _lib.check(self._L.s2pb_lonlat_to_utm(self._ctx, dp(out), dp(a), a.size // 3, int(zone), int(bool(south))))
         return out
 
+    def height_map_to_xyz(self, heights, rpc, off_x, off_y, zone=0, south=False):
+        """The localisation of every pixel of a (h, w) height map and the projection to UTM zone `zone` (1..60; 0: lon, lat,
+        alt as they are) in one device call -> (h, w, 3) float64.  Pixel (i, j) is image pixel (j + off_x, i + off_y) of the
+        camera ``rpc`` (a ctypes structure with the layout of ``triangulation.RPCStruct``); its third coordinate is the height
+        converted to float64.  NaN heights give NaN in all three.  Pixels whose localisation does not converge raise
+        S2pbError(ERR_ARG)."""
+        z = np.ascontiguousarray(heights, np.float64)
+        if z.ndim != 2:
+            raise ValueError("expecting a 2-D height map, got shape %s" % (z.shape,))
+        h, w = z.shape
+        xyz = np.empty((h, w, 3), np.float64)
+        dp = lambda a: a.ctypes.data_as(ctypes.POINTER(ctypes.c_double))
+        _lib.check(self._L.s2pb_height_map_to_xyz(self._ctx, dp(xyz), dp(z), w, h, ctypes.cast(ctypes.pointer(rpc), ctypes.c_void_p),
+                                                  float(off_x), float(off_y), int(zone), int(bool(south))))
+        return xyz
+
     # ------------------------------------------------------------------ DSM rasterisation
     def plyflatten(self, clouds, record_bytes, columns, xoff, yoff, resolution, xsize, ysize):
         """plyflatten with radius 0 and no sigma on the roi (xoff, yoff, xsize, ysize) -> (ysize, xsize, len(columns) - 2)

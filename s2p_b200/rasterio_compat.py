@@ -23,6 +23,22 @@ def read_band(path):
     return np.ascontiguousarray(_read_all(path)[0])
 
 
+def read_band_stored(path):
+    """-> 2-D array of the first band in the dtype it is stored in (rasterio's ``read(1)``): a float64 raster keeps its
+    bits, where read_band rounds to float32."""
+    if _HAVE_RASTERIO:
+        with rasterio.open(path, "r") as f:
+            return np.ascontiguousarray(f.read(1))
+    import cv2
+    a = cv2.imread(path, cv2.IMREAD_UNCHANGED)
+    if a is not None and a.ndim == 2:
+        return np.ascontiguousarray(a)
+    from PIL import Image
+    with Image.open(path) as im:
+        a = np.array(im)
+    return np.ascontiguousarray(a if a.ndim == 2 else a[..., 0])
+
+
 def _read_all(path):
     """-> float32 array (bands, h, w) without rasterio"""
     try:

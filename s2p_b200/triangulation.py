@@ -15,6 +15,10 @@ function with it.
 
 ``height_map`` (s2p/triangulation.py:346-389), the tri-stereo step that triangulates a pair and resamples the altitude onto the
 tile grid, runs as one device call (``s2pb_height_map``); ``install()`` replaces the reference's function with it.
+
+``height_map_to_xyz`` (s2p/triangulation.py:165-217), which localises the merged tri-stereo height map with the reference
+image's camera and projects it to the output CRS, runs as one device call (``s2pb_height_map_to_xyz``) for the same targets
+as ``disp_to_xyz``; ``install()`` replaces the reference's function with it.
 """
 import ctypes
 from ctypes import c_double
@@ -93,6 +97,23 @@ def disp_to_xyz(rpc1, rpc2, H1, H2, disp, mask_rect, img_bbx, mask_orig, A=None,
         lla, err = disp_to_lonlatalt(disp, mask_rect, mask_orig, H1, H2, r1, r2, img_bbx, engine=eng)
         return projection.pyproj_original(lla, out_crs), err
     return eng.disp_to_xyz(disp, mask_rect, mask_orig, H1, H2, r1, r2, img_bbx, *target)
+
+
+def height_map_to_xyz(heights, rpc, off_x=0, off_y=0, out_crs=None, engine=None):
+    """s2p.triangulation.height_map_to_xyz (s2p/triangulation.py:165-217): -> (h, w, 3) float64, every pixel of the height
+    map at ``heights`` (a raster file; band 1, read in its stored dtype) localised by the camera ``rpc`` at image pixel
+    (col + off_x, row + off_y) and its height, in the coordinates of out_crs.  rpc is wrapped as the reference wraps it
+    (``RPCStruct(rpc)``); ctypes structures pass as they are.  NaN heights give NaN in all three coordinates (the reference
+    leaves lon and lat undefined there).  No out_crs, EPSG 4979 / 4326 and the UTM zones of WGS84 run on the device in one
+    call; any other out_crs is localised on the device and projected by the reference's pyproj code (``projection``)."""
+    from . import rasterio_compat
+    h_map = rasterio_compat.read_band_stored(heights)
+    r = _rpc_struct(rpc)
+    eng = engine or get_engine()
+    target = projection.utm_target(out_crs)
+    if target is None:
+        return projection.pyproj_original(eng.height_map_to_xyz(h_map, r, off_x, off_y), out_crs)
+    return eng.height_map_to_xyz(h_map, r, off_x, off_y, *target)
 
 
 def height_map(x, y, w, h, rpc1, rpc2, H1, H2, disp, mask, mask_orig, A=None, engine=None):
@@ -177,4 +198,8 @@ def install():
         if not hasattr(original, "_s2pb_original_height_map"):
             original._s2pb_original_height_map = original.height_map
         original.height_map = height_map
+    if hasattr(original, "height_map_to_xyz"):
+        if not hasattr(original, "_s2pb_original_height_map_to_xyz"):
+            original._s2pb_original_height_map_to_xyz = original.height_map_to_xyz
+        original.height_map_to_xyz = height_map_to_xyz
     return original
