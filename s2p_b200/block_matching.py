@@ -3,7 +3,8 @@
 ``compute_disparity_map`` keeps the reference's signature, file contract and exceptions
 (s2p/block_matching.py:35-336) but, for ``algo in {'mgm', 'mgm_multi', 'mgm_multi_lsd'}``, runs the H100 engine
 through the C ABI instead of spawning the ``mgm`` / ``mgm_multi`` binaries and the three
-``plambda`` / ``backflow`` processes of ``create_rejection_mask``.  ``algo == 'sgbm'`` with both
+``plambda`` / ``backflow`` processes of ``create_rejection_mask`` (and, for ``mgm_multi_lsd``, the two five-command
+weight-map pipelines, see ``lsd_weight_map``).  ``algo == 'sgbm'`` with both
 disparity bounds given (as s2p always passes them) runs the engine's bit-exact restatement of the
 ``sgbm`` binary with s2p's arguments (win 3, P1 8, P2 32, lr 1) and writes no confidence file, as the
 reference does.  Any other ``algo`` (and ``sgbm`` with a bound of None) is handed to the original s2p
@@ -77,23 +78,14 @@ def confidence_path(disp, algo="mgm"):
 
 
 def lsd_weight_map(im):
-    """Regularity weights of 'mgm_multi_lsd' for one rectified image: the reference's own host pipeline
-    (s2p/block_matching.py:199-218: qauto | lsd | cut | pview segments | plambda "255 x - 255 / 2 pow 0.1 fmax"),
-    run as is -- line-segment detection is host pre-processing, not part of the matcher.  -> float32 (h, w)."""
-    import tempfile
+    """Regularity weights of 'mgm_multi_lsd' for one rectified image: what the reference's host pipeline
+    (s2p/block_matching.py:199-218: qauto | lsd | cut | pview segments | plambda "255 x - 255 / 2 pow 0.1 fmax")
+    writes, without starting it.  That is 1 at every pixel, whatever the image: qauto writes into its pipe in NPY, the
+    format iio gives a stream without a file name; lsd reads only PGM and exits; pview draws no segment on its zero
+    image, and the weight law maps 0 to 1.  /bin/sh reports the status of plambda, so the reference goes on
+    (DESIGN.md section 3.4).  -> float32 (h, w)."""
     width, height = rio.image_size(im)
-    tdir = cfg["temporary_dir"] if os.path.isdir(str(cfg["temporary_dir"])) else None
-    fd, out = tempfile.mkstemp(suffix=".tif", dir=tdir)                               # common.tmpfile, s2p/common.py:50-67
-    os.close(fd)
-    cmd = ("qauto %s | lsd  -  - | cut -d' ' -f1,2,3,4 | pview segments %d %d | "
-           "plambda -  \"255 x - 255 / 2 pow 0.1 fmax\" -o %s" % (im, width, height, out))
-    print("\nRUN: %s" % cmd)
-    try:
-        subprocess.run(cmd, shell=True, check=True)
-        return rio.read_band(out)
-    finally:
-        if os.path.exists(out):
-            os.remove(out)
+    return np.ones((height, width), np.float32)
 
 
 def _original_compute_disparity_map():
