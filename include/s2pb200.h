@@ -175,7 +175,9 @@ int s2pb_sgbm(s2pb_ctx *ctx, const float *im1, const float *im2, int w, int h, i
 
 /* ---- rectification warp ---------------------------------------------------- */
 /* dst(j,i) = src sampled at H^-1 (j,i,1), order-5 B-spline with the reference's
- * anti-aliasing rule (3rdparty/homography/LibHomography/Homography.cpp:50-168). */
+ * anti-aliasing rule (3rdparty/homography/LibHomography/Homography.cpp:50-168).
+ * S2PB_ERR_ARG for an empty region of interest, and for a spline image (the region of interest, or
+ * the anti-aliasing intermediate) with a side below 4 pixels, which the reference cannot warp either. */
 int s2pb_homography(s2pb_ctx *ctx, const float *src, int sw, int sh,
                     const double H[9], float *dst, int dw, int dh);
 

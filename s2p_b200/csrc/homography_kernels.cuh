@@ -98,8 +98,8 @@ __global__ void spline_columns_kernel(float *__restrict__ a, int w, int h, float
 // a zero state that far beyond its end (the last segment from initBackward's exact start value).  w x (h / 64)
 // threads instead of w, and no global-memory latency chain: the 2250-column anti-aliasing case drops from 3.6 ms
 // per launch to tens of microseconds.  Out of place (in -> out); lines shorter than 2 * kSplineSeg use the
-// sequential kernel above.
-constexpr int kSplineSeg = 64, kSplineWarm = 32;
+// sequential kernel above.  Both kernels need lines of kSplineMinSide samples at least (map_image refuses shorter ones).
+constexpr int kSplineSeg = 64, kSplineWarm = 32, kSplineMinSide = 4;
 __global__ void __launch_bounds__(128) spline_segments_kernel(const float *__restrict__ in, float *__restrict__ out, int w, int h,
                                                              float scale, double pz)
 {
@@ -139,7 +139,9 @@ __global__ void __launch_bounds__(128) spline_segments_kernel(const float *__res
 #pragma unroll
         for (int q = 0; q < kSplineSeg + kSplineWarm; q++) { if (s + q == h - 1) last = f[q]; if (s + q == h - 2) prev = f[q]; }
         b = (float)(pz / (pz * pz - 1.0)) * fmaf((float)pz, prev, last);
-        if (h - 1 < e) o[(size_t)(h - 1) * st] = b;
+        // o[h-1] is written by the segment that holds h-2, the only one with both values: when h = 64k + 1 the last
+        // segment is the single sample h-1, and its forward value at h-2 (prev) would be missing
+        if (s <= h - 2 && h - 2 < e) o[(size_t)(h - 1) * st] = b;
 #pragma unroll
         for (int q = kSplineSeg + kSplineWarm - 1; q >= 0; q--) {
             const int k = s + q;

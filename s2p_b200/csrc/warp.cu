@@ -47,12 +47,19 @@ static int map_image(s2pb_ctx *ctx, ScratchLease &L, cudaStream_t st, const floa
     const bool useZ = zoomOut < 1.f;
     double matZ[9] = {0};
     float *tmp, *scratch;
-    int tw = w, th = h;
+    const float zoomIn = 1.0f / zoomOut;
+    int tw = w, th = h;                        // the spline image: the source, or the anti-aliasing intermediate
     if (useZ) {
-        const float zoomIn = 1.0f / zoomOut;
         tw = (int)std::ceil((size_t)ow * zoomIn * 1.5);
         th = (int)std::ceil((size_t)oh * zoomIn * 1.5);
         if (tw < 1 || th < 1 || (size_t)tw * th > ((size_t)1 << 31)) return fail(S2PB_ERR_ARG, "homography: degenerate zoom %g", (double)zoomIn);
+    }
+    // Below 4 samples a side the prefilter's initBackward and the border formula's single reflection index outside the
+    // image, and the reference produces no image (prepareSpline's `i < height - 4` wraps around in size_t).
+    if (tw < kSplineMinSide || th < kSplineMinSide)
+        return fail(S2PB_ERR_ARG, "homography: the %s is %d x %d pixels; the order-5 spline needs %d x %d at least",
+                    useZ ? "anti-aliasing intermediate" : "region of interest", tw, th, kSplineMinSide, kSplineMinSide);
+    if (useZ) {
         for (int k = 0; k < 6; k++) matZ[k] = zoomIn * M[k];
         for (int k = 6; k < 9; k++) matZ[k] = M[k];
         tmp = L.take<float>((size_t)tw * th * 4);

@@ -35,6 +35,7 @@ CASES = {
     "zoom_in": _rot(-0.1, 1.7, -60, 20),
     "perspective": np.array([[1.02, 0.03, -10], [0.01, 0.97, 5], [1e-5, -2e-5, 1]]),
     "shifted_crop": _rot(0.02, 1.0, -150, -100),           # needed ROI is a strict sub-window of the source
+    "rows129": np.array([[1, 0, -20], [0, 1.5625, -16.09375], [0, 0, 1.0]]),   # a 256 x 129 ROI: the last prefilter segment of a column is one row
 }
 
 
