@@ -27,6 +27,10 @@
  *                        (s2p/triangulation.py:165-217)
  *   s2pb_plyflatten()    plyflatten_from_plyfiles_list with radius 0 (the external plyflatten package) in plys_to_dsm
  *                        (s2p/__init__.py:432-476)
+ *   s2pb_disp_to_ply()   disparity_to_ply's cloud after its inputs are read (s2p/__init__.py:242-318): disp_to_xyz, filter_xyz,
+ *                        linear_stretching_and_quantization_8bit (s2p/common.py:284-297) and the vertex records of write_to_ply
+ *                        (s2p/triangulation.py:392-429, s2p/ply.py:24-69)
+ *   s2pb_height_map_to_ply() the same for heights_to_ply after heights_fusion (s2p/__init__.py:388-429), from height_map_to_xyz
  *   s2pb_sgbm()          the `sgbm` subprocess (OpenCV 2's StereoSGBM, 3rdparty/sgbm) + create_rejection_mask
  *                        (s2p/block_matching.py:116-134)
  *
@@ -280,6 +284,39 @@ int s2pb_height_map_to_xyz(s2pb_ctx *ctx, double *xyz, const double *heights, in
  * Synchronous on the context's stream. */
 int s2pb_count_3d_neighbors(s2pb_ctx *ctx, int32_t *count, const double *xyz, int nx, int ny, float r, int p);
 int s2pb_remove_isolated_3d_points(s2pb_ctx *ctx, double *xyz, int nx, int ny, float r, int p, int n, int q);
+
+/* ---- the tile's point cloud (s2p/__init__.py disparity_to_ply and heights_to_ply) ---- */
+/* common.linear_stretching_and_quantization_8bit(img, pct) (s2p/common.py:284-297) of n float32 values (every band of the image
+ * together; a uint8 or uint16 image converts exactly) bit for bit with NumPy >= 2: a, b = np.nanpercentile(img, (pct, 100 - pct))
+ * by numpy's 'linear' method (float64 quantiles pct / 100 and (100 - pct) / 100, virtual index (N - 1) q over the N non-NaN values,
+ * the neighbours' difference in float32, the rest of the interpolation in float64), then out = round_half_even(255 * (clip(v, a, b)
+ * - a) / (b - a)) in float64 as uint8, NaN -> 0 (a constant or all-NaN image gives 0 everywhere).
+ * S2PB_ERR_ARG: a null pointer with n > 0, n < 0, pct outside [0, 100].  S2PB_ERR_UNSUPPORTED: n > 2^31 - 1. */
+int s2pb_stretch_8bit(s2pb_ctx *ctx, const float *img, int64_t n, double pct, uint8_t *out);
+/* The vertex records write_to_ply writes for a cloud (s2p/triangulation.py:392-429 -> ply.write_3d_point_cloud_to_ply): the points
+ * of xyz (n points of three float64) whose three coordinates are finite, in order, each packed as x, y, z float64, then, with
+ * nbands = 1, 3 or 4 colour planes (n uint8 each; one band is written three times), red, green, blue (and ir) uint8, then, with conf
+ * (n float32, nullable), confidence float32: 24 + {0, 3, 4} + {0, 4} bytes, no padding.  records holds n such records; *npoints
+ * gets the number written.  S2PB_ERR_ARG: a null pointer, n < 0, nbands not 0, 1, 3 or 4 (the reference raises).
+ * S2PB_ERR_UNSUPPORTED: n > 2^31 - 1. */
+int s2pb_ply_records(s2pb_ctx *ctx, const double *xyz, int64_t n, const uint8_t *colors, int nbands, const float *conf,
+                     uint8_t *records, int64_t *npoints);
+/* disparity_to_ply's cloud (s2p/__init__.py:242-318) in one call: s2pb_disp_to_xyz's argument list without its outputs, then
+ * the 3D filter (remove_isolated_3d_points with r, p, n and q = 1 on the projected cloud, as filter_xyz; off when r == 0 or
+ * n <= 0), nbands colour planes of nx*ny float32 stretched as s2pb_stretch_8bit stretches them with pct, an optional nx*ny
+ * float32 confidence image, and the records of s2pb_ply_records (records: nx*ny records).  Only the npoints records come back.
+ * S2PB_ERR_ARG: as s2pb_disp_to_xyz and s2pb_ply_records, pct outside [0, 100].
+ * S2PB_ERR_UNSUPPORTED: more than 2^31 - 1 points or colour values. */
+int s2pb_disp_to_ply(s2pb_ctx *ctx, const float *dispx, const float *dispy, const float *msk, int nx, int ny, const float *msk_orig,
+                     int w, int h, const double ha[9], const double hb[9], const s2pb_rpc *rpca, const s2pb_rpc *rpcb,
+                     const float orig_img_bounding_box[4], int zone, int south, float r, int p, int n, const float *bands,
+                     int nbands, double pct, const float *conf, uint8_t *records, int64_t *npoints);
+/* heights_to_ply's cloud after heights_fusion (s2p/__init__.py:388-429) in one call: s2pb_height_map_to_xyz's argument list
+ * without its output, then the filter, colours (w*h planes) and records of s2pb_disp_to_ply, without confidence.
+ * S2PB_ERR_ARG: as s2pb_height_map_to_xyz (non-converging localisations included) and s2pb_disp_to_ply. */
+int s2pb_height_map_to_ply(s2pb_ctx *ctx, const double *heights, int w, int h, const s2pb_rpc *rpc, double off_x, double off_y,
+                           int zone, int south, float r, int p, int n, const float *bands, int nbands, double pct,
+                           uint8_t *records, int64_t *npoints);
 
 /* ---- DSM rasterisation (s2p/__init__.py plys_to_dsm) -------------------------- */
 /* One vertex property of a binary little-endian PLY record: its byte offset in the record and its type. */

@@ -87,6 +87,13 @@ _SIGNATURES = {
     "s2pb_cargarse_basura": (c_int, [c_void_p, _f, _f, c_int, c_int]),
     "s2pb_count_3d_neighbors": (c_int, [c_void_p, POINTER(c_int32), POINTER(c_double), c_int, c_int, c_float, c_int]),
     "s2pb_remove_isolated_3d_points": (c_int, [c_void_p, POINTER(c_double), c_int, c_int, c_float, c_int, c_int, c_int]),
+    "s2pb_stretch_8bit": (c_int, [c_void_p, _f, c_int64, c_double, POINTER(c_uint8)]),
+    "s2pb_ply_records": (c_int, [c_void_p, POINTER(c_double), c_int64, POINTER(c_uint8), c_int, _f, POINTER(c_uint8), POINTER(c_int64)]),
+    "s2pb_disp_to_ply": (c_int, [c_void_p, _f, _f, _f, c_int, c_int, _f, c_int, c_int, POINTER(c_double), POINTER(c_double), c_void_p,
+                                 c_void_p, _f, c_int, c_int, c_float, c_int, c_int, _f, c_int, c_double, _f, POINTER(c_uint8),
+                                 POINTER(c_int64)]),
+    "s2pb_height_map_to_ply": (c_int, [c_void_p, POINTER(c_double), c_int, c_int, c_void_p, c_double, c_double, c_int, c_int, c_float,
+                                       c_int, c_int, _f, c_int, c_double, POINTER(c_uint8), POINTER(c_int64)]),
     "s2pb_plyflatten": (c_int, [c_void_p, c_int, POINTER(c_void_p), POINTER(c_int64), c_int, POINTER(PlyColumn), c_int, c_double,
                                 c_double, c_double, c_int, c_int, _f]),
     "s2pb_erode_mask": (c_int, [c_void_p, POINTER(c_uint8), POINTER(c_uint8), c_int, c_int, c_float]),

@@ -1,0 +1,163 @@
+// cloud.cu -- the tile's point cloud as PLY records (cloud_kernels.cuh): the colours of
+// common.linear_stretching_and_quantization_8bit and the vertex records of triangulation.write_to_ply, alone or at the end of
+// disparity_to_ply / heights_to_ply's triangulation and 3D filter on one stream.
+#include "host.h"
+#include "cloud_kernels.cuh"
+
+// bytes of one record: x, y, z float64, 3 colours (1 or 3 bands) or 4 (4 bands) uint8, confidence float32
+static int record_bytes(int nbands, bool conf) { return 24 + (nbands == 4 ? 4 : nbands ? 3 : 0) + (conf ? 4 : 0); }
+
+static bool bands_ok(int nbands) { return nbands == 0 || nbands == 1 || nbands == 3 || nbands == 4; }
+
+// np.nanpercentile(img, (pct, 100 - pct)) of the n values of d_im into d_os (order_stats_bytes())
+static int stretch_bounds_enqueue(s2pb_ctx *ctx, cudaStream_t st, const float *d_im, size_t n, double pct, OrderStats *d_os)
+{
+    return launch_order_stats(ctx, st, d_im, (int)n, kOrdLinear, pct / 100.0, (100.0 - pct) / 100.0, d_os);
+}
+
+// The kept points of the device cloud d_xyz (n points) packed into d_out; their number into *d_total.  Colours: d_colors
+// (nbands uint8 planes) or, when it is null, d_bands (nbands float32 planes) stretched with the bounds of d_os.
+static int pack_enqueue(s2pb_ctx *ctx, HostCall &L, const double *d_xyz, size_t n, int nbands, const uint8_t *d_colors,
+                        const float *d_bands, const OrderStats *d_os, const float *d_conf, uint8_t *d_out, long long *d_total)
+{
+    const int ntiles = (int)((n + kPlyTile - 1) / kPlyTile);
+    int *d_counts = L.take<int>((size_t)ntiles * 4);
+    long long *d_offsets = L.take<long long>((size_t)ntiles * 8);
+    if (int rc = L.error()) return rc;
+    launch(ctx, ply_count_kernel, ntiles, kPlyThreads, 0, L.st, d_xyz, n, d_counts);
+    launch(ctx, ply_scan_kernel, 1, 1024, 0, L.st, d_counts, ntiles, d_offsets, d_total);
+    PlyPackParams P;
+    P.xyz = d_xyz; P.n = n; P.offsets = d_offsets; P.nbands = nbands; P.colors = d_colors; P.bands = d_bands; P.os = d_os;
+    P.conf = d_conf; P.rb = record_bytes(nbands, d_conf != nullptr); P.out = d_out;
+    launch(ctx, ply_pack_kernel, ntiles, kPlyThreads, 0, L.st, P);
+    CK(cudaGetLastError());
+    return S2PB_OK;
+}
+
+// the number of records, then only their bytes come back
+static int download_records(HostCall &L, const long long *d_total, const uint8_t *d_out, int rb, uint8_t *records, int64_t *npoints)
+{
+    long long total = 0;
+    L.download(&total, d_total, 8);
+    if (int rc = L.finish()) return rc;
+    *npoints = total;
+    if (total) L.download(records, d_out, (size_t)total * rb);
+    return L.finish();
+}
+
+extern "C" int s2pb_stretch_8bit(s2pb_ctx *ctx, const float *img, int64_t n, double pct, uint8_t *out)
+{
+    if (!ctx || n < 0 || (n && (!img || !out))) return fail(S2PB_ERR_ARG, "bad argument");
+    if (!(pct >= 0.0 && pct <= 100.0)) return fail(S2PB_ERR_ARG, "percentiles must be in the range [0, 100] (got %g)", pct);
+    if (n > INT32_MAX) return fail(S2PB_ERR_UNSUPPORTED, "at most 2^31 - 1 values");
+    if (n == 0) return S2PB_OK;
+    HostCall L(ctx, "the 8-bit stretch");
+    float *d_im = L.upload(img, (size_t)n * 4);
+    OrderStats *d_os = L.take<OrderStats>(order_stats_bytes());
+    uint8_t *d_out = L.take<uint8_t>((size_t)n);
+    if (int rc = L.error()) return rc;
+    if (int rc = stretch_bounds_enqueue(ctx, L.st, d_im, (size_t)n, pct, d_os)) return rc;
+    launch(ctx, stretch_8bit_kernel, (unsigned)std::min<int64_t>((n + 255) / 256, (int64_t)ctx->sm_count * 16), 256, 0, L.st, d_im,
+           (size_t)n, d_os, d_out);
+    CK(cudaGetLastError());
+    L.download(out, d_out, (size_t)n);
+    return L.finish();
+}
+
+extern "C" int s2pb_ply_records(s2pb_ctx *ctx, const double *xyz, int64_t n, const uint8_t *colors, int nbands, const float *conf,
+                                uint8_t *records, int64_t *npoints)
+{
+    if (!ctx || !npoints || n < 0 || (n && (!xyz || !records || (nbands && !colors)))) return fail(S2PB_ERR_ARG, "bad argument");
+    if (!bands_ok(nbands)) return fail(S2PB_ERR_ARG, "colors must have either 1, 3 or 4 channels (got %d)", nbands);
+    if (n > INT32_MAX) return fail(S2PB_ERR_UNSUPPORTED, "at most 2^31 - 1 points");
+    *npoints = 0;
+    if (n == 0) return S2PB_OK;
+    HostCall L(ctx, "the PLY records");
+    const size_t np = (size_t)n;
+    const int rb = record_bytes(nbands, conf != nullptr);
+    double *d_xyz = L.upload(xyz, np * 24);
+    uint8_t *d_col = nbands ? L.upload(colors, np * nbands) : nullptr;
+    float *d_conf = conf ? L.upload(conf, np * 4) : nullptr;
+    uint8_t *d_out = L.take<uint8_t>(np * rb);
+    long long *d_total = L.take<long long>(8);
+    if (int rc = L.error()) return rc;
+    if (int rc = pack_enqueue(ctx, L, d_xyz, np, nbands, d_col, nullptr, nullptr, d_conf, d_out, d_total)) return rc;
+    return download_records(L, d_total, d_out, rb, records, npoints);
+}
+
+// the common tail of the two steps: filter, colours, records
+static int cloud_tail(s2pb_ctx *ctx, HostCall &L, double *d_xyz, int nx, int ny, float r, int p, int n, const float *bands,
+                      int nbands, double pct, const float *conf, uint8_t *records, int64_t *npoints)
+{
+    const size_t npix = (size_t)nx * ny;
+    const int rb = record_bytes(nbands, conf != nullptr);
+    int *d_work = (r != 0.f && n > 0) ? L.take<int>(npix * 12) : nullptr;
+    float *d_bands = nbands ? L.upload(bands, npix * nbands * 4) : nullptr;
+    OrderStats *d_os = nbands ? L.take<OrderStats>(order_stats_bytes()) : nullptr;
+    float *d_conf = conf ? L.upload(conf, npix * 4) : nullptr;
+    uint8_t *d_out = L.take<uint8_t>(npix * rb);
+    long long *d_total = L.take<long long>(8);
+    if (int rc = L.error()) return rc;
+    if (d_work) {
+        if (int rc = remove_isolated_enqueue(ctx, L.st, d_xyz, nx, ny, r, p, n, 1, d_work)) return rc;
+    }
+    if (nbands) {
+        if (int rc = stretch_bounds_enqueue(ctx, L.st, d_bands, npix * nbands, pct, d_os)) return rc;
+    }
+    if (int rc = pack_enqueue(ctx, L, d_xyz, npix, nbands, nullptr, d_bands, d_os, d_conf, d_out, d_total)) return rc;
+    return download_records(L, d_total, d_out, rb, records, npoints);
+}
+
+static int tail_args_ok(int nx, int ny, const float *bands, int nbands, double pct, uint8_t *records,
+                        int64_t *npoints)
+{
+    if (!records || !npoints || (nbands && !bands)) return fail(S2PB_ERR_ARG, "bad argument");
+    if (!bands_ok(nbands)) return fail(S2PB_ERR_ARG, "colors must have either 1, 3 or 4 channels (got %d)", nbands);
+    if (!(pct >= 0.0 && pct <= 100.0)) return fail(S2PB_ERR_ARG, "percentiles must be in the range [0, 100] (got %g)", pct);
+    if ((size_t)nx * ny * std::max(nbands, 1) > INT32_MAX) return fail(S2PB_ERR_UNSUPPORTED, "at most 2^31 - 1 points and colour values");
+    return S2PB_OK;
+}
+
+extern "C" int s2pb_disp_to_ply(s2pb_ctx *ctx, const float *dispx, const float *dispy, const float *msk, int nx, int ny,
+                                const float *msk_orig, int w, int h, const double ha[9], const double hb[9], const s2pb_rpc *rpca,
+                                const s2pb_rpc *rpcb, const float bbox[4], int zone, int south, float r, int p, int n,
+                                const float *bands, int nbands, double pct, const float *conf, uint8_t *records, int64_t *npoints)
+{
+    if (!ctx || !dispx || !dispy || !msk || !msk_orig || !ha || !hb || !rpca || !rpcb || !bbox || nx < 1 || ny < 1 || w < 1 || h < 1)
+        return fail(S2PB_ERR_ARG, "bad argument");
+    if (zone < 0 || zone > 60) return fail(S2PB_ERR_ARG, "UTM zone %d (1 to 60, or 0 for lon, lat, alt)", zone);
+    if (int rc = tail_args_ok(nx, ny, bands, nbands, pct, records, npoints)) return rc;
+    *npoints = 0;
+    const size_t npix = (size_t)nx * ny, nm = (size_t)w * h;
+    HostCall L(ctx, "the tile's cloud");
+    float *d_dx = L.upload(dispx, npix * 4), *d_dy = L.upload(dispy, npix * 4), *d_m = L.upload(msk, npix * 4);
+    float *d_mo = L.upload(msk_orig, nm * 4);
+    double *d_xyz = L.take<double>(npix * 24);
+    float *d_err = L.take<float>(npix * 4);
+    if (int rc = L.error()) return rc;
+    int rc = triangulate_enqueue(ctx, L.st, d_dx, d_dy, d_m, nx, ny, d_mo, w, h, ha, hb, rpca, rpcb, bbox, d_xyz, d_err);
+    if (rc == S2PB_OK && zone) rc = launch_utm_project(ctx, L.st, zone, south != 0, d_xyz, d_xyz, npix);
+    if (rc != S2PB_OK) return rc;
+    return cloud_tail(ctx, L, d_xyz, nx, ny, r, p, n, bands, nbands, pct, conf, records, npoints);
+}
+
+extern "C" int s2pb_height_map_to_ply(s2pb_ctx *ctx, const double *heights, int w, int h, const s2pb_rpc *rpc, double off_x,
+                                      double off_y, int zone, int south, float r, int p, int n, const float *bands, int nbands,
+                                      double pct, uint8_t *records, int64_t *npoints)
+{
+    if (!ctx || !heights || !rpc || w < 1 || h < 1) return fail(S2PB_ERR_ARG, "bad argument");
+    if (zone < 0 || zone > 60) return fail(S2PB_ERR_ARG, "UTM zone %d (1 to 60, or 0 for lon, lat, alt)", zone);
+    if (int rc = tail_args_ok(w, h, bands, nbands, pct, records, npoints)) return rc;
+    *npoints = 0;
+    const size_t npix = (size_t)w * h;
+    HostCall L(ctx, "the tile's cloud");
+    double *d_z = L.upload(heights, npix * 8), *d_xyz = L.take<double>(npix * 24);
+    int *d_capped = L.take<int>(4);
+    if (int rc = L.error()) return rc;
+    if (int rc = height_map_to_xyz_enqueue(ctx, L.st, d_z, w, h, rpc, off_x, off_y, zone, south, d_xyz, d_capped)) return rc;
+    int capped = 0;
+    L.download(&capped, d_capped, 4);
+    if (int rc = L.finish()) return rc;
+    if (capped) return fail(S2PB_ERR_ARG, "the localisation of %d pixel(s) did not converge in 1000 steps", capped);
+    return cloud_tail(ctx, L, d_xyz, w, h, r, p, n, bands, nbands, pct, nullptr, records, npoints);
+}

@@ -11,7 +11,7 @@
 static_assert(sizeof(s2pb_rpc) == sizeof(RpcModel), "s2pb_rpc must have the layout of the reference's struct rpc");
 
 // disp_to_lonlatalt (c/disp_to_h.c:70-141) on device buffers: lonlatalt nx*ny*3 doubles, err nx*ny floats
-static int triangulate_enqueue(s2pb_ctx *ctx, cudaStream_t st, const float *d_dx, const float *d_dy, const float *d_m, int nx, int ny,
+int triangulate_enqueue(s2pb_ctx *ctx, cudaStream_t st, const float *d_dx, const float *d_dy, const float *d_m, int nx, int ny,
                                const float *d_mo, int w, int h, const double ha[9], const double hb[9], const s2pb_rpc *rpca,
                                const s2pb_rpc *rpcb, const float bbox[4], double *d_out, float *d_err)
 {
@@ -77,6 +77,24 @@ extern "C" int s2pb_disp_to_xyz(s2pb_ctx *ctx, double *xyz, float *err, const fl
     return L.finish();
 }
 
+// every pixel of the device height map d_z localised by the camera into d_out (w*h*3 doubles), then projected to UTM zone
+// `zone` in place (0: none); d_capped (one int, zeroed here) counts the pixels whose iteration hit its cap
+int height_map_to_xyz_enqueue(s2pb_ctx *ctx, cudaStream_t st, const double *d_z, int w, int h, const s2pb_rpc *rpc, double off_x,
+                              double off_y, int zone, int south, double *d_out, int *d_capped)
+{
+    CK(cudaMemsetAsync(d_capped, 0, 4, st));
+    HeightMapParams P;
+    memset(&P, 0, sizeof P);
+    P.heights = d_z; P.w = w; P.h = h; P.off_x = off_x; P.off_y = off_y;
+    memcpy(&P.rpc, rpc, sizeof(RpcModel));
+    P.xyz = d_out; P.capped = d_capped;
+    const dim3 b2(32, 4);
+    launch(ctx, height_map_to_xyz_kernel, grid2d(w, h, b2), b2, 0, st, P);
+    CK(cudaGetLastError());
+    if (zone) return launch_utm_project(ctx, st, zone, south != 0, d_out, d_out, (size_t)w * h);
+    return S2PB_OK;
+}
+
 // s2p.triangulation.height_map_to_xyz (s2p/triangulation.py:165-217) with a UTM (or no) output CRS: every pixel of the height
 // map localised by the camera, then the projection (projection.cu) in place on the device cloud.
 extern "C" int s2pb_height_map_to_xyz(s2pb_ctx *ctx, double *xyz, const double *heights, int w, int h, const s2pb_rpc *rpc,
@@ -89,18 +107,7 @@ extern "C" int s2pb_height_map_to_xyz(s2pb_ctx *ctx, double *xyz, const double *
     double *d_z = L.upload(heights, npix * 8), *d_out = L.take<double>(npix * 24);
     int *d_capped = L.take<int>(4);
     if (int rc = L.error()) return rc;
-    CK(cudaMemsetAsync(d_capped, 0, 4, L.st));
-    HeightMapParams P;
-    memset(&P, 0, sizeof P);
-    P.heights = d_z; P.w = w; P.h = h; P.off_x = off_x; P.off_y = off_y;
-    memcpy(&P.rpc, rpc, sizeof(RpcModel));
-    P.xyz = d_out; P.capped = d_capped;
-    const dim3 b2(32, 4);
-    launch(ctx, height_map_to_xyz_kernel, grid2d(w, h, b2), b2, 0, L.st, P);
-    CK(cudaGetLastError());
-    if (zone) {
-        if (int rc = launch_utm_project(ctx, L.st, zone, south != 0, d_out, d_out, npix)) return rc;
-    }
+    if (int rc = height_map_to_xyz_enqueue(ctx, L.st, d_z, w, h, rpc, off_x, off_y, zone, south, d_out, d_capped)) return rc;
     int capped = 0;
     L.download(xyz, d_out, npix * 24);
     L.download(&capped, d_capped, 4);
@@ -245,6 +252,27 @@ extern "C" int s2pb_count_3d_neighbors(s2pb_ctx *ctx, int32_t *count, const doub
     return L.finish();
 }
 
+// remove_isolated_3d_points on a device cloud of nx * ny < 2^31 points with n > 0; d_work: 3 * nx * ny ints of scratch
+int remove_isolated_enqueue(s2pb_ctx *ctx, cudaStream_t st, double *d_xyz, int nx, int ny, float r, int p, int n, int q, int *d_work)
+{
+    const size_t npix = (size_t)nx * ny;
+    int *d_count = d_work, *d_lab = d_work + npix, *d_saved = d_work + 2 * npix;
+    int rc = pc_count_enqueue(ctx, st, d_xyz, nx, ny, r, p, d_count);
+    if (rc != S2PB_OK) return rc;
+    const unsigned g1 = (unsigned)((npix + 255) / 256);
+    const dim3 b2(32, 8), g2 = grid2d(nx, ny, b2);
+    launch(ctx, pc_label_kernel, g1, 256, 0, st, d_count, (int)npix, n, d_lab, d_saved);
+    if (q >= 0) {                                                       // q < 0: empty windows, nothing is saved
+        q = std::min(q, std::max(nx, ny));
+        launch(ctx, pc_link_kernel, g2, b2, 0, st, d_xyz, nx, ny, r, q, d_lab);
+        cc_flatten(ctx, (int)npix, d_lab, st);
+        launch(ctx, pc_mark_kernel, g2, b2, 0, st, d_xyz, nx, ny, r, q, d_lab, d_saved);
+    }
+    launch(ctx, pc_reject_kernel, g1, 256, 0, st, (int)npix, d_lab, d_saved, d_xyz);
+    CK(cudaGetLastError());
+    return S2PB_OK;
+}
+
 // Same argument list as the reference's remove_isolated_3d_points (c/disp_to_h.c:177-184), plus the context; in place on
 // the host cloud.  Rejection by count, then the closure of the reference's "mercy" sweeps as connected components
 // (pointcloud_kernels.cuh): label, link, flatten, mark the saved components, NaN the rest.
@@ -256,21 +284,9 @@ extern "C" int s2pb_remove_isolated_3d_points(s2pb_ctx *ctx, double *xyz, int nx
     if (n <= 0) return S2PB_OK;                                         // a count is never negative: nothing is rejected
     HostCall L(ctx, "the point cloud");
     double *d_xyz = L.upload(xyz, npix * 24);
-    int *d_count = L.take<int>(npix * 4), *d_lab = L.take<int>(npix * 4), *d_saved = L.take<int>(npix * 4);
+    int *d_work = L.take<int>(npix * 12);
     if (int rc = L.error()) return rc;
-    int rc = pc_count_enqueue(ctx, L.st, d_xyz, nx, ny, r, p, d_count);
-    if (rc != S2PB_OK) return rc;
-    const unsigned g1 = (unsigned)((npix + 255) / 256);
-    const dim3 b2(32, 8), g2 = grid2d(nx, ny, b2);
-    launch(ctx, pc_label_kernel, g1, 256, 0, L.st, d_count, (int)npix, n, d_lab, d_saved);
-    if (q >= 0) {                                                       // q < 0: empty windows, nothing is saved
-        q = std::min(q, std::max(nx, ny));
-        launch(ctx, pc_link_kernel, g2, b2, 0, L.st, d_xyz, nx, ny, r, q, d_lab);
-        cc_flatten(ctx, (int)npix, d_lab, L.st);
-        launch(ctx, pc_mark_kernel, g2, b2, 0, L.st, d_xyz, nx, ny, r, q, d_lab, d_saved);
-    }
-    launch(ctx, pc_reject_kernel, g1, 256, 0, L.st, (int)npix, d_lab, d_saved, d_xyz);
-    CK(cudaGetLastError());
+    if (int rc = remove_isolated_enqueue(ctx, L.st, d_xyz, nx, ny, r, p, n, q, d_work)) return rc;
     L.download(xyz, d_xyz, npix * 24);
     return L.finish();
 }

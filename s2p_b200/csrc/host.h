@@ -1,7 +1,7 @@
 // host.h -- host-side state and helpers shared by the translation units of the C ABI (not a public header).
 //
 // s2pb200.cu owns the context, the slots, the matcher and the matcher's stage entry points; warp.cu, geometry.cu, projection.cu,
-// sgbm.cu and raster.cu each hold one family of entry points.  Every kernel header that defines a non-template kernel is included by one of
+// sgbm.cu, raster.cu and cloud.cu each hold one family of entry points.  Every kernel header that defines a non-template kernel is included by one of
 // those files only, so that its kernels are compiled once; the few launchers another file needs are declared at the end.
 #pragma once
 #include "../../include/s2pb200.h"
@@ -17,7 +17,7 @@
 #include <utility>
 #include <vector>
 
-namespace s2pb { struct RtState; }
+namespace s2pb { struct RtState; struct OrderStats; }
 using namespace s2pb;            // every file that includes this one launches the kernels of namespace s2pb
 
 // ------------------------------------------------------------------ context
@@ -236,6 +236,18 @@ void launch_rejection_mask(s2pb_ctx *ctx, const float *disp, const float *im1, c
                            cudaStream_t st);
 // projection.cu: (lon, lat, alt) -> UTM zone `zone` (1..60) of n device points, in place when d_in == d_out
 int launch_utm_project(s2pb_ctx *ctx, cudaStream_t st, int zone, bool south, const double *d_in, double *d_out, size_t n);
+// geometry.cu: disp_to_lonlatalt, height_map_to_xyz (with the projection to UTM zone `zone`, 0 none) and
+// remove_isolated_3d_points (n > 0; d_work: 3 * nx * ny ints) on device buffers
+int triangulate_enqueue(s2pb_ctx *ctx, cudaStream_t st, const float *d_dx, const float *d_dy, const float *d_m, int nx, int ny,
+                        const float *d_mo, int w, int h, const double ha[9], const double hb[9], const s2pb_rpc *rpca,
+                        const s2pb_rpc *rpcb, const float bbox[4], double *d_out, float *d_err);
+int height_map_to_xyz_enqueue(s2pb_ctx *ctx, cudaStream_t st, const double *d_z, int w, int h, const s2pb_rpc *rpc, double off_x,
+                              double off_y, int zone, int south, double *d_out, int *d_capped);
+int remove_isolated_enqueue(s2pb_ctx *ctx, cudaStream_t st, double *d_xyz, int nx, int ny, float r, int p, int n, int q, int *d_work);
+// sgbm.cu: order statistics of the non-NaN values of n device floats by radix select (sgbm_kernels.cuh) into d_os, which
+// holds order_stats_bytes(); rule kOrdQauto (qauto's thresholds) or kOrdLinear (numpy's 'linear' quantiles q0 and q1)
+size_t order_stats_bytes();
+int launch_order_stats(s2pb_ctx *ctx, cudaStream_t st, const float *d_x, int n, int rule, double q0, double q1, OrderStats *d_os);
 // warp.cu
 void invert_homography(const double i[9], double o[9]);
 int warp_host_to_device(s2pb_ctx *ctx, ScratchLease &L, cudaStream_t st, const float *src, int sw, int sh, const double H[9],

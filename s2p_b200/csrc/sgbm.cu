@@ -9,6 +9,22 @@ extern "C" int s2pb_sgbm_default_params(s2pb_sgbm_params *p)
     return S2PB_OK;
 }
 
+size_t order_stats_bytes() { return sizeof(OrderStats) + kOrdMaxRanks * 256 * sizeof(unsigned); }
+
+// The radix select of sgbm_kernels.cuh: four passes of one 8-bit digit over the n values of d_x, every rank at once.
+int launch_order_stats(s2pb_ctx *ctx, cudaStream_t st, const float *d_x, int n, int rule, double q0, double q1, OrderStats *d_os)
+{
+    unsigned *d_hist = (unsigned *)(d_os + 1);
+    CK(cudaMemsetAsync(d_os, 0, order_stats_bytes(), st));
+    const int hblocks = (int)std::max<size_t>(1, std::min<size_t>(((size_t)n + 255) / 256, (size_t)ctx->sm_count * 4));
+    for (int digit = 3; digit >= 0; digit--) {
+        launch(ctx, sgbm_hist_kernel, hblocks, 256, 0, st, d_x, n, digit, d_os, d_hist);
+        launch(ctx, sgbm_select_kernel, 1, 32, 0, st, digit, rule, q0, q1, d_os, d_hist);
+    }
+    CK(cudaGetLastError());
+    return S2PB_OK;
+}
+
 // The whole `sgbm im1 im2 disp cost dmin dmax win P1 P2 lr` run followed by create_rejection_mask, enqueued on the call's
 // stream.  d_im1 / d_im2 / d_disp: w*h float32, d_mask: w*h uint8 or null, all from L, which is checked before the first launch.
 static int sgbm_enqueue(s2pb_ctx *ctx, HostCall &L, const float *d_im1, const float *d_im2, int w, int h, int dmin, int dmax,
@@ -59,8 +75,7 @@ static int sgbm_enqueue(s2pb_ctx *ctx, HostCall &L, const float *d_im1, const fl
     if (ppix > INT32_MAX) return fail(S2PB_ERR_UNSUPPORTED, "at most 2^31 - 1 padded pixels");
     const size_t vol = any ? (size_t)h * g.w1 * ND : 0;
 
-    SgbmState *d_st = L.take<SgbmState>(sizeof(SgbmState) + 512 * 4);
-    unsigned *d_hist = (unsigned *)(d_st + 1);
+    SgbmState *d_st = L.take<SgbmState>(order_stats_bytes());
     uint8_t *q1 = L.take<uint8_t>(ppix), *q2 = L.take<uint8_t>(ppix);
     short *pix = any ? L.take<short>(vol * 2) : nullptr, *C = any ? L.take<short>(vol * 2) : nullptr;
     short *disp1 = L.take<short>(ppix * 2), *dmed = L.take<short>(ppix * 2);
@@ -68,13 +83,8 @@ static int sgbm_enqueue(s2pb_ctx *ctx, HostCall &L, const float *d_im1, const fl
     int *lab = L.take<int>(ppix * 4), *area = L.take<int>(ppix * 4);
     if (int rc = L.error()) return rc;
 
-    // qauto thresholds: four radix digits of both order statistics
-    CK(cudaMemsetAsync(d_st, 0, sizeof(SgbmState) + 512 * 4, st));
-    const int hblocks = (int)std::min<size_t>((npix + 255) / 256, (size_t)ctx->sm_count * 4);
-    for (int digit = 3; digit >= 0; digit--) {
-        launch(ctx, sgbm_hist_kernel, hblocks, 256, 0, st, d_im1, (int)npix, digit, d_st, d_hist);
-        launch(ctx, sgbm_select_kernel, 1, 32, 0, st, digit, d_st, d_hist);
-    }
+    // qauto thresholds: the two order statistics of get_rminmax
+    if (int rc = launch_order_stats(ctx, st, d_im1, (int)npix, kOrdQauto, 0.0, 0.0, d_st)) return rc;
     launch(ctx, sgbm_quantize_kernel, dim3((g.wp + 255) / 256, h), 256, 0, st, d_im1, d_im2, w, h, off, g.wp, d_st, q1, q2);
     launch(ctx, sgbm_fill_kernel, std::max(1, (int)std::min<size_t>((ppix + 255) / 256, 4096)), 256, 0, st, disp1, ppix, (short)invalid);
     if (any) {

@@ -13,6 +13,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include "union_find.cuh"
+#include "order_stats.h"
 
 namespace s2pb {
 
@@ -23,12 +24,7 @@ constexpr int kSgbmSpeckleWindow = 50;     // speckleWindowSize
 constexpr int kSgbmSpeckleRange = 16;      // speckleRange 1, times DISP_SCALE
 constexpr int kSgbmPixMax = 2 * kSgbmFtzero + (255 >> 2);   // largest per-pixel BT cost: Sobel channel + intensity >> 2
 
-struct SgbmState {
-    unsigned prefix[2];     // radix select: key bits found so far (rank N/200, rank N-1-N/200)
-    unsigned rank[2];       // ... rank still to find below that prefix
-    int n;                  // number of non-NaN pixels of im1
-    float rmin, rmax;       // qauto thresholds
-};
+typedef OrderStats SgbmState;
 
 // float -> unsigned key with the order of the floats (-0 sorts before +0; the two quantise alike)
 __device__ __forceinline__ unsigned sgbm_key(float f)
@@ -41,43 +37,81 @@ __device__ __forceinline__ float sgbm_unkey(unsigned k)
     return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
 }
 
-// one 8-bit digit of both order statistics (digit 3 = most significant); hist[2][256], zeroed by the caller
+// one 8-bit digit of every order statistic (digit 3 = most significant); hist[kOrdMaxRanks][256], zeroed by the caller.
+// Before the first pass every prefix is 0 and the mask keeps no bit, so all ranks count every value.
 __global__ void sgbm_hist_kernel(const float *__restrict__ im, int n, int digit, const SgbmState *__restrict__ st,
                                  unsigned *__restrict__ hist)
 {
-    __shared__ unsigned h[2][256];
-    for (int i = threadIdx.x; i < 512; i += blockDim.x) h[i >> 8][i & 255] = 0;
+    __shared__ unsigned h[kOrdMaxRanks][256];
+    for (int i = threadIdx.x; i < kOrdMaxRanks * 256; i += blockDim.x) h[i >> 8][i & 255] = 0;
     __syncthreads();
     const int shift = 8 * digit;
     const unsigned hi_mask = digit == 3 ? 0u : (0xffffffffu << (shift + 8));
-    const unsigned p0 = st->prefix[0], p1 = st->prefix[1];
+    const int nr = digit == 3 ? 1 : st->nranks;      // the first pass: one histogram of all values serves every rank
+    unsigned p[kOrdMaxRanks];
+    for (int r = 0; r < kOrdMaxRanks; r++) p[r] = st->prefix[r];
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
         const float f = im[i];
         if (isnan(f)) continue;
         const unsigned k = sgbm_key(f), b = (k >> shift) & 255u;
-        if ((k & hi_mask) == p0) atomicAdd(&h[0][b], 1u);
-        if ((k & hi_mask) == p1) atomicAdd(&h[1][b], 1u);
+#pragma unroll
+        for (int r = 0; r < kOrdMaxRanks; r++)
+            if (r < nr && (k & hi_mask) == p[r]) atomicAdd(&h[r][b], 1u);
     }
     __syncthreads();
-    for (int i = threadIdx.x; i < 512; i += blockDim.x)
+    for (int i = threadIdx.x; i < kOrdMaxRanks * 256; i += blockDim.x)
         if (h[i >> 8][i & 255]) atomicAdd(hist + i, h[i >> 8][i & 255]);
 }
 
-// one thread: the digit's bucket for both ranks.  After digit 0 the prefixes are the keys of rmin and rmax
-// (get_rminmax, sgbm.cpp:30-42: rb = N/200, rmin = tx[rb], rmax = tx[N-1-rb] of the sorted non-NaN values).
-__global__ void sgbm_select_kernel(int digit, SgbmState *st, unsigned *hist)
+// numpy's 'linear' quantile q of n sorted values (numpy/lib/_function_base_impl.py: _quantile with get_virtual_index
+// (n - 1) * q, _get_indexes, _get_gamma): the ranks of the two neighbours and the weight gamma
+__device__ __forceinline__ void ord_linear_ranks(unsigned n, double q, unsigned &prev, unsigned &next, double &gamma)
+{
+    const double vi = __dmul_rn((double)(n - 1), q);
+    if (vi >= (double)(n - 1)) {             // index -1 for both: the largest value; gamma = vi - (-1)
+        prev = next = n - 1;
+        gamma = __dadd_rn(vi, 1.0);
+    } else {
+        const double f = floor(vi);
+        prev = (unsigned)f; next = prev + 1;
+        gamma = __dsub_rn(vi, f);
+    }
+}
+
+// numpy's _lerp(a, b, t) for float32 (or narrower) a and b: b - a in the inputs' type, everything else in double
+__device__ __forceinline__ double ord_lerp(float a, float b, double t)
+{
+    const double d = (double)__fsub_rn(b, a);
+    if (t >= 0.5) return __dsub_rn((double)b, __dmul_rn(d, __dsub_rn(1.0, t)));
+    return __dadd_rn((double)a, __dmul_rn(d, t));
+}
+
+// one thread: the digit's bucket for every rank.  After digit 0 the prefixes are the keys of the order statistics.
+// kOrdQauto (get_rminmax, sgbm.cpp:30-42): rb = N/200, rmin = tx[rb], rmax = tx[N-1-rb] of the sorted non-NaN values.
+// kOrdLinear: the floor and ceiling ranks of the virtual index of q[0] and q[1], then their interpolation into lo and hi.
+__global__ void sgbm_select_kernel(int digit, int rule, double q0, double q1, SgbmState *st, unsigned *hist)
 {
     if (threadIdx.x != 0 || blockIdx.x != 0) return;
     if (digit == 3) {
+        st->rule = rule; st->q[0] = q0; st->q[1] = q1;
         unsigned n = 0;
         for (int b = 0; b < 256; b++) n += hist[b];
         st->n = (int)n;
-        const unsigned rb = n / 200;
-        st->rank[0] = rb;
-        st->rank[1] = n ? n - 1 - rb : 0;
-        st->prefix[0] = st->prefix[1] = 0;
+        if (st->rule == kOrdQauto) {
+            const unsigned rb = n / 200;
+            st->nranks = 2;
+            st->rank[0] = rb;
+            st->rank[1] = n ? n - 1 - rb : 0;
+        } else {
+            st->nranks = 4;
+            double g;
+            for (int k = 0; k < 2; k++) ord_linear_ranks(n ? n : 1, st->q[k], st->rank[2 * k], st->rank[2 * k + 1], g);
+        }
+        for (int r = 0; r < kOrdMaxRanks; r++) st->prefix[r] = 0;
+        for (int r = 1; r < st->nranks; r++)                     // the first pass counted every value once, for rank 0
+            for (int b = 0; b < 256; b++) hist[r * 256 + b] = hist[b];
     }
-    for (int r = 0; r < 2; r++) {
+    for (int r = 0; r < st->nranks; r++) {
         unsigned cum = 0, b = 0;
         for (; b < 255; b++) {
             if (st->rank[r] < cum + hist[r * 256 + b]) break;
@@ -86,8 +120,19 @@ __global__ void sgbm_select_kernel(int digit, SgbmState *st, unsigned *hist)
         st->prefix[r] |= b << (8 * digit);
         st->rank[r] -= cum;
     }
-    for (int i = 0; i < 512; i++) hist[i] = 0;
-    if (digit == 0) { st->rmin = sgbm_unkey(st->prefix[0]); st->rmax = sgbm_unkey(st->prefix[1]); }
+    for (int i = 0; i < kOrdMaxRanks * 256; i++) hist[i] = 0;
+    if (digit == 0) {
+        for (int r = 0; r < st->nranks; r++) st->v[r] = sgbm_unkey(st->prefix[r]);
+        st->rmin = st->v[0]; st->rmax = st->v[1];
+        if (st->rule == kOrdLinear) {
+            const double nan = __longlong_as_double(0x7ff8000000000000ll);
+            double g[2];
+            unsigned pr, nx;
+            for (int k = 0; k < 2; k++) ord_linear_ranks(st->n ? (unsigned)st->n : 1u, st->q[k], pr, nx, g[k]);
+            st->lo = st->n ? ord_lerp(st->v[0], st->v[1], g[0]) : nan;
+            st->hi = st->n ? ord_lerp(st->v[2], st->v[3], g[1]) : nan;
+        }
+    }
 }
 
 // qauto / qeasy (sgbm.cpp:44-71) into the padded 8-bit images: g = floor(255 * (x - rmin) / (rmax - rmin)) in float,

@@ -346,6 +346,99 @@ class Engine:
                                                   float(off_x), float(off_y), int(zone), int(bool(south))))
         return xyz
 
+    # ------------------------------------------------------------------ the tile's point cloud as PLY records
+    @staticmethod
+    def ply_dtype(nbands=3, confidence=False):
+        """The packed record write_to_ply writes: x, y, z float64, red, green, blue (and ir with 4 bands) uint8 when there are
+        colours (1, 3 or 4 bands), confidence float32 when asked."""
+        d = [("x", "<f8"), ("y", "<f8"), ("z", "<f8")]
+        if nbands:
+            d += [("red", "u1"), ("green", "u1"), ("blue", "u1")] + ([("ir", "u1")] if nbands == 4 else [])
+        if confidence:
+            d += [("confidence", "<f4")]
+        return np.dtype(d)
+
+    @staticmethod
+    def _bands(colors, shape):
+        """(nbands, h, w) or (h, w) colour planes -> C-contiguous (nbands, h, w) float32 and nbands (0 for None)"""
+        if colors is None:
+            return None, 0
+        c = np.asarray(colors)
+        c = c[None] if c.ndim == 2 else c
+        if c.ndim != 3 or c.shape[1:] != tuple(shape):
+            raise ValueError("expecting colour planes of shape (nbands, %d, %d), got %s" % (shape[0], shape[1], c.shape))
+        return np.ascontiguousarray(c, np.float32), c.shape[0]
+
+    def _records(self, call, npix, nbands, confidence):
+        dt = self.ply_dtype(nbands, confidence)
+        buf = np.empty(npix * dt.itemsize, np.uint8)
+        n = ctypes.c_int64(0)
+        _lib.check(call(buf.ctypes.data_as(ctypes.POINTER(ctypes.c_uint8)), ctypes.byref(n)))
+        return np.frombuffer(buf[:n.value * dt.itemsize].tobytes(), dt)
+
+    def stretch_8bit(self, img, p=1):
+        """common.linear_stretching_and_quantization_8bit(img, p) bit for bit (NumPy >= 2) on the device: the
+        percentiles run over every value of img together -> uint8 of img's shape.  img must convert to float32 exactly."""
+        a = np.ascontiguousarray(img, np.float32)
+        out = np.empty(a.shape, np.uint8)
+        _lib.check(self._L.s2pb_stretch_8bit(self._ctx, _fp(a), a.size, float(p), out.ctypes.data_as(ctypes.POINTER(ctypes.c_uint8))))
+        return out
+
+    def ply_records(self, xyz, colors=None, confidence=None):
+        """The vertex records write_to_ply writes for the cloud xyz (..., 3) float64: its points with three finite coordinates,
+        in order, with the uint8 colours (nbands, ...) and the float32 confidence (...) of those points -> structured array of
+        ply_dtype(nbands, confidence is not None)."""
+        a = np.ascontiguousarray(xyz, np.float64)
+        if a.ndim < 1 or a.shape[-1] != 3:
+            raise ValueError("expecting points of three coordinates, got shape %s" % (a.shape,))
+        n = a.size // 3
+        u8 = lambda v: v.ctypes.data_as(ctypes.POINTER(ctypes.c_uint8))
+        nb, col = 0, None
+        if colors is not None:
+            col = np.ascontiguousarray(colors, np.uint8).reshape(-1, n) if n else np.zeros((np.shape(colors)[0], 0), np.uint8)
+            nb = col.shape[0]
+        conf = None if confidence is None else np.ascontiguousarray(confidence, np.float32).reshape(n)
+        dp = a.ctypes.data_as(ctypes.POINTER(ctypes.c_double))
+        call = lambda out, cnt: self._L.s2pb_ply_records(self._ctx, dp, n, u8(col) if nb else None, nb,
+                                                         _fp(conf) if conf is not None else None, out, cnt)
+        return self._records(call, n, nb, conf is not None)
+
+    def disp_to_ply(self, disp, mask_rect, mask_orig, H1, H2, rpc1, rpc2, img_bbx, zone=0, south=False, r=0.0, p=0, n=0,
+                    colors=None, stretch_p=1, confidence=None, dispy=None):
+        """disp_to_xyz, the 3D filter (remove_isolated_3d_points(r, p, n, q=1); off when r == 0 or n == 0), the 8-bit stretch of
+        the colour planes (nbands, h, w) and the records of ply_records in one device call -> structured array."""
+        dispx, msk, mo = _f32(disp), _f32(mask_rect), _f32(mask_orig)
+        if dispx.ndim != 2 or msk.shape != dispx.shape or mo.ndim != 2:
+            raise ValueError("disp and mask_rect must be 2-D arrays of the same shape, and mask_orig a 2-D array")
+        h, w = dispx.shape
+        dy = np.zeros((h, w), np.float32) if dispy is None else _f32(dispy)
+        bands, nb = self._bands(colors, (h, w))
+        conf = None if confidence is None else _f32(confidence).reshape(h, w)
+        dp = lambda a: a.ctypes.data_as(ctypes.POINTER(ctypes.c_double))
+        Ha = np.ascontiguousarray(np.asarray(H1, np.float64).reshape(9))
+        Hb = np.ascontiguousarray(np.asarray(H2, np.float64).reshape(9))
+        bb = np.ascontiguousarray(np.asarray(img_bbx, np.float32).reshape(4))
+        call = lambda out, cnt: self._L.s2pb_disp_to_ply(
+            self._ctx, _fp(dispx), _fp(dy), _fp(msk), w, h, _fp(mo), mo.shape[1], mo.shape[0], dp(Ha), dp(Hb),
+            ctypes.cast(ctypes.pointer(rpc1), ctypes.c_void_p), ctypes.cast(ctypes.pointer(rpc2), ctypes.c_void_p), _fp(bb),
+            int(zone), int(bool(south)), float(r), operator.index(p), operator.index(n), _fp(bands) if nb else None, nb,
+            float(stretch_p), _fp(conf) if conf is not None else None, out, cnt)
+        return self._records(call, h * w, nb, conf is not None)
+
+    def height_map_to_ply(self, heights, rpc, off_x, off_y, zone=0, south=False, r=0.0, p=0, n=0, colors=None, stretch_p=1):
+        """height_map_to_xyz, the 3D filter, the 8-bit stretch of the colour planes and the records of ply_records in one device
+        call -> structured array (no confidence)."""
+        z = np.ascontiguousarray(heights, np.float64)
+        if z.ndim != 2:
+            raise ValueError("expecting a 2-D height map, got shape %s" % (z.shape,))
+        h, w = z.shape
+        bands, nb = self._bands(colors, (h, w))
+        call = lambda out, cnt: self._L.s2pb_height_map_to_ply(
+            self._ctx, z.ctypes.data_as(ctypes.POINTER(ctypes.c_double)), w, h, ctypes.cast(ctypes.pointer(rpc), ctypes.c_void_p),
+            float(off_x), float(off_y), int(zone), int(bool(south)), float(r), operator.index(p), operator.index(n),
+            _fp(bands) if nb else None, nb, float(stretch_p), out, cnt)
+        return self._records(call, h * w, nb, False)
+
     # ------------------------------------------------------------------ DSM rasterisation
     def plyflatten(self, clouds, record_bytes, columns, xoff, yoff, resolution, xsize, ysize):
         """plyflatten with radius 0 and no sigma on the roi (xoff, yoff, xsize, ysize) -> (ysize, xsize, len(columns) - 2)

@@ -56,6 +56,29 @@ def _read_all(path):
     return np.ascontiguousarray(a.astype(np.float32))
 
 
+def read_stored(path, window=None):
+    """-> (bands, h, w) array in the dtype the raster stores (rasterio's ``read()``); window = (x, y, w, h) or None"""
+    if _HAVE_RASTERIO:
+        with rasterio.open(path, "r") as f:
+            if window is None:
+                return np.ascontiguousarray(f.read())
+            x, y, w, h = window
+            return np.ascontiguousarray(f.read(window=((y, y + h), (x, x + w))))
+    import cv2
+    a = cv2.imread(path, cv2.IMREAD_UNCHANGED)
+    if a is None:
+        from PIL import Image
+        with Image.open(path) as im:
+            a = np.array(im)
+    elif a.ndim == 3:
+        a = a[..., ::-1]              # OpenCV stores BGR
+    a = a[None] if a.ndim == 2 else np.moveaxis(a, 2, 0)
+    if window is not None:
+        x, y, w, h = window
+        a = a[:, y:y + h, x:x + w]
+    return np.ascontiguousarray(a)
+
+
 def band_count(path):
     if _HAVE_RASTERIO:
         with rasterio.open(path, "r") as f:

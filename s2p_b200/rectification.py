@@ -55,11 +55,12 @@ def rectify_pair_and_match(im1, im2, rpc1, rpc2, x, y, w, h, out1, out2, disp, m
 
 def install():
     """Patch an importable s2p: both boundaries (matcher and warp) and the two "next" rows already served
-    (mask erosion, n-view merge) go to the H100 engine, and so do the triangulation steps and the DSM rasterisation."""
-    from . import block_matching, fusion, masking, rasterization, triangulation
+    (mask erosion, n-view merge) go to the H100 engine, and so do the triangulation steps, the tile's point cloud and the DSM rasterisation."""
+    from . import block_matching, cloud, fusion, masking, rasterization, triangulation
     common.install()
     block_matching.install()
     masking.install()
     fusion.install()
     triangulation.install()
     rasterization.install()
+    cloud.install()
