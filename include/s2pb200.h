@@ -216,16 +216,12 @@ typedef struct s2pb_rpc {
     double dmval[4], imval[4];
     double delta;
 } s2pb_rpc;
-/* Same argument list as lib/disp_to_h.so's disp_to_lonlatalt (c/disp_to_h.c:70-76), which
- * s2p.triangulation.disp_to_xyz calls through ctypes (s2p/triangulation.py:118-143), plus the context. */
-int s2pb_disp_to_lonlatalt(s2pb_ctx *ctx, double *lonlatalt, float *err, const float *dispx, const float *dispy,
-                           const float *msk, int nx, int ny, const float *msk_orig, int w, int h,
-                           const double ha[9], const double hb[9], const s2pb_rpc *rpca, const s2pb_rpc *rpcb,
-                           const float orig_img_bounding_box[4]);
 /* s2p.triangulation.disp_to_xyz (s2p/triangulation.py:85-162) for an output CRS of WGS84 / UTM (EPSG 32601-32660 north,
- * 32701-32760 south) in one call: s2pb_disp_to_lonlatalt's argument list, then the UTM zone (1..60, or 0: the output is
- * lon, lat, alt as they are) and south (non-zero: false northing 10 000 000 m).  The cloud is triangulated and projected as
- * s2pb_lonlat_to_utm projects it on the device; xyz (nx*ny*3 float64) and err (nx*ny float32) come back.
+ * 32701-32760 south) in one call: the argument list of lib/disp_to_h.so's disp_to_lonlatalt (c/disp_to_h.c:70-76), which
+ * s2p.triangulation.disp_to_xyz calls through ctypes (s2p/triangulation.py:118-143), plus the context, then the UTM zone
+ * (1..60, or 0: the output is lon, lat, alt as disp_to_lonlatalt writes them) and south (non-zero: false northing
+ * 10 000 000 m).  The cloud is triangulated and projected as s2pb_lonlat_to_utm projects it on the device; xyz (nx*ny*3
+ * float64) and err (nx*ny float32) come back.
  * S2PB_ERR_ARG: a null pointer, a size below 1, a zone outside 0..60. */
 int s2pb_disp_to_xyz(s2pb_ctx *ctx, double *xyz, float *err, const float *dispx, const float *dispy, const float *msk, int nx,
                      int ny, const float *msk_orig, int w, int h, const double ha[9], const double hb[9], const s2pb_rpc *rpca,
@@ -241,17 +237,17 @@ int s2pb_lonlat_to_utm(s2pb_ctx *ctx, double *xyz, const double *lonlatalt, int6
 /* ---- tri-stereo height maps (s2p/__init__.py disparity_to_height and heights_fusion) ---- */
 /* s2p.triangulation.height_map (s2p/triangulation.py:346-389) in one call.  disp, msk: the rectified disparity and mask,
  * nx*ny float32; mask_orig: the tile's mask as s2p reads it, mw*mh float32, unpadded (padded here by one row and column of
- * ones); (x, y, w, h): the tile in the reference image; H1, H2: the rectifying homographies; A (nullable): the pointing
- * correction, H2 <- H2 * A^-1 by the adjugate in C (the Python drop-in applies numpy's inverse itself and passes A = NULL).
- * Triangulates as s2pb_disp_to_lonlatalt inside the bounding box float32(x-1, x+w+2, y-1, y+h+2), keeps the altitude on
+ * ones); (x, y, w, h): the tile in the reference image; H1, H2: the rectifying homographies, H2 with the pointing correction
+ * already applied (H2 * A^-1, which the Python drop-in computes with numpy as the reference does).
+ * Triangulates as s2pb_disp_to_xyz with zone 0 inside the bounding box float32(x-1, x+w+2, y-1, y+h+2), keeps the altitude on
  * the device and writes out (h*w float64, row-major) = affine_transform(nan_to_num(alt).T, H1 * T(x, y),
  * output_shape=(w, h), order=1).T, NaN on the 3x3 dilation of the nearest-neighbour transform of isnan(alt).T (see
  * s2pb_resample_heights).  The third column of H1 * T(x, y) is summed left to right, H1[r][0]*x + H1[r][1]*y + H1[r][2].
  * S2PB_ERR_ARG: the last row of H1 * T(x, y) is not (0, 0, 1), which scipy refuses.
  * S2PB_ERR_UNSUPPORTED: nx or ny below 2 (the reference squeezes such a map to one dimension and fails). */
 int s2pb_height_map(s2pb_ctx *ctx, double *out, const float *disp, const float *msk, int nx, int ny, const float *mask_orig,
-                    int mw, int mh, int x, int y, int w, int h, const double H1[9], const double H2[9], const double *A,
-                    const s2pb_rpc *rpc1, const s2pb_rpc *rpc2);
+                    int mw, int mh, int x, int y, int w, int h, const double H1[9], const double H2[9], const s2pb_rpc *rpc1,
+                    const s2pb_rpc *rpc2);
 /* The resampling stage of s2pb_height_map alone, on a zw*zh float64 map z: scipy.ndimage.affine_transform(nan_to_num(z).T,
  * H, output_shape=(w, h), order=1, mode='constant', cval=0).T bit for bit, then NaN where
  * the 3x3 dilation (zero border) of affine_transform(isnan(z).T, H, output_shape=(w, h), order=0).T is set.

@@ -74,15 +74,13 @@ _SIGNATURES = {
     "s2pb_sgbm_default_params": (c_int, [POINTER(SgbmParams)]),
     "s2pb_sgbm": (c_int, [c_void_p, _f, _f, c_int, c_int, c_int, c_int, POINTER(SgbmParams), _f, POINTER(c_uint8)]),
     "s2pb_merge_n": (c_int, [c_void_p, POINTER(c_void_p), POINTER(c_double), c_int, c_int, c_int, c_int, c_double, _f]),
-    "s2pb_disp_to_lonlatalt": (c_int, [c_void_p, POINTER(c_double), _f, _f, _f, _f, c_int, c_int, _f, c_int, c_int,
-                                       POINTER(c_double), POINTER(c_double), c_void_p, c_void_p, _f]),
     "s2pb_disp_to_xyz": (c_int, [c_void_p, POINTER(c_double), _f, _f, _f, _f, c_int, c_int, _f, c_int, c_int,
                                  POINTER(c_double), POINTER(c_double), c_void_p, c_void_p, _f, c_int, c_int]),
     "s2pb_lonlat_to_utm": (c_int, [c_void_p, POINTER(c_double), POINTER(c_double), c_int64, c_int, c_int]),
     "s2pb_height_map_to_xyz": (c_int, [c_void_p, POINTER(c_double), POINTER(c_double), c_int, c_int, c_void_p, c_double, c_double,
                                        c_int, c_int]),
     "s2pb_height_map": (c_int, [c_void_p, POINTER(c_double), _f, _f, c_int, c_int, _f, c_int, c_int, c_int, c_int, c_int, c_int,
-                                POINTER(c_double), POINTER(c_double), POINTER(c_double), c_void_p, c_void_p]),
+                                POINTER(c_double), POINTER(c_double), c_void_p, c_void_p]),
     "s2pb_resample_heights": (c_int, [c_void_p, POINTER(c_double), c_int, c_int, POINTER(c_double), POINTER(c_double), c_int, c_int]),
     "s2pb_cargarse_basura": (c_int, [c_void_p, _f, _f, c_int, c_int]),
     "s2pb_count_3d_neighbors": (c_int, [c_void_p, POINTER(c_int32), POINTER(c_double), c_int, c_int, c_float, c_int]),

@@ -108,10 +108,11 @@ static int cloud_tail(s2pb_ctx *ctx, HostCall &L, double *d_xyz, int nx, int ny,
     return download_records(L, d_total, d_out, rb, records, npoints);
 }
 
-static int tail_args_ok(int nx, int ny, const float *bands, int nbands, double pct, uint8_t *records,
+// the arguments of the tail, checked before the cloud is made; the cloud's own step checks the rest
+static int tail_args_ok(s2pb_ctx *ctx, int nx, int ny, const float *bands, int nbands, double pct, uint8_t *records,
                         int64_t *npoints)
 {
-    if (!records || !npoints || (nbands && !bands)) return fail(S2PB_ERR_ARG, "bad argument");
+    if (!ctx || nx < 1 || ny < 1 || !records || !npoints || (nbands && !bands)) return fail(S2PB_ERR_ARG, "bad argument");
     if (!bands_ok(nbands)) return fail(S2PB_ERR_ARG, "colors must have either 1, 3 or 4 channels (got %d)", nbands);
     if (!(pct >= 0.0 && pct <= 100.0)) return fail(S2PB_ERR_ARG, "percentiles must be in the range [0, 100] (got %g)", pct);
     if ((size_t)nx * ny * std::max(nbands, 1) > INT32_MAX) return fail(S2PB_ERR_UNSUPPORTED, "at most 2^31 - 1 points and colour values");
@@ -123,21 +124,14 @@ extern "C" int s2pb_disp_to_ply(s2pb_ctx *ctx, const float *dispx, const float *
                                 const s2pb_rpc *rpcb, const float bbox[4], int zone, int south, float r, int p, int n,
                                 const float *bands, int nbands, double pct, const float *conf, uint8_t *records, int64_t *npoints)
 {
-    if (!ctx || !dispx || !dispy || !msk || !msk_orig || !ha || !hb || !rpca || !rpcb || !bbox || nx < 1 || ny < 1 || w < 1 || h < 1)
-        return fail(S2PB_ERR_ARG, "bad argument");
-    if (zone < 0 || zone > 60) return fail(S2PB_ERR_ARG, "UTM zone %d (1 to 60, or 0 for lon, lat, alt)", zone);
-    if (int rc = tail_args_ok(nx, ny, bands, nbands, pct, records, npoints)) return rc;
+    if (int rc = tail_args_ok(ctx, nx, ny, bands, nbands, pct, records, npoints)) return rc;
     *npoints = 0;
-    const size_t npix = (size_t)nx * ny, nm = (size_t)w * h;
     HostCall L(ctx, "the tile's cloud");
-    float *d_dx = L.upload(dispx, npix * 4), *d_dy = L.upload(dispy, npix * 4), *d_m = L.upload(msk, npix * 4);
-    float *d_mo = L.upload(msk_orig, nm * 4);
-    double *d_xyz = L.take<double>(npix * 24);
-    float *d_err = L.take<float>(npix * 4);
-    if (int rc = L.error()) return rc;
-    int rc = triangulate_enqueue(ctx, L.st, d_dx, d_dy, d_m, nx, ny, d_mo, w, h, ha, hb, rpca, rpcb, bbox, d_xyz, d_err);
-    if (rc == S2PB_OK && zone) rc = launch_utm_project(ctx, L.st, zone, south != 0, d_xyz, d_xyz, npix);
-    if (rc != S2PB_OK) return rc;
+    double *d_xyz = nullptr;
+    float *d_err = nullptr;
+    if (int rc = triangulated_cloud(ctx, L, dispx, dispy, msk, nx, ny, msk_orig, w, h, ha, hb, rpca, rpcb, bbox, zone, south, &d_xyz,
+                                    &d_err))
+        return rc;
     return cloud_tail(ctx, L, d_xyz, nx, ny, r, p, n, bands, nbands, pct, conf, records, npoints);
 }
 
@@ -145,19 +139,10 @@ extern "C" int s2pb_height_map_to_ply(s2pb_ctx *ctx, const double *heights, int 
                                       double off_y, int zone, int south, float r, int p, int n, const float *bands, int nbands,
                                       double pct, uint8_t *records, int64_t *npoints)
 {
-    if (!ctx || !heights || !rpc || w < 1 || h < 1) return fail(S2PB_ERR_ARG, "bad argument");
-    if (zone < 0 || zone > 60) return fail(S2PB_ERR_ARG, "UTM zone %d (1 to 60, or 0 for lon, lat, alt)", zone);
-    if (int rc = tail_args_ok(w, h, bands, nbands, pct, records, npoints)) return rc;
+    if (int rc = tail_args_ok(ctx, w, h, bands, nbands, pct, records, npoints)) return rc;
     *npoints = 0;
-    const size_t npix = (size_t)w * h;
     HostCall L(ctx, "the tile's cloud");
-    double *d_z = L.upload(heights, npix * 8), *d_xyz = L.take<double>(npix * 24);
-    int *d_capped = L.take<int>(4);
-    if (int rc = L.error()) return rc;
-    if (int rc = height_map_to_xyz_enqueue(ctx, L.st, d_z, w, h, rpc, off_x, off_y, zone, south, d_xyz, d_capped)) return rc;
-    int capped = 0;
-    L.download(&capped, d_capped, 4);
-    if (int rc = L.finish()) return rc;
-    if (capped) return fail(S2PB_ERR_ARG, "the localisation of %d pixel(s) did not converge in 1000 steps", capped);
+    double *d_xyz = nullptr;
+    if (int rc = localised_cloud(ctx, L, heights, w, h, rpc, off_x, off_y, zone, south, &d_xyz)) return rc;
     return cloud_tail(ctx, L, d_xyz, w, h, r, p, n, bands, nbands, pct, nullptr, records, npoints);
 }

@@ -11,9 +11,9 @@
 static_assert(sizeof(s2pb_rpc) == sizeof(RpcModel), "s2pb_rpc must have the layout of the reference's struct rpc");
 
 // disp_to_lonlatalt (c/disp_to_h.c:70-141) on device buffers: lonlatalt nx*ny*3 doubles, err nx*ny floats
-int triangulate_enqueue(s2pb_ctx *ctx, cudaStream_t st, const float *d_dx, const float *d_dy, const float *d_m, int nx, int ny,
-                               const float *d_mo, int w, int h, const double ha[9], const double hb[9], const s2pb_rpc *rpca,
-                               const s2pb_rpc *rpcb, const float bbox[4], double *d_out, float *d_err)
+static int triangulate_enqueue(s2pb_ctx *ctx, cudaStream_t st, const float *d_dx, const float *d_dy, const float *d_m, int nx,
+                               int ny, const float *d_mo, int w, int h, const double ha[9], const double hb[9],
+                               const s2pb_rpc *rpca, const s2pb_rpc *rpcb, const float bbox[4], double *d_out, float *d_err)
 {
     TriParams P;
     memset(&P, 0, sizeof P);
@@ -30,26 +30,29 @@ int triangulate_enqueue(s2pb_ctx *ctx, cudaStream_t st, const float *d_dx, const
     return S2PB_OK;
 }
 
-// Same argument list as the reference's ctypes entry point disp_to_lonlatalt (c/disp_to_h.c:70-76), plus the context.
-extern "C" int s2pb_disp_to_lonlatalt(s2pb_ctx *ctx, double *lonlatalt, float *err, const float *dispx, const float *dispy,
-                                      const float *msk, int nx, int ny, const float *msk_orig, int w, int h, const double ha[9],
-                                      const double hb[9], const s2pb_rpc *rpca, const s2pb_rpc *rpcb, const float bbox[4])
+// the output CRS of a cloud: UTM zone 1..60, or 0 for lon, lat, alt as they are
+static int cloud_zone_ok(int zone)
 {
-    if (!ctx || !lonlatalt || !err || !dispx || !dispy || !msk || !msk_orig || !ha || !hb || !rpca || !rpcb || !bbox || nx < 1 ||
-        ny < 1 || w < 1 || h < 1)
+    if (zone < 0 || zone > 60) return fail(S2PB_ERR_ARG, "UTM zone %d (1 to 60, or 0 for lon, lat, alt)", zone);
+    return S2PB_OK;
+}
+
+int triangulated_cloud(s2pb_ctx *ctx, HostCall &L, const float *dispx, const float *dispy, const float *msk, int nx, int ny,
+                       const float *msk_orig, int w, int h, const double ha[9], const double hb[9], const s2pb_rpc *rpca,
+                       const s2pb_rpc *rpcb, const float bbox[4], int zone, int south, double **d_xyz, float **d_err)
+{
+    if (!dispx || !dispy || !msk || !msk_orig || !ha || !hb || !rpca || !rpcb || !bbox || nx < 1 || ny < 1 || w < 1 || h < 1)
         return fail(S2PB_ERR_ARG, "bad argument");
+    if (int rc = cloud_zone_ok(zone)) return rc;
     const size_t npix = (size_t)nx * ny, nm = (size_t)w * h;
-    HostCall L(ctx, "the triangulation");
     float *d_dx = L.upload(dispx, npix * 4), *d_dy = L.upload(dispy, npix * 4), *d_m = L.upload(msk, npix * 4);
     float *d_mo = L.upload(msk_orig, nm * 4);
-    double *d_out = L.take<double>(npix * 24);
-    float *d_err = L.take<float>(npix * 4);
+    *d_xyz = L.take<double>(npix * 24);
+    *d_err = L.take<float>(npix * 4);
     if (int rc = L.error()) return rc;
-    int rc = triangulate_enqueue(ctx, L.st, d_dx, d_dy, d_m, nx, ny, d_mo, w, h, ha, hb, rpca, rpcb, bbox, d_out, d_err);
-    if (rc != S2PB_OK) return rc;
-    L.download(lonlatalt, d_out, npix * 24);
-    L.download(err, d_err, npix * 4);
-    return L.finish();
+    int rc = triangulate_enqueue(ctx, L.st, d_dx, d_dy, d_m, nx, ny, d_mo, w, h, ha, hb, rpca, rpcb, bbox, *d_xyz, *d_err);
+    if (rc == S2PB_OK && zone) rc = launch_utm_project(ctx, L.st, zone, south != 0, *d_xyz, *d_xyz, npix);
+    return rc;
 }
 
 // s2p.triangulation.disp_to_xyz (s2p/triangulation.py:85-162) with a UTM (or no) output CRS: disp_to_lonlatalt, then the
@@ -58,40 +61,45 @@ extern "C" int s2pb_disp_to_xyz(s2pb_ctx *ctx, double *xyz, float *err, const fl
                                 int nx, int ny, const float *msk_orig, int w, int h, const double ha[9], const double hb[9],
                                 const s2pb_rpc *rpca, const s2pb_rpc *rpcb, const float bbox[4], int zone, int south)
 {
-    if (!ctx || !xyz || !err || !dispx || !dispy || !msk || !msk_orig || !ha || !hb || !rpca || !rpcb || !bbox || nx < 1 ||
-        ny < 1 || w < 1 || h < 1)
-        return fail(S2PB_ERR_ARG, "bad argument");
-    if (zone < 0 || zone > 60) return fail(S2PB_ERR_ARG, "UTM zone %d (1 to 60, or 0 for lon, lat, alt)", zone);
-    const size_t npix = (size_t)nx * ny, nm = (size_t)w * h;
+    if (!ctx || !xyz || !err) return fail(S2PB_ERR_ARG, "bad argument");
     HostCall L(ctx, "the triangulation");
-    float *d_dx = L.upload(dispx, npix * 4), *d_dy = L.upload(dispy, npix * 4), *d_m = L.upload(msk, npix * 4);
-    float *d_mo = L.upload(msk_orig, nm * 4);
-    double *d_out = L.take<double>(npix * 24);
-    float *d_err = L.take<float>(npix * 4);
-    if (int rc = L.error()) return rc;
-    int rc = triangulate_enqueue(ctx, L.st, d_dx, d_dy, d_m, nx, ny, d_mo, w, h, ha, hb, rpca, rpcb, bbox, d_out, d_err);
-    if (rc == S2PB_OK && zone) rc = launch_utm_project(ctx, L.st, zone, south != 0, d_out, d_out, npix);
-    if (rc != S2PB_OK) return rc;
-    L.download(xyz, d_out, npix * 24);
+    double *d_xyz = nullptr;
+    float *d_err = nullptr;
+    if (int rc = triangulated_cloud(ctx, L, dispx, dispy, msk, nx, ny, msk_orig, w, h, ha, hb, rpca, rpcb, bbox, zone, south, &d_xyz,
+                                    &d_err))
+        return rc;
+    const size_t npix = (size_t)nx * ny;
+    L.download(xyz, d_xyz, npix * 24);
     L.download(err, d_err, npix * 4);
     return L.finish();
 }
 
-// every pixel of the device height map d_z localised by the camera into d_out (w*h*3 doubles), then projected to UTM zone
-// `zone` in place (0: none); d_capped (one int, zeroed here) counts the pixels whose iteration hit its cap
-int height_map_to_xyz_enqueue(s2pb_ctx *ctx, cudaStream_t st, const double *d_z, int w, int h, const s2pb_rpc *rpc, double off_x,
-                              double off_y, int zone, int south, double *d_out, int *d_capped)
+int localised_cloud(s2pb_ctx *ctx, HostCall &L, const double *heights, int w, int h, const s2pb_rpc *rpc, double off_x,
+                    double off_y, int zone, int south, double **d_xyz)
 {
-    CK(cudaMemsetAsync(d_capped, 0, 4, st));
+    if (!heights || !rpc || w < 1 || h < 1) return fail(S2PB_ERR_ARG, "bad argument");
+    if (int rc = cloud_zone_ok(zone)) return rc;
+    const size_t npix = (size_t)w * h;
+    double *d_z = L.upload(heights, npix * 8);
+    *d_xyz = L.take<double>(npix * 24);
+    int *d_capped = L.take<int>(4);
+    if (int rc = L.error()) return rc;
+    CK(cudaMemsetAsync(d_capped, 0, 4, L.st));
     HeightMapParams P;
     memset(&P, 0, sizeof P);
     P.heights = d_z; P.w = w; P.h = h; P.off_x = off_x; P.off_y = off_y;
     memcpy(&P.rpc, rpc, sizeof(RpcModel));
-    P.xyz = d_out; P.capped = d_capped;
+    P.xyz = *d_xyz; P.capped = d_capped;
     const dim3 b2(32, 4);
-    launch(ctx, height_map_to_xyz_kernel, grid2d(w, h, b2), b2, 0, st, P);
+    launch(ctx, height_map_to_xyz_kernel, grid2d(w, h, b2), b2, 0, L.st, P);
     CK(cudaGetLastError());
-    if (zone) return launch_utm_project(ctx, st, zone, south != 0, d_out, d_out, (size_t)w * h);
+    if (zone) {
+        if (int rc = launch_utm_project(ctx, L.st, zone, south != 0, *d_xyz, *d_xyz, npix)) return rc;
+    }
+    int capped = 0;
+    L.download(&capped, d_capped, 4);
+    if (int rc = L.finish()) return rc;
+    if (capped) return fail(S2PB_ERR_ARG, "the localisation of %d pixel(s) did not converge in 1000 steps", capped);
     return S2PB_OK;
 }
 
@@ -100,20 +108,12 @@ int height_map_to_xyz_enqueue(s2pb_ctx *ctx, cudaStream_t st, const double *d_z,
 extern "C" int s2pb_height_map_to_xyz(s2pb_ctx *ctx, double *xyz, const double *heights, int w, int h, const s2pb_rpc *rpc,
                                       double off_x, double off_y, int zone, int south)
 {
-    if (!ctx || !xyz || !heights || !rpc || w < 1 || h < 1) return fail(S2PB_ERR_ARG, "bad argument");
-    if (zone < 0 || zone > 60) return fail(S2PB_ERR_ARG, "UTM zone %d (1 to 60, or 0 for lon, lat, alt)", zone);
-    const size_t npix = (size_t)w * h;
+    if (!ctx || !xyz) return fail(S2PB_ERR_ARG, "bad argument");
     HostCall L(ctx, "the localisation");
-    double *d_z = L.upload(heights, npix * 8), *d_out = L.take<double>(npix * 24);
-    int *d_capped = L.take<int>(4);
-    if (int rc = L.error()) return rc;
-    if (int rc = height_map_to_xyz_enqueue(ctx, L.st, d_z, w, h, rpc, off_x, off_y, zone, south, d_out, d_capped)) return rc;
-    int capped = 0;
-    L.download(xyz, d_out, npix * 24);
-    L.download(&capped, d_capped, 4);
-    if (int rc = L.finish()) return rc;
-    if (capped) return fail(S2PB_ERR_ARG, "the localisation of %d pixel(s) did not converge in 1000 steps", capped);
-    return S2PB_OK;
+    double *d_xyz = nullptr;
+    if (int rc = localised_cloud(ctx, L, heights, w, h, rpc, off_x, off_y, zone, south, &d_xyz)) return rc;
+    L.download(xyz, d_xyz, (size_t)w * h * 24);
+    return L.finish();
 }
 
 // ------------------------------------------------------------------ tri-stereo height maps (section 8f)
@@ -156,21 +156,12 @@ extern "C" int s2pb_resample_heights(s2pb_ctx *ctx, const double *z, int zw, int
 // and resample it onto the tile grid through H1 * T(x, y).
 extern "C" int s2pb_height_map(s2pb_ctx *ctx, double *out, const float *disp, const float *msk, int nx, int ny,
                                const float *mask_orig, int mw, int mh, int x, int y, int w, int h, const double H1[9],
-                               const double H2[9], const double *A, const s2pb_rpc *rpc1, const s2pb_rpc *rpc2)
+                               const double H2[9], const s2pb_rpc *rpc1, const s2pb_rpc *rpc2)
 {
     if (!ctx || !out || !disp || !msk || !mask_orig || !H1 || !H2 || !rpc1 || !rpc2 || nx < 1 || ny < 1 || mw < 1 || mh < 1 ||
         w < 1 || h < 1)
         return fail(S2PB_ERR_ARG, "bad argument");
     if (nx < 2 || ny < 2) return fail(S2PB_ERR_UNSUPPORTED, "a %dx%d rectified map (the reference squeezes it to 1-D)", nx, ny);
-    double Hb[9];
-    if (A) {                                        // H2 * A^-1 (s2p/triangulation.py:114-115)
-        double Ai[9];
-        invert_homography(A, Ai);
-        for (int r = 0; r < 3; r++)
-            for (int q = 0; q < 3; q++) Hb[3 * r + q] = H2[3 * r] * Ai[q] + H2[3 * r + 1] * Ai[3 + q] + H2[3 * r + 2] * Ai[6 + q];
-    } else {
-        memcpy(Hb, H2, sizeof Hb);
-    }
     // H1 * T(x, y): the first two columns are H1's, the third H1 (x, y, 1)^T summed left to right
     double H[9];
     memcpy(H, H1, sizeof H);
@@ -186,7 +177,7 @@ extern "C" int s2pb_height_map(s2pb_ctx *ctx, double *out, const float *disp, co
     CK(cudaMemsetAsync(d_dy, 0, npix * 4, L.st));
     const dim3 b2(32, 8);
     launch(ctx, pad_ones_kernel, grid2d((int)pw, (int)ph, b2), b2, 0, L.st, d_mo0, mw, mh, d_mo);
-    int rc = triangulate_enqueue(ctx, L.st, d_dx, d_dy, d_m, nx, ny, d_mo, (int)pw, (int)ph, H1, Hb, rpc1, rpc2, bbox, d_xyz, d_err);
+    int rc = triangulate_enqueue(ctx, L.st, d_dx, d_dy, d_m, nx, ny, d_mo, (int)pw, (int)ph, H1, H2, rpc1, rpc2, bbox, d_xyz, d_err);
     if (rc == S2PB_OK) rc = resample_heights_enqueue(ctx, L.st, d_xyz + 2, 3, nx, ny, H, d_out, w, h);
     if (rc != S2PB_OK) return rc;
     L.download(out, d_out, (size_t)w * h * 8);

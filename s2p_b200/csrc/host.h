@@ -236,13 +236,16 @@ void launch_rejection_mask(s2pb_ctx *ctx, const float *disp, const float *im1, c
                            cudaStream_t st);
 // projection.cu: (lon, lat, alt) -> UTM zone `zone` (1..60) of n device points, in place when d_in == d_out
 int launch_utm_project(s2pb_ctx *ctx, cudaStream_t st, int zone, bool south, const double *d_in, double *d_out, size_t n);
-// geometry.cu: disp_to_lonlatalt, height_map_to_xyz (with the projection to UTM zone `zone`, 0 none) and
-// remove_isolated_3d_points (n > 0; d_work: 3 * nx * ny ints) on device buffers
-int triangulate_enqueue(s2pb_ctx *ctx, cudaStream_t st, const float *d_dx, const float *d_dy, const float *d_m, int nx, int ny,
-                        const float *d_mo, int w, int h, const double ha[9], const double hb[9], const s2pb_rpc *rpca,
-                        const s2pb_rpc *rpcb, const float bbox[4], double *d_out, float *d_err);
-int height_map_to_xyz_enqueue(s2pb_ctx *ctx, cudaStream_t st, const double *d_z, int w, int h, const s2pb_rpc *rpc, double off_x,
-                              double off_y, int zone, int south, double *d_out, int *d_capped);
+// geometry.cu: the two clouds of a host call, each from host buffers into scratch of L after the checks of its arguments, then
+// projected in place to UTM zone `zone` (0: none).  triangulated_cloud: disp_to_lonlatalt of s2pb_disp_to_xyz's inputs, *d_xyz
+// nx*ny*3 doubles and *d_err nx*ny floats, still in flight on L.st.  localised_cloud: s2pb_height_map_to_xyz's localisation,
+// *d_xyz w*h*3 doubles, complete on return (the pixels whose iteration hit its cap are an error).  remove_isolated_3d_points
+// (n > 0; d_work: 3 * nx * ny ints) on device buffers.
+int triangulated_cloud(s2pb_ctx *ctx, HostCall &L, const float *dispx, const float *dispy, const float *msk, int nx, int ny,
+                       const float *msk_orig, int w, int h, const double ha[9], const double hb[9], const s2pb_rpc *rpca,
+                       const s2pb_rpc *rpcb, const float bbox[4], int zone, int south, double **d_xyz, float **d_err);
+int localised_cloud(s2pb_ctx *ctx, HostCall &L, const double *heights, int w, int h, const s2pb_rpc *rpc, double off_x,
+                    double off_y, int zone, int south, double **d_xyz);
 int remove_isolated_enqueue(s2pb_ctx *ctx, cudaStream_t st, double *d_xyz, int nx, int ny, float r, int p, int n, int q, int *d_work);
 // sgbm.cu: order statistics of the non-NaN values of n device floats by radix select (sgbm_kernels.cuh) into d_os, which
 // holds order_stats_bytes(); rule kOrdQauto (qauto's thresholds) or kOrdLinear (numpy's 'linear' quantiles q0 and q1)

@@ -44,6 +44,28 @@ def _fp(a):
     return a.ctypes.data_as(ctypes.POINTER(ctypes.c_float))
 
 
+def _dp(a):
+    return a.ctypes.data_as(ctypes.POINTER(ctypes.c_double))
+
+
+def _u8(a):
+    return a.ctypes.data_as(ctypes.POINTER(ctypes.c_uint8))
+
+
+def _ip(a):
+    return a.ctypes.data_as(ctypes.POINTER(ctypes.c_int32))
+
+
+def _mat3(H):
+    """a 3x3 matrix as 9 contiguous float64 (the pointer keeps its array alive)"""
+    return _dp(np.ascontiguousarray(np.asarray(H, np.float64).reshape(9)))
+
+
+def _rpc(rpc):
+    """a ctypes structure with the layout of ``triangulation.RPCStruct``, as the ``const s2pb_rpc *`` of the C ABI"""
+    return ctypes.cast(ctypes.pointer(rpc), ctypes.c_void_p)
+
+
 class Engine:
     def __init__(self, device=0):
         L = _lib.lib()
@@ -95,8 +117,7 @@ class Engine:
             pl, pr = np.empty((h, w), np.float32), np.empty((h, w), np.float32)
             _lib.check(self._L.s2pb_mgm_pkr(
                 self._ctx, _fp(im1), _fp(im2), w, h, int(dmin), int(dmax), ctypes.byref(p), _fp(disp), _fp(conf),
-                mask.ctypes.data_as(ctypes.POINTER(ctypes.c_uint8)) if want_mask else None,
-                _fp(right) if want_right else None, _fp(pl), _fp(pr)))
+                _u8(mask) if want_mask else None, _fp(right) if want_right else None, _fp(pl), _fp(pr)))
             out = dict(disp=disp, conf=conf, mask=mask, pkr_left=pl, pkr_right=pr)
             if want_right:
                 out["disp_right"] = right
@@ -104,8 +125,7 @@ class Engine:
         _lib.check(self._L.s2pb_mgm_weighted(
             self._ctx, _fp(im1), _fp(im2), w, h, int(dmin), int(dmax), ctypes.byref(p),
             _fp(wl) if wl is not None else None, _fp(wr) if wr is not None else None, _fp(disp), _fp(conf),
-            mask.ctypes.data_as(ctypes.POINTER(ctypes.c_uint8)) if want_mask else None,
-            _fp(right) if want_right else None))
+            _u8(mask) if want_mask else None, _fp(right) if want_right else None))
         out = dict(disp=disp, conf=conf, mask=mask)
         if want_right:
             out["disp_right"] = right
@@ -134,7 +154,7 @@ class Engine:
         disp = np.empty((h, w), np.float32)
         mask = np.empty((h, w), np.uint8) if want_mask else None
         _lib.check(self._L.s2pb_sgbm(self._ctx, _fp(im1), _fp(im2), w, h, int(dmin), int(dmax), ctypes.byref(p), _fp(disp),
-                                     mask.ctypes.data_as(ctypes.POINTER(ctypes.c_uint8)) if want_mask else None))
+                                     _u8(mask) if want_mask else None))
         return dict(disp=disp, mask=mask)
 
     def mgm_batch(self, refs, secs, dmin, dmax, params=None, want_mask=True, out=None):
@@ -191,13 +211,11 @@ class Engine:
         src = _f32(src)
         if src.ndim != 2:
             raise ValueError("src must be a 2-D array")
-        Hm = np.ascontiguousarray(np.asarray(H, dtype=np.float64).reshape(9))
         if out is None:
             out = np.empty((int(h), int(w)), np.float32)
         elif out.shape != (int(h), int(w)) or out.dtype != np.float32 or not out.flags.c_contiguous:
             raise ValueError("out must be a C-contiguous float32 array of shape (h, w)")     # e.g. a page-locked buffer: DMA'd directly
-        _lib.check(self._L.s2pb_homography(self._ctx, _fp(src), src.shape[1], src.shape[0],
-                                           Hm.ctypes.data_as(ctypes.POINTER(ctypes.c_double)), _fp(out), int(w), int(h)))
+        _lib.check(self._L.s2pb_homography(self._ctx, _fp(src), src.shape[1], src.shape[0], _mat3(H), _fp(out), int(w), int(h)))
         return out
 
     def rectify_match(self, src1, H1, src2, H2, w, h, dmin, dmax, params=None, want_rect=True, want_right=False):
@@ -206,8 +224,6 @@ class Engine:
         src1, src2 = _f32(src1), _f32(src2)
         p = params or default_params("mgm")
         w, h = int(w), int(h)
-        dp = lambda a: np.ascontiguousarray(np.asarray(a, dtype=np.float64).reshape(9)).ctypes.data_as(ctypes.POINTER(ctypes.c_double))
-        Ha, Hb = np.ascontiguousarray(np.asarray(H1, np.float64).reshape(9)), np.ascontiguousarray(np.asarray(H2, np.float64).reshape(9))
         out = dict(disp=np.empty((h, w), np.float32), conf=np.empty((h, w), np.float32), mask=np.empty((h, w), np.uint8))
         if want_rect:
             out["rect1"], out["rect2"] = np.empty((h, w), np.float32), np.empty((h, w), np.float32)
@@ -215,10 +231,9 @@ class Engine:
             out["disp_right"] = np.empty((h, w), np.float32)
         nul = ctypes.POINTER(ctypes.c_float)()
         _lib.check(self._L.s2pb_rectify_match(
-            self._ctx, _fp(src1), src1.shape[1], src1.shape[0], Ha.ctypes.data_as(ctypes.POINTER(ctypes.c_double)),
-            _fp(src2), src2.shape[1], src2.shape[0], Hb.ctypes.data_as(ctypes.POINTER(ctypes.c_double)), w, h, int(dmin), int(dmax),
-            ctypes.byref(p), _fp(out["rect1"]) if want_rect else nul, _fp(out["rect2"]) if want_rect else nul, _fp(out["disp"]),
-            _fp(out["conf"]), out["mask"].ctypes.data_as(ctypes.POINTER(ctypes.c_uint8)), _fp(out["disp_right"]) if want_right else nul))
+            self._ctx, _fp(src1), src1.shape[1], src1.shape[0], _mat3(H1), _fp(src2), src2.shape[1], src2.shape[0], _mat3(H2), w, h,
+            int(dmin), int(dmax), ctypes.byref(p), _fp(out["rect1"]) if want_rect else nul, _fp(out["rect2"]) if want_rect else nul,
+            _fp(out["disp"]), _fp(out["conf"]), _u8(out["mask"]), _fp(out["disp_right"]) if want_right else nul))
         return out
 
     # ------------------------------------------------------------------ n-view merge
@@ -255,8 +270,7 @@ class Engine:
         m = np.ascontiguousarray(mask, dtype=np.uint8)
         h, w = m.shape
         out = np.empty_like(m)
-        u8 = lambda a: a.ctypes.data_as(ctypes.POINTER(ctypes.c_uint8))
-        _lib.check(self._L.s2pb_erode_mask(self._ctx, u8(m), u8(out), w, h, float(radius)))
+        _lib.check(self._L.s2pb_erode_mask(self._ctx, _u8(m), _u8(out), w, h, float(radius)))
         return out
 
     # ------------------------------------------------------------------ 3D outlier filter of triangulation
@@ -278,9 +292,7 @@ class Engine:
         h, w = a.shape[:2]
         out = np.zeros((h, w), np.int32)
         if a.size:
-            _lib.check(self._L.s2pb_count_3d_neighbors(self._ctx, out.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)),
-                                                        a.ctypes.data_as(ctypes.POINTER(ctypes.c_double)), w, h, float(r),
-                                                        operator.index(p)))
+            _lib.check(self._L.s2pb_count_3d_neighbors(self._ctx, _ip(out), _dp(a), w, h, float(r), operator.index(p)))
         return out
 
     def remove_isolated_3d_points(self, xyz, r, p, n, q=1):
@@ -291,15 +303,14 @@ class Engine:
         if not a.flags.writeable:
             raise ValueError("the point cloud is read-only")
         if a.size:
-            _lib.check(self._L.s2pb_remove_isolated_3d_points(self._ctx, a.ctypes.data_as(ctypes.POINTER(ctypes.c_double)), w, h,
-                                                               float(r), operator.index(p), operator.index(n), operator.index(q)))
+            _lib.check(self._L.s2pb_remove_isolated_3d_points(self._ctx, _dp(a), w, h, float(r), operator.index(p),
+                                                               operator.index(n), operator.index(q)))
         return a
 
     # ------------------------------------------------------------------ triangulation into output coordinates
-    def disp_to_xyz(self, disp, mask_rect, mask_orig, H1, H2, rpc1, rpc2, img_bbx, zone=0, south=False, dispy=None):
-        """disp_to_lonlatalt and the projection to UTM zone `zone` (1..60; 0: lon, lat, alt as they are) in one device call
-        -> (xyz (h, w, 3) float64, err (h, w) float32).  rpc1 / rpc2: ctypes structures with the layout of
-        ``triangulation.RPCStruct``; H2 already carries the pointing correction."""
+    @staticmethod
+    def _triangulation(disp, mask_rect, mask_orig, H1, H2, rpc1, rpc2, img_bbx, zone, south, dispy):
+        """-> (h, w) of the rectified map and s2pb_disp_to_xyz's arguments from dispx to south, checked and converted"""
         dispx, msk, mo = _f32(disp), _f32(mask_rect), _f32(mask_orig)
         if dispx.ndim != 2 or msk.shape != dispx.shape or mo.ndim != 2:
             raise ValueError("disp and mask_rect must be 2-D arrays of the same shape, and mask_orig a 2-D array")
@@ -307,16 +318,27 @@ class Engine:
         dy = np.zeros((h, w), np.float32) if dispy is None else _f32(dispy)
         if dy.shape != dispx.shape:
             raise ValueError("dispy must have the shape of disp")
-        dp = lambda a: a.ctypes.data_as(ctypes.POINTER(ctypes.c_double))
-        Ha = np.ascontiguousarray(np.asarray(H1, np.float64).reshape(9))
-        Hb = np.ascontiguousarray(np.asarray(H2, np.float64).reshape(9))
         bb = np.ascontiguousarray(np.asarray(img_bbx, np.float32).reshape(4))
+        return (h, w), (_fp(dispx), _fp(dy), _fp(msk), w, h, _fp(mo), mo.shape[1], mo.shape[0], _mat3(H1), _mat3(H2), _rpc(rpc1),
+                        _rpc(rpc2), _fp(bb), int(zone), int(bool(south)))
+
+    @staticmethod
+    def _localisation(heights, rpc, off_x, off_y, zone, south):
+        """-> (h, w) of the height map and s2pb_height_map_to_xyz's arguments from heights to south, checked and converted"""
+        z = np.ascontiguousarray(heights, np.float64)
+        if z.ndim != 2:
+            raise ValueError("expecting a 2-D height map, got shape %s" % (z.shape,))
+        h, w = z.shape
+        return (h, w), (_dp(z), w, h, _rpc(rpc), float(off_x), float(off_y), int(zone), int(bool(south)))
+
+    def disp_to_xyz(self, disp, mask_rect, mask_orig, H1, H2, rpc1, rpc2, img_bbx, zone=0, south=False, dispy=None):
+        """disp_to_lonlatalt and the projection to UTM zone `zone` (1..60; 0: lon, lat, alt as they are) in one device call
+        -> (xyz (h, w, 3) float64, err (h, w) float32).  rpc1 / rpc2: ctypes structures with the layout of
+        ``triangulation.RPCStruct``; H2 already carries the pointing correction."""
+        (h, w), args = self._triangulation(disp, mask_rect, mask_orig, H1, H2, rpc1, rpc2, img_bbx, zone, south, dispy)
         xyz = np.empty((h, w, 3), np.float64)
         err = np.empty((h, w), np.float32)
-        _lib.check(self._L.s2pb_disp_to_xyz(self._ctx, dp(xyz), _fp(err), _fp(dispx), _fp(dy), _fp(msk), w, h, _fp(mo),
-                                            mo.shape[1], mo.shape[0], dp(Ha), dp(Hb),
-                                            ctypes.cast(ctypes.pointer(rpc1), ctypes.c_void_p),
-                                            ctypes.cast(ctypes.pointer(rpc2), ctypes.c_void_p), _fp(bb), int(zone), int(bool(south))))
+        _lib.check(self._L.s2pb_disp_to_xyz(self._ctx, _dp(xyz), _fp(err), *args))
         return xyz, err
 
     def lonlat_to_utm(self, lonlatalt, zone, south=False):
@@ -326,8 +348,7 @@ class Engine:
         if a.ndim < 1 or a.shape[-1] != 3:
             raise ValueError("expecting points of three coordinates, got shape %s" % (a.shape,))
         out = np.empty_like(a)
-        dp = lambda v: v.ctypes.data_as(ctypes.POINTER(ctypes.c_double))
-        _lib.check(self._L.s2pb_lonlat_to_utm(self._ctx, dp(out), dp(a), a.size // 3, int(zone), int(bool(south))))
+        _lib.check(self._L.s2pb_lonlat_to_utm(self._ctx, _dp(out), _dp(a), a.size // 3, int(zone), int(bool(south))))
         return out
 
     def height_map_to_xyz(self, heights, rpc, off_x, off_y, zone=0, south=False):
@@ -336,14 +357,9 @@ class Engine:
         camera ``rpc`` (a ctypes structure with the layout of ``triangulation.RPCStruct``); its third coordinate is the height
         converted to float64.  NaN heights give NaN in all three.  Pixels whose localisation does not converge raise
         S2pbError(ERR_ARG)."""
-        z = np.ascontiguousarray(heights, np.float64)
-        if z.ndim != 2:
-            raise ValueError("expecting a 2-D height map, got shape %s" % (z.shape,))
-        h, w = z.shape
+        (h, w), args = self._localisation(heights, rpc, off_x, off_y, zone, south)
         xyz = np.empty((h, w, 3), np.float64)
-        dp = lambda a: a.ctypes.data_as(ctypes.POINTER(ctypes.c_double))
-        _lib.check(self._L.s2pb_height_map_to_xyz(self._ctx, dp(xyz), dp(z), w, h, ctypes.cast(ctypes.pointer(rpc), ctypes.c_void_p),
-                                                  float(off_x), float(off_y), int(zone), int(bool(south))))
+        _lib.check(self._L.s2pb_height_map_to_xyz(self._ctx, _dp(xyz), *args))
         return xyz
 
     # ------------------------------------------------------------------ the tile's point cloud as PLY records
@@ -373,7 +389,7 @@ class Engine:
         dt = self.ply_dtype(nbands, confidence)
         buf = np.empty(npix * dt.itemsize, np.uint8)
         n = ctypes.c_int64(0)
-        _lib.check(call(buf.ctypes.data_as(ctypes.POINTER(ctypes.c_uint8)), ctypes.byref(n)))
+        _lib.check(call(_u8(buf), ctypes.byref(n)))
         return np.frombuffer(buf[:n.value * dt.itemsize].tobytes(), dt)
 
     def stretch_8bit(self, img, p=1):
@@ -381,7 +397,7 @@ class Engine:
         percentiles run over every value of img together -> uint8 of img's shape.  img must convert to float32 exactly."""
         a = np.ascontiguousarray(img, np.float32)
         out = np.empty(a.shape, np.uint8)
-        _lib.check(self._L.s2pb_stretch_8bit(self._ctx, _fp(a), a.size, float(p), out.ctypes.data_as(ctypes.POINTER(ctypes.c_uint8))))
+        _lib.check(self._L.s2pb_stretch_8bit(self._ctx, _fp(a), a.size, float(p), _u8(out)))
         return out
 
     def ply_records(self, xyz, colors=None, confidence=None):
@@ -392,14 +408,12 @@ class Engine:
         if a.ndim < 1 or a.shape[-1] != 3:
             raise ValueError("expecting points of three coordinates, got shape %s" % (a.shape,))
         n = a.size // 3
-        u8 = lambda v: v.ctypes.data_as(ctypes.POINTER(ctypes.c_uint8))
         nb, col = 0, None
         if colors is not None:
             col = np.ascontiguousarray(colors, np.uint8).reshape(-1, n) if n else np.zeros((np.shape(colors)[0], 0), np.uint8)
             nb = col.shape[0]
         conf = None if confidence is None else np.ascontiguousarray(confidence, np.float32).reshape(n)
-        dp = a.ctypes.data_as(ctypes.POINTER(ctypes.c_double))
-        call = lambda out, cnt: self._L.s2pb_ply_records(self._ctx, dp, n, u8(col) if nb else None, nb,
+        call = lambda out, cnt: self._L.s2pb_ply_records(self._ctx, _dp(a), n, _u8(col) if nb else None, nb,
                                                          _fp(conf) if conf is not None else None, out, cnt)
         return self._records(call, n, nb, conf is not None)
 
@@ -407,36 +421,22 @@ class Engine:
                     colors=None, stretch_p=1, confidence=None, dispy=None):
         """disp_to_xyz, the 3D filter (remove_isolated_3d_points(r, p, n, q=1); off when r == 0 or n == 0), the 8-bit stretch of
         the colour planes (nbands, h, w) and the records of ply_records in one device call -> structured array."""
-        dispx, msk, mo = _f32(disp), _f32(mask_rect), _f32(mask_orig)
-        if dispx.ndim != 2 or msk.shape != dispx.shape or mo.ndim != 2:
-            raise ValueError("disp and mask_rect must be 2-D arrays of the same shape, and mask_orig a 2-D array")
-        h, w = dispx.shape
-        dy = np.zeros((h, w), np.float32) if dispy is None else _f32(dispy)
+        (h, w), args = self._triangulation(disp, mask_rect, mask_orig, H1, H2, rpc1, rpc2, img_bbx, zone, south, dispy)
         bands, nb = self._bands(colors, (h, w))
         conf = None if confidence is None else _f32(confidence).reshape(h, w)
-        dp = lambda a: a.ctypes.data_as(ctypes.POINTER(ctypes.c_double))
-        Ha = np.ascontiguousarray(np.asarray(H1, np.float64).reshape(9))
-        Hb = np.ascontiguousarray(np.asarray(H2, np.float64).reshape(9))
-        bb = np.ascontiguousarray(np.asarray(img_bbx, np.float32).reshape(4))
         call = lambda out, cnt: self._L.s2pb_disp_to_ply(
-            self._ctx, _fp(dispx), _fp(dy), _fp(msk), w, h, _fp(mo), mo.shape[1], mo.shape[0], dp(Ha), dp(Hb),
-            ctypes.cast(ctypes.pointer(rpc1), ctypes.c_void_p), ctypes.cast(ctypes.pointer(rpc2), ctypes.c_void_p), _fp(bb),
-            int(zone), int(bool(south)), float(r), operator.index(p), operator.index(n), _fp(bands) if nb else None, nb,
-            float(stretch_p), _fp(conf) if conf is not None else None, out, cnt)
+            self._ctx, *args, float(r), operator.index(p), operator.index(n), _fp(bands) if nb else None, nb, float(stretch_p),
+            _fp(conf) if conf is not None else None, out, cnt)
         return self._records(call, h * w, nb, conf is not None)
 
     def height_map_to_ply(self, heights, rpc, off_x, off_y, zone=0, south=False, r=0.0, p=0, n=0, colors=None, stretch_p=1):
         """height_map_to_xyz, the 3D filter, the 8-bit stretch of the colour planes and the records of ply_records in one device
         call -> structured array (no confidence)."""
-        z = np.ascontiguousarray(heights, np.float64)
-        if z.ndim != 2:
-            raise ValueError("expecting a 2-D height map, got shape %s" % (z.shape,))
-        h, w = z.shape
+        (h, w), args = self._localisation(heights, rpc, off_x, off_y, zone, south)
         bands, nb = self._bands(colors, (h, w))
         call = lambda out, cnt: self._L.s2pb_height_map_to_ply(
-            self._ctx, z.ctypes.data_as(ctypes.POINTER(ctypes.c_double)), w, h, ctypes.cast(ctypes.pointer(rpc), ctypes.c_void_p),
-            float(off_x), float(off_y), int(zone), int(bool(south)), float(r), operator.index(p), operator.index(n),
-            _fp(bands) if nb else None, nb, float(stretch_p), out, cnt)
+            self._ctx, *args, float(r), operator.index(p), operator.index(n), _fp(bands) if nb else None, nb, float(stretch_p),
+            out, cnt)
         return self._records(call, h * w, nb, False)
 
     # ------------------------------------------------------------------ DSM rasterisation
@@ -476,15 +476,10 @@ class Engine:
         Hb = np.asarray(H2, np.float64).reshape(3, 3)
         if A is not None:
             Hb = np.dot(Hb, np.linalg.inv(np.asarray(A, np.float64).reshape(3, 3)))
-        dp = lambda a: a.ctypes.data_as(ctypes.POINTER(ctypes.c_double))
-        Ha = np.ascontiguousarray(np.asarray(H1, np.float64).reshape(9))
-        Hb = np.ascontiguousarray(Hb.reshape(9))
         out = np.empty((int(h), int(w)), np.float64)
         ny, nx = disp.shape
-        _lib.check(self._L.s2pb_height_map(self._ctx, dp(out), _fp(disp), _fp(msk), nx, ny, _fp(mo), mo.shape[1], mo.shape[0],
-                                           int(x), int(y), int(w), int(h), dp(Ha), dp(Hb), None,
-                                           ctypes.cast(ctypes.pointer(rpc1), ctypes.c_void_p),
-                                           ctypes.cast(ctypes.pointer(rpc2), ctypes.c_void_p)))
+        _lib.check(self._L.s2pb_height_map(self._ctx, _dp(out), _fp(disp), _fp(msk), nx, ny, _fp(mo), mo.shape[1], mo.shape[0],
+                                           int(x), int(y), int(w), int(h), _mat3(H1), _mat3(Hb), _rpc(rpc1), _rpc(rpc2)))
         return out
 
     def resample_heights(self, z, H, w, h):
@@ -493,10 +488,8 @@ class Engine:
         z = np.ascontiguousarray(z, np.float64)
         if z.ndim != 2:
             raise ValueError("z must be a 2-D array")
-        Hm = np.ascontiguousarray(np.asarray(H, np.float64).reshape(9))
         out = np.empty((int(h), int(w)), np.float64)
-        dp = lambda a: a.ctypes.data_as(ctypes.POINTER(ctypes.c_double))
-        _lib.check(self._L.s2pb_resample_heights(self._ctx, dp(z), z.shape[1], z.shape[0], dp(Hm), dp(out), int(w), int(h)))
+        _lib.check(self._L.s2pb_resample_heights(self._ctx, _dp(z), z.shape[1], z.shape[0], _mat3(H), _dp(out), int(w), int(h)))
         return out
 
     def cargarse_basura(self, img):
@@ -525,12 +518,12 @@ class Engine:
         lo = np.ascontiguousarray(lo, np.int32)
         hi = np.ascontiguousarray(hi, np.int32)
         C = np.empty((h, w, D), np.float32)
-        ip = lambda a: a.ctypes.data_as(ctypes.POINTER(ctypes.c_int32))
         if cost is None:
-            _lib.check(self._L.s2pb_costvolume(self._ctx, _fp(u), _fp(v), w, h, ip(lo), ip(hi), int(gmin), int(D), win, _fp(C)))
+            _lib.check(self._L.s2pb_costvolume(self._ctx, _fp(u), _fp(v), w, h, _ip(lo), _ip(hi), int(gmin), int(D), win, _fp(C)))
         else:
             ci = _lib.COSTS.index(cost) if isinstance(cost, str) else int(cost)
-            _lib.check(self._L.s2pb_costvolume_dist(self._ctx, _fp(u), _fp(v), w, h, ip(lo), ip(hi), int(gmin), int(D), win, ci, _fp(C)))
+            _lib.check(self._L.s2pb_costvolume_dist(self._ctx, _fp(u), _fp(v), w, h, _ip(lo), _ip(hi), int(gmin), int(D), win, ci,
+                                                    _fp(C)))
         return C
 
     def aggregate(self, C, lo, hi, gmin, P1=8.0, P2=32.0, ndir=8, tsgm=3, fix_overcount=1, want_S=True, weights=None,
@@ -544,14 +537,13 @@ class Engine:
         disp = np.empty((h, w), np.float32)
         cost = np.empty((h, w), np.float32)
         conf = np.empty((h, w), np.float32)
-        ip = lambda a: a.ctypes.data_as(ctypes.POINTER(ctypes.c_int32))
         if general or weights is not None:
             wgt = _f32(weights) if weights is not None else None
-            _lib.check(self._L.s2pb_aggregate_w(self._ctx, _fp(C), ip(lo), ip(hi), w, h, int(gmin), D, P1, P2, ndir, tsgm,
+            _lib.check(self._L.s2pb_aggregate_w(self._ctx, _fp(C), _ip(lo), _ip(hi), w, h, int(gmin), D, P1, P2, ndir, tsgm,
                                                 fix_overcount, _fp(wgt) if wgt is not None else None,
                                                 _fp(S) if want_S else None, _fp(disp), _fp(cost), _fp(conf)))
         else:
-            _lib.check(self._L.s2pb_aggregate(self._ctx, _fp(C), ip(lo), ip(hi), w, h, int(gmin), D, P1, P2, ndir, tsgm,
+            _lib.check(self._L.s2pb_aggregate(self._ctx, _fp(C), _ip(lo), _ip(hi), w, h, int(gmin), D, P1, P2, ndir, tsgm,
                                               fix_overcount, _fp(S) if want_S else None, _fp(disp), _fp(cost), _fp(conf)))
         return S, disp, cost, conf
 
@@ -573,8 +565,7 @@ class Engine:
         disp, im1, im2 = _f32(disp), _f32(im1), _f32(im2)
         h, w = disp.shape
         mask = np.empty((h, w), np.uint8)
-        _lib.check(self._L.s2pb_rejection_mask(self._ctx, _fp(disp), _fp(im1), _fp(im2), w, h,
-                                               mask.ctypes.data_as(ctypes.POINTER(ctypes.c_uint8))))
+        _lib.check(self._L.s2pb_rejection_mask(self._ctx, _fp(disp), _fp(im1), _fp(im2), w, h, _u8(mask)))
         return mask
 
 

@@ -2,9 +2,10 @@
 
 The reference triangulates through ``lib/disp_to_h.so`` loaded with ctypes (s2p/triangulation.py:18-20) and calls
 ``lib.disp_to_lonlatalt(lonlatalt, err, dispx, dispy, msk, w, h, msk_orig, ww, hh, H1, H2, byref(rpc1),
-byref(rpc2), bbx)`` (:134-143).  ``s2pb_disp_to_lonlatalt`` takes the same argument list (plus the context) and
-``RPCStruct`` below has the layout of the reference's ``struct rpc`` / ``RPCStruct``; ``install()`` swaps the
-library handle of an importable ``s2p.triangulation`` for an adapter that forwards the very same call.
+byref(rpc2), bbx)`` (:134-143).  ``s2pb_disp_to_xyz`` takes the same argument list (plus the context, then the output
+zone, 0 for lon, lat, alt) and ``RPCStruct`` below has the layout of the reference's ``struct rpc`` / ``RPCStruct``;
+``install()`` swaps the library handle of an importable ``s2p.triangulation`` for an adapter that forwards the very same
+call.
 
 The 3D outlier filter of the same library, ``count_3d_neighbors`` and ``remove_isolated_3d_points`` (c/disp_to_h.c:143-230),
 which ``filter_xyz`` runs on the cloud of a tile (s2p/triangulation.py:275-343), goes through the adapter too.
@@ -25,7 +26,7 @@ from ctypes import c_double
 
 import numpy as np
 
-from . import _lib, projection
+from . import projection
 from .engine import get_engine
 
 
@@ -62,25 +63,7 @@ def rpc_from_geotiff_tag(tag, delta=1.0):
 def disp_to_lonlatalt(disp, mask_rect, mask_orig, H1, H2, rpc1, rpc2, img_bbx, dispy=None, engine=None):
     """numpy-level call: -> (lonlatalt (h, w, 3) float64, err (h, w) float32).
     rpc1 / rpc2: any ctypes structure with the layout of ``RPCStruct`` (the reference's own class works)."""
-    eng = engine or get_engine()
-    dispx = np.ascontiguousarray(disp, np.float32)
-    h, w = dispx.shape
-    dy = np.zeros((h, w), np.float32) if dispy is None else np.ascontiguousarray(dispy, np.float32)
-    msk = np.ascontiguousarray(mask_rect, np.float32)
-    mo = np.ascontiguousarray(mask_orig, np.float32)
-    hh, ww = mo.shape
-    out = np.zeros((h, w, 3), np.float64)
-    err = np.zeros((h, w), np.float32)
-    fp = lambda a: a.ctypes.data_as(ctypes.POINTER(ctypes.c_float))
-    dp = lambda a: a.ctypes.data_as(ctypes.POINTER(ctypes.c_double))
-    Ha = np.ascontiguousarray(np.asarray(H1, np.float64).reshape(9))
-    Hb = np.ascontiguousarray(np.asarray(H2, np.float64).reshape(9))
-    bb = np.ascontiguousarray(np.asarray(img_bbx, np.float32).reshape(4))
-    L = _lib.lib()
-    _lib.check(L.s2pb_disp_to_lonlatalt(eng._ctx, dp(out), fp(err), fp(dispx), fp(dy), fp(msk), w, h, fp(mo), ww, hh,
-                                        dp(Ha), dp(Hb), ctypes.cast(ctypes.pointer(rpc1), ctypes.c_void_p),
-                                        ctypes.cast(ctypes.pointer(rpc2), ctypes.c_void_p), fp(bb)))
-    return out, err
+    return (engine or get_engine()).disp_to_xyz(disp, mask_rect, mask_orig, H1, H2, rpc1, rpc2, img_bbx, zone=0, dispy=dispy)
 
 
 def disp_to_xyz(rpc1, rpc2, H1, H2, disp, mask_rect, img_bbx, mask_orig, A=None, out_crs=None, engine=None):
