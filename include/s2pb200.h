@@ -31,6 +31,8 @@
  *                        linear_stretching_and_quantization_8bit (s2p/common.py:284-297) and the vertex records of write_to_ply
  *                        (s2p/triangulation.py:392-429, s2p/ply.py:24-69)
  *   s2pb_height_map_to_ply() the same for heights_to_ply after heights_fusion (s2p/__init__.py:388-429), from height_map_to_xyz
+ *   s2pb_disp_to_ply_clr(), s2pb_height_map_to_ply_clr() the same two steps with a clr image: its colours in its own type,
+ *                        warped on the device for the pair (s2p/__init__.py:270-280), the raw window for tri-stereo (:404-406)
  *   s2pb_sgbm()          the `sgbm` subprocess (OpenCV 2's StereoSGBM, 3rdparty/sgbm) + create_rejection_mask
  *                        (s2p/block_matching.py:116-134)
  *
@@ -314,9 +316,39 @@ int s2pb_height_map_to_ply(s2pb_ctx *ctx, const double *heights, int w, int h, c
                            int zone, int south, float r, int p, int n, const float *bands, int nbands, double pct,
                            uint8_t *records, int64_t *npoints);
 
-/* ---- DSM rasterisation (s2p/__init__.py plys_to_dsm) -------------------------- */
-/* One vertex property of a binary little-endian PLY record: its byte offset in the record and its type. */
+/* PLY property types: the eight plyfile writes, as double, float, uchar, char, short, ushort, int and uint */
 enum { S2PB_PLY_F64 = 0, S2PB_PLY_F32 = 1, S2PB_PLY_U8 = 2 };
+enum { S2PB_PLY_I8 = 16, S2PB_PLY_I16 = 17, S2PB_PLY_U16 = 18, S2PB_PLY_I32 = 19, S2PB_PLY_U32 = 20 };
+
+/* The tile's point cloud coloured from the image cfg['images'][0]['clr']: the colours keep that image's type, as s2p writes
+ * them (s2p/__init__.py:270-280 and :404-406), and are copied into the records as they are, without a stretch.
+ *
+ * s2pb_ply_records with colour planes of any S2PB_PLY_* type: colors holds nbands planes of n values of color_type,
+ * little-endian, copied byte for byte (NaN colours included) into red, green, blue (and ir) of that type:
+ * 24 + {0, 3, 4} * {1, 2, 4, 8} + {0, 4} bytes per record, at most 60, no padding.
+ * S2PB_ERR_ARG: as s2pb_ply_records, and an unknown color_type. */
+int s2pb_ply_records_typed(s2pb_ctx *ctx, const double *xyz, int64_t n, const void *colors, int nbands, int color_type,
+                           const float *conf, uint8_t *records, int64_t *npoints);
+/* disparity_to_ply with a clr image (s2p/__init__.py:270-280) in one call: s2pb_disp_to_ply's cloud and filter, with float
+ * colours warped on the device.  clr: nbands float32 planes of the cw*ch crop of the clr image that the warp of the rectified
+ * reference needs; hc: H_ref with the crop's origin folded in (H_ref . [[1, 0, x], [0, 1, y], [0, 0, 1]]).  Each band is
+ * warped into nx*ny as s2pb_homography(band, cw, ch, hc, ..., nx, ny) warps it (NaN outside the source), and the float
+ * colours and the optional confidence are packed as s2pb_ply_records_typed packs them.
+ * S2PB_ERR_ARG: as s2pb_disp_to_ply and s2pb_homography, nbands not 1, 3 or 4. */
+int s2pb_disp_to_ply_clr(s2pb_ctx *ctx, const float *dispx, const float *dispy, const float *msk, int nx, int ny,
+                         const float *msk_orig, int w, int h, const double ha[9], const double hb[9], const s2pb_rpc *rpca,
+                         const s2pb_rpc *rpcb, const float orig_img_bounding_box[4], int zone, int south, float r, int p, int n,
+                         const float *clr, int cw, int ch, int nbands, const double hc[9], const float *conf, uint8_t *records,
+                         int64_t *npoints);
+/* heights_to_ply with a clr image (s2p/__init__.py:404-406) after heights_fusion in one call: s2pb_height_map_to_ply's cloud and
+ * filter, then the records of s2pb_ply_records_typed with the colours (nbands planes of w*h values of color_type: the clr
+ * window in its stored type).  S2PB_ERR_ARG: as s2pb_height_map_to_ply, nbands not 1, 3 or 4, an unknown color_type. */
+int s2pb_height_map_to_ply_clr(s2pb_ctx *ctx, const double *heights, int w, int h, const s2pb_rpc *rpc, double off_x,
+                               double off_y, int zone, int south, float r, int p, int n, const void *colors, int nbands,
+                               int color_type, uint8_t *records, int64_t *npoints);
+
+/* ---- DSM rasterisation (s2p/__init__.py plys_to_dsm) -------------------------- */
+/* One vertex property of a binary little-endian PLY record: its byte offset in the record and its type (S2PB_PLY_*). */
 typedef struct s2pb_ply_column {
     int32_t offset;
     int32_t type;            /* S2PB_PLY_* */
@@ -325,7 +357,7 @@ typedef struct s2pb_ply_column {
  * plys_to_dsm runs on a tile's cloud and its neighbours' (s2p/__init__.py:432-476).  records[k]: the npoints[k] vertex records
  * of cloud k, record_bytes each, as they lie in the file; host memory (pageable or page-locked) or device memory, NULL when
  * npoints[k] == 0.  cols[0], cols[1]: x and y; cols[2..ncols-1]: the raster's channels, in that order.  Every property is
- * read as float64.  A point falls in cell (floor((x - xoff) / resolution), floor((yoff - y) / resolution)), in double; points
+ * read as float64 (exactly, for every type).  A point falls in cell (floor((x - xoff) / resolution), floor((yoff - y) / resolution)), in double; points
  * outside the raster or with a NaN coordinate are skipped.  Per cell and channel, over the clouds in order and each cloud's
  * points in order: acc = (float)((double)acc + 1.0 * v) from 0.0f, cnt += 1.0f; raster[(j * xsize + i) * (ncols - 2) + c] =
  * acc / cnt in float, NaN where no point fell.  Deterministic.  Synchronous on the context's stream.

@@ -37,6 +37,7 @@ class PlyColumn(ctypes.Structure):
 
 
 PLY_F64, PLY_F32, PLY_U8 = 0, 1, 2     # S2PB_PLY_*
+PLY_I8, PLY_I16, PLY_U16, PLY_I32, PLY_U32 = 16, 17, 18, 19, 20
 
 COSTS = ("census", "ad", "sd", "ncc", "btad", "btsd")   # S2PB_COST_* = index; the reference's `-t` names
 
@@ -92,6 +93,13 @@ _SIGNATURES = {
                                  POINTER(c_int64)]),
     "s2pb_height_map_to_ply": (c_int, [c_void_p, POINTER(c_double), c_int, c_int, c_void_p, c_double, c_double, c_int, c_int, c_float,
                                        c_int, c_int, _f, c_int, c_double, POINTER(c_uint8), POINTER(c_int64)]),
+    "s2pb_ply_records_typed": (c_int, [c_void_p, POINTER(c_double), c_int64, c_void_p, c_int, c_int, _f, POINTER(c_uint8),
+                                       POINTER(c_int64)]),
+    "s2pb_disp_to_ply_clr": (c_int, [c_void_p, _f, _f, _f, c_int, c_int, _f, c_int, c_int, POINTER(c_double), POINTER(c_double),
+                                     c_void_p, c_void_p, _f, c_int, c_int, c_float, c_int, c_int, _f, c_int, c_int, c_int,
+                                     POINTER(c_double), _f, POINTER(c_uint8), POINTER(c_int64)]),
+    "s2pb_height_map_to_ply_clr": (c_int, [c_void_p, POINTER(c_double), c_int, c_int, c_void_p, c_double, c_double, c_int, c_int,
+                                           c_float, c_int, c_int, c_void_p, c_int, c_int, POINTER(c_uint8), POINTER(c_int64)]),
     "s2pb_plyflatten": (c_int, [c_void_p, c_int, POINTER(c_void_p), POINTER(c_int64), c_int, POINTER(PlyColumn), c_int, c_double,
                                 c_double, c_double, c_int, c_int, _f]),
     "s2pb_erode_mask": (c_int, [c_void_p, POINTER(c_uint8), POINTER(c_uint8), c_int, c_int, c_float]),

@@ -25,14 +25,12 @@ def needed_roi(H, w, h):
     return x0, y0, int(np.ceil(p[0].max() - x0)), int(np.ceil(p[1].max() - y0))
 
 
-def image_apply_homography(out, im, H, w, h):
-    """Same contract as s2p.common.image_apply_homography: ``out`` is written as a float32 TIFF of
-    exactly ``w`` x ``h`` pixels with out(x) = im(H^-1 x), NaN outside the source."""
+def homography_crop(im, H, w, h, cmd):
+    """The part of the image file ``im`` that the warp of its bands by H onto [0,w] x [0,h] reads, as the reference's
+    `homography` binary reads it (main.cpp:94-149): -> (crop, Hc), crop (nbands, rh, rw) float32, every band of the needed
+    ROI clipped to the image, and Hc = H with the crop's origin folded in.  ``cmd`` names the command in the
+    CalledProcessError an empty ROI raises."""
     H = np.asarray(H, dtype=np.float64).reshape(3, 3)
-    cmd = ["s2pb200:homography", im, "-h", " ".join(str(x) for x in H.flatten()), out, "%d" % w, "%d" % h]
-    print("\nRUN: %s" % " ".join(cmd))
-    # read only the part of the source the output needs (the reference does the same through GDAL RasterIO,
-    # main.cpp:112-149), and move the crop's origin into the homography
     sw, sh = rio.image_size(im)
     x, y, rw, rh = needed_roi(H, w, h)
     if x < 0:
@@ -45,11 +43,27 @@ def image_apply_homography(out, im, H, w, h):
     if rw <= 0 or rh <= 0:
         raise subprocess.CalledProcessError(1, cmd, output="ERROR: empty roi")
     Hc = H @ np.array([[1, 0, x], [0, 1, y], [0, 0, 1]], dtype=np.float64)
-    res = []
+    # every band, like the binary (main.cpp loops over GetRasterCount): s2p/__init__.py:276 warps the colour image this way
+    crop = np.stack([rio.read_window(im, x, y, rw, rh, band) for band in range(1, rio.band_count(im) + 1)])
+    return crop, Hc
+
+
+def homography_cmd(out, im, H, w, h):
+    """the `homography` command line s2p.common.image_apply_homography runs"""
+    H = np.asarray(H, dtype=np.float64).reshape(3, 3)
+    return ["s2pb200:homography", im, "-h", " ".join(str(x) for x in H.flatten()), out, "%d" % w, "%d" % h]
+
+
+def image_apply_homography(out, im, H, w, h):
+    """Same contract as s2p.common.image_apply_homography: ``out`` is written as a float32 TIFF of
+    exactly ``w`` x ``h`` pixels with out(x) = im(H^-1 x), NaN outside the source."""
+    cmd = homography_cmd(out, im, H, w, h)
+    print("\nRUN: %s" % " ".join(cmd))
+    # read only the part of the source the output needs (the reference does the same through GDAL RasterIO,
+    # main.cpp:112-149), and move the crop's origin into the homography
+    crop, Hc = homography_crop(im, H, w, h, cmd)
     try:
-        for band in range(1, rio.band_count(im) + 1):      # every band, like the binary (main.cpp loops over GetRasterCount):
-            src = rio.read_window(im, x, y, rw, rh, band)  # s2p/__init__.py:276 warps the colour image through this function
-            res.append(get_engine().homography(src, Hc, w, h))
+        res = [get_engine().homography(band, Hc, w, h) for band in crop]
     except S2pbError as e:
         raise subprocess.CalledProcessError(-e.code, cmd, output=str(e)) from e
     rio.write_float_tiff_bands(out, res)

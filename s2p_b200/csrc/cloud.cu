@@ -1,11 +1,11 @@
 // cloud.cu -- the tile's point cloud as PLY records (cloud_kernels.cuh): the colours of
-// common.linear_stretching_and_quantization_8bit and the vertex records of triangulation.write_to_ply, alone or at the end of
-// disparity_to_ply / heights_to_ply's triangulation and 3D filter on one stream.
+// common.linear_stretching_and_quantization_8bit, or of a clr image in its own type, and the vertex records of
+// triangulation.write_to_ply, alone or at the end of disparity_to_ply / heights_to_ply's triangulation and 3D filter on one stream.
 #include "host.h"
 #include "cloud_kernels.cuh"
 
-// bytes of one record: x, y, z float64, 3 colours (1 or 3 bands) or 4 (4 bands) uint8, confidence float32
-static int record_bytes(int nbands, bool conf) { return 24 + (nbands == 4 ? 4 : nbands ? 3 : 0) + (conf ? 4 : 0); }
+// bytes of one record: x, y, z float64, 3 colours (1 or 3 bands) or 4 (4 bands) of cb bytes, confidence float32
+static int record_bytes(int nbands, int cb, bool conf) { return 24 + (nbands == 4 ? 4 : nbands ? 3 : 0) * cb + (conf ? 4 : 0); }
 
 static bool bands_ok(int nbands) { return nbands == 0 || nbands == 1 || nbands == 3 || nbands == 4; }
 
@@ -16,20 +16,25 @@ static int stretch_bounds_enqueue(s2pb_ctx *ctx, cudaStream_t st, const float *d
 }
 
 // The kept points of the device cloud d_xyz (n points) packed into d_out; their number into *d_total.  Colours: d_colors
-// (nbands uint8 planes) or, when it is null, d_bands (nbands float32 planes) stretched with the bounds of d_os.
-static int pack_enqueue(s2pb_ctx *ctx, HostCall &L, const double *d_xyz, size_t n, int nbands, const uint8_t *d_colors,
+// (nbands planes of values of cb bytes, copied) or, when it is null, d_bands (nbands float32 planes) stretched to uint8 with
+// the bounds of d_os.  Records wider than kPlyMaxRecord bytes go through the wide kernels' smaller CTA tiles.
+static int pack_enqueue(s2pb_ctx *ctx, HostCall &L, const double *d_xyz, size_t n, int nbands, const uint8_t *d_colors, int cb,
                         const float *d_bands, const OrderStats *d_os, const float *d_conf, uint8_t *d_out, long long *d_total)
 {
-    const int ntiles = (int)((n + kPlyTile - 1) / kPlyTile);
+    const int rb = record_bytes(nbands, d_colors ? cb : 1, d_conf != nullptr);
+    const bool wide = rb > kPlyMaxRecord;
+    const int tile = wide ? kPlyThreads * kPlyPerWide : kPlyTile;
+    const int ntiles = (int)((n + tile - 1) / tile);
     int *d_counts = L.take<int>((size_t)ntiles * 4);
     long long *d_offsets = L.take<long long>((size_t)ntiles * 8);
     if (int rc = L.error()) return rc;
-    launch(ctx, ply_count_kernel, ntiles, kPlyThreads, 0, L.st, d_xyz, n, d_counts);
+    launch(ctx, wide ? ply_count_kernel<kPlyPerWide> : ply_count_kernel<kPlyPer>, ntiles, kPlyThreads, 0, L.st, d_xyz, n, d_counts);
     launch(ctx, ply_scan_kernel, 1, 1024, 0, L.st, d_counts, ntiles, d_offsets, d_total);
     PlyPackParams P;
-    P.xyz = d_xyz; P.n = n; P.offsets = d_offsets; P.nbands = nbands; P.colors = d_colors; P.bands = d_bands; P.os = d_os;
-    P.conf = d_conf; P.rb = record_bytes(nbands, d_conf != nullptr); P.out = d_out;
-    launch(ctx, ply_pack_kernel, ntiles, kPlyThreads, 0, L.st, P);
+    P.xyz = d_xyz; P.n = n; P.offsets = d_offsets; P.nbands = nbands; P.cb = d_colors ? cb : 1; P.colors = d_colors;
+    P.bands = d_bands; P.os = d_os; P.conf = d_conf; P.rb = rb; P.out = d_out;
+    launch(ctx, wide ? ply_pack_kernel<kPlyPerWide, kPlyMaxWide> : ply_pack_kernel<kPlyPer, kPlyMaxRecord>, ntiles, kPlyThreads, 0,
+           L.st, P);
     CK(cudaGetLastError());
     return S2PB_OK;
 }
@@ -74,26 +79,58 @@ extern "C" int s2pb_ply_records(s2pb_ctx *ctx, const double *xyz, int64_t n, con
     if (n == 0) return S2PB_OK;
     HostCall L(ctx, "the PLY records");
     const size_t np = (size_t)n;
-    const int rb = record_bytes(nbands, conf != nullptr);
+    const int rb = record_bytes(nbands, 1, conf != nullptr);
     double *d_xyz = L.upload(xyz, np * 24);
     uint8_t *d_col = nbands ? L.upload(colors, np * nbands) : nullptr;
     float *d_conf = conf ? L.upload(conf, np * 4) : nullptr;
     uint8_t *d_out = L.take<uint8_t>(np * rb);
     long long *d_total = L.take<long long>(8);
     if (int rc = L.error()) return rc;
-    if (int rc = pack_enqueue(ctx, L, d_xyz, np, nbands, d_col, nullptr, nullptr, d_conf, d_out, d_total)) return rc;
+    if (int rc = pack_enqueue(ctx, L, d_xyz, np, nbands, d_col, 1, nullptr, nullptr, d_conf, d_out, d_total)) return rc;
     return download_records(L, d_total, d_out, rb, records, npoints);
 }
 
-// the common tail of the two steps: filter, colours, records
+// nbands 1, 3 or 4 and a known colour type: the colours of a clr image
+static int typed_colours_ok(int nbands, int color_type)
+{
+    if (nbands != 1 && nbands != 3 && nbands != 4) return fail(S2PB_ERR_ARG, "colors must have either 1, 3 or 4 channels (got %d)", nbands);
+    if (!ply_type_bytes(color_type)) return fail(S2PB_ERR_ARG, "unknown PLY colour type %d", color_type);
+    return S2PB_OK;
+}
+
+extern "C" int s2pb_ply_records_typed(s2pb_ctx *ctx, const double *xyz, int64_t n, const void *colors, int nbands, int color_type,
+                                      const float *conf, uint8_t *records, int64_t *npoints)
+{
+    if (!ctx || !npoints || n < 0 || (n && (!xyz || !records || (nbands && !colors)))) return fail(S2PB_ERR_ARG, "bad argument");
+    if (!bands_ok(nbands)) return fail(S2PB_ERR_ARG, "colors must have either 1, 3 or 4 channels (got %d)", nbands);
+    const int cb = ply_type_bytes(color_type);
+    if (!cb) return fail(S2PB_ERR_ARG, "unknown PLY colour type %d", color_type);
+    if (n > INT32_MAX) return fail(S2PB_ERR_UNSUPPORTED, "at most 2^31 - 1 points");
+    *npoints = 0;
+    if (n == 0) return S2PB_OK;
+    HostCall L(ctx, "the PLY records");
+    const size_t np = (size_t)n;
+    const int rb = record_bytes(nbands, cb, conf != nullptr);
+    double *d_xyz = L.upload(xyz, np * 24);
+    uint8_t *d_col = nbands ? L.upload((const uint8_t *)colors, np * nbands * cb) : nullptr;
+    float *d_conf = conf ? L.upload(conf, np * 4) : nullptr;
+    uint8_t *d_out = L.take<uint8_t>(np * rb);
+    long long *d_total = L.take<long long>(8);
+    if (int rc = L.error()) return rc;
+    if (int rc = pack_enqueue(ctx, L, d_xyz, np, nbands, d_col, cb, nullptr, nullptr, d_conf, d_out, d_total)) return rc;
+    return download_records(L, d_total, d_out, rb, records, npoints);
+}
+
+// The common tail of the steps: filter, colours, records.  Colours: d_typed (nbands device planes of cb-byte values, copied
+// as they are) or, when it is null, the host float32 planes `bands` stretched with pct.
 static int cloud_tail(s2pb_ctx *ctx, HostCall &L, double *d_xyz, int nx, int ny, float r, int p, int n, const float *bands,
-                      int nbands, double pct, const float *conf, uint8_t *records, int64_t *npoints)
+                      int nbands, double pct, const uint8_t *d_typed, int cb, const float *conf, uint8_t *records, int64_t *npoints)
 {
     const size_t npix = (size_t)nx * ny;
-    const int rb = record_bytes(nbands, conf != nullptr);
+    const int rb = record_bytes(nbands, d_typed ? cb : 1, conf != nullptr);
     int *d_work = (r != 0.f && n > 0) ? L.take<int>(npix * 12) : nullptr;
-    float *d_bands = nbands ? L.upload(bands, npix * nbands * 4) : nullptr;
-    OrderStats *d_os = nbands ? L.take<OrderStats>(order_stats_bytes()) : nullptr;
+    float *d_bands = nbands && !d_typed ? L.upload(bands, npix * nbands * 4) : nullptr;
+    OrderStats *d_os = d_bands ? L.take<OrderStats>(order_stats_bytes()) : nullptr;
     float *d_conf = conf ? L.upload(conf, npix * 4) : nullptr;
     uint8_t *d_out = L.take<uint8_t>(npix * rb);
     long long *d_total = L.take<long long>(8);
@@ -101,10 +138,10 @@ static int cloud_tail(s2pb_ctx *ctx, HostCall &L, double *d_xyz, int nx, int ny,
     if (d_work) {
         if (int rc = remove_isolated_enqueue(ctx, L.st, d_xyz, nx, ny, r, p, n, 1, d_work)) return rc;
     }
-    if (nbands) {
+    if (d_bands) {
         if (int rc = stretch_bounds_enqueue(ctx, L.st, d_bands, npix * nbands, pct, d_os)) return rc;
     }
-    if (int rc = pack_enqueue(ctx, L, d_xyz, npix, nbands, nullptr, d_bands, d_os, d_conf, d_out, d_total)) return rc;
+    if (int rc = pack_enqueue(ctx, L, d_xyz, npix, nbands, d_typed, cb, d_bands, d_os, d_conf, d_out, d_total)) return rc;
     return download_records(L, d_total, d_out, rb, records, npoints);
 }
 
@@ -132,7 +169,7 @@ extern "C" int s2pb_disp_to_ply(s2pb_ctx *ctx, const float *dispx, const float *
     if (int rc = triangulated_cloud(ctx, L, dispx, dispy, msk, nx, ny, msk_orig, w, h, ha, hb, rpca, rpcb, bbox, zone, south, &d_xyz,
                                     &d_err))
         return rc;
-    return cloud_tail(ctx, L, d_xyz, nx, ny, r, p, n, bands, nbands, pct, conf, records, npoints);
+    return cloud_tail(ctx, L, d_xyz, nx, ny, r, p, n, bands, nbands, pct, nullptr, 1, conf, records, npoints);
 }
 
 extern "C" int s2pb_height_map_to_ply(s2pb_ctx *ctx, const double *heights, int w, int h, const s2pb_rpc *rpc, double off_x,
@@ -144,5 +181,47 @@ extern "C" int s2pb_height_map_to_ply(s2pb_ctx *ctx, const double *heights, int 
     HostCall L(ctx, "the tile's cloud");
     double *d_xyz = nullptr;
     if (int rc = localised_cloud(ctx, L, heights, w, h, rpc, off_x, off_y, zone, south, &d_xyz)) return rc;
-    return cloud_tail(ctx, L, d_xyz, w, h, r, p, n, bands, nbands, pct, nullptr, records, npoints);
+    return cloud_tail(ctx, L, d_xyz, w, h, r, p, n, bands, nbands, pct, nullptr, 1, nullptr, records, npoints);
+}
+
+extern "C" int s2pb_disp_to_ply_clr(s2pb_ctx *ctx, const float *dispx, const float *dispy, const float *msk, int nx, int ny,
+                                    const float *msk_orig, int w, int h, const double ha[9], const double hb[9], const s2pb_rpc *rpca,
+                                    const s2pb_rpc *rpcb, const float bbox[4], int zone, int south, float r, int p, int n,
+                                    const float *clr, int cw, int ch, int nbands, const double hc[9], const float *conf,
+                                    uint8_t *records, int64_t *npoints)
+{
+    if (int rc = tail_args_ok(ctx, nx, ny, clr, nbands, 0.0, records, npoints)) return rc;
+    if (int rc = typed_colours_ok(nbands, S2PB_PLY_F32)) return rc;
+    if (!hc || cw < 1 || ch < 1) return fail(S2PB_ERR_ARG, "bad argument");
+    *npoints = 0;
+    HostCall L(ctx, "the tile's cloud");
+    double *d_xyz = nullptr;
+    float *d_err = nullptr;
+    if (int rc = triangulated_cloud(ctx, L, dispx, dispy, msk, nx, ny, msk_orig, w, h, ha, hb, rpca, rpcb, bbox, zone, south, &d_xyz,
+                                    &d_err))
+        return rc;
+    // each band as s2pb_homography warps it, into the plane the records read its colours from
+    const size_t npix = (size_t)nx * ny;
+    float *d_col = L.take<float>(npix * nbands * 4);
+    if (int rc = L.error()) return rc;
+    for (int b = 0; b < nbands; b++)
+        if (int rc = warp_host_to_device(ctx, L, L.st, clr + (size_t)b * cw * ch, cw, ch, hc, d_col + (size_t)b * npix, nx, ny))
+            return rc;
+    return cloud_tail(ctx, L, d_xyz, nx, ny, r, p, n, nullptr, nbands, 0.0, (const uint8_t *)d_col, 4, conf, records, npoints);
+}
+
+extern "C" int s2pb_height_map_to_ply_clr(s2pb_ctx *ctx, const double *heights, int w, int h, const s2pb_rpc *rpc, double off_x,
+                                          double off_y, int zone, int south, float r, int p, int n, const void *colors, int nbands,
+                                          int color_type, uint8_t *records, int64_t *npoints)
+{
+    if (int rc = tail_args_ok(ctx, w, h, (const float *)colors, nbands, 0.0, records, npoints)) return rc;
+    if (int rc = typed_colours_ok(nbands, color_type)) return rc;
+    *npoints = 0;
+    HostCall L(ctx, "the tile's cloud");
+    const int cb = ply_type_bytes(color_type);
+    uint8_t *d_col = L.upload((const uint8_t *)colors, (size_t)w * h * nbands * cb);
+    if (int rc = L.error()) return rc;
+    double *d_xyz = nullptr;
+    if (int rc = localised_cloud(ctx, L, heights, w, h, rpc, off_x, off_y, zone, south, &d_xyz)) return rc;
+    return cloud_tail(ctx, L, d_xyz, w, h, r, p, n, nullptr, nbands, 0.0, d_col, cb, nullptr, records, npoints);
 }

@@ -8,7 +8,10 @@
 //   pack      -> each CTA stages its records in shared memory at the byte offset they have in the output modulo 16, then
 //                writes the 16-byte chunks that lie wholly inside its range with 16-byte stores and the two ragged ends
 //                byte by byte, so neighbouring CTAs never store to the same byte
-// A record is x, y, z float64, then red, green, blue (and ir) uint8, then confidence float32, packed without padding.
+// A record is x, y, z float64, then red, green, blue (and ir), then confidence float32, packed without padding.  The colours
+// are either stretched to uint8, or copied byte for byte from colour planes of one PLY type of 1, 2, 4 or 8 bytes (a `clr`
+// image's own type: float colours keep their bits, NaN included).  Records of up to kPlyMaxRecord bytes are packed by CTAs of
+// kPlyTile points; wider ones (up to kPlyMaxWide) by CTAs of half as many, so that the stage stays within static shared memory.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -19,7 +22,9 @@ namespace s2pb {
 constexpr int kPlyThreads = 256;
 constexpr int kPlyPer = 4;                               // points per thread
 constexpr int kPlyTile = kPlyThreads * kPlyPer;          // points per CTA
-constexpr int kPlyMaxRecord = 32;                        // 24 + 4 colours + 4 confidence
+constexpr int kPlyMaxRecord = 32;                        // 24 + 4 uint8 colours + 4 confidence
+constexpr int kPlyPerWide = 2;                           // points per thread of the wide records
+constexpr int kPlyMaxWide = 60;                          // 24 + 4 float64 colours + 4 confidence
 
 // one value of common.linear_stretching_and_quantization_8bit with the bounds a, b (float64, as numpy forms them):
 // np.clip as its float loop does it (max then min, a NaN operand propagates), then the expression in double, np.round
@@ -47,13 +52,14 @@ __device__ __forceinline__ bool ply_keep(const double *__restrict__ xyz, size_t 
     return isfinite(xyz[3 * i]) && isfinite(xyz[3 * i + 1]) && isfinite(xyz[3 * i + 2]);
 }
 
-// kept points of each CTA tile of kPlyTile points
+// kept points of each CTA tile of kPlyThreads * Per points
+template <int Per>
 __global__ void __launch_bounds__(kPlyThreads) ply_count_kernel(const double *__restrict__ xyz, size_t n, int *__restrict__ counts)
 {
-    const size_t base = (size_t)blockIdx.x * kPlyTile;
+    const size_t base = (size_t)blockIdx.x * (kPlyThreads * Per);
     int c = 0;
 #pragma unroll
-    for (int k = 0; k < kPlyPer; k++) {
+    for (int k = 0; k < Per; k++) {
         const size_t i = base + k * kPlyThreads + threadIdx.x;
         c += i < n && ply_keep(xyz, i);
     }
@@ -119,8 +125,9 @@ struct PlyPackParams {
     size_t n;
     const long long *offsets;   // per CTA tile: the kept points before it (ply_scan_kernel)
     int nbands;                 // 0 (no colour), 1 (grey, written three times), 3 or 4
-    const uint8_t *colors;      // nbands planes of n uint8, or null: ...
-    const float *bands;         // ... nbands planes of n float32, stretched with the bounds of *os
+    int cb;                     // bytes of one colour value: 1, 2, 4 or 8 (1 when stretched)
+    const uint8_t *colors;      // nbands planes of n values of cb bytes, copied as they are, or null: ...
+    const float *bands;         // ... nbands planes of n float32, stretched to uint8 with the bounds of *os
     const OrderStats *os;
     const float *conf;          // n float32, or null (no confidence property)
     int rb;                     // record bytes
@@ -133,11 +140,14 @@ __device__ __forceinline__ void put_bytes(uint8_t *dst, const void *src, int nb)
     for (int k = 0; k < nb; k++) dst[k] = s[k];
 }
 
+// CTA tiles of kPlyThreads * Per points with records of at most MaxRecord bytes: <kPlyPer, kPlyMaxRecord> or
+// <kPlyPerWide, kPlyMaxWide>
+template <int Per, int MaxRecord>
 __global__ void __launch_bounds__(kPlyThreads) ply_pack_kernel(const PlyPackParams P)
 {
-    __shared__ __align__(16) uint8_t stage[kPlyTile * kPlyMaxRecord + 16];
+    __shared__ __align__(16) uint8_t stage[kPlyThreads * Per * MaxRecord + 16];
     __shared__ int ws[kPlyThreads / 32 + 1];
-    const size_t base = (size_t)blockIdx.x * kPlyTile;
+    const size_t base = (size_t)blockIdx.x * (kPlyThreads * Per);
     const size_t gstart = (size_t)P.offsets[blockIdx.x] * P.rb;
     const int shift = (int)(gstart & 15);
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -145,7 +155,7 @@ __global__ void __launch_bounds__(kPlyThreads) ply_pack_kernel(const PlyPackPara
     double a = 0.0, b = 0.0;
     if (!P.colors && P.nbands) { a = P.os->lo; b = P.os->hi; }
     int before = 0;                                          // kept points of this tile in earlier rounds
-    for (int k = 0; k < kPlyPer; k++) {
+    for (int k = 0; k < Per; k++) {
         const size_t i = base + (size_t)k * kPlyThreads + threadIdx.x;
         const bool keep = i < P.n && ply_keep(P.xyz, i);
         // rank of this point among the kept ones of the round: warp ballot, then the warps before it
@@ -162,16 +172,20 @@ __global__ void __launch_bounds__(kPlyThreads) ply_pack_kernel(const PlyPackPara
             const int j = before + ws[wid] + __popc(m & ((1u << lane) - 1));
             uint8_t *r = stage + shift + (size_t)j * P.rb;
             put_bytes(r, P.xyz + 3 * i, 24);
-            if (ncol) {
+            if (ncol && P.colors) {
+                for (int q = 0; q < ncol; q++) {
+                    const int band = P.nbands == 1 ? 0 : q;
+                    put_bytes(r + 24 + q * P.cb, P.colors + ((size_t)band * P.n + i) * P.cb, P.cb);
+                }
+            } else if (ncol) {
                 uint8_t c[4];
                 for (int q = 0; q < ncol; q++) {
                     const int band = P.nbands == 1 ? 0 : q;
-                    const size_t o = (size_t)band * P.n + i;
-                    c[q] = P.colors ? P.colors[o] : stretch_8bit(P.bands[o], a, b);
+                    c[q] = stretch_8bit(P.bands[(size_t)band * P.n + i], a, b);
                 }
                 put_bytes(r + 24, c, ncol);
             }
-            if (P.conf) put_bytes(r + 24 + ncol, P.conf + i, 4);
+            if (P.conf) put_bytes(r + 24 + ncol * P.cb, P.conf + i, 4);
         }
         before += ws[kPlyThreads / 32];
         __syncthreads();

@@ -28,9 +28,14 @@ struct DsmParams {
 __device__ __forceinline__ double dsm_load(const uint8_t *p, int type)
 {
     if (type == S2PB_PLY_U8) return (double)p[0];
-    if (type == S2PB_PLY_F32) {
+    if (type == S2PB_PLY_F32 || type == S2PB_PLY_I32 || type == S2PB_PLY_U32) {
         const uint32_t u = (uint32_t)p[0] | (uint32_t)p[1] << 8 | (uint32_t)p[2] << 16 | (uint32_t)p[3] << 24;
-        return (double)__uint_as_float(u);
+        return type == S2PB_PLY_F32 ? (double)__uint_as_float(u) : type == S2PB_PLY_U32 ? (double)u : (double)(int32_t)u;
+    }
+    if (type == S2PB_PLY_I8) return (double)(int8_t)p[0];
+    if (type == S2PB_PLY_U16 || type == S2PB_PLY_I16) {
+        const uint16_t u = (uint16_t)(p[0] | p[1] << 8);
+        return type == S2PB_PLY_U16 ? (double)u : (double)(int16_t)u;
     }
     unsigned long long u = 0;
 #pragma unroll

@@ -224,6 +224,18 @@ inline void launch(s2pb_ctx *ctx, void (*k)(P...), dim3 grid, dim3 block, size_t
 
 inline dim3 grid2d(int w, int h, dim3 b) { return dim3((w + b.x - 1) / b.x, (h + b.y - 1) / b.y); }
 
+// bytes of a value of PLY property type S2PB_PLY_*, 0 for an unknown type
+inline int ply_type_bytes(int type)
+{
+    switch (type) {
+    case S2PB_PLY_F64: return 8;
+    case S2PB_PLY_F32: case S2PB_PLY_I32: case S2PB_PLY_U32: return 4;
+    case S2PB_PLY_I16: case S2PB_PLY_U16: return 2;
+    case S2PB_PLY_U8: case S2PB_PLY_I8: return 1;
+    default: return 0;
+    }
+}
+
 // ------------------------------------------------------------------ shared between the translation units
 
 // s2pb200.cu: remove_small_cc and the union-find passes it shares with the 3D filter and sgbm (multiscale_kernels.cuh), and

@@ -56,7 +56,7 @@ extern "C" int s2pb_plyflatten(s2pb_ctx *ctx, int nclouds, const void *const *re
     DsmParams P;
     memset(&P, 0, sizeof P);
     for (int c = 0; c < ncols; c++) {
-        const int size = cols[c].type == S2PB_PLY_F64 ? 8 : cols[c].type == S2PB_PLY_F32 ? 4 : cols[c].type == S2PB_PLY_U8 ? 1 : 0;
+        const int size = ply_type_bytes(cols[c].type);
         if (!size) return fail(S2PB_ERR_ARG, "column %d: unknown type %d", c, cols[c].type);
         if (cols[c].offset < 0 || cols[c].offset + size > record_bytes)
             return fail(S2PB_ERR_ARG, "column %d: bytes [%d, %d) outside a %d-byte record", c, cols[c].offset, cols[c].offset + size,

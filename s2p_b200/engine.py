@@ -363,16 +363,35 @@ class Engine:
         return xyz
 
     # ------------------------------------------------------------------ the tile's point cloud as PLY records
+    # numpy colour types -> S2PB_PLY_*: the eight plyfile writes
+    PLY_COLOR_TYPES = {np.dtype(np.int8): _lib.PLY_I8, np.dtype(np.uint8): _lib.PLY_U8, np.dtype("<i2"): _lib.PLY_I16,
+                       np.dtype("<u2"): _lib.PLY_U16, np.dtype("<i4"): _lib.PLY_I32, np.dtype("<u4"): _lib.PLY_U32,
+                       np.dtype("<f4"): _lib.PLY_F32, np.dtype("<f8"): _lib.PLY_F64}
+
     @staticmethod
-    def ply_dtype(nbands=3, confidence=False):
-        """The packed record write_to_ply writes: x, y, z float64, red, green, blue (and ir with 4 bands) uint8 when there are
-        colours (1, 3 or 4 bands), confidence float32 when asked."""
+    def ply_dtype(nbands=3, confidence=False, color_dtype=np.uint8):
+        """The packed record write_to_ply writes: x, y, z float64, red, green, blue (and ir with 4 bands) of color_dtype
+        (little-endian) when there are colours (1, 3 or 4 bands), confidence float32 when asked."""
         d = [("x", "<f8"), ("y", "<f8"), ("z", "<f8")]
         if nbands:
-            d += [("red", "u1"), ("green", "u1"), ("blue", "u1")] + ([("ir", "u1")] if nbands == 4 else [])
+            c = np.dtype(color_dtype).newbyteorder("<")
+            d += [("red", c), ("green", c), ("blue", c)] + ([("ir", c)] if nbands == 4 else [])
         if confidence:
             d += [("confidence", "<f4")]
         return np.dtype(d)
+
+    @classmethod
+    def _typed(cls, colors, shape):
+        """(nbands, h, w) or (h, w) colour planes of one of the eight PLY types -> C-contiguous little-endian (nbands, h, w)
+        planes, nbands and their S2PB_PLY_* type"""
+        c = np.asarray(colors)
+        c = c[None] if c.ndim == 2 else c
+        if c.ndim != 3 or c.shape[1:] != tuple(shape):
+            raise ValueError("expecting colour planes of shape (nbands, %d, %d), got %s" % (shape[0], shape[1], c.shape))
+        dt = c.dtype.newbyteorder("<")
+        if dt not in cls.PLY_COLOR_TYPES:
+            raise TypeError("PLY colours must be one of int8, uint8, int16, uint16, int32, uint32, float32, float64; got %s" % c.dtype)
+        return np.ascontiguousarray(c, dt), c.shape[0], cls.PLY_COLOR_TYPES[dt]
 
     @staticmethod
     def _bands(colors, shape):
@@ -385,8 +404,8 @@ class Engine:
             raise ValueError("expecting colour planes of shape (nbands, %d, %d), got %s" % (shape[0], shape[1], c.shape))
         return np.ascontiguousarray(c, np.float32), c.shape[0]
 
-    def _records(self, call, npix, nbands, confidence):
-        dt = self.ply_dtype(nbands, confidence)
+    def _records(self, call, npix, nbands, confidence, color_dtype=np.uint8):
+        dt = self.ply_dtype(nbands, confidence, color_dtype)
         buf = np.empty(npix * dt.itemsize, np.uint8)
         n = ctypes.c_int64(0)
         _lib.check(call(_u8(buf), ctypes.byref(n)))
@@ -438,6 +457,51 @@ class Engine:
             self._ctx, *args, float(r), operator.index(p), operator.index(n), _fp(bands) if nb else None, nb, float(stretch_p),
             out, cnt)
         return self._records(call, h * w, nb, False)
+
+    def ply_records_typed(self, xyz, colors=None, confidence=None):
+        """ply_records with colours of any of the eight PLY types, copied as they are: colors (nbands, ...) keeps its dtype in
+        the records (a clr image's own type, as write_to_ply writes it) -> structured array of
+        ply_dtype(nbands, confidence is not None, colors.dtype)."""
+        a = np.ascontiguousarray(xyz, np.float64)
+        if a.ndim < 1 or a.shape[-1] != 3:
+            raise ValueError("expecting points of three coordinates, got shape %s" % (a.shape,))
+        n = a.size // 3
+        nb, col, ptype, cdt = 0, None, _lib.PLY_U8, np.uint8
+        if colors is not None:
+            c = np.asarray(colors)
+            col, nb, ptype = self._typed(c.reshape(c.shape[0], 1, n), (1, n))
+            cdt = col.dtype
+        conf = None if confidence is None else np.ascontiguousarray(confidence, np.float32).reshape(n)
+        call = lambda out, cnt: self._L.s2pb_ply_records_typed(self._ctx, _dp(a), n, col.ctypes.data if nb else None, nb, ptype,
+                                                               _fp(conf) if conf is not None else None, out, cnt)
+        return self._records(call, n, nb, conf is not None, cdt)
+
+    def disp_to_ply_clr(self, disp, mask_rect, mask_orig, H1, H2, rpc1, rpc2, img_bbx, zone=0, south=False, r=0.0, p=0, n=0,
+                        clr=None, hc=None, confidence=None, dispy=None):
+        """disp_to_ply with the colours of a clr image: clr (nbands, ch, cw) is the crop of that image which the warp of the
+        rectified reference needs, hc the reference's homography with the crop's origin folded in (common.homography_crop).
+        Every band is warped onto the disparity's grid on the device as homography(band, hc, w, h) warps it, and the records
+        get float32 colours -> structured array of ply_dtype(nbands, confidence is not None, np.float32)."""
+        (h, w), args = self._triangulation(disp, mask_rect, mask_orig, H1, H2, rpc1, rpc2, img_bbx, zone, south, dispy)
+        c = _f32(clr)
+        c = c[None] if c.ndim == 2 else c
+        if c.ndim != 3:
+            raise ValueError("expecting clr planes of shape (nbands, ch, cw), got %s" % (c.shape,))
+        nb, ch, cw = c.shape
+        conf = None if confidence is None else _f32(confidence).reshape(h, w)
+        call = lambda out, cnt: self._L.s2pb_disp_to_ply_clr(
+            self._ctx, *args, float(r), operator.index(p), operator.index(n), _fp(c), cw, ch, nb, _mat3(hc),
+            _fp(conf) if conf is not None else None, out, cnt)
+        return self._records(call, h * w, nb, conf is not None, np.float32)
+
+    def height_map_to_ply_clr(self, heights, rpc, off_x, off_y, zone=0, south=False, r=0.0, p=0, n=0, colors=None):
+        """height_map_to_ply with the colours of a clr image: the planes (nbands, h, w) keep their dtype (one of the eight PLY
+        types) in the records -> structured array of ply_dtype(nbands, False, colors.dtype)."""
+        (h, w), args = self._localisation(heights, rpc, off_x, off_y, zone, south)
+        col, nb, ptype = self._typed(colors, (h, w))
+        call = lambda out, cnt: self._L.s2pb_height_map_to_ply_clr(
+            self._ctx, *args, float(r), operator.index(p), operator.index(n), col.ctypes.data, nb, ptype, out, cnt)
+        return self._records(call, h * w, nb, False, col.dtype)
 
     # ------------------------------------------------------------------ DSM rasterisation
     def plyflatten(self, clouds, record_bytes, columns, xoff, yoff, resolution, xsize, ysize):

@@ -4,7 +4,9 @@ each tile's cloud and its neighbours' (s2p/__init__.py:432-476).
 The clouds' vertex records go to the device as they lie in the files (``s2pb_plyflatten``), where each point is placed in
 its cell and every cell averages its points in order, bit for bit the reference's float accumulation.  Radius > 0, a sigma
 (the Gaussian splat) and PLY files other than binary little-endian with double, float and uchar vertex properties go to the
-original ``plyflatten`` package when it is importable; otherwise they raise ``S2pbError`` with ``ERR_UNSUPPORTED``.
+original ``plyflatten`` package when it is importable; otherwise they raise ``S2pbError`` with ``ERR_UNSUPPORTED``.  The
+colour properties (red, green, blue, ir) may also have the integer types s2p writes for a ``clr`` image in its own type
+(char, short, ushort, int, uint; e.g. ushort for a 12-bit product); like every property they are read as float64.
 
 ``install()`` replaces the name ``plyflatten_from_plyfiles_list`` in the ``s2p`` package, which imports it by name
 (s2p/__init__.py:31), and keeps the original as ``s2p._s2pb_original_plyflatten_from_plyfiles_list``.
@@ -20,6 +22,13 @@ from .engine import get_engine
 _TYPES = {"double": (_lib.PLY_F64, "<f8"), "float64": (_lib.PLY_F64, "<f8"),
           "float": (_lib.PLY_F32, "<f4"), "float32": (_lib.PLY_F32, "<f4"),
           "uchar": (_lib.PLY_U8, "u1"), "uint8": (_lib.PLY_U8, "u1")}
+# ... and the integer types of the colour properties only
+_COLOUR_TYPES = {"char": (_lib.PLY_I8, "i1"), "int8": (_lib.PLY_I8, "i1"),
+                 "short": (_lib.PLY_I16, "<i2"), "int16": (_lib.PLY_I16, "<i2"),
+                 "ushort": (_lib.PLY_U16, "<u2"), "uint16": (_lib.PLY_U16, "<u2"),
+                 "int": (_lib.PLY_I32, "<i4"), "int32": (_lib.PLY_I32, "<i4"),
+                 "uint": (_lib.PLY_U32, "<u4"), "uint32": (_lib.PLY_U32, "<u4")}
+_COLOURS = ("red", "green", "blue", "ir")
 
 
 class UnsupportedPly(ValueError):
@@ -36,7 +45,7 @@ class PlyCloud:
     @property
     def dtype(self):
         """packed structured dtype of a record"""
-        codes = {c: t for c, t in _TYPES.values()}
+        codes = {c: t for c, t in list(_TYPES.values()) + list(_COLOUR_TYPES.values())}
         return np.dtype({"names": self.names, "formats": [codes[t] for t in self.types]})
 
     @property
@@ -82,9 +91,11 @@ def read_ply(path):
         _, n, props = elements[0]
         names, types = [], []
         for p in props:
-            if len(p) != 2 or p[0] not in _TYPES:
-                raise UnsupportedPly("%s: vertex property %s (double, float and uchar only)" % (path, " ".join(p)))
-            types.append(_TYPES[p[0]][0])
+            t = _TYPES.get(p[0]) or (_COLOUR_TYPES.get(p[0]) if len(p) == 2 and p[1] in _COLOURS else None)
+            if len(p) != 2 or t is None:
+                raise UnsupportedPly("%s: vertex property %s (double, float and uchar, and integer colours, only)" %
+                                     (path, " ".join(p)))
+            types.append(t[0])
             names.append(p[1])
         cloud = PlyCloud(None, names, types, comments)
         rb = cloud.dtype.itemsize
