@@ -161,6 +161,28 @@ int s2pb_reserve(s2pb_ctx *ctx, int nslots, int w, int h, int nlabels);
 int s2pb_num_slots(const s2pb_ctx *ctx);
 int s2pb_sync(s2pb_ctx *ctx);
 
+/* ---- workspace layouts ------------------------------------------------------------
+ * Every mgm call of a matcher (the single-scale call, each mgm_multi level including the half-pixel one) runs in one of two
+ * workspace layouts.  The resident layout keeps one f32 volume per scan pass and view (about 33 bytes per voxel and view with
+ * census codes).  The folded layout keeps the running sum of the passes instead, plus a buffer of band-closing scanlines and
+ * one int16 arg-minimum plane per pass (about 5.25 bytes per voxel and view), and runs the passes one after the other.  Both
+ * give the same results, bit for bit.  A call uses the resident layout when it is within the context's workspace limit and
+ * its allocation succeeds, else the folded one; when that does not fit either, S2PB_ERR_NOMEM names both sizes.  The stage
+ * entry points (s2pb_aggregate, s2pb_aggregate_w) run resident only. */
+/* The limit in bytes for each workspace of the context (s2pb_reserve, one per slot); 0 = none (the default), which keeps the
+ * resident layout wherever its allocation succeeds.  It lets several processes share a GPU.  S2PB_ERR_ARG: bytes < 0. */
+int s2pb_set_workspace_limit(s2pb_ctx *ctx, long long bytes);
+/* Bytes of the workspace of a w x h tile whose slab holds D labels (the hull dmax - dmin + 1 of a single-scale call; the
+ * slab is rounded up as the kernels round it), ndir passes, cost_bytes 1 (census codes) or 4 (float costs: the other
+ * distances, or the -wl / -wr weights), in the resident (folded = 0) or folded layout.  No device needed.  A negative S2PB_ERR_*
+ * code for arguments the matcher does not serve. */
+long long s2pb_workspace_bytes(int w, int h, int D, int ndir, int cost_bytes, int folded);
+/* The layout a workspace limit (bytes, 0 = none) selects for that tile: 0 resident, 1 folded, S2PB_ERR_NOMEM for neither.
+ * No device needed; an allocation failure of the resident layout also falls back to the folded one at run time. */
+int s2pb_workspace_layout(int w, int h, int D, int ndir, int cost_bytes, long long limit);
+/* number of mgm calls the context has run in the folded layout */
+long long s2pb_folded_calls(const s2pb_ctx *ctx);
+
 /* ---- the `sgbm` matcher (3rdparty/sgbm/sgbm.cpp + stereosgbm.cpp) ----------------- */
 /* The binary's argv after dmin dmax (`sgbm im1 im2 disp cost dmin dmax win P1 P2 lr`).  What it hardcodes stays
  * constant: fullDP, preFilterCap 63, uniquenessRatio 10, speckle window 50 and range 1, median 3x3. */

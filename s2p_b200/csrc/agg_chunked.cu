@@ -9,18 +9,21 @@ static constexpr int kCkMaxSmem = 224 * 1024;      // dynamic part: the 227 KB o
 int agg_chunked_configure()
 {
     cudaError_t e = cudaSuccess;
-#define CFG(T, S) e = cudaFuncSetAttribute(aggregate_chunked_kernel<T, S, 4, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kCkMaxSmem); if (e) return -1; \
-                  e = cudaFuncSetAttribute(aggregate_chunked_kernel<T, S, 2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kCkMaxSmem); if (e) return -1;
+#define CFG1(T, S, F) e = cudaFuncSetAttribute(aggregate_chunked_kernel<T, S, 4, false, F>, cudaFuncAttributeMaxDynamicSharedMemorySize, kCkMaxSmem); if (e) return -1; \
+                      e = cudaFuncSetAttribute(aggregate_chunked_kernel<T, S, 2, false, F>, cudaFuncAttributeMaxDynamicSharedMemorySize, kCkMaxSmem); if (e) return -1;
+#define CFG(T, S) CFG1(T, S, false) CFG1(T, S, true)
     CFG(1, false) CFG(2, false) CFG(3, false) CFG(4, false) CFG(1, true) CFG(2, true) CFG(3, true) CFG(4, true)
 #undef CFG
-#define CFG_GEN(T) e = cudaFuncSetAttribute(aggregate_chunked_kernel<T, false, 2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kCkMaxSmem); if (e) return -1;
+#undef CFG1
+#define CFG_GEN(T) e = cudaFuncSetAttribute(aggregate_chunked_kernel<T, false, 2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kCkMaxSmem); if (e) return -1; \
+                   e = cudaFuncSetAttribute(aggregate_chunked_kernel<T, false, 2, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kCkMaxSmem); if (e) return -1;
     CFG_GEN(1) CFG_GEN(2) CFG_GEN(3) CFG_GEN(4)
 #undef CFG_GEN
     return 0;
 }
 
 // 0 ok, -1 CUDA error, -2 this shape is not served
-int agg_chunked_launch(int tsgm, const ChunkedParams &P, int sm_count, cudaStream_t st)
+template <bool FOLD> static int chunked_launch(int tsgm, const ChunkedArgs<FOLD> &P, int sm_count, cudaStream_t st)
 {
     if (P.DP < 32 || P.DP > 2048 || (P.DP & 31)) return -2;
     const bool gen = P.A.general != 0;          // float costs (and weights): no cost table, pipeline depth 2 (ck_stage)
@@ -35,9 +38,9 @@ int agg_chunked_launch(int tsgm, const ChunkedParams &P, int sm_count, cudaStrea
     if (grid > total) grid = total;
     const bool scaled = P.A.lut != nullptr;
     const int threads = warps * 32;
-#define GO2(T, ST) do { if (scaled) aggregate_chunked_kernel<T, true, ST, false><<<grid, threads, SM.bytes, st>>>(P); \
-                        else aggregate_chunked_kernel<T, false, ST, false><<<grid, threads, SM.bytes, st>>>(P); } while (0)
-#define GO(T) do { if (gen) aggregate_chunked_kernel<T, false, 2, true><<<grid, threads, SM.bytes, st>>>(P); \
+#define GO2(T, ST) do { if (scaled) aggregate_chunked_kernel<T, true, ST, false, FOLD><<<grid, threads, SM.bytes, st>>>(P); \
+                        else aggregate_chunked_kernel<T, false, ST, false, FOLD><<<grid, threads, SM.bytes, st>>>(P); } while (0)
+#define GO(T) do { if (gen) aggregate_chunked_kernel<T, false, 2, true, FOLD><<<grid, threads, SM.bytes, st>>>(P); \
                    else if (stage == 4) GO2(T, 4); else GO2(T, 2); } while (0)
     switch (tsgm) {
     case 1: GO(1); break;
@@ -50,5 +53,7 @@ int agg_chunked_launch(int tsgm, const ChunkedParams &P, int sm_count, cudaStrea
 #undef GO2
     return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }
+int agg_chunked_launch(int tsgm, const ChunkedParams &P, int sm_count, cudaStream_t st) { return chunked_launch<false>(tsgm, P, sm_count, st); }
+int agg_chunked_fold_launch(int tsgm, const ChunkedFoldParams &P, int sm_count, cudaStream_t st) { return chunked_launch<true>(tsgm, P, sm_count, st); }
 
 }  // namespace s2pb

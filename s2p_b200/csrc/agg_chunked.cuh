@@ -51,6 +51,12 @@ struct ChunkedParams {
     int gmin[kMaxPV];                       // ... and the label of slot 0
     int DP;                                 // slots per pixel (multiple of 32, <= 2048)
 };
+// the folded layout (FoldView, agg_kernel.cuh): one pass index per launch; bands of ck_warps scanlines index the boundary buffer
+struct ChunkedFoldParams : ChunkedParams {
+    FoldView fv[kMaxPV];
+    int first;
+};
+template <bool FOLD> using ChunkedArgs = typename std::conditional<FOLD, ChunkedFoldParams, ChunkedParams>::type;
 
 // shared memory carve-up for a run-time DP
 struct CkSmem {
@@ -71,9 +77,9 @@ struct CkSmem {
     }
 };
 
-template <int TSGM, int TYPE, bool SCALED, int STAGE, bool GEN>
-__device__ __forceinline__ void run_band_chunked(const PassDesc &pd, const short *__restrict__ lo_img, const short *__restrict__ hi_img,
-                                                 int gmin, int DP, int band, float P1, float P2,
+template <int TSGM, int TYPE, bool SCALED, int STAGE, bool GEN, bool FOLD>
+__device__ __forceinline__ void run_band_chunked(const PassDesc &pd, const FoldView &fv, int first, const short *__restrict__ lo_img,
+                                                 const short *__restrict__ hi_img, int gmin, int DP, int band, float P1, float P2,
                                                  const float *__restrict__ lut, const int *abort_flag, unsigned char *smem)
 {
     constexpr bool useA = (TYPE == 0) ? true : (TSGM == 4);
@@ -149,9 +155,11 @@ __device__ __forceinline__ void run_band_chunked(const PassDesc &pd, const short
     range_words(0, nl0, nh0); range_words(1, nl1, nh1); range_words(2, nl2, nh2);
     const bool stage_prev = prev && from_r0;
     const long long prevbase = rowbase - pd.strideS;
-    const char *psrc = reinterpret_cast<const char *>(pd.L + prevbase * DP);
+    // (FOLD: the previous band's closing scanline is stored contiguously in the boundary buffer)
+    const char *psrc = FOLD ? reinterpret_cast<const char *>(fv.Lb + (long long)(band > 0 ? band - 1 : 0) * nI * DP)
+                            : reinterpret_cast<const char *>(pd.L + prevbase * DP);
     const float *pmsrc = pd.Lmin + prevbase;
-    const long long lstepb = strideI * (long long)(DP * 4);
+    const long long lstepb = (FOLD ? 1 : strideI) * (long long)(DP * 4);
     const unsigned r0_s = smem_s + (unsigned)SM.r0_off, r0m_s = smem_s + (unsigned)SM.r0m_off, r0rng_s = smem_s + (unsigned)SM.r0rng_off;
     long long ppix = prevbase;                               // pixel index of the previous-band pixel to stage next
     const int *prev_progress = (band > 0) ? pd.progress + (band - 1) : nullptr;
@@ -196,8 +204,10 @@ __device__ __forceinline__ void run_band_chunked(const PassDesc &pd, const short
         }
     };
 
-    float *out = pd.L + rowbase * DP;
+    float *out = (FOLD ? fv.S : pd.L) + rowbase * DP;        // FOLD: the running sum S instead of L_p
     float *lmin_out = pd.Lmin + rowbase;
+    float *lb_out = FOLD ? fv.Lb + (long long)band * nI * DP : nullptr;    // FOLD: the band-closing scanline's vectors
+    short *am_out = FOLD ? fv.am + rowbase : nullptr;
     long long upix = rowbase;                                // pixel index of the pixel computed next (for the range halves)
 
     // one neighbour's contribution for slot kk of chunk e: update_costW, mgm_core.cc:92-121
@@ -273,11 +283,13 @@ __device__ __forceinline__ void run_band_chunked(const PassDesc &pd, const short
             const CT *cp = cst + (size_t)slot * DP;
             float *mine = myring + (i & (kCkRing - 1)) * VS + kCkPad;
             float lm = S2PB_INF;
+            int la = -1;                                     // FOLD: my last slot attaining lm
             if (weighted) { wv = wst[slot]; P1w = __fmul_rn(P1, wv); }
             for (int e = 0; e < NC; e++) {
                 const int kk = 32 * e + lane;
                 float L = S2PB_INF;
                 if (e >= ea && e <= eb) {
+                    const float sv = (FOLD && !first) ? __ldcg(out + kk) : 0.f;     // FOLD: S so far (0 before pass 0)
                     float c;
                     if constexpr (GEN) c = cp[kk];
                     else {
@@ -306,11 +318,25 @@ __device__ __forceinline__ void run_band_chunked(const PassDesc &pd, const short
                         L = c + acc;
                     }
                     mine[kk] = L;
-                    lm = fminf(lm, L);
-                    out[kk] = L;
+                    if constexpr (FOLD) {
+                        // S + L_p in pass order, as the WTA adds; the arg-minimum rule of the chunked WTA (wta_chunked_kernel)
+                        if (L <= lm) la = kk;
+                        lm = fminf(lm, L);
+                        out[kk] = __fadd_rn(sv, L);
+                        if (publish) lb_out[kk] = L;
+                    } else {
+                        lm = fminf(lm, L);
+                        out[kk] = L;
+                    }
                 }
             }
             const float m = warp_min_f32(lm);
+            if constexpr (FOLD) {
+                const int a = __reduce_max_sync(0xffffffffu, lm == m ? la : -1);
+                if (lane == 0) *am_out = (short)a;
+                am_out += strideI;
+                lb_out += DP;
+            }
             if (lane == 0) {
                 mine[32 * ea - 1] = S2PB_INF;                  // guards on both sides of the span
                 mine[32 * (eb + 1)] = S2PB_INF;
@@ -331,8 +357,9 @@ __device__ __forceinline__ void run_band_chunked(const PassDesc &pd, const short
     cp_async_wait<0>();
 }
 
-template <int TSGM, bool SCALED, int STAGE, bool GEN>
-__global__ void __launch_bounds__(kCkThreads) aggregate_chunked_kernel(const __grid_constant__ ChunkedParams P)
+// FOLD: the folded layout (ChunkedFoldParams), as in aggregate_kernel
+template <int TSGM, bool SCALED, int STAGE, bool GEN, bool FOLD = false>
+__global__ void __launch_bounds__(kCkThreads) aggregate_chunked_kernel(const __grid_constant__ ChunkedArgs<FOLD> P)
 {
     extern __shared__ __align__(16) unsigned char smem[];
     __shared__ int s_item;
@@ -350,8 +377,11 @@ __global__ void __launch_bounds__(kCkThreads) aggregate_chunked_kernel(const __g
         const int band = item / P.A.nPV, pvi = item - band * P.A.nPV;
         const PassDesc &pd = P.A.pv[pvi];
         if (band >= (pd.nS + kCkWarps - 1) / kCkWarps) continue;
-        if (pd.type == 0) run_band_chunked<TSGM, 0, SCALED, STAGE, GEN>(pd, P.lo[pvi], P.hi[pvi], P.gmin[pvi], P.DP, band, P.A.P1, P.A.P2, P.A.lut, P.A.abort_flag, smem);
-        else run_band_chunked<TSGM, 1, SCALED, STAGE, GEN>(pd, P.lo[pvi], P.hi[pvi], P.gmin[pvi], P.DP, band, P.A.P1, P.A.P2, P.A.lut, P.A.abort_flag, smem);
+        FoldView fv{};
+        int first = 0;
+        if constexpr (FOLD) { fv = P.fv[pvi]; first = P.first; }
+        if (pd.type == 0) run_band_chunked<TSGM, 0, SCALED, STAGE, GEN, FOLD>(pd, fv, first, P.lo[pvi], P.hi[pvi], P.gmin[pvi], P.DP, band, P.A.P1, P.A.P2, P.A.lut, P.A.abort_flag, smem);
+        else run_band_chunked<TSGM, 1, SCALED, STAGE, GEN, FOLD>(pd, fv, first, P.lo[pvi], P.hi[pvi], P.gmin[pvi], P.DP, band, P.A.P1, P.A.P2, P.A.lut, P.A.abort_flag, smem);
     }
 }
 

@@ -3,7 +3,8 @@
 
 namespace s2pb {
 
-#define DECL(n) template <> int agg_launch_lpl<n>(int, const AggParams &, int, cudaStream_t, int); template <> int agg_configure_lpl<n>();
+#define DECL(n) template <> int agg_launch_lpl<n>(int, const AggParams &, int, cudaStream_t, int); template <> int agg_configure_lpl<n>(); \
+    template <> int agg_fold_launch_lpl<n>(int, const AggFoldParams &, int, cudaStream_t);
 S2PB_FOR_EACH_LPL(DECL)
 #undef DECL
 
@@ -19,6 +20,16 @@ int agg_launch(int LPL, int tsgm, const AggParams &P, int sm_count, cudaStream_t
 {
     switch (LPL) {
 #define CASE(n) case n: return agg_launch_lpl<n>(tsgm, P, sm_count, st, ctas_per_sm);
+    S2PB_FOR_EACH_LPL(CASE)
+#undef CASE
+    default: return -2;
+    }
+}
+
+int agg_fold_launch(int LPL, int tsgm, const AggFoldParams &P, int sm_count, cudaStream_t st)
+{
+    switch (LPL) {
+#define CASE(n) case n: return agg_fold_launch_lpl<n>(tsgm, P, sm_count, st);
     S2PB_FOR_EACH_LPL(CASE)
 #undef CASE
     default: return -2;

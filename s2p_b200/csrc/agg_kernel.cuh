@@ -18,6 +18,8 @@
 //   Lmin_p  f32  [H][W]       per-pass vector minimum; only the band-closing scanlines are written (the next band
 //                             reads them back); the per-pass LAST arg-minimum for the consensus is recomputed by the
 //                             WTA kernel from L_p
+// The folded layout (FOLD, DESIGN.md section 3.6) replaces the L_p volumes by the running sum S, a buffer of band-closing
+// scanlines and one int16 arg-minimum plane per pass (FoldView below).
 // DP = 32*LPL slots per pixel (LPL labels per lane); a warp owns one pixel, lane l owns
 // slots [l*LPL, (l+1)*LPL), so every access to a pixel's vector is one fully coalesced
 // 64*LPL- or 128*LPL-byte request whatever the scan direction of the pass.
@@ -296,6 +298,19 @@ struct AggParams {
     const float *lut;
     int general;     // 1: GEN flavour (float costs, optional per-pixel weights)
 };
+// The folded layout (DESIGN.md section 3.6): a launch carries one pass index and, instead of the pass volume L_p, each
+// pass-view updates the running sum S of its view, keeps only its band-closing scanlines (the next band reads them) and
+// records the pass's last arg-minimum per pixel for the consensus.
+struct FoldView {
+    float *S;        // [H][W][DP] sum of the passes so far, added in pass order as the WTA adds them
+    float *Lb;       // [bands][nI][DP] L_p of each band's closing scanline, at (band, i)
+    short *am;       // [H][W] the LAST slot attaining the minimum of L_p (wta_add_pass)
+};
+struct AggFoldParams : AggParams {
+    FoldView fv[kMaxPV];
+    int first;       // 1: the launch carries pass 0 (S = 0 + L_0), else S = S + L_p
+};
+template <bool FOLD> using AggArgs = typename std::conditional<FOLD, AggFoldParams, AggParams>::type;
 
 // cp.async pipeline depth in pixel steps (kStage) and slots of the previous-band ring (kR0 > kStage + 1,
 // because pixel 0 is staged ahead of the pipeline); shallower for the widest volumes.  (16 labels per lane would
@@ -401,9 +416,32 @@ template <int NBYTES> __device__ __forceinline__ void warp_cp_async_s(unsigned s
     }
 }
 
-template <int LPL, int TSGM, int TYPE, bool SCALED, bool GEN>
-__device__ __forceinline__ void run_band(const PassDesc &pd, int band, float P1, float P2, const float *__restrict__ lut,
-                                         const int *abort_flag, unsigned char *smem)
+// FOLD: one pixel's pass vector L (minimum m) into the running sum S at out: S = 0 + L_0 for pass 0, S + L_p after it -- the
+// additions and their order are those of wta_add_pass, so S after pass p is the WTA's running sum -- and the LAST slot attaining m
+// into *am, wta_add_pass's rule (slot lane*LPL + e).  S is read here, after the recursion: held across it, it made the widest and
+// the float-cost instantiations spill.
+template <int LPL>
+__device__ __forceinline__ void fold_store(float *out, short *am, const float (&L)[LPL], float m, int first, int lane)
+{
+    float t[LPL];
+    if (first) {
+#pragma unroll
+        for (int e = 0; e < LPL; e++) t[e] = 0.f;
+    } else ld_vec_cg<LPL>(out, t);
+    int a = -1;
+#pragma unroll
+    for (int e = 0; e < LPL; e++) {
+        t[e] = __fadd_rn(t[e], L[e]);
+        if (L[e] == m) a = lane * LPL + e;
+    }
+    st_vec<LPL>(out, t);
+    a = __reduce_max_sync(0xffffffffu, a);
+    if (lane == 0) *am = (short)a;
+}
+
+template <int LPL, int TSGM, int TYPE, bool SCALED, bool GEN, bool FOLD>
+__device__ __forceinline__ void run_band(const PassDesc &pd, const FoldView &fv, int first, int band, float P1, float P2,
+                                         const float *__restrict__ lut, const int *abort_flag, unsigned char *smem)
 {
     constexpr int DP = 32 * LPL;
     constexpr bool useA = (TYPE == 0) ? true : (TSGM == 4);
@@ -463,9 +501,11 @@ __device__ __forceinline__ void run_band(const PassDesc &pd, int band, float P1,
     //      previous band's last scanline (warp 0 only)
     const bool stage_prev = prevA && from_r0;
     const long long prevbase = rowbaseA - pd.strideS;
-    const char *psrc = reinterpret_cast<const char *>(pd.L + prevbase * DP);
+    // (FOLD: the previous band's closing scanline is stored contiguously in the boundary buffer)
+    const char *psrc = FOLD ? reinterpret_cast<const char *>(fv.Lb + (long long)(band > 0 ? band - 1 : 0) * nI * DP)
+                            : reinterpret_cast<const char *>(pd.L + prevbase * DP);
     const float *pmsrc = pd.Lmin + prevbase;
-    const long long lstepb = strideI * (DP * 4);
+    const long long lstepb = (FOLD ? 1 : strideI) * (DP * 4);
     const unsigned r0_s = smem_s + (unsigned)SM::r0_off, r0m_s = smem_s + (unsigned)SM::r0m_off;
     const int *prev_progress = (band > 0) ? pd.progress + (band - 1) : nullptr;
     int jp = 0, avail = 0;
@@ -504,9 +544,11 @@ __device__ __forceinline__ void run_band(const PassDesc &pd, int band, float P1,
 
     // ---- global output cursors
     const long long lstep = strideI * DP;                    // floats per pixel step along the scanline
-    float *outA = pd.L + rowbaseA * DP + lane * LPL;
+    float *outA = (FOLD ? fv.S : pd.L) + rowbaseA * DP + lane * LPL;      // FOLD: the running sum S instead of L_p
     float *outB = outA + (long long)pd.strideS * DP;
     float *lminB = pd.Lmin + rowbaseA + pd.strideS;          // only the band's last scanline publishes its minima
+    float *lbB = FOLD ? fv.Lb + (long long)band * nI * DP + lane * LPL : nullptr;   // FOLD: ... and its vectors
+    short *amA = FOLD ? fv.am + rowbaseA : nullptr, *amB = FOLD ? amA + pd.strideS : nullptr;
 
     auto fetch_prev = [&](int j, NbVec<LPL> &dst) {
         const int slot = j & srcmask;
@@ -651,8 +693,10 @@ __device__ __forceinline__ void run_band(const PassDesc &pd, int band, float P1,
                 hNew.m = mAm;
                 fill_edges<LPL>(hNew, lane);
                 if (MSG) nb_message<LPL>(hNew, P1, P2);
-                st_vec<LPL>(outA, LA);
+                if constexpr (FOLD) fold_store<LPL>(outA, amA, LA, mAm, first, lane);
+                else st_vec<LPL>(outA, LA);
                 outA += lstep;
+                if (FOLD) amA += strideI;
             }
             if (actB) {
 #pragma unroll
@@ -665,8 +709,12 @@ __device__ __forceinline__ void run_band(const PassDesc &pd, int band, float P1,
                     fill_edges<LPL>(wAB, lane);
                 }
                 if (usePrev) st_vec<LPL>(myring + (iB & (kRing - 1)) * DP, MSG ? wAB.v : LB);
-                st_vec<LPL>(outB, LB);
+                if constexpr (FOLD) {
+                    fold_store<LPL>(outB, amB, LB, mBm, first, lane);
+                    if (publish) st_vec<LPL>(lbB + (long long)iB * DP, LB);
+                } else st_vec<LPL>(outB, LB);
                 outB += lstep;
+                if (FOLD) amB += strideI;
                 if (!MSG && lane == 0 && usePrev) myringm[iB & (kRing - 1)] = mBm;
                 if (publish) {
                     if (lane == 0) *lminB = mBm;
@@ -725,8 +773,9 @@ template <int LPL, int TSGM> struct AggOcc {
     static constexpr int regs = (LPL <= 4) ? 112 : (two_wide ? 128 : 255);
     static constexpr int ctas = (regs <= 128) ? 2 : 1;
 };
-template <int LPL, int TSGM, bool SCALED, bool GEN>
-__global__ void __launch_bounds__(kAggThreads) __maxnreg__((AggOcc<LPL, TSGM>::regs)) aggregate_kernel(const __grid_constant__ AggParams P)
+// FOLD: the folded layout (AggFoldParams): one pass index per launch, S, boundary buffer and arg-minimum plane instead of L_p
+template <int LPL, int TSGM, bool SCALED, bool GEN, bool FOLD = false>
+__global__ void __launch_bounds__(kAggThreads) __maxnreg__((AggOcc<LPL, TSGM>::regs)) aggregate_kernel(const __grid_constant__ AggArgs<FOLD> P)
 {
     extern __shared__ __align__(16) unsigned char smem[];
     __shared__ int s_item;
@@ -740,8 +789,14 @@ __global__ void __launch_bounds__(kAggThreads) __maxnreg__((AggOcc<LPL, TSGM>::r
         const int band = item / P.nPV, pvi = item - band * P.nPV;
         const PassDesc &pd = P.pv[pvi];
         if (band >= pd.nBands) continue;
-        if (pd.type == 0) run_band<LPL, TSGM, 0, SCALED, GEN>(pd, band, P.P1, P.P2, P.lut, P.abort_flag, smem);
-        else run_band<LPL, TSGM, 1, SCALED, GEN>(pd, band, P.P1, P.P2, P.lut, P.abort_flag, smem);
+        if constexpr (FOLD) {
+            if (pd.type == 0) run_band<LPL, TSGM, 0, SCALED, GEN, true>(pd, P.fv[pvi], P.first, band, P.P1, P.P2, P.lut, P.abort_flag, smem);
+            else run_band<LPL, TSGM, 1, SCALED, GEN, true>(pd, P.fv[pvi], P.first, band, P.P1, P.P2, P.lut, P.abort_flag, smem);
+        } else {
+            const FoldView none{};
+            if (pd.type == 0) run_band<LPL, TSGM, 0, SCALED, GEN, false>(pd, none, 0, band, P.P1, P.P2, P.lut, P.abort_flag, smem);
+            else run_band<LPL, TSGM, 1, SCALED, GEN, false>(pd, none, 0, band, P.P1, P.P2, P.lut, P.abort_flag, smem);
+        }
     }
 }
 

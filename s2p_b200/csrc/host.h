@@ -32,7 +32,10 @@ struct ViewWS {
     short *lo, *hi;        // per-pixel label range
     uint64_t *census;
     void *C;               // [H][W][DP] costs: u8 codes (census popcounts, agg_kernel.cuh) or float (general flavour)
-    float *L[kMaxPasses];
+    float *L[kMaxPasses];  // resident layout: one volume per pass
+    float *S;              // folded layout (FoldView, agg_kernel.cuh): the running sum of the passes [H][W][DP],
+    float *Lb;             // ... the band-closing scanlines of the pass in flight,
+    short *am[kMaxPasses]; // ... and each pass's last arg-minimum [H][W]
     float *Lmin[kMaxPasses];
     int *progress;         // [kMaxPasses][maxBands]
     float *disp, *cost, *conf, *tmp;
@@ -42,6 +45,7 @@ struct Slot {
     size_t bytes = 0;
     int w = 0, h = 0, DP = 0, ndir = 0;
     int cbytes = 1;               // bytes per stored cost: 1 = 8-bit census codes, 4 = float (general flavour)
+    bool folded = false;          // the workspace holds the folded layout (slot_ensure picks it when the resident one does not fit)
     ViewWS v[2];
     int *next_item = nullptr;
     float *lut = nullptr;
@@ -79,6 +83,8 @@ struct s2pb_ctx {
     int *scratch_flag = nullptr;   // pinned + mapped: device -> host one-word answers
     int *d_scratch = nullptr;      // 64 words of device memory (hull accumulators of mgm_multi)
     std::atomic<long long> launches{0};   // (mgm_multi tiles of a batch are enqueued from several host threads)
+    size_t ws_limit = 0;                  // s2pb_set_workspace_limit: bytes per workspace, 0 = none
+    std::atomic<long long> folded_calls{0};   // mgm_calls that ran in the folded layout (s2pb_folded_calls)
     // destination of the PKR images of s2pb_mgm_pkr (device, per view), or null: every mgm_call writes them, the last one stays
     float *pkr_dst[2] = {nullptr, nullptr};
     // deadline of the matcher call in flight (timeout_ms counted from the API entry; has_deadline = false: none)

@@ -659,6 +659,52 @@ __global__ void __launch_bounds__(kWtaThreads) __maxnreg__((LPL <= 4) ? 64 : 128
     else wta_pixels<LPL, GEN, 0>(P, sSrow);
 }
 
+// The WTA of the folded layout (FoldView, agg_kernel.cuh): the aggregation has summed S in pass order and recorded each pass's
+// last arg-minimum, so a pixel reads its S vector, its costs (for the overcount fix) and one short per pass, and ends in
+// wta_finish as wta_kernel does -- the same winner, consensus, sub-pixel fit, PKR and outputs.
+struct FoldPlanes {
+    const float *S;                     // [npix][DP]
+    const short *am[kMaxPasses];        // [npix] per pass (passes >= ndir: unused)
+};
+// a pixel's costs in the WTA's slot mapping (WtaMap)
+template <int LPL, bool GEN> __device__ __forceinline__ void wta_ld_cost(const WtaParams &P, size_t p, int lane, float (&c)[LPL])
+{
+    constexpr int DP = 32 * LPL;
+    if constexpr (GEN) wta_ld_pass<LPL>(reinterpret_cast<const float *>(P.C) + p * DP, lane, c);
+    else if constexpr (WtaMap<LPL>::interleaved) {
+        const uint8_t *cp = reinterpret_cast<const uint8_t *>(P.C) + p * DP + lane;
+#pragma unroll
+        for (int e = 0; e < LPL; e++) c[e] = cost_value(__ldg(cp + 32 * e), P.lut);
+    } else {
+        const CostPack<LPL> cp = ld_cost<LPL, true>(reinterpret_cast<const uint8_t *>(P.C) + p * DP + lane * LPL);
+#pragma unroll
+        for (int e = 0; e < LPL; e++) c[e] = cost_value(cost_code(cp, e), P.lut);
+    }
+}
+template <int LPL, bool GEN>
+__global__ void __launch_bounds__(kWtaThreads) wta_fold_kernel(const WtaParams P, const FoldPlanes F)
+{
+    constexpr int DP = 32 * LPL;
+    __shared__ float sS[kWtaThreads / 32][DP];
+    float *sSrow = sS[threadIdx.x >> 5];
+    const int lane = threadIdx.x & 31;
+    const short *amp = F.am[0];                   // lanes 0 .. ndir-1: the arg-minimum plane of pass `lane`
+#pragma unroll
+    for (int q = 1; q < kMaxPasses; q++) if (lane == q) amp = F.am[q];
+    const size_t warp = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = ((size_t)gridDim.x * blockDim.x) >> 5;
+    for (size_t p = warp; p < P.npix; p += nwarps) {
+        const int plo = __ldg(P.lo + p), phi = __ldg(P.hi + p);
+        const int a = lane < P.ndir ? __ldg(amp + p) : -1;
+        float s[LPL], c[LPL];
+        wta_ld_pass<LPL>(F.S + p * DP, lane, s);
+        wta_ld_cost<LPL, GEN>(P, p, lane, c);
+        int am[kMaxPasses];
+#pragma unroll
+        for (int d = 0; d < kMaxPasses; d++) am[d] = __shfl_sync(0xffffffffu, a, d);
+        wta_finish<LPL>(P, p, lane, s, am, c, sSrow, plo, phi);
+    }
+}
+
 // The same WTA reading only the labels that can still win (DESIGN.md 3.2).  Census flavour, unit weights: every message of
 // the aggregation is >= 0, so L_p[d] >= C[d] in every pass, S[d] >= C[d] and S[d] >= L_0[d].  With T = S[d0] of one probe
 // slot d0 (any slot gives a valid bound; the first slot holding the pixel's smallest cost code is the probe), a slot with
@@ -792,8 +838,9 @@ __global__ void __launch_bounds__(kWtaThreads) __maxnreg__((LPL <= 4) ? 64 : 128
 // label range (slot 32*e + lane), so a 40-label pixel of a 512-slot slab reads 2 x 128 B per pass instead of 2 KB.
 // Per lane it keeps, for every pass, the running minimum and the LAST slot attaining it, and for S the running
 // first minimum; S itself goes to shared memory for the sub-pixel fit.  Same arithmetic as wta_kernel<LPL, GEN>.
-template <bool GEN>
-__global__ void __launch_bounds__(kWtaThreads) wta_chunked_kernel(const WtaParams P, int DP)
+// FOLD: the folded layout's WTA (F): S is read as the aggregation summed it, and each pass's arg-minimum from its plane.
+template <bool GEN, bool FOLD = false>
+__global__ void __launch_bounds__(kWtaThreads) wta_chunked_kernel(const WtaParams P, int DP, const FoldPlanes F)
 {
     extern __shared__ float sS_all[];                    // [warps][DP]
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
@@ -811,13 +858,16 @@ __global__ void __launch_bounds__(kWtaThreads) wta_chunked_kernel(const WtaParam
         for (int e = ea; e <= eb; e++) {
             const int kk = 32 * e + lane;
             float s = 0.f;
+            if constexpr (FOLD) s = __ldcg(F.S + p * DP + kk);
+            else {
 #pragma unroll
-            for (int d = 0; d < kMaxPasses; d++)
-                if (d < P.ndir) {
-                    const float v = __ldcg(P.L[d] + p * DP + kk);
-                    if (v < pm[d]) { pm[d] = v; pa[d] = kk; } else if (v == pm[d]) pa[d] = kk;
-                    s += v;
-                }
+                for (int d = 0; d < kMaxPasses; d++)
+                    if (d < P.ndir) {
+                        const float v = __ldcg(P.L[d] + p * DP + kk);
+                        if (v < pm[d]) { pm[d] = v; pa[d] = kk; } else if (v == pm[d]) pa[d] = kk;
+                        s += v;
+                    }
+            }
             const float c = GEN ? reinterpret_cast<const float *>(P.C)[p * DP + kk]
                                 : cost_value(reinterpret_cast<const uint8_t *>(P.C)[p * DP + kk], P.lut);
             if (P.fix_overcount == 1) s = fmaf(-(float)(P.ndir - 1), c, s);
@@ -830,8 +880,11 @@ __global__ void __launch_bounds__(kWtaThreads) wta_chunked_kernel(const WtaParam
         for (int d = 0; d < kMaxPasses; d++) {
             confi_src[d] = -1;
             if (d < P.ndir) {
-                const float md = warp_min_f32(pm[d]);
-                confi_src[d] = __reduce_max_sync(0xffffffffu, (pm[d] == md) ? pa[d] : -1);
+                if constexpr (FOLD) confi_src[d] = __ldg(F.am[d] + p);
+                else {
+                    const float md = warp_min_f32(pm[d]);
+                    confi_src[d] = __reduce_max_sync(0xffffffffu, (pm[d] == md) ? pa[d] : -1);
+                }
             }
         }
         const float m = warp_min_f32(best);

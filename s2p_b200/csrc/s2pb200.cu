@@ -40,9 +40,21 @@ int fail(int code, const char *fmt, ...)
 // chunk-skipping kernel on float-cost slabs wider than 1024 slots (agg_chunked.cuh, ck_warps)
 static int max_bands(int w, int h) { return ((w > h ? w : h) + 1) / 2; }
 
-static int slot_layout(Slot &s, int w, int h, int DP, int ndir, int cbytes, bool allocate)
+// Scanlines of the boundary buffer of the folded layout: one per band of the pass, for the larger of the two scan geometries
+// (rows: h scanlines of w pixels; columns: w of h).  A band holds kNW scanlines in the register-resident kernel and ck_warps in
+// the chunk-skipping one, which serves the slabs wider than 512 slots (wide_slab).
+static size_t boundary_pixels(int w, int h, int DP, bool gen)
 {
-    // carve one allocation; called first with allocate=false to size it
+    const int nw = DP > 512 ? ck_warps(DP, gen) : kNW;
+    const size_t rows = (size_t)((h + nw - 1) / nw) * w, cols = (size_t)((w + nw - 1) / nw) * h;
+    return rows > cols ? rows : cols;
+}
+
+// The workspace of one slot, in the resident layout (eight pass volumes per view) or the folded one (the running sum S, the
+// boundary buffer and one arg-minimum plane per pass, DESIGN.md section 3.6).  Carves one allocation; called with
+// allocate=false to size it (s.bytes).
+static int slot_layout(Slot &s, int w, int h, int DP, int ndir, int cbytes, bool folded, bool allocate)
+{
     size_t npix = (size_t)w * h, off = 0;
     auto take = [&](size_t bytes) { size_t o = off; off = align_up(off + bytes, 256); return o; };
     char *b = (char *)s.base;
@@ -60,8 +72,15 @@ static int slot_layout(Slot &s, int w, int h, int DP, int ndir, int cbytes, bool
         o = take((size_t)h * 4); if (allocate) v.rowthr = (float *)(b + o);
         o = take(256); if (allocate) v.rtstate = (RtState *)(b + o);
         o = take(npix * DP * cbytes); if (allocate) v.C = (void *)(b + o);
+        for (int p = 0; p < kMaxPasses; p++) { v.L[p] = nullptr; v.am[p] = nullptr; }
+        v.S = v.Lb = nullptr;
+        if (folded) {
+            o = take(npix * DP * 4); if (allocate) v.S = (float *)(b + o);
+            o = take(boundary_pixels(w, h, DP, cbytes == 4) * DP * 4); if (allocate) v.Lb = (float *)(b + o);
+            for (int p = 0; p < ndir; p++) { o = take(npix * 2); if (allocate) v.am[p] = (short *)(b + o); }
+        }
         for (int p = 0; p < ndir; p++) {
-            o = take(npix * DP * 4); if (allocate) v.L[p] = (float *)(b + o);
+            if (!folded) { o = take(npix * DP * 4); if (allocate) v.L[p] = (float *)(b + o); }
             o = take(npix * 4); if (allocate) v.Lmin[p] = (float *)(b + o);
         }
         o = take((size_t)kMaxPasses * mb * 4); if (allocate) v.progress = (int *)(b + o);
@@ -95,24 +114,62 @@ static int slot_io_ensure(Slot &s, size_t npix)
     return S2PB_OK;
 }
 
-static int slot_ensure(s2pb_ctx *ctx, Slot &s, int w, int h, int DP, int ndir, int cbytes = 1)
+static size_t layout_bytes(int w, int h, int DP, int ndir, int cbytes, bool folded)
 {
     Slot probe;
-    slot_layout(probe, w, h, DP, ndir, cbytes, false);
-    if (!s.base || probe.bytes > s.bytes) {
-        if (s.base) { CK(cudaStreamSynchronize(s.stream)); CK(cudaFree(s.base)); s.base = nullptr; }
-        cudaError_t e = cudaMalloc(&s.base, probe.bytes);
-        if (e != cudaSuccess) {
-            cudaGetLastError();
-            s.base = nullptr; s.bytes = 0;
-            return fail(S2PB_ERR_NOMEM, "workspace of %.2f GiB for a %dx%dx%d tile does not fit: %s",
-                        probe.bytes / 1073741824.0, w, h, DP, cudaGetErrorString(e));
-        }
-        s.bytes = probe.bytes;
+    slot_layout(probe, w, h, DP, ndir, cbytes, folded, false);
+    return probe.bytes;
+}
+
+// The layout a workspace limit (0: none) selects: 0 resident when it is within the limit, else 1 folded when that is, else -1
+// (slot_ensure also falls back to the folded layout when the resident one's allocation fails)
+static bool fits(size_t bytes, size_t limit) { return limit == 0 || bytes <= limit; }
+static int plan_layout(size_t resident, size_t folded, size_t limit)
+{
+    return fits(resident, limit) ? 0 : fits(folded, limit) ? 1 : -1;
+}
+
+// s.base holds at least `bytes` afterwards, or false (nothing allocated; the CUDA error in *err)
+static int slot_alloc(Slot &s, size_t bytes, cudaError_t *err)
+{
+    *err = cudaSuccess;
+    if (s.base && bytes <= s.bytes) return S2PB_OK;
+    if (s.base) { CK(cudaStreamSynchronize(s.stream)); CK(cudaFree(s.base)); s.base = nullptr; s.bytes = 0; }
+    *err = cudaMalloc(&s.base, bytes);
+    if (*err != cudaSuccess) { cudaGetLastError(); s.base = nullptr; s.bytes = 0; return S2PB_OK; }
+    s.bytes = bytes;
+    return S2PB_OK;
+}
+
+// Size the slot's workspace for a tile and carve it.  The resident layout when it is within the context's workspace limit
+// (s2pb_set_workspace_limit) and its allocation succeeds, else the folded one (allow_fold: the matcher's calls; the stage entry
+// points run resident only), else S2PB_ERR_NOMEM naming both sizes.
+static int slot_ensure(s2pb_ctx *ctx, Slot &s, int w, int h, int DP, int ndir, int cbytes = 1, bool allow_fold = true)
+{
+    const size_t limit = ctx->ws_limit;
+    const size_t res = layout_bytes(w, h, DP, ndir, cbytes, false), fold = layout_bytes(w, h, DP, ndir, cbytes, true);
+    if (s.base && limit != 0 && s.bytes > limit) {        // allocated before the limit was lowered: give it back
+        CK(cudaStreamSynchronize(s.stream)); CK(cudaFree(s.base)); s.base = nullptr; s.bytes = 0;
     }
-    s.w = w; s.h = h; s.DP = DP; s.ndir = ndir; s.cbytes = cbytes;
+    const int plan = plan_layout(res, fold, limit);
+    cudaError_t e = cudaErrorMemoryAllocation;
+    bool folded = false;
+    int rc;
+    if (plan == 0 && (rc = slot_alloc(s, res, &e)) != S2PB_OK) return rc;
+    if (plan >= 0 && e != cudaSuccess && allow_fold) {
+        folded = true;
+        if ((rc = slot_alloc(s, fold, &e)) != S2PB_OK) return rc;
+    }
+    if (e != cudaSuccess) {
+        char why[128];
+        if (!fits(allow_fold ? fold : res, limit)) snprintf(why, sizeof why, "the workspace limit is %.2f GiB", limit / 1073741824.0);
+        else snprintf(why, sizeof why, "%s", cudaGetErrorString(e));
+        return fail(S2PB_ERR_NOMEM, "workspace for a %dx%dx%d tile does not fit: %.2f GiB resident, %.2f GiB folded%s: %s",
+                    w, h, DP, res / 1073741824.0, fold / 1073741824.0, allow_fold ? "" : " (not available here)", why);
+    }
+    s.w = w; s.h = h; s.DP = DP; s.ndir = ndir; s.cbytes = cbytes; s.folded = folded;
     size_t keep = s.bytes;
-    slot_layout(s, w, h, DP, ndir, cbytes, true);
+    slot_layout(s, w, h, DP, ndir, cbytes, folded, true);
     s.bytes = keep;
     return S2PB_OK;
 }
@@ -186,7 +243,9 @@ extern "C" s2pb_ctx *s2pb_create(int device)
     // function attributes are per device: every context sets them for its own (not once per process)
     if (agg_configure() != 0 || agg_chunked_configure() != 0 ||
         cudaFuncSetAttribute(wta_chunked_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * 2048 * 4) != cudaSuccess ||
-        cudaFuncSetAttribute(wta_chunked_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * 2048 * 4) != cudaSuccess) {
+        cudaFuncSetAttribute(wta_chunked_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * 2048 * 4) != cudaSuccess ||
+        cudaFuncSetAttribute(wta_chunked_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * 2048 * 4) != cudaSuccess ||
+        cudaFuncSetAttribute(wta_chunked_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * 2048 * 4) != cudaSuccess) {
         fail(S2PB_ERR_CUDA, "cudaFuncSetAttribute failed for the aggregation kernels"); delete ctx; return nullptr;
     }
     return ctx;
@@ -235,6 +294,14 @@ extern "C" int s2pb_default_params(const char *algo, s2pb_mgm_params *p)
 
 extern "C" int s2pb_num_slots(const s2pb_ctx *ctx) { return ctx ? (int)ctx->slots.size() : 0; }
 extern "C" long long s2pb_kernel_launches(const s2pb_ctx *ctx) { return ctx ? ctx->launches.load() : 0LL; }
+extern "C" long long s2pb_folded_calls(const s2pb_ctx *ctx) { return ctx ? ctx->folded_calls.load() : 0LL; }
+
+extern "C" int s2pb_set_workspace_limit(s2pb_ctx *ctx, long long bytes)
+{
+    if (!ctx || bytes < 0) return fail(S2PB_ERR_ARG, "bad argument");
+    ctx->ws_limit = (size_t)bytes;
+    return S2PB_OK;
+}
 
 extern "C" int s2pb_sync(s2pb_ctx *ctx)
 {
@@ -366,6 +433,32 @@ static int slab_lpl(int D, int *lpl)
     return S2PB_OK;
 }
 
+// the workspace arithmetic of a w x h tile of D labels, for the C ABI (no device): slot_layout of the slab slab_lpl gives
+static int workspace_args(int w, int h, int D, int ndir, int cost_bytes, int *DP)
+{
+    if (w < 2 || h < 2 || D < 1) return fail(S2PB_ERR_ARG, "bad tile shape %dx%d, %d labels", w, h, D);
+    if (ndir != 2 && ndir != 4 && ndir != 8) return fail(S2PB_ERR_ARG, "ndir must be 2, 4 or 8");
+    if (cost_bytes != 1 && cost_bytes != 4) return fail(S2PB_ERR_ARG, "cost_bytes must be 1 (census codes) or 4 (float costs)");
+    int LPL, rc = slab_lpl(D, &LPL);
+    if (rc != S2PB_OK) return rc;
+    *DP = 32 * LPL;
+    return S2PB_OK;
+}
+extern "C" long long s2pb_workspace_bytes(int w, int h, int D, int ndir, int cost_bytes, int folded)
+{
+    int DP, rc = workspace_args(w, h, D, ndir, cost_bytes, &DP);
+    if (rc != S2PB_OK) return rc;
+    return (long long)layout_bytes(w, h, DP, ndir, cost_bytes, folded != 0);
+}
+extern "C" int s2pb_workspace_layout(int w, int h, int D, int ndir, int cost_bytes, long long limit)
+{
+    int DP, rc = workspace_args(w, h, D, ndir, cost_bytes, &DP);
+    if (rc != S2PB_OK) return rc;
+    if (limit < 0) return fail(S2PB_ERR_ARG, "negative limit");
+    const int plan = plan_layout(layout_bytes(w, h, DP, ndir, cost_bytes, false), layout_bytes(w, h, DP, ndir, cost_bytes, true), (size_t)limit);
+    return plan >= 0 ? plan : fail(S2PB_ERR_NOMEM, "neither layout fits the limit");
+}
+
 static void fill_pass(PassDesc &pd, int pass, int w, int h)
 {
     const long long W = w, H = h;
@@ -431,6 +524,56 @@ static int launch_aggregate(s2pb_ctx *ctx, Slot &s, int nviews, int w, int h, in
                     wide_slab(LPL) ? "chunk-skipping" : "register-resident", 32 * LPL, tsgm, general ? " (float costs)" : "");
     if (r != 0) return fail(S2PB_ERR_CUDA, "aggregation launch failed: %s", cudaGetErrorString(cudaGetLastError()));
     ctx->launches++;
+    return S2PB_OK;
+}
+
+// The same aggregation in the folded layout: one launch per pass index, in pass order on stream st, each carrying pass p of the
+// `nviews` views; every launch adds its pass into the views' S, so the order of the launches is the order of the sum.  The
+// item queue is reset before every launch; each pass has its own progress counters, reset once.
+static int launch_aggregate_folded(s2pb_ctx *ctx, Slot &s, int nviews, int w, int h, int LPL, float P1, float P2, int ndir,
+                                   int tsgm, const float *lut, cudaStream_t st, bool general, const float *const *wgt,
+                                   const int *gminv, int first_view)
+{
+    const int mb = max_bands(w, h);
+    int *counter = s.next_item + 16 * first_view;
+    for (int vi = first_view; vi < first_view + nviews; vi++) CK(cudaMemsetAsync(s.v[vi].progress, 0, (size_t)kMaxPasses * mb * 4, st));
+    for (int p = 0; p < ndir; p++) {
+        ChunkedFoldParams Q;                  // (its AggFoldParams part is what the register-resident kernel takes)
+        AggFoldParams F;
+        memset(&Q, 0, sizeof Q);
+        memset(&F, 0, sizeof F);
+        AggParams &P = F;
+        for (int vi = first_view; vi < first_view + nviews; vi++) {
+            const int q = P.nPV++;
+            PassDesc &pd = P.pv[q];
+            fill_pass(pd, p, w, h);
+            pd.C = s.v[vi].C; pd.L = nullptr; pd.Lmin = s.v[vi].Lmin[p];
+            pd.W = (general && wgt) ? wgt[vi] : nullptr;
+            pd.progress = s.v[vi].progress + (size_t)p * mb;
+            if (pd.nBands > P.maxBands) P.maxBands = pd.nBands;
+            F.fv[q] = FoldView{s.v[vi].S, s.v[vi].Lb, s.v[vi].am[p]};
+            Q.lo[q] = s.v[vi].lo; Q.hi[q] = s.v[vi].hi; Q.gmin[q] = gminv ? gminv[vi] : 0;
+        }
+        P.P1 = P1; P.P2 = P2; P.next_item = counter; P.abort_flag = ctx->abort_flag; P.lut = general ? nullptr : lut;
+        P.general = general ? 1 : 0;
+        F.first = p == 0;
+        CK(cudaMemsetAsync(counter, 0, 4, st));
+        int r;
+        if (wide_slab(LPL)) {
+            Q.A = P;
+            Q.DP = 32 * LPL;
+            for (int q = 0; q < P.nPV; q++) Q.fv[q] = F.fv[q];
+            Q.first = F.first;
+            r = agg_chunked_fold_launch(tsgm, Q, ctx->sm_count, st);
+        } else {
+            r = agg_fold_launch(LPL, tsgm, F, ctx->sm_count, st);
+        }
+        if (r == -2)
+            return fail(S2PB_ERR_UNSUPPORTED, "no folded %s aggregation kernel serves a slab of %d slots with TSGM %d%s",
+                        wide_slab(LPL) ? "chunk-skipping" : "register-resident", 32 * LPL, tsgm, general ? " (float costs)" : "");
+        if (r != 0) return fail(S2PB_ERR_CUDA, "aggregation launch failed: %s", cudaGetErrorString(cudaGetLastError()));
+        ctx->launches++;
+    }
     return S2PB_OK;
 }
 
@@ -502,12 +645,39 @@ static int launch_wta(s2pb_ctx *ctx, int LPL, const WtaParams &P, cudaStream_t s
     if (P.S == nullptr && wide_slab(LPL)) {
         const int DP = 32 * LPL;
         const size_t smem = (size_t)(kWtaThreads / 32) * DP * sizeof(float);
-        if (general) launch(ctx, wta_chunked_kernel<true>, sm * 16, kWtaThreads, smem, st, P, DP);
-        else launch(ctx, wta_chunked_kernel<false>, sm * 16, kWtaThreads, smem, st, P, DP);
+        if (general) launch(ctx, wta_chunked_kernel<true>, sm * 16, kWtaThreads, smem, st, P, DP, FoldPlanes{});
+        else launch(ctx, wta_chunked_kernel<false>, sm * 16, kWtaThreads, smem, st, P, DP, FoldPlanes{});
     } else {
         const bool pruned = ctx->wta_prune && !general && P.ndir == kMaxPasses && P.S == nullptr && P.pkr == nullptr &&
                             wta_pruned_width(LPL);
         rc = with_lpl(LPL, [&](auto k) { constexpr int K = decltype(k)::value; launch_wta_t<K>(ctx, P, st, general, pruned); });
+    }
+    if (rc != S2PB_OK) return rc;
+    CK(cudaGetLastError());
+    return S2PB_OK;
+}
+
+// The WTA of one view in the folded layout (wta_fold_kernel, or its chunk-skipping counterpart on a wide slab): S and the
+// arg-minimum planes of the view instead of its pass volumes.  No dense S output (the stage entry points run resident).
+static int launch_wta_folded(s2pb_ctx *ctx, int LPL, const WtaParams &P, const ViewWS &v, cudaStream_t st, bool general)
+{
+    const int sm = ctx->sm_count;
+    FoldPlanes F;
+    memset(&F, 0, sizeof F);
+    F.S = v.S;
+    for (int d = 0; d < kMaxPasses; d++) F.am[d] = v.am[d];
+    int rc = S2PB_OK;
+    if (wide_slab(LPL)) {
+        const int DP = 32 * LPL;
+        const size_t smem = (size_t)(kWtaThreads / 32) * DP * sizeof(float);
+        if (general) launch(ctx, wta_chunked_kernel<true, true>, sm * 16, kWtaThreads, smem, st, P, DP, F);
+        else launch(ctx, wta_chunked_kernel<false, true>, sm * 16, kWtaThreads, smem, st, P, DP, F);
+    } else {
+        rc = with_lpl(LPL, [&](auto k) {
+            constexpr int K = decltype(k)::value;
+            if (general) launch(ctx, wta_fold_kernel<K, true>, sm * 16, kWtaThreads, 0, st, P, F);
+            else launch(ctx, wta_fold_kernel<K, false>, sm * 16, kWtaThreads, 0, st, P, F);
+        });
     }
     if (rc != S2PB_OK) return rc;
     CK(cudaGetLastError());
@@ -764,7 +934,21 @@ static int mgm_call(s2pb_ctx *ctx, Slot &s, int w, int h, const float *const img
     // ---- 8-pass MGM of both views (mgm_multiscale.cc:194-202: P1 / ZOOMFACTOR) in one persistent launch, or two when the
     // views' slabs differ in width
     const float P1 = p->P1 / (float)zoom;
-    if (LPLv[0] == LPLv[1]) {
+    if (s.folded) {
+        // the folded layout (slot_ensure): one launch per pass, in pass order; the views side by side as below when their slabs
+        // differ in width
+        ctx->folded_calls++;
+        if (LPLv[0] == LPLv[1]) {
+            rc = launch_aggregate_folded(ctx, s, 2, w, h, LPLv[0], P1, p->P2, p->ndir, p->tsgm, lut, st, general, wgt, gminv, 0);
+        } else {
+            CK(cudaEventRecord(s.fork, st));
+            CK(cudaStreamWaitEvent(s.stream2, s.fork, 0));
+            rc = launch_aggregate_folded(ctx, s, 1, w, h, LPLv[0], P1, p->P2, p->ndir, p->tsgm, lut, st, general, wgt, gminv, 0);
+            if (rc == S2PB_OK) rc = launch_aggregate_folded(ctx, s, 1, w, h, LPLv[1], P1, p->P2, p->ndir, p->tsgm, lut, s.stream2, general, wgt, gminv, 1);
+            CK(cudaEventRecord(s.join, s.stream2));
+            CK(cudaStreamWaitEvent(st, s.join, 0));
+        }
+    } else if (LPLv[0] == LPLv[1]) {
         // With another tile's aggregation queued or running (tiles in flight) the launch takes one CTA per SM instead of two, so
         // two tiles' aggregations share the SMs: a pass is a chain of bands, two CTAs per SM on 16 pass-views run it twice as
         // many bands deep as one CTA per SM does, and a good part of each launch is the chain filling and draining.  (This
@@ -790,7 +974,7 @@ static int mgm_call(s2pb_ctx *ctx, Slot &s, int w, int h, const float *const img
         fill_wta(W, s.v[vi], p->ndir, gminv[vi], p, lut, npix);
         W.inv_zoom_div = (float)zoom;
         W.pkr = ctx->pkr_dst[vi];
-        rc = launch_wta(ctx, LPLv[vi], W, st, general);
+        rc = s.folded ? launch_wta_folded(ctx, LPLv[vi], W, s.v[vi], st, general) : launch_wta(ctx, LPLv[vi], W, st, general);
         if (rc != S2PB_OK) return rc;
     }
     if (timed) CK(cudaEventRecord(s.ev[4], st));
@@ -1415,7 +1599,7 @@ static int stage_aggregate(s2pb_ctx *ctx, const float *C, const int32_t *lo, con
     if (rc == S2PB_OK) rc = L.error();
     if (rc != S2PB_OK) return rc;
     Slot &s = ctx->slots[0];          // the workspace of slot 0 holds the slab
-    rc = slot_ensure(ctx, s, w, h, DP, ndir, general ? 4 : 1);
+    rc = slot_ensure(ctx, s, w, h, DP, ndir, general ? 4 : 1, false);
     if (rc != S2PB_OK) return rc;
     size_t totp = npix * DP;
     if (general) launch(ctx, pad_cost_kernel, (unsigned)((totp + 255) / 256), 256, 0, L.st, dCf, npix, D, DP, (float *)s.v[0].C);

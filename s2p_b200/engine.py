@@ -36,6 +36,22 @@ def device_count():
     return _lib.lib().s2pb_device_count()
 
 
+def workspace_bytes(w, h, nlabels, ndir=8, cost_bytes=1, folded=False):
+    """Bytes of one workspace for a w x h tile whose slab holds ``nlabels`` labels, in the resident or the folded layout
+    (s2pb_workspace_bytes; no device needed).  ``cost_bytes``: 1 for census codes, 4 for the other distances or the weights."""
+    r = _lib.lib().s2pb_workspace_bytes(int(w), int(h), int(nlabels), int(ndir), int(cost_bytes), int(bool(folded)))
+    _lib.check(int(r) if r < 0 else 0)
+    return int(r)
+
+
+def workspace_layout(w, h, nlabels, ndir=8, cost_bytes=1, limit=0):
+    """'resident' or 'folded': the layout a workspace limit of ``limit`` bytes (0: none) selects for that tile; raises S2pbError
+    (S2PB_ERR_NOMEM) when neither fits (s2pb_workspace_layout)."""
+    r = _lib.lib().s2pb_workspace_layout(int(w), int(h), int(nlabels), int(ndir), int(cost_bytes), int(limit))
+    _lib.check(r if r < 0 else 0)
+    return "folded" if r == 1 else "resident"
+
+
 def _f32(a):
     return np.ascontiguousarray(a, dtype=np.float32)
 
@@ -200,6 +216,15 @@ class Engine:
         ms = (ctypes.c_float * len(_lib.T_NAMES))()
         _lib.check(self._L.s2pb_last_timings(self._ctx, int(slot), ms))
         return dict(zip(_lib.T_NAMES, [float(x) for x in ms]))
+
+    def set_workspace_limit(self, nbytes):
+        """Cap each workspace of this engine at ``nbytes`` (0: no cap).  A tile whose resident workspace exceeds the cap runs in the
+        folded layout, with the same results (s2pb_set_workspace_limit)."""
+        _lib.check(self._L.s2pb_set_workspace_limit(self._ctx, int(nbytes)))
+
+    def folded_calls(self):
+        """matcher calls (pyramid levels of mgm_multi included) that ran in the folded layout"""
+        return int(self._L.s2pb_folded_calls(self._ctx))
 
     def kernel_launches(self):
         return int(self._L.s2pb_kernel_launches(self._ctx))
@@ -649,5 +674,10 @@ def get_engine(device=None):
             device = (ident[0] - 1) % n if ident else 0
     key = (os.getpid(), device)
     if key not in _engines:
-        _engines[key] = Engine(device)
+        eng = Engine(device)
+        # S2PB_WORKSPACE_LIMIT (GiB per workspace): the setting reaches s2p's pool workers through their environment
+        limit = os.environ.get("S2PB_WORKSPACE_LIMIT")
+        if limit:
+            eng.set_workspace_limit(int(float(limit) * 2 ** 30))
+        _engines[key] = eng
     return _engines[key]
