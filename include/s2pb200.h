@@ -37,6 +37,8 @@
  *                        (s2p/__init__.py:479-525)
  *   s2pb_sgbm()          the `sgbm` subprocess (OpenCV 2's StereoSGBM, 3rdparty/sgbm) + create_rejection_mask
  *                        (s2p/block_matching.py:116-134)
+ *   s2pb_pair_tile_to_ply() rectification_pair, stereo_matching and disparity_to_ply of a two-view tile (s2p/__init__.py:102-318)
+ *                        in one call, from the source crops to the records of cloud.ply
  *
  * Conventions: all images are single-band, row-major, C-contiguous float32,
  * NaN = no data.  Disparity d at ref pixel (x,y) means the match is at
@@ -414,6 +416,49 @@ int s2pb_deflate_blocks(s2pb_ctx *ctx, const float *raster, int W, int H, int ba
 
 /* masking.erosion (s2p/masking.py:87-97 = `morsi diskR erosion`, c/morsi.c:54-66,280-298) on a 0/1 mask */
 int s2pb_erode_mask(s2pb_ctx *ctx, const uint8_t *in, uint8_t *out, int w, int h, float radius);
+
+/* ---- a two-view tile from its source images to its point cloud (s2p.main steps 3 to 5 with two images) ---------- */
+enum { S2PB_MATCHER_MGM = 0, S2PB_MATCHER_SGBM = 1 };
+/* The inputs of s2pb_pair_tile_to_ply, stage by stage.  Host pointers. */
+typedef struct s2pb_pair_tile {
+    /* rectify_pair's two warps: the crops of the two images and their rectifying homographies with the crops' origins folded in */
+    const float *src1, *src2;
+    int32_t sw1, sh1, sw2, sh2;
+    double H1[9], H2[9];
+    int32_t w, h;                /* the rectified size */
+    int32_t dmin, dmax;          /* the matcher's range, as compute_disparity_map hands it to the matcher */
+    /* the matcher */
+    int32_t matcher;             /* S2PB_MATCHER_MGM (mgm, mgm_multi, mgm_multi_lsd by mgm.scales and wl / wr) or _SGBM */
+    s2pb_mgm_params mgm;
+    s2pb_sgbm_params sgbm;
+    const float *wl, *wr;        /* MGM: the -wl / -wr weight images (w*h float32), both or neither */
+    float erode_radius;          /* masking.erosion of the mask: 0 none, else a disk radius in (1, 64] */
+    /* disparity_to_ply's cloud: s2pb_disp_to_ply's arguments from msk_orig to south, and the filter's r, p, n */
+    const float *msk_orig;
+    int32_t mw, mh;
+    float bbox[4];
+    const s2pb_rpc *rpc1, *rpc2;
+    double ha[9], hb[9];         /* H_ref and H_sec . A^-1 as disparity_to_ply reads them */
+    int32_t zone, south;
+    float r;
+    int32_t p, n;
+    /* the colours: the rectified reference stretched with pct, or, when clr is not null, clr_bands float32 planes of the cw x ch
+     * crop of the clr image warped by hc as s2pb_disp_to_ply_clr warps them */
+    double pct;
+    const float *clr;
+    int32_t cw, ch, clr_bands;
+    double hc[9];
+    int32_t with_conf;           /* MGM: the confidence column */
+} s2pb_pair_tile;
+/* s2pb_homography x 2 -> s2pb_mgm_weighted or s2pb_sgbm -> s2pb_erode_mask when erode_radius > 0 -> s2pb_disp_to_ply, or
+ * s2pb_disp_to_ply_clr with a clr crop, on the disparity, the eroded mask as float32 and a zero dispy, in one call: the rectified pair, the
+ * disparity, the confidence and the mask stay on the device between the stages, and the records and every intermediate are
+ * those of that sequence, bit for bit.  records: w*h records of the record size of the colours and the confidence; *npoints
+ * gets the number written.  Nullable host copies of the intermediates (w*h each): rect1, rect2, disp, conf (MGM), mask (0/1,
+ * after the erosion), disp_right (MGM).  Errors as the calls of the sequence, S2PB_ERR_TIMEOUT from the MGM matcher included;
+ * S2PB_ERR_ARG also for conf, disp_right or with_conf with sgbm.  Synchronous. */
+int s2pb_pair_tile_to_ply(s2pb_ctx *ctx, const s2pb_pair_tile *t, uint8_t *records, int64_t *npoints, float *rect1, float *rect2,
+                          float *disp, float *conf, uint8_t *mask, float *disp_right);
 
 /* ---- stage-level entry points (host buffers; used by the parity tests) ----- */
 /* census_tools.cc:127-153.  codes: w*h uint64, first neighbour in the top bit. */

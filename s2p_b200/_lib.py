@@ -31,6 +31,23 @@ class SgbmParams(ctypes.Structure):
     _fields_ = [("win", c_int32), ("P1", c_int32), ("P2", c_int32), ("lr_diff", c_int32)]
 
 
+class PairTile(ctypes.Structure):
+    """Mirror of ``s2pb_pair_tile``: the inputs of s2pb_pair_tile_to_ply."""
+    _fields_ = [
+        ("src1", POINTER(c_float)), ("src2", POINTER(c_float)), ("sw1", c_int32), ("sh1", c_int32), ("sw2", c_int32),
+        ("sh2", c_int32), ("H1", c_double * 9), ("H2", c_double * 9), ("w", c_int32), ("h", c_int32), ("dmin", c_int32),
+        ("dmax", c_int32), ("matcher", c_int32), ("mgm", MgmParams), ("sgbm", SgbmParams), ("wl", POINTER(c_float)),
+        ("wr", POINTER(c_float)), ("erode_radius", c_float), ("msk_orig", POINTER(c_float)), ("mw", c_int32), ("mh", c_int32),
+        ("bbox", c_float * 4), ("rpc1", c_void_p), ("rpc2", c_void_p), ("ha", c_double * 9), ("hb", c_double * 9),
+        ("zone", c_int32), ("south", c_int32), ("r", c_float), ("p", c_int32), ("n", c_int32), ("pct", c_double),
+        ("clr", POINTER(c_float)), ("cw", c_int32), ("ch", c_int32), ("clr_bands", c_int32), ("hc", c_double * 9),
+        ("with_conf", c_int32),
+    ]
+
+
+MATCHER_MGM, MATCHER_SGBM = 0, 1     # S2PB_MATCHER_*
+
+
 class PlyColumn(ctypes.Structure):
     """Mirror of ``s2pb_ply_column``: byte offset of a vertex property in a PLY record and its PLY_* type."""
     _fields_ = [("offset", c_int32), ("type", c_int32)]
@@ -109,6 +126,8 @@ _SIGNATURES = {
     "s2pb_mosaic_deflate": (c_int, [c_void_p, c_int, POINTER(c_void_p), POINTER(c_int32), POINTER(c_int32), POINTER(c_int64),
                                     POINTER(c_int64), c_int, c_int, c_int, POINTER(c_uint8), c_int64, POINTER(c_int32)]),
     "s2pb_deflate_blocks": (c_int, [c_void_p, _f, c_int, c_int, c_int, POINTER(c_uint8), c_int64, POINTER(c_int32)]),
+    "s2pb_pair_tile_to_ply": (c_int, [c_void_p, POINTER(PairTile), POINTER(c_uint8), POINTER(c_int64), _f, _f, _f, _f, POINTER(c_uint8),
+                                      _f]),
     "s2pb_erode_mask": (c_int, [c_void_p, POINTER(c_uint8), POINTER(c_uint8), c_int, c_int, c_float]),
     "s2pb_census": (c_int, [c_void_p, _f, c_int, c_int, c_int, POINTER(c_uint64)]),
     "s2pb_costvolume": (c_int, [c_void_p, _f, _f, c_int, c_int, POINTER(c_int32), POINTER(c_int32), c_int, c_int, c_int, _f]),

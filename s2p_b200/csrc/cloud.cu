@@ -91,7 +91,7 @@ extern "C" int s2pb_ply_records(s2pb_ctx *ctx, const double *xyz, int64_t n, con
 }
 
 // nbands 1, 3 or 4 and a known colour type: the colours of a clr image
-static int typed_colours_ok(int nbands, int color_type)
+int typed_colours_ok(int nbands, int color_type)
 {
     if (nbands != 1 && nbands != 3 && nbands != 4) return fail(S2PB_ERR_ARG, "colors must have either 1, 3 or 4 channels (got %d)", nbands);
     if (!ply_type_bytes(color_type)) return fail(S2PB_ERR_ARG, "unknown PLY colour type %d", color_type);
@@ -121,17 +121,15 @@ extern "C" int s2pb_ply_records_typed(s2pb_ctx *ctx, const double *xyz, int64_t 
     return download_records(L, d_total, d_out, rb, records, npoints);
 }
 
-// The common tail of the steps: filter, colours, records.  Colours: d_typed (nbands device planes of cb-byte values, copied
-// as they are) or, when it is null, the host float32 planes `bands` stretched with pct.
-static int cloud_tail(s2pb_ctx *ctx, HostCall &L, double *d_xyz, int nx, int ny, float r, int p, int n, const float *bands,
-                      int nbands, double pct, const uint8_t *d_typed, int cb, const float *conf, uint8_t *records, int64_t *npoints)
+// The common tail of the steps on device inputs: filter, colours, records.  Colours: d_typed (nbands device planes of cb-byte
+// values, copied as they are) or, when it is null, the device float32 planes d_bands stretched with pct.
+int cloud_tail_device(s2pb_ctx *ctx, HostCall &L, double *d_xyz, int nx, int ny, float r, int p, int n, const float *d_bands,
+                      int nbands, double pct, const uint8_t *d_typed, int cb, const float *d_conf, uint8_t *records, int64_t *npoints)
 {
     const size_t npix = (size_t)nx * ny;
-    const int rb = record_bytes(nbands, d_typed ? cb : 1, conf != nullptr);
+    const int rb = record_bytes(nbands, d_typed ? cb : 1, d_conf != nullptr);
     int *d_work = (r != 0.f && n > 0) ? L.take<int>(npix * 12) : nullptr;
-    float *d_bands = nbands && !d_typed ? L.upload(bands, npix * nbands * 4) : nullptr;
     OrderStats *d_os = d_bands ? L.take<OrderStats>(order_stats_bytes()) : nullptr;
-    float *d_conf = conf ? L.upload(conf, npix * 4) : nullptr;
     uint8_t *d_out = L.take<uint8_t>(npix * rb);
     long long *d_total = L.take<long long>(8);
     if (int rc = L.error()) return rc;
@@ -145,8 +143,18 @@ static int cloud_tail(s2pb_ctx *ctx, HostCall &L, double *d_xyz, int nx, int ny,
     return download_records(L, d_total, d_out, rb, records, npoints);
 }
 
+// The common tail of the steps with host inputs: the float32 planes `bands` (when d_typed is null) and conf go to the device first.
+static int cloud_tail(s2pb_ctx *ctx, HostCall &L, double *d_xyz, int nx, int ny, float r, int p, int n, const float *bands,
+                      int nbands, double pct, const uint8_t *d_typed, int cb, const float *conf, uint8_t *records, int64_t *npoints)
+{
+    const size_t npix = (size_t)nx * ny;
+    float *d_bands = nbands && !d_typed ? L.upload(bands, npix * nbands * 4) : nullptr;
+    float *d_conf = conf ? L.upload(conf, npix * 4) : nullptr;
+    return cloud_tail_device(ctx, L, d_xyz, nx, ny, r, p, n, d_bands, nbands, pct, d_typed, cb, d_conf, records, npoints);
+}
+
 // the arguments of the tail, checked before the cloud is made; the cloud's own step checks the rest
-static int tail_args_ok(s2pb_ctx *ctx, int nx, int ny, const float *bands, int nbands, double pct, uint8_t *records,
+int tail_args_ok(s2pb_ctx *ctx, int nx, int ny, const float *bands, int nbands, double pct, uint8_t *records,
                         int64_t *npoints)
 {
     if (!ctx || nx < 1 || ny < 1 || !records || !npoints || (nbands && !bands)) return fail(S2PB_ERR_ARG, "bad argument");

@@ -37,22 +37,36 @@ static int cloud_zone_ok(int zone)
     return S2PB_OK;
 }
 
-int triangulated_cloud(s2pb_ctx *ctx, HostCall &L, const float *dispx, const float *dispy, const float *msk, int nx, int ny,
-                       const float *msk_orig, int w, int h, const double ha[9], const double hb[9], const s2pb_rpc *rpca,
-                       const s2pb_rpc *rpcb, const float bbox[4], int zone, int south, double **d_xyz, float **d_err)
+int triangulated_cloud_device(s2pb_ctx *ctx, HostCall &L, const float *d_dx, const float *d_dy, const float *d_m, int nx, int ny,
+                              const float *d_mo, int w, int h, const double ha[9], const double hb[9], const s2pb_rpc *rpca,
+                              const s2pb_rpc *rpcb, const float bbox[4], int zone, int south, double **d_xyz, float **d_err)
 {
-    if (!dispx || !dispy || !msk || !msk_orig || !ha || !hb || !rpca || !rpcb || !bbox || nx < 1 || ny < 1 || w < 1 || h < 1)
-        return fail(S2PB_ERR_ARG, "bad argument");
-    if (int rc = cloud_zone_ok(zone)) return rc;
-    const size_t npix = (size_t)nx * ny, nm = (size_t)w * h;
-    float *d_dx = L.upload(dispx, npix * 4), *d_dy = L.upload(dispy, npix * 4), *d_m = L.upload(msk, npix * 4);
-    float *d_mo = L.upload(msk_orig, nm * 4);
+    const size_t npix = (size_t)nx * ny;
     *d_xyz = L.take<double>(npix * 24);
     *d_err = L.take<float>(npix * 4);
     if (int rc = L.error()) return rc;
     int rc = triangulate_enqueue(ctx, L.st, d_dx, d_dy, d_m, nx, ny, d_mo, w, h, ha, hb, rpca, rpcb, bbox, *d_xyz, *d_err);
     if (rc == S2PB_OK && zone) rc = launch_utm_project(ctx, L.st, zone, south != 0, *d_xyz, *d_xyz, npix);
     return rc;
+}
+
+int triangulated_cloud_args_ok(int nx, int ny, int w, int h, const double ha[9], const double hb[9], const s2pb_rpc *rpca,
+                               const s2pb_rpc *rpcb, const float bbox[4], int zone)
+{
+    if (!ha || !hb || !rpca || !rpcb || !bbox || nx < 1 || ny < 1 || w < 1 || h < 1) return fail(S2PB_ERR_ARG, "bad argument");
+    return cloud_zone_ok(zone);
+}
+
+int triangulated_cloud(s2pb_ctx *ctx, HostCall &L, const float *dispx, const float *dispy, const float *msk, int nx, int ny,
+                       const float *msk_orig, int w, int h, const double ha[9], const double hb[9], const s2pb_rpc *rpca,
+                       const s2pb_rpc *rpcb, const float bbox[4], int zone, int south, double **d_xyz, float **d_err)
+{
+    if (!dispx || !dispy || !msk || !msk_orig) return fail(S2PB_ERR_ARG, "bad argument");
+    if (int rc = triangulated_cloud_args_ok(nx, ny, w, h, ha, hb, rpca, rpcb, bbox, zone)) return rc;
+    const size_t npix = (size_t)nx * ny, nm = (size_t)w * h;
+    float *d_dx = L.upload(dispx, npix * 4), *d_dy = L.upload(dispy, npix * 4), *d_m = L.upload(msk, npix * 4);
+    float *d_mo = L.upload(msk_orig, nm * 4);
+    return triangulated_cloud_device(ctx, L, d_dx, d_dy, d_m, nx, ny, d_mo, w, h, ha, hb, rpca, rpcb, bbox, zone, south, d_xyz, d_err);
 }
 
 // s2p.triangulation.disp_to_xyz (s2p/triangulation.py:85-162) with a UTM (or no) output CRS: disp_to_lonlatalt, then the

@@ -1,7 +1,7 @@
 // host.h -- host-side state and helpers shared by the translation units of the C ABI (not a public header).
 //
 // s2pb200.cu owns the context, the slots, the matcher and the matcher's stage entry points; warp.cu, geometry.cu, projection.cu,
-// sgbm.cu, raster.cu, cloud.cu and mosaic.cu each hold one family of entry points.  Every kernel header that defines a non-template kernel is included by one of
+// sgbm.cu, raster.cu, cloud.cu, mosaic.cu and pair_tile.cu each hold one family of entry points.  Every kernel header that defines a non-template kernel is included by one of
 // those files only, so that its kernels are compiled once; the few launchers another file needs are declared at the end.
 #pragma once
 #include "../../include/s2pb200.h"
@@ -252,6 +252,14 @@ void cc_flatten(s2pb_ctx *ctx, int n, int *lab, cudaStream_t st);
 void cc_area(s2pb_ctx *ctx, int n, const int *lab, int *area, cudaStream_t st);
 void launch_rejection_mask(s2pb_ctx *ctx, const float *disp, const float *im1, const float *im2, int w, int h, uint8_t *mask,
                            cudaStream_t st);
+// s2pb200.cu: morsi's disk erosion of a device mask (erode_radius_ok: the radii s2pb_erode_mask accepts); the matcher of
+// s2pb_mgm_weighted between device buffers on slot 0, st being that slot's stream (the deadline of p->timeout_ms counts from the
+// call, which waits for st through it: S2PB_ERR_TIMEOUT); d_wl / d_wr: device weight images or null
+int erode_radius_ok(float radius);
+void launch_erode_mask(s2pb_ctx *ctx, const uint8_t *in, uint8_t *out, int w, int h, float radius, cudaStream_t st);
+int mgm_match_device(s2pb_ctx *ctx, cudaStream_t st, const float *d_im1, const float *d_im2, int w, int h, int dmin, int dmax,
+                     const s2pb_mgm_params *p, const float *d_wl, const float *d_wr, float *d_disp, float *d_conf, uint8_t *d_mask,
+                     float *d_dispR);
 // projection.cu: (lon, lat, alt) -> UTM zone `zone` (1..60) of n device points, in place when d_in == d_out
 int launch_utm_project(s2pb_ctx *ctx, cudaStream_t st, int zone, bool south, const double *d_in, double *d_out, size_t n);
 // geometry.cu: the two clouds of a host call, each from host buffers into scratch of L after the checks of its arguments, then
@@ -262,6 +270,12 @@ int launch_utm_project(s2pb_ctx *ctx, cudaStream_t st, int zone, bool south, con
 int triangulated_cloud(s2pb_ctx *ctx, HostCall &L, const float *dispx, const float *dispy, const float *msk, int nx, int ny,
                        const float *msk_orig, int w, int h, const double ha[9], const double hb[9], const s2pb_rpc *rpca,
                        const s2pb_rpc *rpcb, const float bbox[4], int zone, int south, double **d_xyz, float **d_err);
+// triangulated_cloud_device: the same from device disparities and masks, after triangulated_cloud_args_ok checked the rest.
+int triangulated_cloud_args_ok(int nx, int ny, int w, int h, const double ha[9], const double hb[9], const s2pb_rpc *rpca,
+                               const s2pb_rpc *rpcb, const float bbox[4], int zone);
+int triangulated_cloud_device(s2pb_ctx *ctx, HostCall &L, const float *d_dx, const float *d_dy, const float *d_m, int nx, int ny,
+                              const float *d_mo, int w, int h, const double ha[9], const double hb[9], const s2pb_rpc *rpca,
+                              const s2pb_rpc *rpcb, const float bbox[4], int zone, int south, double **d_xyz, float **d_err);
 int localised_cloud(s2pb_ctx *ctx, HostCall &L, const double *heights, int w, int h, const s2pb_rpc *rpc, double off_x,
                     double off_y, int zone, int south, double **d_xyz);
 int remove_isolated_enqueue(s2pb_ctx *ctx, cudaStream_t st, double *d_xyz, int nx, int ny, float r, int p, int n, int q, int *d_work);
@@ -269,6 +283,16 @@ int remove_isolated_enqueue(s2pb_ctx *ctx, cudaStream_t st, double *d_xyz, int n
 // holds order_stats_bytes(); rule kOrdQauto (qauto's thresholds) or kOrdLinear (numpy's 'linear' quantiles q0 and q1)
 size_t order_stats_bytes();
 int launch_order_stats(s2pb_ctx *ctx, cudaStream_t st, const float *d_x, int n, int rule, double q0, double q1, OrderStats *d_os);
+// the `sgbm` run and its rejection mask on device buffers of L (see s2pb_sgbm for what it refuses)
+int sgbm_enqueue(s2pb_ctx *ctx, HostCall &L, const float *d_im1, const float *d_im2, int w, int h, int dmin, int dmax,
+                 const s2pb_sgbm_params *p, float *d_disp, uint8_t *d_mask);
+// cloud.cu: the checks of the cloud steps' tail arguments (colours, pct, records) and of a clr image's bands and type, and the
+// tail itself on device inputs -- 3D filter, colours (d_typed planes of cb-byte values copied, else the float32 planes d_bands
+// stretched with pct), confidence (nullable) -- down to the records and their number in host memory, synchronised
+int tail_args_ok(s2pb_ctx *ctx, int nx, int ny, const float *bands, int nbands, double pct, uint8_t *records, int64_t *npoints);
+int typed_colours_ok(int nbands, int color_type);
+int cloud_tail_device(s2pb_ctx *ctx, HostCall &L, double *d_xyz, int nx, int ny, float r, int p, int n, const float *d_bands,
+                      int nbands, double pct, const uint8_t *d_typed, int cb, const float *d_conf, uint8_t *records, int64_t *npoints);
 // warp.cu
 void invert_homography(const double i[9], double o[9]);
 int warp_host_to_device(s2pb_ctx *ctx, ScratchLease &L, cudaStream_t st, const float *src, int sw, int sh, const double H[9],

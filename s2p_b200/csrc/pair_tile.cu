@@ -1,0 +1,93 @@
+// pair_tile.cu -- a two-view tile from its source crops to the records of cloud.ply in one call: rectify_pair's two warps, the
+// matcher and its rejection mask, masking.erosion and disparity_to_ply chained on one stream, the intermediates staying on the
+// device (s2p/__init__.py:102-318).
+#include "host.h"
+
+// the eroded 0/1 mask as the float32 image disparity_to_ply hands to the triangulation (a PNG read back as uint8, then float32)
+__global__ void mask_to_float_kernel(const uint8_t *__restrict__ in, float *__restrict__ out, size_t n)
+{
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) out[i] = (float)in[i];
+}
+
+// what the stages would refuse that can be seen before the first launch
+static int pair_tile_args_ok(s2pb_ctx *ctx, const s2pb_pair_tile *t, uint8_t *records, int64_t *npoints, const float *conf,
+                             const float *disp_right)
+{
+    if (!ctx || !t || !t->src1 || !t->src2 || !t->msk_orig || t->sw1 < 1 || t->sh1 < 1 || t->sw2 < 1 || t->sh2 < 1 || t->w < 1 ||
+        t->h < 1 || t->mw < 1 || t->mh < 1)
+        return fail(S2PB_ERR_ARG, "bad argument");
+    if (t->matcher != S2PB_MATCHER_MGM && t->matcher != S2PB_MATCHER_SGBM) return fail(S2PB_ERR_ARG, "unknown matcher %d", t->matcher);
+    if (t->matcher == S2PB_MATCHER_SGBM && (conf || disp_right || t->with_conf || t->wl || t->wr))
+        return fail(S2PB_ERR_ARG, "sgbm has no confidence, right disparity or weight images");
+    if ((t->wl == nullptr) != (t->wr == nullptr)) return fail(S2PB_ERR_ARG, "the weight images come in pairs (-wl and -wr)");
+    if (t->erode_radius != 0.f) {
+        if (int rc = erode_radius_ok(t->erode_radius)) return rc;
+    }
+    if (int rc = triangulated_cloud_args_ok(t->w, t->h, t->mw, t->mh, t->ha, t->hb, t->rpc1, t->rpc2, t->bbox, t->zone)) return rc;
+    if (t->clr) {
+        if (int rc = tail_args_ok(ctx, t->w, t->h, t->clr, t->clr_bands, 0.0, records, npoints)) return rc;
+        if (int rc = typed_colours_ok(t->clr_bands, S2PB_PLY_F32)) return rc;
+        if (t->cw < 1 || t->ch < 1) return fail(S2PB_ERR_ARG, "bad argument");
+        return S2PB_OK;
+    }
+    return tail_args_ok(ctx, t->w, t->h, nullptr, 0, t->pct, records, npoints);      // colours: the call's own rectified reference
+}
+
+extern "C" int s2pb_pair_tile_to_ply(s2pb_ctx *ctx, const s2pb_pair_tile *t, uint8_t *records, int64_t *npoints, float *rect1,
+                                     float *rect2, float *disp, float *conf, uint8_t *mask, float *disp_right)
+{
+    if (int rc = pair_tile_args_ok(ctx, t, records, npoints, conf, disp_right)) return rc;
+    *npoints = 0;
+    const int w = t->w, h = t->h;
+    const size_t npix = (size_t)w * h;
+    const bool mgm = t->matcher == S2PB_MATCHER_MGM, erode = t->erode_radius != 0.f;
+    HostCall L(ctx, "the pair tile");
+    float *d_r1 = L.take<float>(npix * 4), *d_r2 = L.take<float>(npix * 4), *d_disp = L.take<float>(npix * 4);
+    float *d_conf = mgm ? L.take<float>(npix * 4) : nullptr, *d_dispR = disp_right ? L.take<float>(npix * 4) : nullptr;
+    uint8_t *d_mask = L.take<uint8_t>(npix), *d_eroded = erode ? L.take<uint8_t>(npix) : d_mask;
+    float *d_msk = L.take<float>(npix * 4), *d_dy = L.take<float>(npix * 4);
+    const float *d_wl = t->wl ? L.upload(t->wl, npix * 4) : nullptr, *d_wr = t->wr ? L.upload(t->wr, npix * 4) : nullptr;
+    const float *d_mo = L.upload(t->msk_orig, (size_t)t->mw * t->mh * 4);
+    if (int rc = L.error()) return rc;
+
+    // rectification_pair: both warps straight into the matcher's inputs
+    if (int rc = warp_host_to_device(ctx, L, L.st, t->src1, t->sw1, t->sh1, t->H1, d_r1, w, h)) return rc;
+    if (int rc = warp_host_to_device(ctx, L, L.st, t->src2, t->sw2, t->sh2, t->H2, d_r2, w, h)) return rc;
+    if (rect1) L.download(rect1, d_r1, npix * 4);
+    if (rect2) L.download(rect2, d_r2, npix * 4);
+
+    // stereo_matching: the matcher and its rejection mask, then the erosion of the mask
+    if (mgm) {
+        if (int rc = mgm_match_device(ctx, L.st, d_r1, d_r2, w, h, t->dmin, t->dmax, &t->mgm, d_wl, d_wr, d_disp, d_conf, d_mask,
+                                      d_dispR))
+            return rc;
+    } else if (int rc = sgbm_enqueue(ctx, L, d_r1, d_r2, w, h, t->dmin, t->dmax, &t->sgbm, d_disp, d_mask)) {
+        return rc;
+    }
+    if (erode) launch_erode_mask(ctx, d_mask, d_eroded, w, h, t->erode_radius, L.st);
+    launch(ctx, mask_to_float_kernel, (unsigned)((npix + 255) / 256), 256, 0, L.st, d_eroded, d_msk, npix);
+    CK(cudaGetLastError());
+    CK(cudaMemsetAsync(d_dy, 0, npix * 4, L.st));
+    if (disp) L.download(disp, d_disp, npix * 4);
+    if (conf) L.download(conf, d_conf, npix * 4);
+    if (mask) L.download(mask, d_eroded, npix);
+    if (disp_right) L.download(disp_right, d_dispR, npix * 4);
+
+    // disparity_to_ply: the cloud, its colours and its records
+    double *d_xyz = nullptr;
+    float *d_err = nullptr;
+    if (int rc = triangulated_cloud_device(ctx, L, d_disp, d_dy, d_msk, w, h, d_mo, t->mw, t->mh, t->ha, t->hb, t->rpc1, t->rpc2,
+                                           t->bbox, t->zone, t->south, &d_xyz, &d_err))
+        return rc;
+    const float *d_cc = t->with_conf ? d_conf : nullptr;
+    if (!t->clr) return cloud_tail_device(ctx, L, d_xyz, w, h, t->r, t->p, t->n, d_r1, 1, t->pct, nullptr, 1, d_cc, records, npoints);
+    float *d_col = L.take<float>(npix * t->clr_bands * 4);
+    if (int rc = L.error()) return rc;
+    for (int b = 0; b < t->clr_bands; b++)
+        if (int rc = warp_host_to_device(ctx, L, L.st, t->clr + (size_t)b * t->cw * t->ch, t->cw, t->ch, t->hc, d_col + (size_t)b * npix,
+                                         w, h))
+            return rc;
+    return cloud_tail_device(ctx, L, d_xyz, w, h, t->r, t->p, t->n, nullptr, t->clr_bands, 0.0, (const uint8_t *)d_col, 4, d_cc,
+                             records, npoints);
+}

@@ -1665,16 +1665,27 @@ extern "C" int s2pb_remove_small_cc(s2pb_ctx *ctx, const float *in, float *out, 
     return L.finish();
 }
 
+int erode_radius_ok(float radius)
+{
+    if (!(radius > 1.f) || radius > 64.f) return fail(S2PB_ERR_ARG, "disk radius must be in (1, 64]");   // build_disk, c/morsi.c:282
+    return S2PB_OK;
+}
+
+void launch_erode_mask(s2pb_ctx *ctx, const uint8_t *in, uint8_t *out, int w, int h, float radius, cudaStream_t st)
+{
+    dim3 b2(32, 8);
+    launch(ctx, erode_mask_kernel, grid2d(w, h, b2), b2, 0, st, in, out, w, h, radius);
+}
+
 extern "C" int s2pb_erode_mask(s2pb_ctx *ctx, const uint8_t *in, uint8_t *out, int w, int h, float radius)
 {
     if (!ctx || !in || !out || w < 1 || h < 1) return fail(S2PB_ERR_ARG, "bad argument");
-    if (!(radius > 1.f) || radius > 64.f) return fail(S2PB_ERR_ARG, "disk radius must be in (1, 64]");   // build_disk, c/morsi.c:282
+    if (int rc = erode_radius_ok(radius)) return rc;
     size_t npix = (size_t)w * h;
     HostCall L(ctx, "the mask erosion");
     uint8_t *a = L.upload(in, npix), *b = L.take<uint8_t>(npix);
     if (int rc = L.error()) return rc;
-    dim3 b2(32, 8);
-    launch(ctx, erode_mask_kernel, grid2d(w, h, b2), b2, 0, L.st, a, b, w, h, radius);
+    launch_erode_mask(ctx, a, b, w, h, radius, L.st);
     CK(cudaGetLastError());
     L.download(out, b, npix);
     return L.finish();
@@ -1735,5 +1746,20 @@ extern "C" int s2pb_rectify_match(s2pb_ctx *ctx, const float *src1, int sw1, int
     CK(cudaMemcpyAsync(conf, s.d_conf, npix * 4, cudaMemcpyDeviceToHost, st));
     if (mask) CK(cudaMemcpyAsync(mask, s.d_mask, npix, cudaMemcpyDeviceToHost, st));
     if (disp_right) CK(cudaMemcpyAsync(disp_right, s.d_dispR, npix * 4, cudaMemcpyDeviceToHost, st));
+    return sync_or_timeout(ctx, st);
+}
+
+// The matcher of s2pb_mgm_weighted between device buffers on slot 0 (st is that slot's stream, as HostCall's): the deadline counts
+// from here, and the call waits for the stream through the timeout.
+int mgm_match_device(s2pb_ctx *ctx, cudaStream_t st, const float *d_im1, const float *d_im2, int w, int h, int dmin, int dmax,
+                     const s2pb_mgm_params *p, const float *d_wl, const float *d_wr, float *d_disp, float *d_conf, uint8_t *d_mask,
+                     float *d_dispR)
+{
+    if (int rc = check_params(p, w, h, dmin, dmax)) return rc;
+    set_deadline(ctx, p->timeout_ms);
+    MgmExtra x;
+    x.wl = d_wl; x.wr = d_wr;
+    int rc = mgm_enqueue(ctx, ctx->slots[0], d_im1, d_im2, w, h, dmin, dmax, p, d_disp, d_conf, d_mask, d_dispR, st, -1, &x);
+    if (rc != S2PB_OK) return rc;
     return sync_or_timeout(ctx, st);
 }

@@ -27,9 +27,12 @@ int launch_order_stats(s2pb_ctx *ctx, cudaStream_t st, const float *d_x, int n, 
 
 // The whole `sgbm im1 im2 disp cost dmin dmax win P1 P2 lr` run followed by create_rejection_mask, enqueued on the call's
 // stream.  d_im1 / d_im2 / d_disp: w*h float32, d_mask: w*h uint8 or null, all from L, which is checked before the first launch.
-static int sgbm_enqueue(s2pb_ctx *ctx, HostCall &L, const float *d_im1, const float *d_im2, int w, int h, int dmin, int dmax,
-                        const s2pb_sgbm_params *p, float *d_disp, uint8_t *d_mask)
+// S2PB_ERR_ARG / S2PB_ERR_UNSUPPORTED for what s2pb_sgbm refuses, before anything is enqueued.
+int sgbm_enqueue(s2pb_ctx *ctx, HostCall &L, const float *d_im1, const float *d_im2, int w, int h, int dmin, int dmax,
+                 const s2pb_sgbm_params *p, float *d_disp, uint8_t *d_mask)
 {
+    if (dmin >= dmax) return fail(S2PB_ERR_ARG, "mindisp(%d) > maxdisp(%d)", -dmax, -dmin);     // sgbm.cpp:174-177
+    if (p->win < 1 || p->win % 2 == 0) return fail(S2PB_ERR_ARG, "SADWindowSize must be odd and positive (got %d)", p->win);
     const cudaStream_t st = L.st;
     // sgbm.cpp:166-192: OpenCV's convention is the opposite of s2p's; the label count is rounded up to a multiple of 16
     const int mindisp = -dmax, maxdisp = -dmin;
@@ -124,8 +127,6 @@ extern "C" int s2pb_sgbm(s2pb_ctx *ctx, const float *im1, const float *im2, int 
                          const s2pb_sgbm_params *p, float *disp, uint8_t *mask)
 {
     if (!ctx || !im1 || !im2 || !p || !disp || w < 1 || h < 1) return fail(S2PB_ERR_ARG, "bad argument");
-    if (dmin >= dmax) return fail(S2PB_ERR_ARG, "mindisp(%d) > maxdisp(%d)", -dmax, -dmin);     // sgbm.cpp:174-177
-    if (p->win < 1 || p->win % 2 == 0) return fail(S2PB_ERR_ARG, "SADWindowSize must be odd and positive (got %d)", p->win);
     const size_t npix = (size_t)w * h;
     HostCall L(ctx, "sgbm");
     float *d_im1 = L.upload(im1, npix * 4), *d_im2 = L.upload(im2, npix * 4), *d_disp = L.take<float>(npix * 4);

@@ -519,6 +519,64 @@ class Engine:
             _fp(conf) if conf is not None else None, out, cnt)
         return self._records(call, h * w, nb, conf is not None, np.float32)
 
+    PAIR_TILE_OUTPUTS = ("rect1", "rect2", "disp", "conf", "mask", "disp_right")
+
+    def pair_tile_to_ply(self, src1, H1, src2, H2, w, h, dmin, dmax, mask_orig, H_ref, H_sec, rpc1, rpc2, img_bbx, zone=0, south=False,
+                         params=None, weights=None, erode_radius=0, r=0.0, p=0, n=0, stretch_p=1, clr=None, hc=None,
+                         confidence=False, want=()):
+        """A two-view tile from its source crops to its cloud's records in one device call (s2pb_pair_tile_to_ply): homography
+        of src1 by H1 and of src2 by H2 onto w x h, the matcher (``params``: MgmParams, or SgbmParams for sgbm; ``weights`` =
+        (wl, wr) for mgm_multi_lsd) on [dmin, dmax], the erosion of its mask (erode_radius 0: none), then disp_to_ply on the
+        disparity and the eroded mask (H_ref, H_sec: the triangulation's homographies, H_sec with the pointing correction)
+        coloured by the stretch of the rectified reference, or by the clr crop (nbands, ch, cw) warped by hc, with the
+        confidence column when ``confidence``.  -> (records, dict of the intermediates named in ``want``, a subset of
+        PAIR_TILE_OUTPUTS)."""
+        src1, src2, mo = _f32(src1), _f32(src2), _f32(mask_orig)
+        if src1.ndim != 2 or src2.ndim != 2 or mo.ndim != 2:
+            raise ValueError("src1, src2 and mask_orig must be 2-D arrays")
+        unknown = set(want) - set(self.PAIR_TILE_OUTPUTS)
+        if unknown:
+            raise ValueError("unknown outputs %s (one of %s)" % (sorted(unknown), ", ".join(self.PAIR_TILE_OUTPUTS)))
+        w, h = int(w), int(h)
+        t = _lib.PairTile()
+        t.src1, t.sw1, t.sh1, t.src2, t.sw2, t.sh2 = _fp(src1), src1.shape[1], src1.shape[0], _fp(src2), src2.shape[1], src2.shape[0]
+        t.w, t.h, t.dmin, t.dmax = w, h, int(dmin), int(dmax)
+        params = params if params is not None else default_params("mgm")
+        if isinstance(params, SgbmParams):
+            t.matcher, t.sgbm = _lib.MATCHER_SGBM, params
+        else:
+            t.matcher, t.mgm = _lib.MATCHER_MGM, params
+        if weights is not None:
+            wl, wr = _f32(weights[0]), _f32(weights[1])
+            if wl.shape != (h, w) or wr.shape != (h, w):
+                raise ValueError("the weight images must have the shape of the rectified images")
+            t.wl, t.wr = _fp(wl), _fp(wr)
+        t.erode_radius = float(erode_radius)
+        t.msk_orig, t.mw, t.mh = _fp(mo), mo.shape[1], mo.shape[0]
+        t.bbox[:] = [float(v) for v in np.asarray(img_bbx, np.float32).reshape(4)]
+        t.rpc1, t.rpc2 = _rpc(rpc1), _rpc(rpc2)
+        for name, H in (("H1", H1), ("H2", H2), ("ha", H_ref), ("hb", H_sec)):
+            getattr(t, name)[:] = [float(v) for v in np.asarray(H, np.float64).reshape(9)]
+        t.zone, t.south = int(zone), int(bool(south))
+        t.r, t.p, t.n, t.pct = float(r), operator.index(p), operator.index(n), float(stretch_p)
+        nb, cdt = 1, np.uint8
+        if clr is not None:
+            c = _f32(clr)
+            c = c[None] if c.ndim == 2 else c
+            if c.ndim != 3:
+                raise ValueError("expecting clr planes of shape (nbands, ch, cw), got %s" % (c.shape,))
+            nb, cdt = c.shape[0], np.float32
+            t.clr, t.clr_bands, t.ch, t.cw = _fp(c), c.shape[0], c.shape[1], c.shape[2]
+            t.hc[:] = [float(v) for v in np.asarray(hc, np.float64).reshape(9)]
+        t.with_conf = int(bool(confidence))
+        out = {k: np.empty((h, w), np.uint8 if k == "mask" else np.float32) for k in self.PAIR_TILE_OUTPUTS if k in want}
+        ptr = lambda k, conv: conv(out[k]) if k in out else None
+        call = lambda rec, cnt: self._L.s2pb_pair_tile_to_ply(
+            self._ctx, ctypes.byref(t), rec, cnt, ptr("rect1", _fp), ptr("rect2", _fp), ptr("disp", _fp), ptr("conf", _fp),
+            ptr("mask", _u8), ptr("disp_right", _fp))
+        records = self._records(call, h * w, nb, bool(confidence), cdt)
+        return records, out
+
     def height_map_to_ply_clr(self, heights, rpc, off_x, off_y, zone=0, south=False, r=0.0, p=0, n=0, colors=None):
         """height_map_to_ply with the colours of a clr image: the planes (nbands, h, w) keep their dtype (one of the eight PLY
         types) in the records -> structured array of ply_dtype(nbands, False, colors.dtype)."""

@@ -8,13 +8,18 @@ from one to the other without changing s2p/__init__.py; the drop-ins of `common.
 file hand-off.  A pipeline that calls both steps from the same worker can use `rectify_and_match` instead: same files out
 (rectified pair, disparity, confidence, mask), bit-identical to the two-step path, one TIFF decode and two host<->device
 round trips fewer per tile.  INTEGRATION.md shows the ten lines of s2p/__init__.py this replaces.
+
+With two images, `pair_tile` goes further: steps 3, 4 and 5 of a tile (rectification_pair, stereo_matching, disparity_to_ply)
+in one device call from the source images to cloud.ply, the intermediates written only where s2p keeps them (INTEGRATION.md
+section 2b).
 """
+import os
 import subprocess
 
 import numpy as np
 
-from . import _lib, rasterio_compat as rio
-from .block_matching import _NATIVE, confidence_path, disparity_bounds, matcher_params
+from . import _lib, cloud, common, projection, rasterio_compat as rio, triangulation
+from .block_matching import _NATIVE, SGBM_ARGS, confidence_path, disparity_bounds, matcher_params
 from .common import needed_roi
 from .engine import S2pbError, get_engine
 
@@ -57,3 +62,128 @@ def rectify_and_match(out1, out2, disp, mask, im1, im2, H1, H2, w, h, algo, disp
     rio.write_float_tiff(disp, out["disp"])
     rio.write_float_tiff(confidence_path(disp, algo), out["conf"])
     rio.write_mask_png(mask, out["mask"])
+
+
+# ------------------------------------------------------------------ steps 3 to 5 of a two-view tile in one device call
+
+SERVED = ("mgm", "mgm_multi", "mgm_multi_lsd", "sgbm")
+CONFIDENCE_COLUMN = ("mgm", "mgm_multi")    # the algos whose confidence file disparity_to_ply finds at `extra`
+
+
+def fall_through_reason(cfg):
+    """Why ``pair_tile`` runs the three steps instead of the device call for this configuration, or None."""
+    if len(cfg['images']) != 2:
+        return "not a two-view run"
+    if cfg['matching_algorithm'] not in SERVED:
+        return "algo %r is not served" % cfg['matching_algorithm']
+    if projection.utm_target(cfg['out_crs']) is None:
+        return "output CRS %r is not a UTM zone of WGS84" % cfg['out_crs']
+    if not cloud.numpy_stretch_is_float64():
+        return "NumPy < 2 stretches the colours in float32"
+    clr = cfg['images'][0]['clr']
+    if clr and not cloud._clr_bands_ok(clr):
+        return "the clr image does not open with 1, 3 or 4 bands"
+    return None
+
+
+def erosion_radius(radius):
+    """masking.erosion's radius as the device call takes it: nothing happens below 2 (s2p/masking.py:87-97)"""
+    return int(radius) if radius >= 2 else 0
+
+
+def _stepwise(s2p, tile):
+    s2p.rectification_pair(tile, 1)
+    s2p.stereo_matching(tile, 1)
+    s2p.disparity_to_ply(tile)
+
+
+def pair_tile(tile, engine=None):
+    """``rectification_pair(tile, 1)``, ``stereo_matching(tile, 1)`` and ``disparity_to_ply(tile)`` of a two-view run
+    (s2p/__init__.py:102-318) with one device call between the rectification's host algebra and cloud.ply.
+
+    ``rectification_pair`` itself runs -- pointing, SIFT matches and those of the neighbours, ``rectify_pair``'s algebra, the text
+    files it writes and removes -- with its two ``common.image_apply_homography`` calls intercepted; then ``s2pb_pair_tile_to_ply``
+    warps, matches, erodes and triangulates, and only the files the three steps leave are written, byte for byte: with
+    ``clean_intermediate`` none of the rasters that ``stereo_matching`` and ``disparity_to_ply`` would delete.  The three steps
+    run instead whenever ``fall_through_reason`` gives one, and when the device refuses the tile as unsupported.  Raises
+    MaxDisparityRangeError before any device work and subprocess.TimeoutExpired as ``compute_disparity_map`` does."""
+    import s2p
+    import s2p.common as s2p_common
+    from s2p.config import cfg
+    if fall_through_reason(cfg):
+        return _stepwise(s2p, tile)
+
+    calls = []
+    saved = s2p_common.image_apply_homography
+    s2p_common.image_apply_homography = lambda out, im, H, ww, hh: calls.append((out, im, H, ww, hh))
+    try:
+        s2p.rectification_pair(tile, 1)
+    finally:
+        s2p_common.image_apply_homography = saved
+    if len(calls) != 2 or calls[0][3:] != calls[1][3:]:
+        raise RuntimeError("rectify_pair did not warp its two images the way s2p/rectification.py:379-380 does")
+    (rect1, im1, H1, w, h), (rect2, im2, H2, _, _) = calls
+
+    out_dir = tile['dir']
+    pair_dir = os.path.join(out_dir, 'pair_1')
+    algo = cfg['matching_algorithm']
+    clean = cfg['clean_intermediate']
+    disp_min, disp_max = np.loadtxt(os.path.join(pair_dir, 'disp_min_max.txt'))
+    disp_min, disp_max = disparity_bounds(w, disp_min, disp_max, cfg['max_disp_range'])
+    src1, H1c = _crop(im1, H1, w, h)
+    src2, H2c = _crop(im2, H2, w, h)
+
+    eng = engine or get_engine()
+    if algo == "sgbm":
+        params, weights = eng.sgbm_params(**SGBM_ARGS), None
+    else:
+        params = matcher_params(algo, cfg['mgm_timeout'])
+        weights = (np.ones((h, w), np.float32),) * 2 if algo == "mgm_multi_lsd" else None     # block_matching.lsd_weight_map
+    x, y, tw, th = tile['coordinates']
+    H_ref = np.loadtxt(os.path.join(pair_dir, 'H_ref.txt'))
+    H_sec = np.dot(np.loadtxt(os.path.join(pair_dir, 'H_sec.txt')),
+                   np.linalg.inv(np.loadtxt(os.path.join(cfg['out_dir'], 'global_pointing_pair_1.txt'))))
+    mask_orig = os.path.join(out_dir, 'mask.png')
+    r, p, n = cloud._filter_args(cfg)
+    clr, hc = None, None
+    ply_file = os.path.join(out_dir, 'cloud.ply')
+    if cfg['images'][0]['clr']:
+        im = cfg['images'][0]['clr']
+        clr, hc = common.homography_crop(im, H_ref, w, h, common.homography_cmd("<colours of %s>" % ply_file, im, H_ref, w, h))
+    conf_file = confidence_path(os.path.join(pair_dir, 'rectified_disp.tif'), algo) if algo != "sgbm" else None
+    want = () if clean else ("rect1", "rect2", "disp", "mask")
+    if conf_file:
+        want += ("conf",)
+
+    cmd = ["s2pb200:rectify+%s+ply" % algo, im1, im2, ply_file]
+    print("\nRUN: %s" % " ".join(cmd))
+    try:
+        records, out = eng.pair_tile_to_ply(
+            src1, H1c, src2, H2c, w, h, disp_min, disp_max, rio.read_stored(mask_orig).squeeze(), H_ref, H_sec,
+            triangulation._rpc_struct(cfg['images'][0]['rpcm']), triangulation._rpc_struct(cfg['images'][1]['rpcm']),
+            (x, x + tw, y, y + th), *projection.utm_target(cfg['out_crs']), params=params, weights=weights,
+            erode_radius=erosion_radius(cfg['msk_erosion']), r=r, p=p, n=n, clr=clr, hc=hc,
+            confidence=algo in CONFIDENCE_COLUMN, want=want)
+    except S2pbError as e:
+        if e.code == _lib.ERR_TIMEOUT:
+            raise subprocess.TimeoutExpired(cmd, cfg['mgm_timeout']) from e
+        if e.code == _lib.ERR_UNSUPPORTED:      # the steps' own handling of the tile (their error or the original tool)
+            for out_file, im, H, ww, hh in calls:
+                saved(out_file, im, H, ww, hh)
+            s2p.stereo_matching(tile, 1)
+            return s2p.disparity_to_ply(tile)
+        raise subprocess.CalledProcessError(-e.code, cmd, output=str(e)) from e
+
+    if not clean:
+        rio.write_float_tiff(rect1, out["rect1"])
+        rio.write_float_tiff(rect2, out["rect2"])
+        rio.write_float_tiff(os.path.join(pair_dir, 'rectified_disp.tif'), out["disp"])
+        rio.write_mask_png(os.path.join(pair_dir, 'rectified_mask.png'), out["mask"])
+    if conf_file:
+        rio.write_float_tiff(conf_file, out["conf"])
+    cloud.write_ply(ply_file, records, cloud._comments(cfg))
+    if clean:
+        for f in ('disp_min_max.txt', 'H_ref.txt', 'H_sec.txt'):
+            cloud._remove(os.path.join(pair_dir, f))
+        cloud._remove(mask_orig)
+
