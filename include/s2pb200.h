@@ -39,6 +39,10 @@
  *                        (s2p/block_matching.py:116-134)
  *   s2pb_pair_tile_to_ply() rectification_pair, stereo_matching and disparity_to_ply of a two-view tile (s2p/__init__.py:102-318)
  *                        in one call, from the source crops to the records of cloud.ply
+ *   s2pb_pair_tile_to_height_map() rectification_pair, stereo_matching and disparity_to_height of one pair of a tri-stereo
+ *                        tile (s2p/__init__.py:102-239) in one call, from the source crops to the pair's height map
+ *   s2pb_heights_tile_to_ply() heights_to_ply of a tri-stereo tile, its heights_fusion included (s2p/__init__.py:355-429), in
+ *                        one call, from the pairs' height maps to the records of cloud.ply
  *
  * Conventions: all images are single-band, row-major, C-contiguous float32,
  * NaN = no data.  Disparity d at ref pixel (x,y) means the match is at
@@ -419,7 +423,7 @@ int s2pb_erode_mask(s2pb_ctx *ctx, const uint8_t *in, uint8_t *out, int w, int h
 
 /* ---- a two-view tile from its source images to its point cloud (s2p.main steps 3 to 5 with two images) ---------- */
 enum { S2PB_MATCHER_MGM = 0, S2PB_MATCHER_SGBM = 1 };
-/* The inputs of s2pb_pair_tile_to_ply, stage by stage.  Host pointers. */
+/* The inputs of s2pb_pair_tile_to_ply and s2pb_pair_tile_to_height_map, stage by stage.  Host pointers. */
 typedef struct s2pb_pair_tile {
     /* rectify_pair's two warps: the crops of the two images and their rectifying homographies with the crops' origins folded in */
     const float *src1, *src2;
@@ -459,6 +463,56 @@ typedef struct s2pb_pair_tile {
  * S2PB_ERR_ARG also for conf, disp_right or with_conf with sgbm.  Synchronous. */
 int s2pb_pair_tile_to_ply(s2pb_ctx *ctx, const s2pb_pair_tile *t, uint8_t *records, int64_t *npoints, float *rect1, float *rect2,
                           float *disp, float *conf, uint8_t *mask, float *disp_right);
+
+/* ---- a tri-stereo tile from its source images to its point cloud (s2p.main steps 3 to 5 with three or more images) ---- */
+/* One pair i of the tile: s2pb_homography x 2 -> s2pb_mgm_weighted or s2pb_sgbm -> s2pb_erode_mask when erode_radius > 0 ->
+ * s2pb_height_map on the disparity and the eroded mask as float32, in one call, with the intermediates on the device.  It
+ * reads the warp fields of t (src1 to h), the matcher fields (dmin to wr), erode_radius, msk_orig, mw, mh, rpc1, rpc2, and
+ * ha = H_ref as H_ref.txt holds it and hb = H_sec . A^-1 (the pointing correction applied), s2pb_height_map's H1 and H2.  It
+ * ignores the cloud-only fields: bbox, zone, south, r, p, n, pct, clr, cw, ch, clr_bands, hc and with_conf.  (x, y, w, h): the
+ * tile in the reference image; heights: w*h float64, the pair's height map.  The heights, their NaN set and every
+ * intermediate are those of that sequence, bit for bit.  Nullable host copies of the intermediates (t->w * t->h each): rect1,
+ * rect2, disp, conf (MGM), mask (0/1, after the erosion), disp_right (MGM).  Errors as the calls of the sequence: S2PB_ERR_TIMEOUT
+ * from the MGM matcher, S2PB_ERR_UNSUPPORTED for a rectified size below 2 x 2, and S2PB_ERR_ARG also for conf or disp_right
+ * with sgbm.  Synchronous. */
+int s2pb_pair_tile_to_height_map(s2pb_ctx *ctx, const s2pb_pair_tile *t, int x, int y, int w, int h, double *heights, float *rect1,
+                                 float *rect2, float *disp, float *conf, uint8_t *mask, float *disp_right);
+#define S2PB_MAX_FUSION 16
+/* The inputs of s2pb_heights_tile_to_ply, stage by stage.  Host pointers. */
+typedef struct s2pb_heights_tile {
+    /* heights_fusion: n_maps (1..S2PB_MAX_FUSION) w*h height maps of the pairs, all of map_type (S2PB_PLY_F32 or S2PB_PLY_F64) as
+     * they are stored, their offsets (the global mean heights), cargarse_basura, and merge_n's operator (the op codes of
+     * s2pb_merge_n, S2PB_FUSE_SUB_F32 included) and threshold */
+    int32_t n_maps, w, h, map_type;
+    const void *maps[S2PB_MAX_FUSION];
+    double offsets[S2PB_MAX_FUSION];
+    int32_t cargarse_basura, op;
+    double threshold;
+    /* height_map_to_xyz: the reference image's camera, the tile's origin in that image, the output UTM zone (0: lon, lat, alt) */
+    const s2pb_rpc *rpc;
+    double off_x, off_y;
+    int32_t zone, south;
+    /* the filter of filter_xyz (off when r == 0 or n <= 0) */
+    float r;
+    int32_t p, n;
+    /* the colours: nbands (0, 1, 3 or 4) planes of w*h values; stretch != 0: float32 stretched with pct as
+     * s2pb_height_map_to_ply stretches them; else values of PLY type color_type copied as s2pb_height_map_to_ply_clr copies them */
+    const void *colors;
+    int32_t nbands, color_type, stretch;
+    double pct;
+} s2pb_heights_tile;
+/* heights_fusion then heights_to_ply's cloud (s2p/__init__.py:355-429) in one call: with cargarse_basura, each map rounded to
+ * float32 (as the reference's tools read a float64 map) and cleaned as s2pb_cargarse_basura cleans it, then merged by
+ * s2pb_merge_n's rule; without it the maps are merged in their stored type, a float64 map subtracted from its offset in float64
+ * without a rounding first (as s2p/fusion.py:49 does with the float64 array rasterio reads).  The merged float32 map, converted
+ * to float64 exactly, goes through s2pb_height_map_to_ply (stretch) or s2pb_height_map_to_ply_clr (typed colours).  records: w*h
+ * records of the record size of the colours; *npoints gets the number written.  Nullable host copies of the intermediates:
+ * cleaned (null, or n_maps nullable pointers to w*h float32: each cleaned map, with cargarse_basura only) and merged (w*h
+ * float32).  Errors as the calls of the sequence: S2PB_ERR_UNSUPPORTED for more than S2PB_MAX_FUSION maps, or a map below
+ * 2 x 2 with cargarse_basura; S2PB_ERR_ARG also for a map_type other than float32 / float64, or cleaned without
+ * cargarse_basura.  Synchronous. */
+int s2pb_heights_tile_to_ply(s2pb_ctx *ctx, const s2pb_heights_tile *t, uint8_t *records, int64_t *npoints, float *const *cleaned,
+                             float *merged);
 
 /* ---- stage-level entry points (host buffers; used by the parity tests) ----- */
 /* census_tools.cc:127-153.  codes: w*h uint64, first neighbour in the top bit. */

@@ -32,7 +32,7 @@ class SgbmParams(ctypes.Structure):
 
 
 class PairTile(ctypes.Structure):
-    """Mirror of ``s2pb_pair_tile``: the inputs of s2pb_pair_tile_to_ply."""
+    """Mirror of ``s2pb_pair_tile``: the inputs of s2pb_pair_tile_to_ply and s2pb_pair_tile_to_height_map."""
     _fields_ = [
         ("src1", POINTER(c_float)), ("src2", POINTER(c_float)), ("sw1", c_int32), ("sh1", c_int32), ("sw2", c_int32),
         ("sh2", c_int32), ("H1", c_double * 9), ("H2", c_double * 9), ("w", c_int32), ("h", c_int32), ("dmin", c_int32),
@@ -46,6 +46,18 @@ class PairTile(ctypes.Structure):
 
 
 MATCHER_MGM, MATCHER_SGBM = 0, 1     # S2PB_MATCHER_*
+MAX_FUSION = 16                      # S2PB_MAX_FUSION
+
+
+class HeightsTile(ctypes.Structure):
+    """Mirror of ``s2pb_heights_tile``: the inputs of s2pb_heights_tile_to_ply."""
+    _fields_ = [
+        ("n_maps", c_int32), ("w", c_int32), ("h", c_int32), ("map_type", c_int32), ("maps", c_void_p * MAX_FUSION),
+        ("offsets", c_double * MAX_FUSION), ("cargarse_basura", c_int32), ("op", c_int32), ("threshold", c_double),
+        ("rpc", c_void_p), ("off_x", c_double), ("off_y", c_double), ("zone", c_int32), ("south", c_int32), ("r", c_float),
+        ("p", c_int32), ("n", c_int32), ("colors", c_void_p), ("nbands", c_int32), ("color_type", c_int32), ("stretch", c_int32),
+        ("pct", c_double),
+    ]
 
 
 class PlyColumn(ctypes.Structure):
@@ -128,6 +140,9 @@ _SIGNATURES = {
     "s2pb_deflate_blocks": (c_int, [c_void_p, _f, c_int, c_int, c_int, POINTER(c_uint8), c_int64, POINTER(c_int32)]),
     "s2pb_pair_tile_to_ply": (c_int, [c_void_p, POINTER(PairTile), POINTER(c_uint8), POINTER(c_int64), _f, _f, _f, _f, POINTER(c_uint8),
                                       _f]),
+    "s2pb_pair_tile_to_height_map": (c_int, [c_void_p, POINTER(PairTile), c_int, c_int, c_int, c_int, POINTER(c_double), _f, _f, _f, _f,
+                                             POINTER(c_uint8), _f]),
+    "s2pb_heights_tile_to_ply": (c_int, [c_void_p, POINTER(HeightsTile), POINTER(c_uint8), POINTER(c_int64), POINTER(_f), _f]),
     "s2pb_erode_mask": (c_int, [c_void_p, POINTER(c_uint8), POINTER(c_uint8), c_int, c_int, c_float]),
     "s2pb_census": (c_int, [c_void_p, _f, c_int, c_int, c_int, POINTER(c_uint64)]),
     "s2pb_costvolume": (c_int, [c_void_p, _f, _f, c_int, c_int, POINTER(c_int32), POINTER(c_int32), c_int, c_int, c_int, _f]),

@@ -10,6 +10,10 @@
 // array np.loadtxt returned, s2p/__init__.py:371-374): NumPy >= 2 (NEP 50) subtracts in float64, NumPy < 2
 // (value-based casting) in float32.  `sub_f32` selects the latter; the Python drop-in asks the NumPy it runs under.
 // Sums follow NumPy's pairwise scheme (8 accumulators from 8 values on), so np.mean / np.nanmean agree for every n.
+//
+// The rasters are read in the type they are stored in (fusion_kernel<float> or <double>): a float64 height map, which
+// triangulation.height_map returns and common.rasterio_write keeps, is subtracted in float64 without a rounding to float32
+// first, as `f.read(1) - offsets[i]` does with the float64 array rasterio returns for it (under any NumPy).
 #pragma once
 #include <cuda_runtime.h>
 
@@ -19,7 +23,7 @@ constexpr int kMaxFusion = 16;
 enum { FUSE_AVERAGE_IF_CLOSE = 0, FUSE_NANMEDIAN = 1, FUSE_NANMEAN = 2, FUSE_NANMIN = 3, FUSE_NANMAX = 4,
        FUSE_MEDIAN = 5, FUSE_MEAN = 6, FUSE_MIN = 7, FUSE_MAX = 8, FUSE_OP_COUNT = 9 };
 struct FusionParams {
-    const float *in[kMaxFusion];
+    const void *in[kMaxFusion];   // float or double rasters, as the kernel's instantiation reads them
     double offset[kMaxFusion];
     int n, op, sub_f32;
     double threshold, mean_offset;
@@ -46,6 +50,14 @@ __device__ __forceinline__ double np_sum(const double *a, int n)
     return res;
 }
 
+// one stored value minus its offset, in float64 (sub_f32: in float32, NumPy < 2's rule for a float32 raster)
+__device__ __forceinline__ double fusion_input(float in, double offset, int sub_f32)
+{
+    return sub_f32 ? (double)(in - (float)offset) : (double)in - offset;
+}
+__device__ __forceinline__ double fusion_input(double in, double offset, int) { return in - offset; }
+
+template <typename T>
 __global__ void fusion_kernel(const FusionParams P)
 {
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -53,8 +65,7 @@ __global__ void fusion_kernel(const FusionParams P)
     double v[kMaxFusion], a[kMaxFusion];
     int m = 0;
     for (int k = 0; k < P.n; k++) {
-        const float in = P.in[k][i];
-        const double x = P.sub_f32 ? (double)(in - (float)P.offset[k]) : (double)in - P.offset[k];
+        const double x = fusion_input(static_cast<const T *>(P.in[k])[i], P.offset[k], P.sub_f32);
         a[k] = x;
         if (x == x) {                       // insertion sort of the non-NaN values
             int q = m++;

@@ -88,13 +88,10 @@ extern "C" int s2pb_disp_to_xyz(s2pb_ctx *ctx, double *xyz, float *err, const fl
     return L.finish();
 }
 
-int localised_cloud(s2pb_ctx *ctx, HostCall &L, const double *heights, int w, int h, const s2pb_rpc *rpc, double off_x,
-                    double off_y, int zone, int south, double **d_xyz)
+int localised_cloud_device(s2pb_ctx *ctx, HostCall &L, const double *d_z, int w, int h, const s2pb_rpc *rpc, double off_x,
+                           double off_y, int zone, int south, double **d_xyz)
 {
-    if (!heights || !rpc || w < 1 || h < 1) return fail(S2PB_ERR_ARG, "bad argument");
-    if (int rc = cloud_zone_ok(zone)) return rc;
     const size_t npix = (size_t)w * h;
-    double *d_z = L.upload(heights, npix * 8);
     *d_xyz = L.take<double>(npix * 24);
     int *d_capped = L.take<int>(4);
     if (int rc = L.error()) return rc;
@@ -115,6 +112,21 @@ int localised_cloud(s2pb_ctx *ctx, HostCall &L, const double *heights, int w, in
     if (int rc = L.finish()) return rc;
     if (capped) return fail(S2PB_ERR_ARG, "the localisation of %d pixel(s) did not converge in 1000 steps", capped);
     return S2PB_OK;
+}
+
+int localised_cloud_args_ok(int w, int h, const s2pb_rpc *rpc, int zone)
+{
+    if (!rpc || w < 1 || h < 1) return fail(S2PB_ERR_ARG, "bad argument");
+    return cloud_zone_ok(zone);
+}
+
+int localised_cloud(s2pb_ctx *ctx, HostCall &L, const double *heights, int w, int h, const s2pb_rpc *rpc, double off_x,
+                    double off_y, int zone, int south, double **d_xyz)
+{
+    if (!heights) return fail(S2PB_ERR_ARG, "bad argument");
+    if (int rc = localised_cloud_args_ok(w, h, rpc, zone)) return rc;
+    double *d_z = L.upload(heights, (size_t)w * h * 8);
+    return localised_cloud_device(ctx, L, d_z, w, h, rpc, off_x, off_y, zone, south, d_xyz);
 }
 
 // s2p.triangulation.height_map_to_xyz (s2p/triangulation.py:165-217) with a UTM (or no) output CRS: every pixel of the height
@@ -168,53 +180,91 @@ extern "C" int s2pb_resample_heights(s2pb_ctx *ctx, const double *z, int zw, int
 // s2p.triangulation.height_map (s2p/triangulation.py:346-389) with p = 1: triangulate inside the bounding box
 // float32(x-1, x+w+2, y-1, y+h+2) against mask_orig padded by one row / column of ones, keep the altitude on the device
 // and resample it onto the tile grid through H1 * T(x, y).
-extern "C" int s2pb_height_map(s2pb_ctx *ctx, double *out, const float *disp, const float *msk, int nx, int ny,
-                               const float *mask_orig, int mw, int mh, int x, int y, int w, int h, const double H1[9],
-                               const double H2[9], const s2pb_rpc *rpc1, const s2pb_rpc *rpc2)
+// H1 * T(x, y): the first two columns are H1's, the third H1 (x, y, 1)^T summed left to right
+static void tile_homography(const double H1[9], int x, int y, double H[9])
 {
-    if (!ctx || !out || !disp || !msk || !mask_orig || !H1 || !H2 || !rpc1 || !rpc2 || nx < 1 || ny < 1 || mw < 1 || mh < 1 ||
-        w < 1 || h < 1)
+    memcpy(H, H1, 9 * sizeof(double));
+    for (int r = 0; r < 3; r++) H[3 * r + 2] = H1[3 * r] * x + H1[3 * r + 1] * y + H1[3 * r + 2];
+}
+
+int height_map_args_ok(int nx, int ny, int mw, int mh, int x, int y, int w, int h, const double H1[9], const double H2[9],
+                       const s2pb_rpc *rpc1, const s2pb_rpc *rpc2)
+{
+    if (!H1 || !H2 || !rpc1 || !rpc2 || nx < 1 || ny < 1 || mw < 1 || mh < 1 || w < 1 || h < 1)
         return fail(S2PB_ERR_ARG, "bad argument");
     if (nx < 2 || ny < 2) return fail(S2PB_ERR_UNSUPPORTED, "a %dx%d rectified map (the reference squeezes it to 1-D)", nx, ny);
-    // H1 * T(x, y): the first two columns are H1's, the third H1 (x, y, 1)^T summed left to right
     double H[9];
-    memcpy(H, H1, sizeof H);
-    for (int r = 0; r < 3; r++) H[3 * r + 2] = H1[3 * r] * x + H1[3 * r + 1] * y + H1[3 * r + 2];
+    tile_homography(H1, x, y, H);
     if (!affine_last_row(H)) return fail(S2PB_ERR_ARG, "the last row of H1 * T(x, y) is not (0, 0, 1)");
+    return S2PB_OK;
+}
+
+int height_map_device(s2pb_ctx *ctx, HostCall &L, const float *d_dx, const float *d_m, int nx, int ny, const float *d_mo0, int mw,
+                      int mh, int x, int y, int w, int h, const double H1[9], const double H2[9], const s2pb_rpc *rpc1,
+                      const s2pb_rpc *rpc2, double *d_out)
+{
+    double H[9];
+    tile_homography(H1, x, y, H);
     const float bbox[4] = {(float)(x - 1), (float)(x + w + 2), (float)(y - 1), (float)(y + h + 2)};
     const size_t npix = (size_t)nx * ny, pw = (size_t)mw + 2, ph = (size_t)mh + 2;
-    HostCall L(ctx, "the height map");
-    float *d_dx = L.upload(disp, npix * 4), *d_dy = L.take<float>(npix * 4), *d_m = L.upload(msk, npix * 4);
-    float *d_mo0 = L.upload(mask_orig, (size_t)mw * mh * 4), *d_mo = L.take<float>(pw * ph * 4), *d_err = L.take<float>(npix * 4);
-    double *d_xyz = L.take<double>(npix * 24), *d_out = L.take<double>((size_t)w * h * 8);
+    float *d_dy = L.take<float>(npix * 4), *d_mo = L.take<float>(pw * ph * 4), *d_err = L.take<float>(npix * 4);
+    double *d_xyz = L.take<double>(npix * 24);
     if (int rc = L.error()) return rc;
     CK(cudaMemsetAsync(d_dy, 0, npix * 4, L.st));
     const dim3 b2(32, 8);
     launch(ctx, pad_ones_kernel, grid2d((int)pw, (int)ph, b2), b2, 0, L.st, d_mo0, mw, mh, d_mo);
     int rc = triangulate_enqueue(ctx, L.st, d_dx, d_dy, d_m, nx, ny, d_mo, (int)pw, (int)ph, H1, H2, rpc1, rpc2, bbox, d_xyz, d_err);
     if (rc == S2PB_OK) rc = resample_heights_enqueue(ctx, L.st, d_xyz + 2, 3, nx, ny, H, d_out, w, h);
-    if (rc != S2PB_OK) return rc;
+    return rc;
+}
+
+// s2p.triangulation.height_map (s2p/triangulation.py:346-389) with p = 1: triangulate inside the bounding box
+// float32(x-1, x+w+2, y-1, y+h+2) against mask_orig padded by one row / column of ones, keep the altitude on the device
+// and resample it onto the tile grid through H1 * T(x, y).
+extern "C" int s2pb_height_map(s2pb_ctx *ctx, double *out, const float *disp, const float *msk, int nx, int ny,
+                               const float *mask_orig, int mw, int mh, int x, int y, int w, int h, const double H1[9],
+                               const double H2[9], const s2pb_rpc *rpc1, const s2pb_rpc *rpc2)
+{
+    if (!ctx || !out || !disp || !msk || !mask_orig) return fail(S2PB_ERR_ARG, "bad argument");
+    if (int rc = height_map_args_ok(nx, ny, mw, mh, x, y, w, h, H1, H2, rpc1, rpc2)) return rc;
+    const size_t npix = (size_t)nx * ny;
+    HostCall L(ctx, "the height map");
+    float *d_dx = L.upload(disp, npix * 4), *d_m = L.upload(msk, npix * 4);
+    float *d_mo0 = L.upload(mask_orig, (size_t)mw * mh * 4);
+    double *d_out = L.take<double>((size_t)w * h * 8);
+    if (int rc = L.error()) return rc;
+    if (int rc = height_map_device(ctx, L, d_dx, d_m, nx, ny, d_mo0, mw, mh, x, y, w, h, H1, H2, rpc1, rpc2, d_out)) return rc;
     L.download(out, d_out, (size_t)w * h * 8);
     return L.finish();
 }
 
 // s2p.common.cargarse_basura (s2p/common.py:251-262) on the float32 image its tools read: 5x5 min / max and plambda in one
 // kernel, then remove_small_cc(200, 5)
+int basura_args_ok(int w, int h)
+{
+    if (w < 2 || h < 2) return fail(S2PB_ERR_UNSUPPORTED, "a %dx%d image: the reference's morphoop reads outside it", w, h);
+    if ((size_t)w * h > INT32_MAX) return fail(S2PB_ERR_UNSUPPORTED, "at most 2^31 - 1 pixels");
+    return S2PB_OK;
+}
+
+int basura_enqueue(s2pb_ctx *ctx, cudaStream_t st, const float *d_in, float *d_out, int w, int h, float *d_m, int *lab, int *area)
+{
+    const dim3 bb(kBasuraTx, kBasuraTy);
+    launch(ctx, basura_minmax_kernel, grid2d(w, h, bb), bb, 0, st, d_in, w, h, d_m);
+    CK(cudaGetLastError());
+    return launch_remove_small_cc(ctx, d_m, d_out, w, h, 200, 5.f, lab, area, st);
+}
+
 extern "C" int s2pb_cargarse_basura(s2pb_ctx *ctx, const float *in, float *out, int w, int h)
 {
     if (!ctx || !in || !out || w < 1 || h < 1) return fail(S2PB_ERR_ARG, "bad argument");
-    if (w < 2 || h < 2) return fail(S2PB_ERR_UNSUPPORTED, "a %dx%d image: the reference's morphoop reads outside it", w, h);
+    if (int rc = basura_args_ok(w, h)) return rc;
     const size_t npix = (size_t)w * h;
-    if (npix > INT32_MAX) return fail(S2PB_ERR_UNSUPPORTED, "at most 2^31 - 1 pixels");
     HostCall L(ctx, "cargarse_basura");
     float *a = L.upload(in, npix * 4), *m = L.take<float>(npix * 4), *b = L.take<float>(npix * 4);
     int *lab = L.take<int>(npix * 4), *area = L.take<int>(npix * 4);
     if (int rc = L.error()) return rc;
-    const dim3 bb(kBasuraTx, kBasuraTy);
-    launch(ctx, basura_minmax_kernel, grid2d(w, h, bb), bb, 0, L.st, a, w, h, m);
-    CK(cudaGetLastError());
-    int rc = launch_remove_small_cc(ctx, m, b, w, h, 200, 5.f, lab, area, L.st);
-    if (rc != S2PB_OK) return rc;
+    if (int rc = basura_enqueue(ctx, L.st, a, b, w, h, m, lab, area)) return rc;
     L.download(out, b, npix * 4);
     return L.finish();
 }

@@ -1,7 +1,7 @@
 // host.h -- host-side state and helpers shared by the translation units of the C ABI (not a public header).
 //
 // s2pb200.cu owns the context, the slots, the matcher and the matcher's stage entry points; warp.cu, geometry.cu, projection.cu,
-// sgbm.cu, raster.cu, cloud.cu, mosaic.cu and pair_tile.cu each hold one family of entry points.  Every kernel header that defines a non-template kernel is included by one of
+// sgbm.cu, raster.cu, cloud.cu, mosaic.cu, pair_tile.cu and heights_tile.cu each hold one family of entry points.  Every kernel header that defines a non-template kernel is included by one of
 // those files only, so that its kernels are compiled once; the few launchers another file needs are declared at the end.
 #pragma once
 #include "../../include/s2pb200.h"
@@ -278,6 +278,21 @@ int triangulated_cloud_device(s2pb_ctx *ctx, HostCall &L, const float *d_dx, con
                               const s2pb_rpc *rpcb, const float bbox[4], int zone, int south, double **d_xyz, float **d_err);
 int localised_cloud(s2pb_ctx *ctx, HostCall &L, const double *heights, int w, int h, const s2pb_rpc *rpc, double off_x,
                     double off_y, int zone, int south, double **d_xyz);
+// localised_cloud_device: the same from device heights d_z, after localised_cloud_args_ok checked the rest.
+int localised_cloud_args_ok(int w, int h, const s2pb_rpc *rpc, int zone);
+int localised_cloud_device(s2pb_ctx *ctx, HostCall &L, const double *d_z, int w, int h, const s2pb_rpc *rpc, double off_x,
+                           double off_y, int zone, int south, double **d_xyz);
+// s2pb_height_map from the device disparity d_dx and mask d_m (nx*ny) and the unpadded device mask_orig d_mo0 (mw*mh) into the
+// device heights d_out (w*h), in flight on L.st, after height_map_args_ok checked its arguments.
+int height_map_args_ok(int nx, int ny, int mw, int mh, int x, int y, int w, int h, const double H1[9], const double H2[9],
+                       const s2pb_rpc *rpc1, const s2pb_rpc *rpc2);
+int height_map_device(s2pb_ctx *ctx, HostCall &L, const float *d_dx, const float *d_m, int nx, int ny, const float *d_mo0, int mw,
+                      int mh, int x, int y, int w, int h, const double H1[9], const double H2[9], const s2pb_rpc *rpc1,
+                      const s2pb_rpc *rpc2, double *d_out);
+// s2pb_cargarse_basura of a device w*h float32 image into d_out (d_m: w*h floats, lab and area: w*h ints of scratch), after
+// basura_args_ok
+int basura_args_ok(int w, int h);
+int basura_enqueue(s2pb_ctx *ctx, cudaStream_t st, const float *d_in, float *d_out, int w, int h, float *d_m, int *lab, int *area);
 int remove_isolated_enqueue(s2pb_ctx *ctx, cudaStream_t st, double *d_xyz, int nx, int ny, float r, int p, int n, int q, int *d_work);
 // sgbm.cu: order statistics of the non-NaN values of n device floats by radix select (sgbm_kernels.cuh) into d_os, which
 // holds order_stats_bytes(); rule kOrdQauto (qauto's thresholds) or kOrdLinear (numpy's 'linear' quantiles q0 and q1)
@@ -293,6 +308,10 @@ int tail_args_ok(s2pb_ctx *ctx, int nx, int ny, const float *bands, int nbands, 
 int typed_colours_ok(int nbands, int color_type);
 int cloud_tail_device(s2pb_ctx *ctx, HostCall &L, double *d_xyz, int nx, int ny, float r, int p, int n, const float *d_bands,
                       int nbands, double pct, const uint8_t *d_typed, int cb, const float *d_conf, uint8_t *records, int64_t *npoints);
+// raster.cu: s2pb_merge_n's checks of n and op, and its merge of n device rasters (float32, or float64 when f64) into d_out
+int fusion_args_ok(int n, int op);
+void fusion_enqueue(s2pb_ctx *ctx, cudaStream_t st, const void *const *d_in, bool f64, const double *offsets, int n, size_t npix,
+                    int op, double threshold, float *d_out);
 // warp.cu
 void invert_homography(const double i[9], double o[9]);
 int warp_host_to_device(s2pb_ctx *ctx, ScratchLease &L, cudaStream_t st, const float *src, int sw, int sh, const double H[9],

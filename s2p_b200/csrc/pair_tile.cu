@@ -1,6 +1,7 @@
-// pair_tile.cu -- a two-view tile from its source crops to the records of cloud.ply in one call: rectify_pair's two warps, the
-// matcher and its rejection mask, masking.erosion and disparity_to_ply chained on one stream, the intermediates staying on the
-// device (s2p/__init__.py:102-318).
+// pair_tile.cu -- one pair of a tile from its source crops on, in one call: rectify_pair's two warps, the matcher and its
+// rejection mask and masking.erosion chained on one stream (pair_match), then, for a two-view tile, disparity_to_ply down to
+// the records of cloud.ply, or, for a pair of a tri-stereo tile, disparity_to_height down to the pair's height map; the
+// intermediates stay on the device (s2p/__init__.py:102-318).
 #include "host.h"
 
 // the eroded 0/1 mask as the float32 image disparity_to_ply hands to the triangulation (a PNG read back as uint8, then float32)
@@ -10,45 +11,43 @@ __global__ void mask_to_float_kernel(const uint8_t *__restrict__ in, float *__re
     if (i < n) out[i] = (float)in[i];
 }
 
-// what the stages would refuse that can be seen before the first launch
-static int pair_tile_args_ok(s2pb_ctx *ctx, const s2pb_pair_tile *t, uint8_t *records, int64_t *npoints, const float *conf,
-                             const float *disp_right)
+// what the warps, the matcher and the erosion would refuse that can be seen before the first launch
+// (with_conf: the confidence column is asked for)
+static int pair_match_args_ok(const s2pb_pair_tile *t, const float *conf, const float *disp_right, bool with_conf)
 {
-    if (!ctx || !t || !t->src1 || !t->src2 || !t->msk_orig || t->sw1 < 1 || t->sh1 < 1 || t->sw2 < 1 || t->sh2 < 1 || t->w < 1 ||
-        t->h < 1 || t->mw < 1 || t->mh < 1)
+    if (!t->src1 || !t->src2 || !t->msk_orig || t->sw1 < 1 || t->sh1 < 1 || t->sw2 < 1 || t->sh2 < 1 || t->w < 1 || t->h < 1 ||
+        t->mw < 1 || t->mh < 1)
         return fail(S2PB_ERR_ARG, "bad argument");
     if (t->matcher != S2PB_MATCHER_MGM && t->matcher != S2PB_MATCHER_SGBM) return fail(S2PB_ERR_ARG, "unknown matcher %d", t->matcher);
-    if (t->matcher == S2PB_MATCHER_SGBM && (conf || disp_right || t->with_conf || t->wl || t->wr))
+    if (t->matcher == S2PB_MATCHER_SGBM && (conf || disp_right || with_conf || t->wl || t->wr))
         return fail(S2PB_ERR_ARG, "sgbm has no confidence, right disparity or weight images");
     if ((t->wl == nullptr) != (t->wr == nullptr)) return fail(S2PB_ERR_ARG, "the weight images come in pairs (-wl and -wr)");
     if (t->erode_radius != 0.f) {
         if (int rc = erode_radius_ok(t->erode_radius)) return rc;
     }
-    if (int rc = triangulated_cloud_args_ok(t->w, t->h, t->mw, t->mh, t->ha, t->hb, t->rpc1, t->rpc2, t->bbox, t->zone)) return rc;
-    if (t->clr) {
-        if (int rc = tail_args_ok(ctx, t->w, t->h, t->clr, t->clr_bands, 0.0, records, npoints)) return rc;
-        if (int rc = typed_colours_ok(t->clr_bands, S2PB_PLY_F32)) return rc;
-        if (t->cw < 1 || t->ch < 1) return fail(S2PB_ERR_ARG, "bad argument");
-        return S2PB_OK;
-    }
-    return tail_args_ok(ctx, t->w, t->h, nullptr, 0, t->pct, records, npoints);      // colours: the call's own rectified reference
+    return S2PB_OK;
 }
 
-extern "C" int s2pb_pair_tile_to_ply(s2pb_ctx *ctx, const s2pb_pair_tile *t, uint8_t *records, int64_t *npoints, float *rect1,
-                                     float *rect2, float *disp, float *conf, uint8_t *mask, float *disp_right)
+// The device results of the front half of a pair tile that the back halves read (w*h each, scratch of the call)
+struct PairMatch {
+    const float *rect1;       // the rectified reference
+    const float *disp, *conf; // the disparity and, with MGM, its confidence
+    const float *msk;         // the eroded 0/1 mask as float32
+};
+
+// rectify_pair's two warps, the matcher and its rejection mask, and masking.erosion, on L's stream: the buffers come from L,
+// the intermediates named by non-null host pointers are copied back (in flight on L.st), the matcher waits for its stream
+static int pair_match(s2pb_ctx *ctx, HostCall &L, const s2pb_pair_tile *t, float *rect1, float *rect2, float *disp, float *conf,
+                      uint8_t *mask, float *disp_right, PairMatch *m)
 {
-    if (int rc = pair_tile_args_ok(ctx, t, records, npoints, conf, disp_right)) return rc;
-    *npoints = 0;
     const int w = t->w, h = t->h;
     const size_t npix = (size_t)w * h;
     const bool mgm = t->matcher == S2PB_MATCHER_MGM, erode = t->erode_radius != 0.f;
-    HostCall L(ctx, "the pair tile");
     float *d_r1 = L.take<float>(npix * 4), *d_r2 = L.take<float>(npix * 4), *d_disp = L.take<float>(npix * 4);
     float *d_conf = mgm ? L.take<float>(npix * 4) : nullptr, *d_dispR = disp_right ? L.take<float>(npix * 4) : nullptr;
     uint8_t *d_mask = L.take<uint8_t>(npix), *d_eroded = erode ? L.take<uint8_t>(npix) : d_mask;
-    float *d_msk = L.take<float>(npix * 4), *d_dy = L.take<float>(npix * 4);
+    float *d_msk = L.take<float>(npix * 4);
     const float *d_wl = t->wl ? L.upload(t->wl, npix * 4) : nullptr, *d_wr = t->wr ? L.upload(t->wr, npix * 4) : nullptr;
-    const float *d_mo = L.upload(t->msk_orig, (size_t)t->mw * t->mh * 4);
     if (int rc = L.error()) return rc;
 
     // rectification_pair: both warps straight into the matcher's inputs
@@ -68,20 +67,53 @@ extern "C" int s2pb_pair_tile_to_ply(s2pb_ctx *ctx, const s2pb_pair_tile *t, uin
     if (erode) launch_erode_mask(ctx, d_mask, d_eroded, w, h, t->erode_radius, L.st);
     launch(ctx, mask_to_float_kernel, (unsigned)((npix + 255) / 256), 256, 0, L.st, d_eroded, d_msk, npix);
     CK(cudaGetLastError());
-    CK(cudaMemsetAsync(d_dy, 0, npix * 4, L.st));
     if (disp) L.download(disp, d_disp, npix * 4);
     if (conf) L.download(conf, d_conf, npix * 4);
     if (mask) L.download(mask, d_eroded, npix);
     if (disp_right) L.download(disp_right, d_dispR, npix * 4);
+    m->rect1 = d_r1; m->disp = d_disp; m->conf = d_conf; m->msk = d_msk;
+    return S2PB_OK;
+}
+
+// what the stages of s2pb_pair_tile_to_ply would refuse that can be seen before the first launch
+static int pair_tile_args_ok(s2pb_ctx *ctx, const s2pb_pair_tile *t, uint8_t *records, int64_t *npoints, const float *conf,
+                             const float *disp_right)
+{
+    if (!ctx || !t) return fail(S2PB_ERR_ARG, "bad argument");
+    if (int rc = pair_match_args_ok(t, conf, disp_right, t->with_conf != 0)) return rc;
+    if (int rc = triangulated_cloud_args_ok(t->w, t->h, t->mw, t->mh, t->ha, t->hb, t->rpc1, t->rpc2, t->bbox, t->zone)) return rc;
+    if (t->clr) {
+        if (int rc = tail_args_ok(ctx, t->w, t->h, t->clr, t->clr_bands, 0.0, records, npoints)) return rc;
+        if (int rc = typed_colours_ok(t->clr_bands, S2PB_PLY_F32)) return rc;
+        if (t->cw < 1 || t->ch < 1) return fail(S2PB_ERR_ARG, "bad argument");
+        return S2PB_OK;
+    }
+    return tail_args_ok(ctx, t->w, t->h, nullptr, 0, t->pct, records, npoints);      // colours: the call's own rectified reference
+}
+
+extern "C" int s2pb_pair_tile_to_ply(s2pb_ctx *ctx, const s2pb_pair_tile *t, uint8_t *records, int64_t *npoints, float *rect1,
+                                     float *rect2, float *disp, float *conf, uint8_t *mask, float *disp_right)
+{
+    if (int rc = pair_tile_args_ok(ctx, t, records, npoints, conf, disp_right)) return rc;
+    *npoints = 0;
+    const int w = t->w, h = t->h;
+    const size_t npix = (size_t)w * h;
+    HostCall L(ctx, "the pair tile");
+    PairMatch m;
+    if (int rc = pair_match(ctx, L, t, rect1, rect2, disp, conf, mask, disp_right, &m)) return rc;
 
     // disparity_to_ply: the cloud, its colours and its records
+    float *d_dy = L.take<float>(npix * 4);
+    const float *d_mo = L.upload(t->msk_orig, (size_t)t->mw * t->mh * 4);
+    if (int rc = L.error()) return rc;
+    CK(cudaMemsetAsync(d_dy, 0, npix * 4, L.st));
     double *d_xyz = nullptr;
     float *d_err = nullptr;
-    if (int rc = triangulated_cloud_device(ctx, L, d_disp, d_dy, d_msk, w, h, d_mo, t->mw, t->mh, t->ha, t->hb, t->rpc1, t->rpc2,
+    if (int rc = triangulated_cloud_device(ctx, L, m.disp, d_dy, m.msk, w, h, d_mo, t->mw, t->mh, t->ha, t->hb, t->rpc1, t->rpc2,
                                            t->bbox, t->zone, t->south, &d_xyz, &d_err))
         return rc;
-    const float *d_cc = t->with_conf ? d_conf : nullptr;
-    if (!t->clr) return cloud_tail_device(ctx, L, d_xyz, w, h, t->r, t->p, t->n, d_r1, 1, t->pct, nullptr, 1, d_cc, records, npoints);
+    const float *d_cc = t->with_conf ? m.conf : nullptr;
+    if (!t->clr) return cloud_tail_device(ctx, L, d_xyz, w, h, t->r, t->p, t->n, m.rect1, 1, t->pct, nullptr, 1, d_cc, records, npoints);
     float *d_col = L.take<float>(npix * t->clr_bands * 4);
     if (int rc = L.error()) return rc;
     for (int b = 0; b < t->clr_bands; b++)
@@ -90,4 +122,25 @@ extern "C" int s2pb_pair_tile_to_ply(s2pb_ctx *ctx, const s2pb_pair_tile *t, uin
             return rc;
     return cloud_tail_device(ctx, L, d_xyz, w, h, t->r, t->p, t->n, nullptr, t->clr_bands, 0.0, (const uint8_t *)d_col, 4, d_cc,
                              records, npoints);
+}
+
+extern "C" int s2pb_pair_tile_to_height_map(s2pb_ctx *ctx, const s2pb_pair_tile *t, int x, int y, int tw, int th, double *heights,
+                                            float *rect1, float *rect2, float *disp, float *conf, uint8_t *mask, float *disp_right)
+{
+    if (!ctx || !t || !heights) return fail(S2PB_ERR_ARG, "bad argument");
+    if (int rc = pair_match_args_ok(t, conf, disp_right, false)) return rc;
+    if (int rc = height_map_args_ok(t->w, t->h, t->mw, t->mh, x, y, tw, th, t->ha, t->hb, t->rpc1, t->rpc2)) return rc;
+    HostCall L(ctx, "the pair's height map");
+    PairMatch m;
+    if (int rc = pair_match(ctx, L, t, rect1, rect2, disp, conf, mask, disp_right, &m)) return rc;
+
+    // disparity_to_height: triangulation.height_map on the device disparity and eroded mask
+    const float *d_mo = L.upload(t->msk_orig, (size_t)t->mw * t->mh * 4);
+    double *d_out = L.take<double>((size_t)tw * th * 8);
+    if (int rc = L.error()) return rc;
+    if (int rc = height_map_device(ctx, L, m.disp, m.msk, t->w, t->h, d_mo, t->mw, t->mh, x, y, tw, th, t->ha, t->hb, t->rpc1,
+                                   t->rpc2, d_out))
+        return rc;
+    L.download(heights, d_out, (size_t)tw * th * 8);
+    return L.finish();
 }

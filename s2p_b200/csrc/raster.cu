@@ -10,29 +10,50 @@
 
 // ------------------------------------------------------------------ n-view merge (section 8f)
 
-extern "C" int s2pb_merge_n(s2pb_ctx *ctx, const float *const *inputs, const double *offsets, int n, int w, int h, int op,
-                            double threshold, float *out)
+static_assert(S2PB_MAX_FUSION == kMaxFusion, "the public bound on the merged maps is the merge kernel's");
+
+// what the merge refuses: n outside 1..kMaxFusion, an operator code (S2PB_FUSE_SUB_F32 aside) it does not know
+int fusion_args_ok(int n, int op)
 {
-    if (!ctx || !inputs || !offsets || !out || n < 1 || w < 1 || h < 1) return fail(S2PB_ERR_ARG, "bad argument");
+    if (n < 1) return fail(S2PB_ERR_ARG, "bad argument");
     if (n > kMaxFusion) return fail(S2PB_ERR_UNSUPPORTED, "at most %d rasters can be merged", kMaxFusion);
-    const int sub_f32 = (op & S2PB_FUSE_SUB_F32) ? 1 : 0;
     op &= ~S2PB_FUSE_SUB_F32;
     if (op < FUSE_AVERAGE_IF_CLOSE || op >= FUSE_OP_COUNT) return fail(S2PB_ERR_ARG, "unknown averaging operator %d", op);
-    const size_t npix = (size_t)w * h;
-    HostCall L(ctx, "the merge");
-    float *o = L.take<float>(npix * 4);
+    return S2PB_OK;
+}
+
+// merge_n of n device rasters of npix float32 (f64: float64) values into the float32 d_out, after fusion_args_ok
+void fusion_enqueue(s2pb_ctx *ctx, cudaStream_t st, const void *const *d_in, bool f64, const double *offsets, int n, size_t npix,
+                    int op, double threshold, float *d_out)
+{
     FusionParams P;
     memset(&P, 0, sizeof P);
     double s = 0;
     for (int k = 0; k < n; k++) {
-        if (!inputs[k]) return fail(S2PB_ERR_ARG, "null raster %d", k);
-        P.in[k] = L.upload(inputs[k], npix * 4);
+        P.in[k] = d_in[k];
         P.offset[k] = offsets[k];
         s += offsets[k];                     // np.mean of a short list: plain left-to-right sum / n
     }
+    P.n = n; P.op = op & ~S2PB_FUSE_SUB_F32; P.sub_f32 = (op & S2PB_FUSE_SUB_F32) ? 1 : 0; P.threshold = threshold;
+    P.mean_offset = s / n; P.npix = npix; P.out = d_out;
+    launch(ctx, f64 ? fusion_kernel<double> : fusion_kernel<float>, (unsigned)((npix + 255) / 256), 256, 0, st, P);
+}
+
+extern "C" int s2pb_merge_n(s2pb_ctx *ctx, const float *const *inputs, const double *offsets, int n, int w, int h, int op,
+                            double threshold, float *out)
+{
+    if (!ctx || !inputs || !offsets || !out || w < 1 || h < 1) return fail(S2PB_ERR_ARG, "bad argument");
+    if (int rc = fusion_args_ok(n, op)) return rc;
+    const size_t npix = (size_t)w * h;
+    HostCall L(ctx, "the merge");
+    float *o = L.take<float>(npix * 4);
+    const void *d_in[kMaxFusion] = {};
+    for (int k = 0; k < n; k++) {
+        if (!inputs[k]) return fail(S2PB_ERR_ARG, "null raster %d", k);
+        d_in[k] = L.upload(inputs[k], npix * 4);
+    }
     if (int rc = L.error()) return rc;
-    P.n = n; P.op = op; P.sub_f32 = sub_f32; P.threshold = threshold; P.mean_offset = s / n; P.npix = npix; P.out = o;
-    launch(ctx, fusion_kernel, (unsigned)((npix + 255) / 256), 256, 0, L.st, P);
+    fusion_enqueue(ctx, L.st, d_in, false, offsets, n, npix, op, threshold, o);
     CK(cudaGetLastError());
     L.download(out, o, npix * 4);
     return L.finish();

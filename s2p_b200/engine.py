@@ -521,23 +521,17 @@ class Engine:
 
     PAIR_TILE_OUTPUTS = ("rect1", "rect2", "disp", "conf", "mask", "disp_right")
 
-    def pair_tile_to_ply(self, src1, H1, src2, H2, w, h, dmin, dmax, mask_orig, H_ref, H_sec, rpc1, rpc2, img_bbx, zone=0, south=False,
-                         params=None, weights=None, erode_radius=0, r=0.0, p=0, n=0, stretch_p=1, clr=None, hc=None,
-                         confidence=False, want=()):
-        """A two-view tile from its source crops to its cloud's records in one device call (s2pb_pair_tile_to_ply): homography
-        of src1 by H1 and of src2 by H2 onto w x h, the matcher (``params``: MgmParams, or SgbmParams for sgbm; ``weights`` =
-        (wl, wr) for mgm_multi_lsd) on [dmin, dmax], the erosion of its mask (erode_radius 0: none), then disp_to_ply on the
-        disparity and the eroded mask (H_ref, H_sec: the triangulation's homographies, H_sec with the pointing correction)
-        coloured by the stretch of the rectified reference, or by the clr crop (nbands, ch, cw) warped by hc, with the
-        confidence column when ``confidence``.  -> (records, dict of the intermediates named in ``want``, a subset of
-        PAIR_TILE_OUTPUTS)."""
+    @staticmethod
+    def _pair_tile(src1, H1, src2, H2, w, h, dmin, dmax, mask_orig, H_ref, H_sec, rpc1, rpc2, params, weights, erode_radius, want):
+        """-> (PairTile with the fields of the warps, the matcher, the erosion, msk_orig, the cameras, ha and hb filled; the arrays
+        its pointers refer to)"""
         src1, src2, mo = _f32(src1), _f32(src2), _f32(mask_orig)
         if src1.ndim != 2 or src2.ndim != 2 or mo.ndim != 2:
             raise ValueError("src1, src2 and mask_orig must be 2-D arrays")
-        unknown = set(want) - set(self.PAIR_TILE_OUTPUTS)
+        unknown = set(want) - set(Engine.PAIR_TILE_OUTPUTS)
         if unknown:
-            raise ValueError("unknown outputs %s (one of %s)" % (sorted(unknown), ", ".join(self.PAIR_TILE_OUTPUTS)))
-        w, h = int(w), int(h)
+            raise ValueError("unknown outputs %s (one of %s)" % (sorted(unknown), ", ".join(Engine.PAIR_TILE_OUTPUTS)))
+        keep = [src1, src2, mo]
         t = _lib.PairTile()
         t.src1, t.sw1, t.sh1, t.src2, t.sw2, t.sh2 = _fp(src1), src1.shape[1], src1.shape[0], _fp(src2), src2.shape[1], src2.shape[0]
         t.w, t.h, t.dmin, t.dmax = w, h, int(dmin), int(dmax)
@@ -551,12 +545,36 @@ class Engine:
             if wl.shape != (h, w) or wr.shape != (h, w):
                 raise ValueError("the weight images must have the shape of the rectified images")
             t.wl, t.wr = _fp(wl), _fp(wr)
+            keep += [wl, wr]
         t.erode_radius = float(erode_radius)
         t.msk_orig, t.mw, t.mh = _fp(mo), mo.shape[1], mo.shape[0]
-        t.bbox[:] = [float(v) for v in np.asarray(img_bbx, np.float32).reshape(4)]
         t.rpc1, t.rpc2 = _rpc(rpc1), _rpc(rpc2)
         for name, H in (("H1", H1), ("H2", H2), ("ha", H_ref), ("hb", H_sec)):
             getattr(t, name)[:] = [float(v) for v in np.asarray(H, np.float64).reshape(9)]
+        return t, keep
+
+    def _pair_outputs(self, want, h, w):
+        """the host arrays of the intermediates named in ``want`` and the pointer arguments from rect1 to disp_right"""
+        out = {k: np.empty((h, w), np.uint8 if k == "mask" else np.float32) for k in self.PAIR_TILE_OUTPUTS if k in want}
+        ptr = lambda k, conv: conv(out[k]) if k in out else None
+        return out, (ptr("rect1", _fp), ptr("rect2", _fp), ptr("disp", _fp), ptr("conf", _fp), ptr("mask", _u8), ptr("disp_right", _fp))
+
+    PAIR_TILE_OUTPUTS = ("rect1", "rect2", "disp", "conf", "mask", "disp_right")
+
+    def pair_tile_to_ply(self, src1, H1, src2, H2, w, h, dmin, dmax, mask_orig, H_ref, H_sec, rpc1, rpc2, img_bbx, zone=0, south=False,
+                         params=None, weights=None, erode_radius=0, r=0.0, p=0, n=0, stretch_p=1, clr=None, hc=None,
+                         confidence=False, want=()):
+        """A two-view tile from its source crops to its cloud's records in one device call (s2pb_pair_tile_to_ply): homography
+        of src1 by H1 and of src2 by H2 onto w x h, the matcher (``params``: MgmParams, or SgbmParams for sgbm; ``weights`` =
+        (wl, wr) for mgm_multi_lsd) on [dmin, dmax], the erosion of its mask (erode_radius 0: none), then disp_to_ply on the
+        disparity and the eroded mask (H_ref, H_sec: the triangulation's homographies, H_sec with the pointing correction)
+        coloured by the stretch of the rectified reference, or by the clr crop (nbands, ch, cw) warped by hc, with the
+        confidence column when ``confidence``.  -> (records, dict of the intermediates named in ``want``, a subset of
+        PAIR_TILE_OUTPUTS)."""
+        w, h = int(w), int(h)
+        t, keep = self._pair_tile(src1, H1, src2, H2, w, h, dmin, dmax, mask_orig, H_ref, H_sec, rpc1, rpc2, params, weights,
+                                  erode_radius, want)
+        t.bbox[:] = [float(v) for v in np.asarray(img_bbx, np.float32).reshape(4)]
         t.zone, t.south = int(zone), int(bool(south))
         t.r, t.p, t.n, t.pct = float(r), operator.index(p), operator.index(n), float(stretch_p)
         nb, cdt = 1, np.uint8
@@ -569,12 +587,87 @@ class Engine:
             t.clr, t.clr_bands, t.ch, t.cw = _fp(c), c.shape[0], c.shape[1], c.shape[2]
             t.hc[:] = [float(v) for v in np.asarray(hc, np.float64).reshape(9)]
         t.with_conf = int(bool(confidence))
-        out = {k: np.empty((h, w), np.uint8 if k == "mask" else np.float32) for k in self.PAIR_TILE_OUTPUTS if k in want}
-        ptr = lambda k, conv: conv(out[k]) if k in out else None
-        call = lambda rec, cnt: self._L.s2pb_pair_tile_to_ply(
-            self._ctx, ctypes.byref(t), rec, cnt, ptr("rect1", _fp), ptr("rect2", _fp), ptr("disp", _fp), ptr("conf", _fp),
-            ptr("mask", _u8), ptr("disp_right", _fp))
+        out, ptrs = self._pair_outputs(want, h, w)
+        call = lambda rec, cnt: self._L.s2pb_pair_tile_to_ply(self._ctx, ctypes.byref(t), rec, cnt, *ptrs)
         records = self._records(call, h * w, nb, bool(confidence), cdt)
+        return records, out
+
+    def pair_tile_to_height_map(self, src1, H1, src2, H2, w, h, dmin, dmax, mask_orig, H_ref, H_sec, rpc1, rpc2, tile, params=None,
+                                weights=None, erode_radius=0, want=()):
+        """One pair of a tri-stereo tile from its source crops to its height map in one device call
+        (s2pb_pair_tile_to_height_map): the warps, the matcher and the erosion of pair_tile_to_ply, then height_map on the
+        disparity and the eroded mask for the tile (x, y, tw, th) of the reference image (H_ref: H_ref.txt; H_sec: H_sec.txt
+        times the inverse of the pointing correction).  -> ((th, tw) float64 heights, dict of the intermediates named in
+        ``want``, a subset of PAIR_TILE_OUTPUTS)."""
+        w, h = int(w), int(h)
+        x, y, tw, th = (int(v) for v in tile)
+        t, keep = self._pair_tile(src1, H1, src2, H2, w, h, dmin, dmax, mask_orig, H_ref, H_sec, rpc1, rpc2, params, weights,
+                                  erode_radius, want)
+        heights = np.empty((th, tw), np.float64)
+        out, ptrs = self._pair_outputs(want, h, w)
+        _lib.check(self._L.s2pb_pair_tile_to_height_map(self._ctx, ctypes.byref(t), x, y, tw, th, _dp(heights), *ptrs))
+        return heights, out
+
+    HEIGHTS_TILE_OUTPUTS = ("cleaned", "merged")
+
+    def heights_tile_to_ply(self, maps, offsets, rpc, off_x, off_y, zone=0, south=False, cargarse_basura=False,
+                            averaging="average_if_close", threshold=1.0, sub_f32=None, r=0.0, p=0, n=0, colors=None, stretch_p=1,
+                            clr=None, want=()):
+        """A tri-stereo tile from its pairs' height maps to its cloud's records in one device call (s2pb_heights_tile_to_ply):
+        with ``cargarse_basura``, each map rounded to float32 and cleaned as cargarse_basura cleans it; then merge_n of the
+        maps (the cleaned ones, else as they are: float32 maps as float32, any other type as float64, which every stored
+        height type converts to exactly) with ``offsets``, ``averaging`` and ``threshold``; then height_map_to_ply of the merged
+        map coloured by the stretch of the float32 planes ``colors`` (as height_map_to_ply) or by the typed planes ``clr`` (as
+        height_map_to_ply_clr).  sub_f32: as merge_n.  -> (records, dict of the intermediates named in ``want``: 'cleaned',
+        the list of cleaned float32 maps, and 'merged', the merged float32 map)."""
+        unknown = set(want) - set(self.HEIGHTS_TILE_OUTPUTS)
+        if unknown:
+            raise ValueError("unknown outputs %s (one of %s)" % (sorted(unknown), ", ".join(self.HEIGHTS_TILE_OUTPUTS)))
+        if "cleaned" in want and not cargarse_basura:
+            raise ValueError("the cleaned maps exist with cargarse_basura only")
+        if averaging.startswith("numpy."):
+            averaging = "np." + averaging[6:]
+        if averaging not in self.FUSION_OPS:
+            raise NotImplementedError("averaging operator %r (supported: %s)" % (averaging, ", ".join(sorted(self.FUSION_OPS))))
+        if sub_f32 is None:
+            sub_f32 = self.numpy_subtracts_in_float32()
+        maps = [np.asarray(m) for m in maps]
+        if not maps or len(maps) != len(offsets):
+            raise ValueError("%d maps, %d offsets" % (len(maps), len(offsets)))
+        if len(maps) > _lib.MAX_FUSION:
+            raise NotImplementedError("at most %d height maps can be merged, got %d" % (_lib.MAX_FUSION, len(maps)))
+        if any(m.ndim != 2 or m.shape != maps[0].shape for m in maps):
+            raise ValueError("the height maps must be 2-D arrays of the same shape")
+        f32 = all(m.dtype == np.float32 for m in maps)
+        maps = [np.ascontiguousarray(m, np.float32 if f32 else np.float64) for m in maps]
+        h, w = maps[0].shape
+        t = _lib.HeightsTile()
+        t.n_maps, t.w, t.h, t.map_type = len(maps), w, h, _lib.PLY_F32 if f32 else _lib.PLY_F64
+        for k, m in enumerate(maps):
+            t.maps[k], t.offsets[k] = m.ctypes.data, float(offsets[k])
+        t.cargarse_basura = int(bool(cargarse_basura))
+        t.op, t.threshold = self.FUSION_OPS[averaging] | (self.FUSE_SUB_F32 if sub_f32 else 0), float(threshold)
+        t.rpc, t.off_x, t.off_y, t.zone, t.south = _rpc(rpc), float(off_x), float(off_y), int(zone), int(bool(south))
+        t.r, t.p, t.n = float(r), operator.index(p), operator.index(n)
+        if clr is not None:
+            if colors is not None:
+                raise ValueError("colors (stretched) or clr (typed), not both")
+            col, nb, t.color_type = self._typed(clr, (h, w))
+            cdt = col.dtype
+        else:
+            col, nb = self._bands(colors, (h, w))
+            cdt, t.stretch, t.pct = np.uint8, 1, float(stretch_p)
+        t.colors, t.nbands = (col.ctypes.data if nb else None), nb
+        out = {}
+        cleaned = None
+        if "cleaned" in want:
+            out["cleaned"] = [np.empty((h, w), np.float32) for _ in maps]
+            cleaned = (_lib._f * len(maps))(*[_fp(c) for c in out["cleaned"]])
+        if "merged" in want:
+            out["merged"] = np.empty((h, w), np.float32)
+        call = lambda rec, cnt: self._L.s2pb_heights_tile_to_ply(self._ctx, ctypes.byref(t), rec, cnt, cleaned,
+                                                                 _fp(out["merged"]) if "merged" in out else None)
+        records = self._records(call, h * w, nb, False, cdt)
         return records, out
 
     def height_map_to_ply_clr(self, heights, rpc, off_x, off_y, zone=0, south=False, r=0.0, p=0, n=0, colors=None):

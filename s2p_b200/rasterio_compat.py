@@ -122,6 +122,22 @@ def write_float_tiff(path, a):
     Image.fromarray(a, mode="F").save(path, format="TIFF")
 
 
+def write_float64_tiff(path, a):
+    """Single-band float64 raster, as common.rasterio_write writes the float64 height map of a pair (s2p/common.py:125-156:
+    rasterio with the profile driver, count, width, height and dtype only); without rasterio a plain float64 TIFF."""
+    a = np.ascontiguousarray(a, dtype=np.float64)
+    if _HAVE_RASTERIO:
+        h, w = a.shape
+        with rasterio.Env():
+            with rasterio.open(path, "w", driver="GTiff", count=1, width=w, height=h, dtype=a.dtype) as f:
+                f.write(a[None])
+                f.update_tags()
+        return
+    import cv2
+    if not cv2.imwrite(path, a):
+        raise IOError("cv2.imwrite failed for %s" % path)
+
+
 def write_float_tiff_like(path, a, template):
     """Single-band float32 raster at `path` with the metadata (CRS, transform, ...) of the raster `template`, which may be
     `path` itself; without rasterio a plain float32 TIFF."""
