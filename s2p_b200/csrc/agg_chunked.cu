@@ -23,7 +23,7 @@ int agg_chunked_configure()
 }
 
 // 0 ok, -1 CUDA error, -2 this shape is not served
-template <bool FOLD> static int chunked_launch(int tsgm, const ChunkedArgs<FOLD> &P, int sm_count, cudaStream_t st)
+template <bool FOLD> int agg_chunked_launch(int tsgm, const ChunkedArgs<FOLD> &P, int sm_count, cudaStream_t st)
 {
     if (P.DP < 32 || P.DP > 2048 || (P.DP & 31)) return -2;
     const bool gen = P.A.general != 0;          // float costs (and weights): no cost table, pipeline depth 2 (ck_stage)
@@ -53,7 +53,7 @@ template <bool FOLD> static int chunked_launch(int tsgm, const ChunkedArgs<FOLD>
 #undef GO2
     return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }
-int agg_chunked_launch(int tsgm, const ChunkedParams &P, int sm_count, cudaStream_t st) { return chunked_launch<false>(tsgm, P, sm_count, st); }
-int agg_chunked_fold_launch(int tsgm, const ChunkedFoldParams &P, int sm_count, cudaStream_t st) { return chunked_launch<true>(tsgm, P, sm_count, st); }
+template int agg_chunked_launch<false>(int, const ChunkedParams &, int, cudaStream_t);
+template int agg_chunked_launch<true>(int, const ChunkedFoldParams &, int, cudaStream_t);
 
 }  // namespace s2pb

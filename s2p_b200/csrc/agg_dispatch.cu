@@ -3,8 +3,7 @@
 
 namespace s2pb {
 
-#define DECL(n) template <> int agg_launch_lpl<n>(int, const AggParams &, int, cudaStream_t, int); template <> int agg_configure_lpl<n>(); \
-    template <> int agg_fold_launch_lpl<n>(int, const AggFoldParams &, int, cudaStream_t);
+#define DECL(n) template <> int agg_configure_lpl<n>();
 S2PB_FOR_EACH_LPL(DECL)
 #undef DECL
 
@@ -16,24 +15,16 @@ int agg_configure()
     return 0;
 }
 
-int agg_launch(int LPL, int tsgm, const AggParams &P, int sm_count, cudaStream_t st, int ctas_per_sm)
+template <bool FOLD> int agg_launch(int LPL, int tsgm, const AggArgs<FOLD> &P, int sm_count, cudaStream_t st, int ctas_per_sm)
 {
     switch (LPL) {
-#define CASE(n) case n: return agg_launch_lpl<n>(tsgm, P, sm_count, st, ctas_per_sm);
+#define CASE(n) case n: return agg_launch_lpl<n, FOLD>(tsgm, P, sm_count, st, ctas_per_sm);
     S2PB_FOR_EACH_LPL(CASE)
 #undef CASE
     default: return -2;
     }
 }
-
-int agg_fold_launch(int LPL, int tsgm, const AggFoldParams &P, int sm_count, cudaStream_t st)
-{
-    switch (LPL) {
-#define CASE(n) case n: return agg_fold_launch_lpl<n>(tsgm, P, sm_count, st);
-    S2PB_FOR_EACH_LPL(CASE)
-#undef CASE
-    default: return -2;
-    }
-}
+template int agg_launch<false>(int, int, const AggParams &, int, cudaStream_t, int);
+template int agg_launch<true>(int, int, const AggFoldParams &, int, cudaStream_t, int);
 
 }  // namespace s2pb

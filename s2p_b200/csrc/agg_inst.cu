@@ -26,17 +26,18 @@ template <> int agg_configure_lpl<kLPL>()
     return 0;
 }
 
-template <bool FOLD> static int launch_lpl(int tsgm, const AggArgs<FOLD> &P, int sm_count, cudaStream_t st, int ctas_per_sm)
+template <int LPL, bool FOLD> int agg_launch_lpl(int tsgm, const AggArgs<FOLD> &P, int sm_count, cudaStream_t st, int ctas_per_sm)
 {
     // persistent CTAs, one (or two) per SM; bands are pulled from a global queue in dependency order
     const int total = P.maxBands * P.nPV;
     dim3 block(kAggThreads);
     const bool scaled = P.lut != nullptr;
-#define GO(T) do { int per = AggOcc<kLPL, T>::ctas; if (ctas_per_sm > 0 && ctas_per_sm < per) per = ctas_per_sm; \
+    constexpr size_t smem = AggSmem<LPL, false>::bytes, smem_gen = AggSmem<LPL, true>::bytes;
+#define GO(T) do { int per = AggOcc<LPL, T>::ctas; if (ctas_per_sm > 0 && ctas_per_sm < per) per = ctas_per_sm; \
                    int grid = sm_count * per; if (grid > total) grid = total; \
-                   if (P.general) aggregate_kernel<kLPL, T, false, true, FOLD><<<grid, block, kSmemGen, st>>>(P); \
-                   else if (scaled) aggregate_kernel<kLPL, T, true, false, FOLD><<<grid, block, kSmem, st>>>(P); \
-                   else aggregate_kernel<kLPL, T, false, false, FOLD><<<grid, block, kSmem, st>>>(P); } while (0)
+                   if (P.general) aggregate_kernel<LPL, T, false, true, FOLD><<<grid, block, smem_gen, st>>>(P); \
+                   else if (scaled) aggregate_kernel<LPL, T, true, false, FOLD><<<grid, block, smem, st>>>(P); \
+                   else aggregate_kernel<LPL, T, false, false, FOLD><<<grid, block, smem, st>>>(P); } while (0)
     switch (tsgm) {
     case 1: GO(1); break;
     case 2: GO(2); break;
@@ -47,14 +48,8 @@ template <bool FOLD> static int launch_lpl(int tsgm, const AggArgs<FOLD> &P, int
 #undef GO
     return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }
-template <> int agg_launch_lpl<kLPL>(int tsgm, const AggParams &P, int sm_count, cudaStream_t st, int ctas_per_sm)
-{
-    return launch_lpl<false>(tsgm, P, sm_count, st, ctas_per_sm);
-}
-template <> int agg_fold_launch_lpl<kLPL>(int tsgm, const AggFoldParams &P, int sm_count, cudaStream_t st)
-{
-    return launch_lpl<true>(tsgm, P, sm_count, st, 0);
-}
+template int agg_launch_lpl<kLPL, false>(int, const AggParams &, int, cudaStream_t, int);
+template int agg_launch_lpl<kLPL, true>(int, const AggFoldParams &, int, cudaStream_t, int);
 
 }  // namespace s2pb
 static_assert(s2pb::AggSmem<S2PB_LPL, false>::bytes <= 227 * 1024 && s2pb::AggSmem<S2PB_LPL, true>::bytes <= 227 * 1024,

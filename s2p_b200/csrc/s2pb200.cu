@@ -480,97 +480,56 @@ static void fill_pass(PassDesc &pd, int pass, int w, int h)
 // (mgm_costvolume.cc:63-72 allocates one vector per pixel of its own length).  Both flavours: census codes and float costs.
 static bool wide_slab(int LPL) { return 32 * LPL > 512; }
 
-// Enqueue the 8-pass aggregation of `nviews` views of slot s in ONE persistent launch.
+// Enqueue the MGM aggregation of `nviews` views of slot s, from view first_view, on stream st.  The resident layout: ONE persistent
+// launch carrying the ndir passes of the views.  The folded layout (s.folded): ndir launches in pass order, launch p carrying pass p
+// of the views; each adds its pass into the views' S, so the order of the launches is the order of the sum.  Each pass has its own
+// progress counters, reset once; the item queue is reset before every launch.
 // general: the float-cost flavour; wgt[vi] = that view's weight image or nullptr (general only)
 // gminv: label of slot 0 per view (read by the chunk-skipping kernel only)
+// ctas_per_sm > 0 caps the persistent CTAs per SM of a resident launch (agg_launch); the folded launches take no cap
 static int launch_aggregate(s2pb_ctx *ctx, Slot &s, int nviews, int w, int h, int LPL, float P1, float P2, int ndir, int tsgm,
                             const float *lut, cudaStream_t st, bool general = false, const float *const *wgt = nullptr,
                             const int *gminv = nullptr, int first_view = 0, int ctas_per_sm = 0)
 {
-    AggParams P;
-    memset(&P, 0, sizeof P);
-    int mb = max_bands(w, h);
-    P.nPV = 0; P.maxBands = 0;
-    for (int vi = first_view; vi < first_view + nviews; vi++) {
-        CK(cudaMemsetAsync(s.v[vi].progress, 0, (size_t)kMaxPasses * mb * 4, st));
-        for (int p = 0; p < ndir; p++) {
-            PassDesc &pd = P.pv[P.nPV++];
-            fill_pass(pd, p, w, h);
-            pd.C = s.v[vi].C; pd.L = s.v[vi].L[p]; pd.Lmin = s.v[vi].Lmin[p];
-            pd.W = (general && wgt) ? wgt[vi] : nullptr;
-            pd.progress = s.v[vi].progress + (size_t)p * mb;
-            if (pd.nBands > P.maxBands) P.maxBands = pd.nBands;
-        }
-    }
+    const int mb = max_bands(w, h), sm = ctx->sm_count;
     int *counter = s.next_item + 16 * first_view;          // two launches may be in flight at once: one work counter each
-    P.P1 = P1; P.P2 = P2; P.next_item = counter; P.abort_flag = ctx->abort_flag; P.lut = general ? nullptr : lut;
-    P.general = general ? 1 : 0;
-    CK(cudaMemsetAsync(counter, 0, 4, st));
-    int r;
-    if (wide_slab(LPL)) {
-        ChunkedParams Q;
-        memset(&Q, 0, sizeof Q);
-        Q.A = P;
-        Q.DP = 32 * LPL;
-        int q = 0;
-        for (int vi = first_view; vi < first_view + nviews; vi++)
-            for (int p = 0; p < ndir; p++, q++) { Q.lo[q] = s.v[vi].lo; Q.hi[q] = s.v[vi].hi; Q.gmin[q] = gminv[vi]; }
-        r = agg_chunked_launch(tsgm, Q, ctx->sm_count, st);
-    } else {
-        r = agg_launch(LPL, tsgm, P, ctx->sm_count, st, ctas_per_sm);
-    }
-    if (r == -2)
-        return fail(S2PB_ERR_UNSUPPORTED, "no %s aggregation kernel serves a slab of %d slots with TSGM %d%s",
-                    wide_slab(LPL) ? "chunk-skipping" : "register-resident", 32 * LPL, tsgm, general ? " (float costs)" : "");
-    if (r != 0) return fail(S2PB_ERR_CUDA, "aggregation launch failed: %s", cudaGetErrorString(cudaGetLastError()));
-    ctx->launches++;
-    return S2PB_OK;
-}
-
-// The same aggregation in the folded layout: one launch per pass index, in pass order on stream st, each carrying pass p of the
-// `nviews` views; every launch adds its pass into the views' S, so the order of the launches is the order of the sum.  The
-// item queue is reset before every launch; each pass has its own progress counters, reset once.
-static int launch_aggregate_folded(s2pb_ctx *ctx, Slot &s, int nviews, int w, int h, int LPL, float P1, float P2, int ndir,
-                                   int tsgm, const float *lut, cudaStream_t st, bool general, const float *const *wgt,
-                                   const int *gminv, int first_view)
-{
-    const int mb = max_bands(w, h);
-    int *counter = s.next_item + 16 * first_view;
     for (int vi = first_view; vi < first_view + nviews; vi++) CK(cudaMemsetAsync(s.v[vi].progress, 0, (size_t)kMaxPasses * mb * 4, st));
-    for (int p = 0; p < ndir; p++) {
-        ChunkedFoldParams Q;                  // (its AggFoldParams part is what the register-resident kernel takes)
-        AggFoldParams F;
-        memset(&Q, 0, sizeof Q);
+    const int passes = s.folded ? 1 : ndir;                // per launch
+    for (int p0 = 0; p0 < ndir; p0 += passes) {
+        AggFoldParams F;                      // a resident launch takes its AggParams part,
+        ChunkedFoldParams Q;                  // and a resident chunk-skipping one this one's ChunkedParams part
         memset(&F, 0, sizeof F);
+        memset(&Q, 0, sizeof Q);
         AggParams &P = F;
-        for (int vi = first_view; vi < first_view + nviews; vi++) {
-            const int q = P.nPV++;
-            PassDesc &pd = P.pv[q];
-            fill_pass(pd, p, w, h);
-            pd.C = s.v[vi].C; pd.L = nullptr; pd.Lmin = s.v[vi].Lmin[p];
-            pd.W = (general && wgt) ? wgt[vi] : nullptr;
-            pd.progress = s.v[vi].progress + (size_t)p * mb;
-            if (pd.nBands > P.maxBands) P.maxBands = pd.nBands;
-            F.fv[q] = FoldView{s.v[vi].S, s.v[vi].Lb, s.v[vi].am[p]};
-            Q.lo[q] = s.v[vi].lo; Q.hi[q] = s.v[vi].hi; Q.gmin[q] = gminv ? gminv[vi] : 0;
-        }
+        for (int vi = first_view; vi < first_view + nviews; vi++)
+            for (int p = p0; p < p0 + passes; p++) {
+                // slot_layout leaves null what the other layout holds: L_p in the folded layout, the FoldView in the resident one
+                const int q = P.nPV++;
+                PassDesc &pd = P.pv[q];
+                fill_pass(pd, p, w, h);
+                pd.C = s.v[vi].C; pd.L = s.v[vi].L[p]; pd.Lmin = s.v[vi].Lmin[p];
+                pd.W = (general && wgt) ? wgt[vi] : nullptr;
+                pd.progress = s.v[vi].progress + (size_t)p * mb;
+                if (pd.nBands > P.maxBands) P.maxBands = pd.nBands;
+                Q.fv[q] = F.fv[q] = FoldView{s.v[vi].S, s.v[vi].Lb, s.v[vi].am[p]};
+                Q.lo[q] = s.v[vi].lo; Q.hi[q] = s.v[vi].hi; Q.gmin[q] = gminv ? gminv[vi] : 0;
+            }
         P.P1 = P1; P.P2 = P2; P.next_item = counter; P.abort_flag = ctx->abort_flag; P.lut = general ? nullptr : lut;
         P.general = general ? 1 : 0;
-        F.first = p == 0;
+        Q.first = F.first = p0 == 0;
         CK(cudaMemsetAsync(counter, 0, 4, st));
         int r;
         if (wide_slab(LPL)) {
             Q.A = P;
             Q.DP = 32 * LPL;
-            for (int q = 0; q < P.nPV; q++) Q.fv[q] = F.fv[q];
-            Q.first = F.first;
-            r = agg_chunked_fold_launch(tsgm, Q, ctx->sm_count, st);
+            r = s.folded ? agg_chunked_launch<true>(tsgm, Q, sm, st) : agg_chunked_launch<false>(tsgm, Q, sm, st);
         } else {
-            r = agg_fold_launch(LPL, tsgm, F, ctx->sm_count, st);
+            r = s.folded ? agg_launch<true>(LPL, tsgm, F, sm, st) : agg_launch<false>(LPL, tsgm, F, sm, st, ctas_per_sm);
         }
         if (r == -2)
-            return fail(S2PB_ERR_UNSUPPORTED, "no folded %s aggregation kernel serves a slab of %d slots with TSGM %d%s",
-                        wide_slab(LPL) ? "chunk-skipping" : "register-resident", 32 * LPL, tsgm, general ? " (float costs)" : "");
+            return fail(S2PB_ERR_UNSUPPORTED, "no %s%s aggregation kernel serves a slab of %d slots with TSGM %d%s",
+                        s.folded ? "folded " : "", wide_slab(LPL) ? "chunk-skipping" : "register-resident", 32 * LPL, tsgm,
+                        general ? " (float costs)" : "");
         if (r != 0) return fail(S2PB_ERR_CUDA, "aggregation launch failed: %s", cudaGetErrorString(cudaGetLastError()));
         ctx->launches++;
     }
@@ -627,56 +586,49 @@ static int launch_cost(s2pb_ctx *ctx, int LPL, bool general, const CostGenParams
     return S2PB_OK;
 }
 
-template <int LPL> static void launch_wta_t(s2pb_ctx *ctx, const WtaParams &P, cudaStream_t st, bool general, bool pruned)
+template <int LPL> static void launch_wta_t(s2pb_ctx *ctx, const WtaParams &P, const FoldPlanes *F, cudaStream_t st, bool general,
+                                            bool pruned)
 {
     const int sm = ctx->sm_count;
+    if (F) {
+        if (general) launch(ctx, wta_fold_kernel<LPL, true>, sm * 16, kWtaThreads, 0, st, P, *F);
+        else launch(ctx, wta_fold_kernel<LPL, false>, sm * 16, kWtaThreads, 0, st, P, *F);
+        return;
+    }
     if constexpr (wta_pruned_width(LPL))
         if (pruned) { launch(ctx, wta_pruned_kernel<LPL>, sm * 16, kWtaThreads, 0, st, P); return; }
     if (general) launch(ctx, wta_kernel<LPL, true>, sm * 16, kWtaThreads, 0, st, P);
     else launch(ctx, wta_kernel<LPL, false>, sm * 16, kWtaThreads, 0, st, P);
 }
-// The WTA of one view.  A wide slab without a dense S: wta_chunked_kernel.  The census flavour's eight-pass WTA without a dense
-// S or PKR output, on the widths wta_pruned_kernel serves: that kernel, which reads only the labels that can still win, unless
-// the context was created with S2PB_WTA_PRUNE=0 (s2pb_ctx::wta_prune).  Everything else: wta_kernel.
-static int launch_wta(s2pb_ctx *ctx, int LPL, const WtaParams &P, cudaStream_t st, bool general = false)
-{
-    const int sm = ctx->sm_count;
-    int rc = S2PB_OK;
-    if (P.S == nullptr && wide_slab(LPL)) {
-        const int DP = 32 * LPL;
-        const size_t smem = (size_t)(kWtaThreads / 32) * DP * sizeof(float);
-        if (general) launch(ctx, wta_chunked_kernel<true>, sm * 16, kWtaThreads, smem, st, P, DP, FoldPlanes{});
-        else launch(ctx, wta_chunked_kernel<false>, sm * 16, kWtaThreads, smem, st, P, DP, FoldPlanes{});
-    } else {
-        const bool pruned = ctx->wta_prune && !general && P.ndir == kMaxPasses && P.S == nullptr && P.pkr == nullptr &&
-                            wta_pruned_width(LPL);
-        rc = with_lpl(LPL, [&](auto k) { constexpr int K = decltype(k)::value; launch_wta_t<K>(ctx, P, st, general, pruned); });
-    }
-    if (rc != S2PB_OK) return rc;
-    CK(cudaGetLastError());
-    return S2PB_OK;
-}
-
-// The WTA of one view in the folded layout (wta_fold_kernel, or its chunk-skipping counterpart on a wide slab): S and the
-// arg-minimum planes of the view instead of its pass volumes.  No dense S output (the stage entry points run resident).
-static int launch_wta_folded(s2pb_ctx *ctx, int LPL, const WtaParams &P, const ViewWS &v, cudaStream_t st, bool general)
+// The WTA of view vi of slot s.  A wide slab without a dense S: wta_chunked_kernel.  In the folded layout, S and the arg-minimum
+// planes of the view instead of its pass volumes: wta_fold_kernel, or wta_chunked_kernel's FOLD instantiation on a wide slab; no
+// dense S output (the stage entry points run resident).  In the resident layout, the census flavour's eight-pass WTA without a
+// dense S or PKR output, on the widths wta_pruned_kernel serves: that kernel, which reads only the labels that can still win,
+// unless the context was created with S2PB_WTA_PRUNE=0 (s2pb_ctx::wta_prune).  Everything else: wta_kernel.
+static int launch_wta(s2pb_ctx *ctx, const Slot &s, int vi, int LPL, const WtaParams &P, cudaStream_t st, bool general)
 {
     const int sm = ctx->sm_count;
     FoldPlanes F;
     memset(&F, 0, sizeof F);
-    F.S = v.S;
-    for (int d = 0; d < kMaxPasses; d++) F.am[d] = v.am[d];
+    if (s.folded) {
+        F.S = s.v[vi].S;
+        for (int d = 0; d < kMaxPasses; d++) F.am[d] = s.v[vi].am[d];
+    }
     int rc = S2PB_OK;
-    if (wide_slab(LPL)) {
+    if (P.S == nullptr && wide_slab(LPL)) {
         const int DP = 32 * LPL;
         const size_t smem = (size_t)(kWtaThreads / 32) * DP * sizeof(float);
-        if (general) launch(ctx, wta_chunked_kernel<true, true>, sm * 16, kWtaThreads, smem, st, P, DP, F);
-        else launch(ctx, wta_chunked_kernel<false, true>, sm * 16, kWtaThreads, smem, st, P, DP, F);
+        auto go = [&](auto kernel) { launch(ctx, kernel, sm * 16, kWtaThreads, smem, st, P, DP, F); };
+        if (s.folded && general) go(wta_chunked_kernel<true, true>);
+        else if (s.folded) go(wta_chunked_kernel<false, true>);
+        else if (general) go(wta_chunked_kernel<true>);
+        else go(wta_chunked_kernel<false>);
     } else {
+        const bool pruned = ctx->wta_prune && !general && P.ndir == kMaxPasses && P.S == nullptr && P.pkr == nullptr &&
+                            wta_pruned_width(LPL);
         rc = with_lpl(LPL, [&](auto k) {
             constexpr int K = decltype(k)::value;
-            if (general) launch(ctx, wta_fold_kernel<K, true>, sm * 16, kWtaThreads, 0, st, P, F);
-            else launch(ctx, wta_fold_kernel<K, false>, sm * 16, kWtaThreads, 0, st, P, F);
+            launch_wta_t<K>(ctx, P, s.folded ? &F : nullptr, st, general, pruned);
         });
     }
     if (rc != S2PB_OK) return rc;
@@ -931,24 +883,11 @@ static int mgm_call(s2pb_ctx *ctx, Slot &s, int w, int h, const float *const img
     }
     if (timed) CK(cudaEventRecord(s.ev[2], st));
     TRACE(st, "  census + cost");
-    // ---- 8-pass MGM of both views (mgm_multiscale.cc:194-202: P1 / ZOOMFACTOR) in one persistent launch, or two when the
-    // views' slabs differ in width
+    // ---- 8-pass MGM of both views (mgm_multiscale.cc:194-202: P1 / ZOOMFACTOR) in one launch_aggregate, or two when the views'
+    // slabs differ in width; in the folded layout (slot_ensure) each is a launch per pass
     const float P1 = p->P1 / (float)zoom;
-    if (s.folded) {
-        // the folded layout (slot_ensure): one launch per pass, in pass order; the views side by side as below when their slabs
-        // differ in width
-        ctx->folded_calls++;
-        if (LPLv[0] == LPLv[1]) {
-            rc = launch_aggregate_folded(ctx, s, 2, w, h, LPLv[0], P1, p->P2, p->ndir, p->tsgm, lut, st, general, wgt, gminv, 0);
-        } else {
-            CK(cudaEventRecord(s.fork, st));
-            CK(cudaStreamWaitEvent(s.stream2, s.fork, 0));
-            rc = launch_aggregate_folded(ctx, s, 1, w, h, LPLv[0], P1, p->P2, p->ndir, p->tsgm, lut, st, general, wgt, gminv, 0);
-            if (rc == S2PB_OK) rc = launch_aggregate_folded(ctx, s, 1, w, h, LPLv[1], P1, p->P2, p->ndir, p->tsgm, lut, s.stream2, general, wgt, gminv, 1);
-            CK(cudaEventRecord(s.join, s.stream2));
-            CK(cudaStreamWaitEvent(st, s.join, 0));
-        }
-    } else if (LPLv[0] == LPLv[1]) {
+    if (s.folded) ctx->folded_calls++;
+    if (LPLv[0] == LPLv[1]) {
         // With another tile's aggregation queued or running (tiles in flight) the launch takes one CTA per SM instead of two, so
         // two tiles' aggregations share the SMs: a pass is a chain of bands, two CTAs per SM on 16 pass-views run it twice as
         // many bands deep as one CTA per SM does, and a good part of each launch is the chain filling and draining.  (This
@@ -974,7 +913,7 @@ static int mgm_call(s2pb_ctx *ctx, Slot &s, int w, int h, const float *const img
         fill_wta(W, s.v[vi], p->ndir, gminv[vi], p, lut, npix);
         W.inv_zoom_div = (float)zoom;
         W.pkr = ctx->pkr_dst[vi];
-        rc = s.folded ? launch_wta_folded(ctx, LPLv[vi], W, s.v[vi], st, general) : launch_wta(ctx, LPLv[vi], W, st, general);
+        rc = launch_wta(ctx, s, vi, LPLv[vi], W, st, general);
         if (rc != S2PB_OK) return rc;
     }
     if (timed) CK(cudaEventRecord(s.ev[4], st));
@@ -1615,7 +1554,7 @@ static int stage_aggregate(s2pb_ctx *ctx, const float *C, const int32_t *lo, con
     fill_wta(W, s.v[0], ndir, gmin, &prm, nullptr, npix);
     W.lo = dlo; W.hi = dhi;
     W.S = dS; W.Dout = D;
-    rc = launch_wta(ctx, LPL, W, L.st, general);
+    rc = launch_wta(ctx, s, 0, LPL, W, L.st, general);
     if (rc != S2PB_OK) return rc;
     L.download(disp, s.v[0].disp, npix * 4);
     if (cost) L.download(cost, s.v[0].cost, npix * 4);
