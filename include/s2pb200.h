@@ -141,9 +141,12 @@ int s2pb_mgm_pkr(s2pb_ctx *ctx, const float *im1, const float *im2, int w, int h
                  float *pkr_left, float *pkr_right);
 
 /* Same, device pointers on both sides, enqueued on `stream` (a cudaStream_t
- * passed as void*, NULL = the context's own stream) and NOT synchronised when
+ * passed as void*, NULL = the slot's own stream) and NOT synchronised when
  * timeout_ms <= 0.  `slot` selects one of the context's workspaces
- * (0 <= slot < s2pb_num_slots) so that several tiles can be in flight.
+ * (0 <= slot < s2pb_num_slots) so that several tiles can be in flight.  A slot
+ * owns its workspace, its streams and its abort word; a call that exceeds its
+ * timeout raises only its own slot's abort word and waits for its stream and
+ * the slot's streams, so calls on other slots are not disturbed.
  * nodata_hint: bit 1 = the secondary image may hold NaN pixels (the reference
  * then gives them the label range [dmin, dmin+1], main_mgm.cc:214-216, which can
  * widen the right view's volume); 0 = neither image holds NaN; < 0 = unknown, the
@@ -158,7 +161,9 @@ int s2pb_mgm_device(s2pb_ctx *ctx, int slot, const float *d_im1, const float *d_
  * Arrays of n host pointers.  For the multi-scale algorithms (scales >= 0), which read a
  * label hull back at every pyramid level, the tiles are driven by one host thread per
  * workspace inside the call (at most four); a context may also be used from several
- * caller threads as long as each uses its own slot. */
+ * caller threads as long as each uses its own slot.  The timeout is the per-tile
+ * timeout_ms times n for the whole batch; on any error or timeout every slot is
+ * aborted and drained before the call returns. */
 int s2pb_mgm_batch(s2pb_ctx *ctx, int n, const float *const *im1, const float *const *im2,
                    int w, int h, int dmin, int dmax, const s2pb_mgm_params *p,
                    float *const *disp, float *const *conf, uint8_t *const *mask);

@@ -10,7 +10,6 @@
 #include <cuda_runtime.h>
 #include <algorithm>
 #include <atomic>
-#include <chrono>
 #include <list>
 #include <mutex>
 #include <string>
@@ -70,6 +69,7 @@ struct Slot {
     cudaEvent_t fork = nullptr, join = nullptr;
     cudaEvent_t ev[S2PB_T_COUNT + 1] = {};
     cudaEvent_t done = nullptr;
+    int *abort = nullptr;         // this slot's word of s2pb_ctx::abort_words: a timeout of a call on this slot raises it
     bool timed = false;
     bool direct_out = false;      // the last host-API call wrote its results straight into the caller's pinned buffers
 };
@@ -79,17 +79,12 @@ struct s2pb_ctx {
     bool wta_prune = true;         // S2PB_WTA_PRUNE (read when the context is created): 0 wta_kernel for every shape, the
                                    // same-device reference of wta_pruned_kernel (DESIGN.md 3.2); unset or any other value prunes
     std::vector<Slot> slots;
-    int *abort_flag = nullptr;     // pinned + mapped: the host raises it on timeout
-    int *scratch_flag = nullptr;   // pinned + mapped: device -> host one-word answers
-    int *d_scratch = nullptr;      // 64 words of device memory (hull accumulators of mgm_multi)
+    // pinned + mapped, one word per slot (Slot::abort; at most 64 slots): the persistent aggregation kernels of a slot stop
+    // waiting on band hand-offs while its word is raised, so a timed-out call drains without touching other slots' calls
+    int *abort_words = nullptr;
     std::atomic<long long> launches{0};   // (mgm_multi tiles of a batch are enqueued from several host threads)
     size_t ws_limit = 0;                  // s2pb_set_workspace_limit: bytes per workspace, 0 = none
     std::atomic<long long> folded_calls{0};   // mgm_calls that ran in the folded layout (s2pb_folded_calls)
-    // destination of the PKR images of s2pb_mgm_pkr (device, per view), or null: every mgm_call writes them, the last one stays
-    float *pkr_dst[2] = {nullptr, nullptr};
-    // deadline of the matcher call in flight (timeout_ms counted from the API entry; has_deadline = false: none)
-    std::chrono::steady_clock::time_point deadline;
-    bool has_deadline = false;
     // DCT coefficient tables of the matched image's round trip, one entry per image width (dct_tables)
     struct DctTab { int n; double *T10, *T01, *TR01, *mc, *ms; };
     std::list<DctTab> dct;          // a list: entries stay put while other host threads hold pointers to them

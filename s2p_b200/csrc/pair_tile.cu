@@ -1,7 +1,7 @@
-// pair_tile.cu -- one pair of a tile from its source crops on, in one call: rectify_pair's two warps, the matcher and its
-// rejection mask and masking.erosion chained on one stream (pair_match), then, for a two-view tile, disparity_to_ply down to
-// the records of cloud.ply, or, for a pair of a tri-stereo tile, disparity_to_height down to the pair's height map; the
-// intermediates stay on the device (s2p/__init__.py:102-318).
+// pair_tile.cu -- one pair of a tile from its source crops on, in one call: rectify_pair's two warps and the matcher with its
+// rejection mask chained on one stream (rectify_and_match, all of s2pb_rectify_match), then masking.erosion (pair_match) and,
+// for a two-view tile, disparity_to_ply down to the records of cloud.ply, or, for a pair of a tri-stereo tile,
+// disparity_to_height down to the pair's height map; the intermediates stay on the device (s2p/__init__.py:102-318).
 #include "host.h"
 
 // the eroded 0/1 mask as the float32 image disparity_to_ply hands to the triangulation (a PNG read back as uint8, then float32)
@@ -28,25 +28,27 @@ static int pair_match_args_ok(const s2pb_pair_tile *t, const float *conf, const 
     return S2PB_OK;
 }
 
-// The device results of the front half of a pair tile that the back halves read (w*h each, scratch of the call)
+// The device results of a pair's front half (w*h each, scratch of the call)
 struct PairMatch {
     const float *rect1;       // the rectified reference
     const float *disp, *conf; // the disparity and, with MGM, its confidence
-    const float *msk;         // the eroded 0/1 mask as float32
+    uint8_t *mask;            // the rejection mask
+    const float *dispR;       // MGM's right disparity, when asked for
+    const float *msk;         // pair_match: the eroded 0/1 mask as float32
 };
 
-// rectify_pair's two warps, the matcher and its rejection mask, and masking.erosion, on L's stream: the buffers come from L,
-// the intermediates named by non-null host pointers are copied back (in flight on L.st), the matcher waits for its stream
-static int pair_match(s2pb_ctx *ctx, HostCall &L, const s2pb_pair_tile *t, float *rect1, float *rect2, float *disp, float *conf,
-                      uint8_t *mask, float *disp_right, PairMatch *m)
+// rectify_pair's two warps and the matcher (t->matcher) with its rejection mask, on L's stream: the buffers come from L, the
+// rectified pair is copied back when rect1 / rect2 are not null (in flight on L.st), and MGM waits for its stream through its
+// timeout.  want_right: MGM's right disparity.
+static int rectify_and_match(s2pb_ctx *ctx, HostCall &L, const s2pb_pair_tile *t, float *rect1, float *rect2, bool want_right,
+                             PairMatch *m)
 {
     const int w = t->w, h = t->h;
     const size_t npix = (size_t)w * h;
-    const bool mgm = t->matcher == S2PB_MATCHER_MGM, erode = t->erode_radius != 0.f;
+    const bool mgm = t->matcher == S2PB_MATCHER_MGM;
     float *d_r1 = L.take<float>(npix * 4), *d_r2 = L.take<float>(npix * 4), *d_disp = L.take<float>(npix * 4);
-    float *d_conf = mgm ? L.take<float>(npix * 4) : nullptr, *d_dispR = disp_right ? L.take<float>(npix * 4) : nullptr;
-    uint8_t *d_mask = L.take<uint8_t>(npix), *d_eroded = erode ? L.take<uint8_t>(npix) : d_mask;
-    float *d_msk = L.take<float>(npix * 4);
+    float *d_conf = mgm ? L.take<float>(npix * 4) : nullptr, *d_dispR = want_right ? L.take<float>(npix * 4) : nullptr;
+    uint8_t *d_mask = L.take<uint8_t>(npix);
     const float *d_wl = t->wl ? L.upload(t->wl, npix * 4) : nullptr, *d_wr = t->wr ? L.upload(t->wr, npix * 4) : nullptr;
     if (int rc = L.error()) return rc;
 
@@ -56,7 +58,7 @@ static int pair_match(s2pb_ctx *ctx, HostCall &L, const s2pb_pair_tile *t, float
     if (rect1) L.download(rect1, d_r1, npix * 4);
     if (rect2) L.download(rect2, d_r2, npix * 4);
 
-    // stereo_matching: the matcher and its rejection mask, then the erosion of the mask
+    // stereo_matching: the matcher and its rejection mask
     if (mgm) {
         if (int rc = mgm_match_device(ctx, L.st, d_r1, d_r2, w, h, t->dmin, t->dmax, &t->mgm, d_wl, d_wr, d_disp, d_conf, d_mask,
                                       d_dispR))
@@ -64,14 +66,57 @@ static int pair_match(s2pb_ctx *ctx, HostCall &L, const s2pb_pair_tile *t, float
     } else if (int rc = sgbm_enqueue(ctx, L, d_r1, d_r2, w, h, t->dmin, t->dmax, &t->sgbm, d_disp, d_mask)) {
         return rc;
     }
-    if (erode) launch_erode_mask(ctx, d_mask, d_eroded, w, h, t->erode_radius, L.st);
+    m->rect1 = d_r1; m->disp = d_disp; m->conf = d_conf; m->mask = d_mask; m->dispR = d_dispR; m->msk = nullptr;
+    return S2PB_OK;
+}
+
+// Steps 3 and 4 of a tile in one call (s2p/__init__.py:147-155 rectify_pair's two warps, :184-190 compute_disparity_map): both
+// images are warped straight into the matcher's device inputs and matched there; the rectified pair never travels through
+// files or host memory unless the caller asks for a copy (rect1 / rect2).
+extern "C" int s2pb_rectify_match(s2pb_ctx *ctx, const float *src1, int sw1, int sh1, const double H1[9],
+                                  const float *src2, int sw2, int sh2, const double H2[9], int w, int h, int dmin, int dmax,
+                                  const s2pb_mgm_params *p, float *rect1, float *rect2, float *disp, float *conf, uint8_t *mask,
+                                  float *disp_right)
+{
+    if (!ctx || !src1 || !src2 || !H1 || !H2 || !p || !disp || !conf || sw1 < 1 || sh1 < 1 || sw2 < 1 || sh2 < 1 ||
+        w < 1 || h < 1)
+        return fail(S2PB_ERR_ARG, "bad argument");
+    s2pb_pair_tile t = {};
+    t.src1 = src1; t.sw1 = sw1; t.sh1 = sh1; std::copy(H1, H1 + 9, t.H1);
+    t.src2 = src2; t.sw2 = sw2; t.sh2 = sh2; std::copy(H2, H2 + 9, t.H2);
+    t.w = w; t.h = h; t.dmin = dmin; t.dmax = dmax;
+    t.matcher = S2PB_MATCHER_MGM; t.mgm = *p;
+    const size_t npix = (size_t)w * h;
+    HostCall L(ctx, "the rectified pair");
+    PairMatch m;
+    if (int rc = rectify_and_match(ctx, L, &t, rect1, rect2, disp_right != nullptr, &m)) return rc;
+    L.download(disp, m.disp, npix * 4);
+    L.download(conf, m.conf, npix * 4);
+    if (mask) L.download(mask, m.mask, npix);
+    if (disp_right) L.download(disp_right, m.dispR, npix * 4);
+    return L.finish();
+}
+
+// rectify_and_match, then masking.erosion of the mask and its float32 copy (m->msk): the intermediates named by non-null host
+// pointers are copied back (in flight on L.st)
+static int pair_match(s2pb_ctx *ctx, HostCall &L, const s2pb_pair_tile *t, float *rect1, float *rect2, float *disp, float *conf,
+                      uint8_t *mask, float *disp_right, PairMatch *m)
+{
+    const int w = t->w, h = t->h;
+    const size_t npix = (size_t)w * h;
+    const bool erode = t->erode_radius != 0.f;
+    if (int rc = rectify_and_match(ctx, L, t, rect1, rect2, disp_right != nullptr, m)) return rc;
+    uint8_t *d_eroded = erode ? L.take<uint8_t>(npix) : m->mask;
+    float *d_msk = L.take<float>(npix * 4);
+    if (int rc = L.error()) return rc;
+    if (erode) launch_erode_mask(ctx, m->mask, d_eroded, w, h, t->erode_radius, L.st);
     launch(ctx, mask_to_float_kernel, (unsigned)((npix + 255) / 256), 256, 0, L.st, d_eroded, d_msk, npix);
     CK(cudaGetLastError());
-    if (disp) L.download(disp, d_disp, npix * 4);
-    if (conf) L.download(conf, d_conf, npix * 4);
+    if (disp) L.download(disp, m->disp, npix * 4);
+    if (conf) L.download(conf, m->conf, npix * 4);
     if (mask) L.download(mask, d_eroded, npix);
-    if (disp_right) L.download(disp_right, d_dispR, npix * 4);
-    m->rect1 = d_r1; m->disp = d_disp; m->conf = d_conf; m->msk = d_msk;
+    if (disp_right) L.download(disp_right, m->dispR, npix * 4);
+    m->msk = d_msk;
     return S2PB_OK;
 }
 

@@ -12,11 +12,13 @@
 #include "agg_dispatch.h"
 #include "agg_chunked.cuh"
 
+#include <chrono>
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
 #include <cstdlib>
+#include <optional>
 #include <thread>
 #include <type_traits>
 
@@ -193,6 +195,7 @@ static int slot_host_ensure(Slot &s, size_t npix)
 
 static int slot_init(s2pb_ctx *ctx, Slot &s)
 {
+    s.abort = ctx->abort_words + (&s - ctx->slots.data());
     CK(cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking));
     CK(cudaStreamCreateWithFlags(&s.stream2, cudaStreamNonBlocking));
     CK(cudaMalloc((void **)&s.d_small, 256));
@@ -231,12 +234,10 @@ extern "C" s2pb_ctx *s2pb_create(int device)
     ctx->device = device;
     ctx->sm_count = prop.multiProcessorCount;
     if (const char *e = getenv("S2PB_WTA_PRUNE")) ctx->wta_prune = atoi(e) != 0;
-    if (cudaHostAlloc((void **)&ctx->abort_flag, 16 * sizeof(int), cudaHostAllocMapped) != cudaSuccess) {
+    if (cudaHostAlloc((void **)&ctx->abort_words, 64 * sizeof(int), cudaHostAllocMapped) != cudaSuccess) {
         fail(S2PB_ERR_CUDA, "cudaHostAlloc failed"); delete ctx; return nullptr;
     }
-    ctx->scratch_flag = ctx->abort_flag + 8;
-    for (int i = 0; i < 16; i++) ctx->abort_flag[i] = 0;
-    if (cudaMalloc((void **)&ctx->d_scratch, 256) != cudaSuccess) { fail(S2PB_ERR_CUDA, "cudaMalloc failed"); delete ctx; return nullptr; }
+    for (int i = 0; i < 64; i++) ctx->abort_words[i] = 0;
     ctx->slots.reserve(64);
     ctx->slots.resize(1);
     if (slot_init(ctx, ctx->slots[0]) != S2PB_OK) { delete ctx; return nullptr; }
@@ -271,8 +272,7 @@ extern "C" void s2pb_destroy(s2pb_ctx *ctx)
     }
     for (auto &b : ctx->pool) cudaFree(b.p);
     for (auto &t : ctx->dct) for (double *q : {t.T10, t.T01, t.TR01, t.mc, t.ms}) if (q) cudaFree(q);
-    if (ctx->abort_flag) cudaFreeHost(ctx->abort_flag);
-    if (ctx->d_scratch) cudaFree(ctx->d_scratch);
+    if (ctx->abort_words) cudaFreeHost(ctx->abort_words);
     delete ctx;
 }
 
@@ -325,33 +325,49 @@ static int ensure_slots(s2pb_ctx *ctx, int nslots)
     return S2PB_OK;
 }
 
-// ------------------------------------------------------------------ timeouts
+// ------------------------------------------------------------------ matcher calls and timeouts
+
+using Deadline = std::optional<std::chrono::steady_clock::time_point>;
+
+// One call into the matcher: what its entry point decides once and every stage of the call reads.  Calls on different slots
+// may run at once from different host threads, so nothing of a call is kept on the context.
+struct MatchCall {
+    Slot &s;                                   // the workspace
+    cudaStream_t st;                           // the stream the call is enqueued on: the slot's, or the caller's
+    Deadline deadline;                         // none: the call waits without a timeout
+    const float *wl = nullptr, *wr = nullptr;  // device weight images (-wl / -wr) at full resolution, both or neither
+    float *pkr[2] = {nullptr, nullptr};        // device destinations of the PKR images of the two views, or none
+};
 
 // The timeout contract (timeout_ms -> S2PB_ERR_TIMEOUT -> subprocess.TimeoutExpired upstream) counts from the API
 // entry: every host-side wait of a matcher call goes through sync_or_timeout, also the per-level read-backs of mgm_multi.
-static void set_deadline(s2pb_ctx *ctx, long long timeout_ms)
+static Deadline deadline_after(long long timeout_ms)
 {
-    ctx->has_deadline = timeout_ms > 0;
-    if (ctx->has_deadline) ctx->deadline = std::chrono::steady_clock::now() + std::chrono::milliseconds(timeout_ms);
+    if (timeout_ms <= 0) return std::nullopt;
+    return std::chrono::steady_clock::now() + std::chrono::milliseconds(timeout_ms);
 }
-// stop everything that is in flight on any slot: raise the abort flag (the persistent aggregation kernels drain), wait
-// for every slot stream -- some of them DMA into the caller's buffers -- then clear the flag
-static void drain_all(s2pb_ctx *ctx, bool abort)
+// stop everything that is in flight on any slot (s2pb_mgm_batch, which drives them all, on an error): raise every slot's abort
+// word (the persistent aggregation kernels drain), wait for every slot stream -- some of them DMA into the caller's buffers --
+// then clear the words
+static void drain_all(s2pb_ctx *ctx)
 {
-    if (abort) *(volatile int *)ctx->abort_flag = 1;
-    for (auto &s : ctx->slots) if (s.stream) cudaStreamSynchronize(s.stream);
-    if (abort) *(volatile int *)ctx->abort_flag = 0;
+    for (auto &s : ctx->slots) *(volatile int *)s.abort = 1;
+    for (auto &s : ctx->slots) { cudaStreamSynchronize(s.stream); cudaStreamSynchronize(s.stream2); }
+    for (auto &s : ctx->slots) *(volatile int *)s.abort = 0;
 }
-static int sync_or_timeout(s2pb_ctx *ctx, cudaStream_t st)
+// Wait for the call's stream.  Past the deadline, only the call's own slot is stopped: its abort word is raised until the
+// call's stream and the slot's streams have drained, so calls on other slots run on undisturbed.
+static int sync_or_timeout(const MatchCall &c)
 {
-    if (!ctx->has_deadline) { CK(cudaStreamSynchronize(st)); return S2PB_OK; }
+    if (!c.deadline) { CK(cudaStreamSynchronize(c.st)); return S2PB_OK; }
     for (;;) {
-        cudaError_t e = cudaStreamQuery(st);
+        cudaError_t e = cudaStreamQuery(c.st);
         if (e == cudaSuccess) return S2PB_OK;
         if (e != cudaErrorNotReady) return fail(S2PB_ERR_CUDA, "stream failed: %s", cudaGetErrorString(e));
-        if (std::chrono::steady_clock::now() > ctx->deadline) {
-            drain_all(ctx, true);
-            cudaStreamSynchronize(st);
+        if (std::chrono::steady_clock::now() > *c.deadline) {
+            *(volatile int *)c.s.abort = 1;
+            for (cudaStream_t q : {c.st, c.s.stream, c.s.stream2}) cudaStreamSynchronize(q);
+            *(volatile int *)c.s.abort = 0;
             return fail(S2PB_ERR_TIMEOUT, "matcher exceeded its timeout");
         }
         std::this_thread::sleep_for(std::chrono::microseconds(100));
@@ -514,7 +530,7 @@ static int launch_aggregate(s2pb_ctx *ctx, Slot &s, int nviews, int w, int h, in
                 Q.fv[q] = F.fv[q] = FoldView{s.v[vi].S, s.v[vi].Lb, s.v[vi].am[p]};
                 Q.lo[q] = s.v[vi].lo; Q.hi[q] = s.v[vi].hi; Q.gmin[q] = gminv ? gminv[vi] : 0;
             }
-        P.P1 = P1; P.P2 = P2; P.next_item = counter; P.abort_flag = ctx->abort_flag; P.lut = general ? nullptr : lut;
+        P.P1 = P1; P.P2 = P2; P.next_item = counter; P.abort_flag = s.abort; P.lut = general ? nullptr : lut;
         P.general = general ? 1 : 0;
         Q.first = F.first = p0 == 0;
         CK(cudaMemsetAsync(counter, 0, 4, st));
@@ -766,8 +782,6 @@ struct Level {
     float *dl, *dr, *conf;                 // results of this level's mgm_call
     float *wl = nullptr, *wr = nullptr;    // regularity weights of this level (-wl / -wr), or none
 };
-// device weight images at full resolution, both or neither (s2pb_mgm_weighted)
-struct MgmExtra { const float *wl = nullptr, *wr = nullptr; };
 
 static GaussTaps gauss_taps(float sigma)
 {   // mgm_multiscale.cc:66-71
@@ -817,7 +831,8 @@ static bool general_flavour(const s2pb_mgm_params *p, const float *const wgt[2])
     return p->cost != S2PB_COST_CENSUS || (wgt[0] && wgt[1]);
 }
 
-// One mgm_call (mgm_multiscale.cc:161-335) on the slot's workspace, which slot_ensure has sized for the wider slab.
+// One mgm_call (mgm_multiscale.cc:161-335) on the workspace of c's slot, which slot_ensure has sized for the wider slab, on c's
+// stream; the PKR images go to c.pkr.
 //   img:   the NaN-free images; lo / hi: each view's per-pixel label range; gminv: the label of each view's slot 0
 //   LPLv:  labels per lane of each view's slab (wide_slab: the chunk-skipping kernels)
 //   zoom:  ZOOMFACTOR, 1 or 2 (labels of half pixels: SUBPIX = 2); wgt: the views' weight images, or none
@@ -826,10 +841,11 @@ static bool general_flavour(const s2pb_mgm_params *p, const float *const wgt[2])
 //   timed (single scale): record s.ev[1..4] after the stages (s2pb_last_timings), and size the aggregation's grid by
 //   whether another slot's aggregation is in flight (other_aggregation_pending reads those events)
 // Enqueues only: no host synchronisation (except S2PB_TRACE=1).
-static int mgm_call(s2pb_ctx *ctx, Slot &s, int w, int h, const float *const img[2], short *const lo[2], short *const hi[2],
-                    const int gminv[2], const int LPLv[2], int zoom, const float *const wgt[2], const s2pb_mgm_params *p,
-                    float *outL, float *&outR, cudaStream_t st, bool timed)
+static int mgm_call(s2pb_ctx *ctx, const MatchCall &c, int w, int h, const float *const img[2], short *const lo[2],
+                    short *const hi[2], const int gminv[2], const int LPLv[2], int zoom, const float *const wgt[2],
+                    const s2pb_mgm_params *p, float *outL, float *&outR, bool timed)
 {
+    Slot &s = c.s; const cudaStream_t st = c.st;
     const bool general = general_flavour(p, wgt);
     const bool census = p->cost == S2PB_COST_CENSUS, ncc = p->cost == S2PB_COST_NCC;
     const size_t npix = (size_t)w * h;
@@ -912,7 +928,7 @@ static int mgm_call(s2pb_ctx *ctx, Slot &s, int w, int h, const float *const img
         WtaParams W;
         fill_wta(W, s.v[vi], p->ndir, gminv[vi], p, lut, npix);
         W.inv_zoom_div = (float)zoom;
-        W.pkr = ctx->pkr_dst[vi];
+        W.pkr = c.pkr[vi];
         rc = launch_wta(ctx, s, vi, LPLv[vi], W, st, general);
         if (rc != S2PB_OK) return rc;
     }
@@ -943,9 +959,12 @@ static int mgm_call(s2pb_ctx *ctx, Slot &s, int w, int h, const float *const img
 }
 
 // One mgm_call of a pyramid level: the label ranges of both views from the level's bounds, one slab for both views
-// sized by the wider hull, then the speckle filter (mgm_multiscale.cc:328-334).
-static int mgm_call_level(s2pb_ctx *ctx, Slot &s, Level &L, int zoom, const s2pb_mgm_params *p, cudaStream_t st, bool weighted)
+// sized by the wider hull, then the speckle filter (mgm_multiscale.cc:328-334).  Weighted by the level's weight maps when the
+// call has weight images.
+static int mgm_call_level(s2pb_ctx *ctx, const MatchCall &c, Level &L, int zoom, const s2pb_mgm_params *p)
 {
+    Slot &s = c.s; const cudaStream_t st = c.st;
+    const bool weighted = c.wl && c.wr;
     const int w = L.w, h = L.h, n = w * h;
     const float *wgt[2] = {weighted ? L.wl : nullptr, weighted ? L.wr : nullptr};
     const bool general = general_flavour(p, wgt);
@@ -965,7 +984,7 @@ static int mgm_call_level(s2pb_ctx *ctx, Slot &s, Level &L, int zoom, const s2pb
     CK(cudaGetLastError());
     int hull[4];
     CK(cudaMemcpyAsync(hull, d_hull, sizeof hull, cudaMemcpyDeviceToHost, st));
-    int rc = sync_or_timeout(ctx, st);
+    int rc = sync_or_timeout(c);
     if (rc != S2PB_OK) return rc;
     int gminv[2] = {hull[0], hull[2]}, gmaxv[2] = {hull[1], hull[3]};
     int D = 0;
@@ -984,7 +1003,7 @@ static int mgm_call_level(s2pb_ctx *ctx, Slot &s, Level &L, int zoom, const s2pb
     const int LPLv[2] = {LPL, LPL};
     const bool cc = p->remove_small_cc > 0;
     float *lrL = cc ? tl : L.dl, *lrR = cc ? tr : L.dr;
-    rc = mgm_call(ctx, s, w, h, img, lo, hi, gminv, LPLv, zoom, wgt, p, lrL, lrR, st, false);
+    rc = mgm_call(ctx, c, w, h, img, lo, hi, gminv, LPLv, zoom, wgt, p, lrL, lrR, false);
     if (rc != S2PB_OK) return rc;
     if (cc) {
         rc = launch_remove_small_cc(ctx, lrL, L.dl, w, h, p->remove_small_cc, 5.f, lab, area, st);   // mgm_multiscale.cc:332-333
@@ -999,13 +1018,13 @@ static int mgm_call_level(s2pb_ctx *ctx, Slot &s, Level &L, int zoom, const s2pb
 }
 
 // main() of mgm_multi (main_mgm_multi.cc:88-256) + recursive_multiscale (mgm_multiscale.cc:339-410)
-static int mgm_multi_enqueue(s2pb_ctx *ctx, Slot &s, const float *d_im1, const float *d_im2, int w, int h, int dmin, int dmax,
-                             const s2pb_mgm_params *p, float *d_disp, float *d_conf, uint8_t *d_mask, float *d_dispR, cudaStream_t st,
-                             const MgmExtra *x)
+static int mgm_multi_enqueue(s2pb_ctx *ctx, const MatchCall &call, const float *d_im1, const float *d_im2, int w, int h, int dmin,
+                             int dmax, const s2pb_mgm_params *p, float *d_disp, float *d_conf, uint8_t *d_mask, float *d_dispR)
 {
+    Slot &s = call.s; const cudaStream_t st = call.st;
     const int n = w * h;
     dim3 b2(32, 8);
-    const bool weighted = x && x->wl && x->wr;
+    const bool weighted = call.wl && call.wr;
     // pyramid shape: downsample while max > 100, min > 50 and scale < -S (mgm_multiscale.cc:362)
     std::vector<Level> lv(1);
     lv[0].w = w; lv[0].h = h;
@@ -1033,8 +1052,8 @@ static int mgm_multi_enqueue(s2pb_ctx *ctx, Slot &s, const float *d_im1, const f
         }
     }
     if (weighted) {
-        CK(cudaMemcpyAsync(lv[0].wl, x->wl, (size_t)n * 4, cudaMemcpyDeviceToDevice, st));
-        CK(cudaMemcpyAsync(lv[0].wr, x->wr, (size_t)n * 4, cudaMemcpyDeviceToDevice, st));
+        CK(cudaMemcpyAsync(lv[0].wl, call.wl, (size_t)n * 4, cudaMemcpyDeviceToDevice, st));
+        CK(cudaMemcpyAsync(lv[0].wr, call.wr, (size_t)n * 4, cudaMemcpyDeviceToDevice, st));
     }
     s.timed = false;
     // level 0: NaN -> 0, initial bounds (main_mgm_multi.cc:160-196; the sentinel for no-data is dmin in both views)
@@ -1075,7 +1094,7 @@ static int mgm_multi_enqueue(s2pb_ctx *ctx, Slot &s, const float *d_im1, const f
             CK(cudaGetLastError());
         }
         s.arena_off = arena_mark;
-        rc = mgm_call_level(ctx, s, L, 1, p, st, weighted);
+        rc = mgm_call_level(ctx, call, L, 1, p);
         if (rc != S2PB_OK) return rc;
     }
     Level &L0 = lv[0];
@@ -1088,10 +1107,9 @@ static int mgm_multi_enqueue(s2pb_ctx *ctx, Slot &s, const float *d_im1, const f
         launch(ctx, update_ranges_kernel, grid2d(w, h, b2), b2, 0, st, L0.dr, 1.f, w, h, L0.dminR, L0.dmaxR, L0.dminR, L0.dmaxR, w, h, 2.f, 4, c, d);
         L0.dminL = a; L0.dmaxL = b; L0.dminR = c; L0.dmaxR = d;
         s.arena_off = mark2;
-        float *keep[2] = {ctx->pkr_dst[0], ctx->pkr_dst[1]};          // ... and with its own img_dict: the PKR images written are the ZOOM = 1 call's
-        ctx->pkr_dst[0] = ctx->pkr_dst[1] = nullptr;
-        rc = mgm_call_level(ctx, s, L0, p->subpix, p, st, false);   // fresh `param` without the weight images (main_mgm_multi.cc:207)
-        ctx->pkr_dst[0] = keep[0]; ctx->pkr_dst[1] = keep[1];
+        MatchCall half = call;        // fresh `param` without the weight images (main_mgm_multi.cc:207), and with its own img_dict:
+        half.wl = half.wr = nullptr; half.pkr[0] = half.pkr[1] = nullptr;     // the PKR images written are the ZOOM = 1 call's
+        rc = mgm_call_level(ctx, half, L0, p->subpix, p);
         if (rc != S2PB_OK) return rc;
     }
     float *outL = d_disp;
@@ -1114,12 +1132,12 @@ static int mgm_multi_enqueue(s2pb_ctx *ctx, Slot &s, const float *d_im1, const f
 
 // ------------------------------------------------------------------ the matcher (device level)
 
-static int mgm_enqueue(s2pb_ctx *ctx, Slot &s, const float *d_im1, const float *d_im2, int w, int h, int dmin, int dmax,
-                       const s2pb_mgm_params *p, float *d_disp, float *d_conf, uint8_t *d_mask, float *d_dispR, cudaStream_t st,
-                       int nodata_hint, const MgmExtra *x = nullptr)
+static int mgm_enqueue(s2pb_ctx *ctx, const MatchCall &c, const float *d_im1, const float *d_im2, int w, int h, int dmin, int dmax,
+                       const s2pb_mgm_params *p, float *d_disp, float *d_conf, uint8_t *d_mask, float *d_dispR, int nodata_hint)
 {
-    if (p->scales >= 0) return mgm_multi_enqueue(ctx, s, d_im1, d_im2, w, h, dmin, dmax, p, d_disp, d_conf, d_mask, d_dispR, st, x);
-    const float *wgt[2] = {x ? x->wl : nullptr, x ? x->wr : nullptr};
+    if (p->scales >= 0) return mgm_multi_enqueue(ctx, c, d_im1, d_im2, w, h, dmin, dmax, p, d_disp, d_conf, d_mask, d_dispR);
+    Slot &s = c.s; const cudaStream_t st = c.st;
+    const float *wgt[2] = {c.wl, c.wr};
     const bool general = general_flavour(p, wgt);
     const size_t npix = (size_t)w * h;
     const int n = (int)npix;
@@ -1129,7 +1147,7 @@ static int mgm_enqueue(s2pb_ctx *ctx, Slot &s, const float *d_im1, const float *
         launch(ctx, has_nan_kernel, ctx->sm_count * 4, 256, 0, st, d_im2, n, flag);
         int hflag = 0;
         CK(cudaMemcpyAsync(&hflag, flag, 4, cudaMemcpyDeviceToHost, st));
-        int rs = sync_or_timeout(ctx, st);
+        int rs = sync_or_timeout(c);
         if (rs != S2PB_OK) return rs;
         nodata_hint = hflag ? 3 : 0;
     }
@@ -1154,7 +1172,7 @@ static int mgm_enqueue(s2pb_ctx *ctx, Slot &s, const float *d_im1, const float *
     const float *img[2] = {s.v[0].img, s.v[1].img};
     short *lo[2] = {s.v[0].lo, s.v[1].lo}, *hi[2] = {s.v[0].hi, s.v[1].hi};
     float *outL = d_disp, *outR = d_dispR;
-    rc = mgm_call(ctx, s, w, h, img, lo, hi, gminv, LPLv, 1, wgt, p, outL, outR, st, true);
+    rc = mgm_call(ctx, c, w, h, img, lo, hi, gminv, LPLv, 1, wgt, p, outL, outR, true);
     if (rc != S2PB_OK) return rc;
     // ---- no-data restore (main_mgm.cc:231-236), mask
     launch(ctx, nan_restore_kernel, (n + 255) / 256, 256, 0, st, outL, d_im1, n);
@@ -1178,11 +1196,10 @@ extern "C" int s2pb_mgm_device(s2pb_ctx *ctx, int slot, const float *d_im1, cons
     rc = ensure_slots(ctx, slot + 1);
     if (rc != S2PB_OK) return rc;
     Slot &s = ctx->slots[slot];
-    cudaStream_t st = stream ? (cudaStream_t)stream : s.stream;
-    set_deadline(ctx, p->timeout_ms);
-    rc = mgm_enqueue(ctx, s, d_im1, d_im2, w, h, dmin, dmax, p, d_disp, d_conf, d_mask, d_disp_right, st, nodata_hint);
+    const MatchCall c{s, stream ? (cudaStream_t)stream : s.stream, deadline_after(p->timeout_ms)};
+    rc = mgm_enqueue(ctx, c, d_im1, d_im2, w, h, dmin, dmax, p, d_disp, d_conf, d_mask, d_disp_right, nodata_hint);
     if (rc != S2PB_OK) return rc;
-    if (p->timeout_ms > 0) return sync_or_timeout(ctx, st);
+    if (c.deadline) return sync_or_timeout(c);
     return S2PB_OK;
 }
 
@@ -1195,12 +1212,13 @@ static bool is_pinned_host(const void *p)
     return a.type == cudaMemoryTypeHost;
 }
 
-// stage the inputs of one tile through pinned memory and enqueue everything on the slot's stream
-static int mgm_host_enqueue(s2pb_ctx *ctx, Slot &s, const float *im1, const float *im2, int w, int h, int dmin, int dmax,
-                            const s2pb_mgm_params *p, bool want_mask, bool want_right,
-                            float *o_disp = nullptr, float *o_conf = nullptr, uint8_t *o_mask = nullptr,
-                            const float *wl = nullptr, const float *wr = nullptr)
+// stage the inputs of one tile through pinned memory and enqueue everything on the stream of c, the slot's own; wl / wr: host
+// weight images, both or neither
+static int mgm_host_enqueue(s2pb_ctx *ctx, const MatchCall &c, const float *im1, const float *im2, int w, int h, int dmin,
+                            int dmax, const s2pb_mgm_params *p, bool want_mask, bool want_right, float *o_disp, float *o_conf,
+                            uint8_t *o_mask, const float *wl = nullptr, const float *wr = nullptr)
 {
+    Slot &s = c.s;
     size_t npix = (size_t)w * h;
     int rc = slot_host_ensure(s, npix);
     if (rc != S2PB_OK) return rc;
@@ -1221,14 +1239,14 @@ static int mgm_host_enqueue(s2pb_ctx *ctx, Slot &s, const float *im1, const floa
     if (rc != S2PB_OK) return rc;
     CK(cudaMemcpyAsync(s.d_in[0], src1, npix * 4, cudaMemcpyHostToDevice, s.stream));
     CK(cudaMemcpyAsync(s.d_in[1], src2, npix * 4, cudaMemcpyHostToDevice, s.stream));
-    MgmExtra x;
+    MatchCall cw = c;
     if (wl && wr) {        // not a hot path: plain (driver-staged) copies of the caller's weight images
         CK(cudaMemcpyAsync(s.d_w[0], wl, npix * 4, cudaMemcpyHostToDevice, s.stream));
         CK(cudaMemcpyAsync(s.d_w[1], wr, npix * 4, cudaMemcpyHostToDevice, s.stream));
-        x.wl = s.d_w[0]; x.wr = s.d_w[1];
+        cw.wl = s.d_w[0]; cw.wr = s.d_w[1];
     }
-    rc = mgm_enqueue(ctx, s, s.d_in[0], s.d_in[1], w, h, dmin, dmax, p, s.d_disp, s.d_conf, want_mask ? s.d_mask : nullptr,
-                     want_right ? s.d_dispR : nullptr, s.stream, sec_nodata ? 2 : 0, &x);
+    rc = mgm_enqueue(ctx, cw, s.d_in[0], s.d_in[1], w, h, dmin, dmax, p, s.d_disp, s.d_conf, want_mask ? s.d_mask : nullptr,
+                     want_right ? s.d_dispR : nullptr, sec_nodata ? 2 : 0);
     if (rc != S2PB_OK) return rc;
     // results go straight into the caller's buffers when those are page-locked (o_* != nullptr), else to the staging block
     s.direct_out = o_disp && o_conf && is_pinned_host(o_disp) && is_pinned_host(o_conf) && (!want_mask || (o_mask && is_pinned_host(o_mask)));
@@ -1249,31 +1267,44 @@ static void copy_staged_outputs(const Slot &s, size_t npix, float *disp, float *
     if (mask) memcpy(mask, s.h_mask, npix);
 }
 
+// s2pb_mgm, s2pb_mgm_weighted and s2pb_mgm_pkr: one tile from host buffers on slot 0.  wl / wr: host weight images or null;
+// pkr_left / pkr_right: host destinations of the PKR images, or null.
+static int mgm_host(s2pb_ctx *ctx, const float *im1, const float *im2, int w, int h, int dmin, int dmax, const s2pb_mgm_params *p,
+                    const float *wl, const float *wr, float *disp, float *conf, uint8_t *mask, float *disp_right, float *pkr_left,
+                    float *pkr_right)
+{
+    if (!ctx || !im1 || !im2 || !disp || !conf) return fail(S2PB_ERR_ARG, "null argument");
+    if ((wl == nullptr) != (wr == nullptr)) return fail(S2PB_ERR_ARG, "the weight images come in pairs (-wl and -wr)");
+    int rc = check_params(p, w, h, dmin, dmax);
+    if (rc != S2PB_OK) return rc;
+    const size_t npix = (size_t)w * h;
+    // the lease holds the device PKR images, and waits for slot 0's stream on every return: after an error nothing may still
+    // DMA into the caller's buffers
+    HostCall L(ctx, "the PKR images");
+    Slot &s = ctx->slots[0];
+    MatchCall c{s, s.stream, deadline_after(p->timeout_ms)};
+    if (pkr_left) { c.pkr[0] = L.take<float>(npix * 4); c.pkr[1] = L.take<float>(npix * 4); }
+    if ((rc = L.error()) != S2PB_OK) return rc;
+    rc = mgm_host_enqueue(ctx, c, im1, im2, w, h, dmin, dmax, p, mask != nullptr, disp_right != nullptr, disp, conf, mask, wl, wr);
+    if (rc == S2PB_OK) rc = sync_or_timeout(c);
+    if (rc != S2PB_OK) return rc;
+    copy_staged_outputs(s, npix, disp, conf, mask);
+    if (disp_right) memcpy(disp_right, s.h_dispR, npix * 4);
+    if (pkr_left) { L.download(pkr_left, c.pkr[0], npix * 4); L.download(pkr_right, c.pkr[1], npix * 4); }
+    return L.finish();
+}
+
 extern "C" int s2pb_mgm(s2pb_ctx *ctx, const float *im1, const float *im2, int w, int h, int dmin, int dmax,
                         const s2pb_mgm_params *p, float *disp, float *conf, uint8_t *mask, float *disp_right)
 {
-    return s2pb_mgm_weighted(ctx, im1, im2, w, h, dmin, dmax, p, nullptr, nullptr, disp, conf, mask, disp_right);
+    return mgm_host(ctx, im1, im2, w, h, dmin, dmax, p, nullptr, nullptr, disp, conf, mask, disp_right, nullptr, nullptr);
 }
 
 extern "C" int s2pb_mgm_weighted(s2pb_ctx *ctx, const float *im1, const float *im2, int w, int h, int dmin, int dmax,
                                  const s2pb_mgm_params *p, const float *wl, const float *wr,
                                  float *disp, float *conf, uint8_t *mask, float *disp_right)
 {
-    if (!ctx || !im1 || !im2 || !disp || !conf) return fail(S2PB_ERR_ARG, "null argument");
-    if ((wl == nullptr) != (wr == nullptr)) return fail(S2PB_ERR_ARG, "the weight images come in pairs (-wl and -wr)");
-    int rc = check_params(p, w, h, dmin, dmax);
-    if (rc != S2PB_OK) return rc;
-    CK(cudaSetDevice(ctx->device));
-    Slot &s = ctx->slots[0];
-    set_deadline(ctx, p->timeout_ms);
-    rc = mgm_host_enqueue(ctx, s, im1, im2, w, h, dmin, dmax, p, mask != nullptr, disp_right != nullptr, disp, conf, mask, wl, wr);
-    if (rc != S2PB_OK) { cudaStreamSynchronize(s.stream); return rc; }      // nothing may still DMA into the caller's buffers
-    rc = sync_or_timeout(ctx, s.stream);
-    if (rc != S2PB_OK) return rc;
-    size_t npix = (size_t)w * h;
-    copy_staged_outputs(s, npix, disp, conf, mask);
-    if (disp_right) memcpy(disp_right, s.h_dispR, npix * 4);
-    return S2PB_OK;
+    return mgm_host(ctx, im1, im2, w, h, dmin, dmax, p, wl, wr, disp, conf, mask, disp_right, nullptr, nullptr);
 }
 
 // `mgm ... -confidence_pkrL f -confidence_pkrR g` (main_mgm.cc:147,250-262; mgm_multi likewise): s2pb_mgm plus the peak-ratio
@@ -1282,18 +1313,8 @@ extern "C" int s2pb_mgm_pkr(s2pb_ctx *ctx, const float *im1, const float *im2, i
                             const s2pb_mgm_params *p, float *disp, float *conf, uint8_t *mask, float *disp_right,
                             float *pkr_left, float *pkr_right)
 {
-    if (!ctx || !pkr_left || !pkr_right) return fail(S2PB_ERR_ARG, "null argument");
-    const size_t npix = (size_t)w * h;
-    HostCall L(ctx, "the PKR images");
-    float *d0 = L.take<float>(npix * 4), *d1 = L.take<float>(npix * 4);
-    if (int rc = L.error()) return rc;
-    ctx->pkr_dst[0] = d0; ctx->pkr_dst[1] = d1;
-    int rc = s2pb_mgm_weighted(ctx, im1, im2, w, h, dmin, dmax, p, nullptr, nullptr, disp, conf, mask, disp_right);
-    ctx->pkr_dst[0] = ctx->pkr_dst[1] = nullptr;
-    if (rc != S2PB_OK) return rc;
-    L.download(pkr_left, d0, npix * 4);
-    L.download(pkr_right, d1, npix * 4);
-    return L.finish();
+    if (!pkr_left || !pkr_right) return fail(S2PB_ERR_ARG, "null argument");
+    return mgm_host(ctx, im1, im2, w, h, dmin, dmax, p, nullptr, nullptr, disp, conf, mask, disp_right, pkr_left, pkr_right);
 }
 
 extern "C" int s2pb_reserve(s2pb_ctx *ctx, int nslots, int w, int h, int nlabels)
@@ -1325,7 +1346,8 @@ extern "C" int s2pb_mgm_batch(s2pb_ctx *ctx, int n, const float *const *im1, con
     CK(cudaSetDevice(ctx->device));
     const int ns = (int)ctx->slots.size();
     const size_t npix = (size_t)w * h;
-    set_deadline(ctx, p->timeout_ms * (long long)(n > 0 ? n : 1));       // the per-tile timeout times the number of tiles
+    const Deadline deadline = deadline_after(p->timeout_ms * (long long)(n > 0 ? n : 1));   // the per-tile timeout times the number of tiles
+    auto call = [&](int si) { Slot &s = ctx->slots[si]; return MatchCall{s, s.stream, deadline}; };
     if (p->scales >= 0 && ns > 1 && n > 1) {
         // mgm_multi reads a label hull back at every pyramid level, so a tile's enqueue blocks its host thread: one thread per
         // workspace keeps several tiles in flight (their kernels overlap on the device, each on its slot's stream)
@@ -1337,39 +1359,38 @@ extern "C" int s2pb_mgm_batch(s2pb_ctx *ctx, int n, const float *const *im1, con
         for (int k = 0; k < T; k++)
             th.emplace_back([&, k]() {
                 cudaSetDevice(ctx->device);
-                Slot &s = ctx->slots[k];
+                const MatchCall c = call(k);
                 for (int t = k; t < n && !stop.load(); t += T) {
-                    int r = mgm_host_enqueue(ctx, s, im1[t], im2[t], w, h, dmin, dmax, p, mask && mask[t], false, disp[t], conf[t],
+                    int r = mgm_host_enqueue(ctx, c, im1[t], im2[t], w, h, dmin, dmax, p, mask && mask[t], false, disp[t], conf[t],
                                              mask ? mask[t] : nullptr);
-                    if (r == S2PB_OK) r = sync_or_timeout(ctx, s.stream);
+                    if (r == S2PB_OK) r = sync_or_timeout(c);
                     if (r != S2PB_OK) { codes[k] = r; errs[k] = g_err; stop.store(true); break; }
-                    copy_staged_outputs(s, npix, disp[t], conf[t], mask ? mask[t] : nullptr);
+                    copy_staged_outputs(c.s, npix, disp[t], conf[t], mask ? mask[t] : nullptr);
                 }
             });
         for (auto &t : th) t.join();
         for (int k = 0; k < T; k++)
-            if (codes[k] != S2PB_OK) { drain_all(ctx, true); g_err = errs[k]; return codes[k]; }
+            if (codes[k] != S2PB_OK) { drain_all(ctx); g_err = errs[k]; return codes[k]; }
         return S2PB_OK;
     }
     std::vector<int> inflight(ns, -1);
     auto collect = [&](int si) -> int {
-        Slot &s = ctx->slots[si];
         int t = inflight[si];
         if (t < 0) return S2PB_OK;
-        int r = sync_or_timeout(ctx, s.stream);
+        int r = sync_or_timeout(call(si));
         if (r != S2PB_OK) return r;
-        copy_staged_outputs(s, npix, disp[t], conf[t], mask ? mask[t] : nullptr);
+        copy_staged_outputs(ctx->slots[si], npix, disp[t], conf[t], mask ? mask[t] : nullptr);
         inflight[si] = -1;
         return S2PB_OK;
     };
     // on any error the other slots still have kernels and copies in flight, some of them into the caller's page-locked
     // buffers: stop and wait for all of them before returning (the caller may free its arrays right away)
-    auto bail = [&](int code) -> int { std::string keep = g_err; drain_all(ctx, true); g_err = keep; return code; };
+    auto bail = [&](int code) -> int { std::string keep = g_err; drain_all(ctx); g_err = keep; return code; };
     for (int t = 0; t < n; t++) {
         int si = t % ns;
         rc = collect(si);
         if (rc != S2PB_OK) return bail(rc);
-        rc = mgm_host_enqueue(ctx, ctx->slots[si], im1[t], im2[t], w, h, dmin, dmax, p, mask && mask[t], false, disp[t], conf[t],
+        rc = mgm_host_enqueue(ctx, call(si), im1[t], im2[t], w, h, dmin, dmax, p, mask && mask[t], false, disp[t], conf[t],
                               mask ? mask[t] : nullptr);
         if (rc != S2PB_OK) return bail(rc);
         inflight[si] = t;
@@ -1652,41 +1673,7 @@ extern "C" int s2pb_rejection_mask(s2pb_ctx *ctx, const float *disp, const float
     return L.finish();
 }
 
-// ------------------------------------------------------------------ warp (warp.cu) and match
-
-// Steps 3 and 4 of a tile in one call (s2p/__init__.py:147-155 rectify_pair's two warps, :184-190 compute_disparity_map): both
-// images are warped straight into the matcher's device inputs and matched there; the rectified pair never travels through
-// files or host memory unless the caller asks for a copy (rect1 / rect2).
-extern "C" int s2pb_rectify_match(s2pb_ctx *ctx, const float *src1, int sw1, int sh1, const double H1[9],
-                                  const float *src2, int sw2, int sh2, const double H2[9], int w, int h, int dmin, int dmax,
-                                  const s2pb_mgm_params *p, float *rect1, float *rect2, float *disp, float *conf, uint8_t *mask,
-                                  float *disp_right)
-{
-    if (!ctx || !src1 || !src2 || !H1 || !H2 || !disp || !conf || sw1 < 1 || sh1 < 1 || sw2 < 1 || sh2 < 1) return fail(S2PB_ERR_ARG, "bad argument");
-    int rc = check_params(p, w, h, dmin, dmax);
-    if (rc != S2PB_OK) return rc;
-    CK(cudaSetDevice(ctx->device));
-    Slot &s = ctx->slots[0];
-    cudaStream_t st = s.stream;
-    const size_t npix = (size_t)w * h;
-    rc = slot_io_ensure(s, npix);
-    if (rc != S2PB_OK) return rc;
-    set_deadline(ctx, p->timeout_ms);
-    ScratchLease L(ctx, st);
-    rc = warp_host_to_device(ctx, L, st, src1, sw1, sh1, H1, s.d_in[0], w, h);
-    if (rc == S2PB_OK) rc = warp_host_to_device(ctx, L, st, src2, sw2, sh2, H2, s.d_in[1], w, h);
-    if (rc != S2PB_OK) return rc;
-    if (rect1) CK(cudaMemcpyAsync(rect1, s.d_in[0], npix * 4, cudaMemcpyDeviceToHost, st));
-    if (rect2) CK(cudaMemcpyAsync(rect2, s.d_in[1], npix * 4, cudaMemcpyDeviceToHost, st));
-    rc = mgm_enqueue(ctx, s, s.d_in[0], s.d_in[1], w, h, dmin, dmax, p, s.d_disp, s.d_conf, mask ? s.d_mask : nullptr,
-                     disp_right ? s.d_dispR : nullptr, st, -1);
-    if (rc != S2PB_OK) return rc;
-    CK(cudaMemcpyAsync(disp, s.d_disp, npix * 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(conf, s.d_conf, npix * 4, cudaMemcpyDeviceToHost, st));
-    if (mask) CK(cudaMemcpyAsync(mask, s.d_mask, npix, cudaMemcpyDeviceToHost, st));
-    if (disp_right) CK(cudaMemcpyAsync(disp_right, s.d_dispR, npix * 4, cudaMemcpyDeviceToHost, st));
-    return sync_or_timeout(ctx, st);
-}
+// ------------------------------------------------------------------ the matcher of pair_tile.cu
 
 // The matcher of s2pb_mgm_weighted between device buffers on slot 0 (st is that slot's stream, as HostCall's): the deadline counts
 // from here, and the call waits for the stream through the timeout.
@@ -1695,10 +1682,8 @@ int mgm_match_device(s2pb_ctx *ctx, cudaStream_t st, const float *d_im1, const f
                      float *d_dispR)
 {
     if (int rc = check_params(p, w, h, dmin, dmax)) return rc;
-    set_deadline(ctx, p->timeout_ms);
-    MgmExtra x;
-    x.wl = d_wl; x.wr = d_wr;
-    int rc = mgm_enqueue(ctx, ctx->slots[0], d_im1, d_im2, w, h, dmin, dmax, p, d_disp, d_conf, d_mask, d_dispR, st, -1, &x);
+    const MatchCall c{ctx->slots[0], st, deadline_after(p->timeout_ms), d_wl, d_wr};
+    int rc = mgm_enqueue(ctx, c, d_im1, d_im2, w, h, dmin, dmax, p, d_disp, d_conf, d_mask, d_dispR, -1);
     if (rc != S2PB_OK) return rc;
-    return sync_or_timeout(ctx, st);
+    return sync_or_timeout(c);
 }
