@@ -259,7 +259,7 @@ typedef struct s2pb_rpc {
  * (1..60, or 0: the output is lon, lat, alt as disp_to_lonlatalt writes them) and south (non-zero: false northing
  * 10 000 000 m).  The cloud is triangulated and projected as s2pb_lonlat_to_utm projects it on the device; xyz (nx*ny*3
  * float64) and err (nx*ny float32) come back.
- * S2PB_ERR_ARG: a null pointer, a size below 1, a zone outside 0..60. */
+ * S2PB_ERR_ARG: a null pointer, a size below 1, a zone outside 0..60 (S2PB_ZONE_EGM96 aside). */
 int s2pb_disp_to_xyz(s2pb_ctx *ctx, double *xyz, float *err, const float *dispx, const float *dispy, const float *msk, int nx,
                      int ny, const float *msk_orig, int w, int h, const double ha[9], const double hb[9], const s2pb_rpc *rpca,
                      const s2pb_rpc *rpcb, const float orig_img_bounding_box[4], int zone, int south);
@@ -268,8 +268,29 @@ int s2pb_disp_to_xyz(s2pb_ctx *ctx, double *xyz, float *err, const float *dispx,
  * runs for +proj=utm (Poder / Engsager, Krueger's series to order n^6; Karney 2011), k0 = 0.9996, central meridian
  * 6 zone - 183, false easting 500 000 m.  The altitude passes through.  A point with a NaN coordinate becomes NaN in all
  * three; a point outside the projection's domain (|lat| > 90, or too far from the central meridian) +inf in all three.
- * Within 1e-6 m of the exact map.  S2PB_ERR_ARG: a null pointer with n > 0, n < 0, a zone outside 1..60. */
+ * Within 1e-6 m of the exact map.  S2PB_ERR_ARG: a null pointer with n > 0, n < 0, a zone outside 1..60 (S2PB_ZONE_EGM96
+ * aside). */
 int s2pb_lonlat_to_utm(s2pb_ctx *ctx, double *xyz, const double *lonlatalt, int64_t n, int zone, int south);
+
+/* Heights above the EGM96 geoid (EPSG:5773), the vertical datum of s2p's `out_geoid` targets EPSG:326zz+5773 / 327zz+5773
+ * (and EPSG:4326+5773 for zone 0).  OR S2PB_ZONE_EGM96 into the `zone` argument of s2pb_disp_to_xyz, s2pb_lonlat_to_utm,
+ * s2pb_height_map_to_xyz and the PLY calls, or into the zone field of s2pb_pair_tile and s2pb_heights_tile: every point then
+ * gets z = z - N(lon, lat) in float64, N interpolated in the context's geoid grid at the point's WGS84 longitude and
+ * latitude, before the UTM map (which leaves x and y as they are without the flag).  The cloud's 3D filter runs on the
+ * shifted cloud.  Bilinear rule: node (i, j) lies at (lon0 + i dlon, lat0 - j dlat); for x = ((lon - lon0) mod 360) / dlon
+ * and y = (lat0 - lat) / dlat, i = floor(x), j = floor(y) (at most h - 1), fx = x - i, fy = y - j, column i + 1 is column 0
+ * past the last one and row j + 1 the last row past it; from the float32 nodes a = (i, j), b = (i+1, j), c = (i, j+1),
+ * d = (i+1, j+1), in float64, t = a + fx (b - a), u = c + fx (d - c), N = t + fy (u - t): PROJ's bilinear vgridshift on a
+ * grid such as us_nga_egm96_15.tif up to rounding, exact at the nodes and on a constant grid.  A NaN point stays NaN in all three coordinates; a point with
+ * |lat| > 90 becomes +inf in all three.  S2PB_ERR_ARG: the flag on a context without a grid; any bit other than the flag
+ * or a zone outside the call's range once the flag is removed. */
+#define S2PB_ZONE_EGM96 0x100
+/* Upload the geoid grid of S2PB_ZONE_EGM96 to the context's device, replacing the one it holds (grid NULL: drop it).  grid:
+ * h rows of w float32 node values in metres, row 0 northernmost, node (i, j) at (lon0 + i dlon, lat0 - j dlat) degrees.  The
+ * grid must be global: w dlon >= 360 (longitude wraps), lat0 >= 90 and lat0 - (h - 1) dlat <= -90.  Synchronous.
+ * S2PB_ERR_ARG: w or h below 2, w * h above 2^31 - 1, a non-finite origin, a spacing that is not positive and finite, a grid
+ * that is not global.  S2PB_ERR_NOMEM: the grid does not fit the device. */
+int s2pb_set_geoid(s2pb_ctx *ctx, const float *grid, int w, int h, double lon0, double lat0, double dlon, double dlat);
 
 /* ---- tri-stereo height maps (s2p/__init__.py disparity_to_height and heights_fusion) ---- */
 /* s2p.triangulation.height_map (s2p/triangulation.py:346-389) in one call.  disp, msk: the rectified disparity and mask,
@@ -303,7 +324,7 @@ int s2pb_cargarse_basura(s2pb_ctx *ctx, const float *in, float *out, int w, int 
  * lat, alt as they are) north or south (south != 0) as s2pb_lonlat_to_utm projects it; xyz (w*h*3 float64) comes back.
  * The third coordinate is z bit for bit.  A NaN height gives NaN in all three (the reference leaves lon and lat undefined
  * there); an iteration whose residual turns NaN stops, as the reference's does, with a NaN lon and lat.
- * S2PB_ERR_ARG: a null pointer, a size below 1, a zone outside 0..60, or pixels whose iteration did not meet the
+ * S2PB_ERR_ARG: a null pointer, a size below 1, a zone outside 0..60 (S2PB_ZONE_EGM96 aside), or pixels whose iteration did not meet the
  * reference's stopping test within 1000 steps (the reference would not return; the message gives their number). */
 int s2pb_height_map_to_xyz(s2pb_ctx *ctx, double *xyz, const double *heights, int w, int h, const s2pb_rpc *rpc, double off_x,
                            double off_y, int zone, int south);
@@ -493,7 +514,8 @@ typedef struct s2pb_heights_tile {
     double offsets[S2PB_MAX_FUSION];
     int32_t cargarse_basura, op;
     double threshold;
-    /* height_map_to_xyz: the reference image's camera, the tile's origin in that image, the output UTM zone (0: lon, lat, alt) */
+    /* height_map_to_xyz: the reference image's camera, the tile's origin in that image, the output UTM zone (0: lon, lat, alt;
+     * S2PB_ZONE_EGM96 may be OR'ed in) */
     const s2pb_rpc *rpc;
     double off_x, off_y;
     int32_t zone, south;

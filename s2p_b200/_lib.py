@@ -46,6 +46,7 @@ class PairTile(ctypes.Structure):
 
 
 MATCHER_MGM, MATCHER_SGBM = 0, 1     # S2PB_MATCHER_*
+ZONE_EGM96 = 0x100                   # S2PB_ZONE_EGM96
 MAX_FUSION = 16                      # S2PB_MAX_FUSION
 
 
@@ -111,6 +112,7 @@ _SIGNATURES = {
     "s2pb_disp_to_xyz": (c_int, [c_void_p, POINTER(c_double), _f, _f, _f, _f, c_int, c_int, _f, c_int, c_int,
                                  POINTER(c_double), POINTER(c_double), c_void_p, c_void_p, _f, c_int, c_int]),
     "s2pb_lonlat_to_utm": (c_int, [c_void_p, POINTER(c_double), POINTER(c_double), c_int64, c_int, c_int]),
+    "s2pb_set_geoid": (c_int, [c_void_p, _f, c_int, c_int, c_double, c_double, c_double, c_double]),
     "s2pb_height_map_to_xyz": (c_int, [c_void_p, POINTER(c_double), POINTER(c_double), c_int, c_int, c_void_p, c_double, c_double,
                                        c_int, c_int]),
     "s2pb_height_map": (c_int, [c_void_p, POINTER(c_double), _f, _f, c_int, c_int, _f, c_int, c_int, c_int, c_int, c_int, c_int,

@@ -12,7 +12,8 @@ with no temporary file; for tri-stereo, the tile's window of the image in its st
 ``s2pb_height_map_to_ply_clr``).
 
 The steps fall through to the original when the device path would not write the reference's file:
-- an output CRS other than WGS84 and its UTM zones (the original then uses the installed ``disp_to_xyz`` / filter drop-ins);
+- an output CRS other than WGS84 and its UTM zones, with or without EGM96 heights (those only where the grid is found; the
+  original then uses the installed ``disp_to_xyz`` / filter drop-ins);
 - NumPy < 2, whose casting rules make the stretch float32;
 - colours whose band count the reference refuses, or whose type does not convert exactly to float32 (the original raises or
   stretches them itself);
@@ -148,13 +149,14 @@ def disparity_to_ply(tile, engine=None):
     H1 = np.loadtxt(H_ref)
     H2 = np.dot(np.loadtxt(H_sec), np.linalg.inv(np.loadtxt(pointing)))   # pointing correction (s2p/triangulation.py:114-115)
     r, p, n = _filter_args(cfg)
+    eng = engine or get_engine()
     cloud = (disp_img, mask_rect_img, mask_orig_img, H1, H2, triangulation._rpc_struct(rpc1), triangulation._rpc_struct(rpc2),
-             (x, x + w, y, y + h), *target)
+             (x, x + w, y, y + h), *projection.utm_target(cfg['out_crs'], eng))
     if clr:
         crop, hc = common.homography_crop(clr, H1, ww, hh, common.homography_cmd("<colours of %s>" % ply_file, clr, H1, ww, hh))
-        records = (engine or get_engine()).disp_to_ply_clr(*cloud, r=r, p=p, n=n, clr=crop, hc=hc, confidence=confidence)
+        records = eng.disp_to_ply_clr(*cloud, r=r, p=p, n=n, clr=crop, hc=hc, confidence=confidence)
     else:
-        records = (engine or get_engine()).disp_to_ply(*cloud, r=r, p=p, n=n, colors=colors, confidence=confidence)
+        records = eng.disp_to_ply(*cloud, r=r, p=p, n=n, colors=colors, confidence=confidence)
     write_ply(ply_file, records, _comments(cfg))
 
     if cfg['clean_intermediate']:
@@ -196,11 +198,12 @@ def heights_to_ply(tile, engine=None):
     height_map = os.path.join(out_dir, 'height_map.tif')
     heights = rasterio_compat.read_band_stored(height_map)
     r, p, n = _filter_args(cfg)
-    cloud = (heights, triangulation._rpc_struct(cfg['images'][0]['rpcm']), x, y, *target)
+    eng = engine or get_engine()
+    cloud = (heights, triangulation._rpc_struct(cfg['images'][0]['rpcm']), x, y, *projection.utm_target(cfg['out_crs'], eng))
     if clr:
-        records = (engine or get_engine()).height_map_to_ply_clr(*cloud, r=r, p=p, n=n, colors=colors)
+        records = eng.height_map_to_ply_clr(*cloud, r=r, p=p, n=n, colors=colors)
     else:
-        records = (engine or get_engine()).height_map_to_ply(*cloud, r=r, p=p, n=n, colors=colors)
+        records = eng.height_map_to_ply(*cloud, r=r, p=p, n=n, colors=colors)
     write_ply(plyfile, records, _comments(cfg))
 
     if cfg['clean_intermediate']:

@@ -30,13 +30,6 @@ static int triangulate_enqueue(s2pb_ctx *ctx, cudaStream_t st, const float *d_dx
     return S2PB_OK;
 }
 
-// the output CRS of a cloud: UTM zone 1..60, or 0 for lon, lat, alt as they are
-static int cloud_zone_ok(int zone)
-{
-    if (zone < 0 || zone > 60) return fail(S2PB_ERR_ARG, "UTM zone %d (1 to 60, or 0 for lon, lat, alt)", zone);
-    return S2PB_OK;
-}
-
 int triangulated_cloud_device(s2pb_ctx *ctx, HostCall &L, const float *d_dx, const float *d_dy, const float *d_m, int nx, int ny,
                               const float *d_mo, int w, int h, const double ha[9], const double hb[9], const s2pb_rpc *rpca,
                               const s2pb_rpc *rpcb, const float bbox[4], int zone, int south, double **d_xyz, float **d_err)
@@ -46,15 +39,15 @@ int triangulated_cloud_device(s2pb_ctx *ctx, HostCall &L, const float *d_dx, con
     *d_err = L.take<float>(npix * 4);
     if (int rc = L.error()) return rc;
     int rc = triangulate_enqueue(ctx, L.st, d_dx, d_dy, d_m, nx, ny, d_mo, w, h, ha, hb, rpca, rpcb, bbox, *d_xyz, *d_err);
-    if (rc == S2PB_OK && zone) rc = launch_utm_project(ctx, L.st, zone, south != 0, *d_xyz, *d_xyz, npix);
+    if (rc == S2PB_OK) rc = launch_cloud_project(ctx, L.st, zone, south != 0, *d_xyz, *d_xyz, npix);
     return rc;
 }
 
-int triangulated_cloud_args_ok(int nx, int ny, int w, int h, const double ha[9], const double hb[9], const s2pb_rpc *rpca,
-                               const s2pb_rpc *rpcb, const float bbox[4], int zone)
+int triangulated_cloud_args_ok(const s2pb_ctx *ctx, int nx, int ny, int w, int h, const double ha[9], const double hb[9],
+                               const s2pb_rpc *rpca, const s2pb_rpc *rpcb, const float bbox[4], int zone)
 {
     if (!ha || !hb || !rpca || !rpcb || !bbox || nx < 1 || ny < 1 || w < 1 || h < 1) return fail(S2PB_ERR_ARG, "bad argument");
-    return cloud_zone_ok(zone);
+    return cloud_crs_ok(ctx, zone, true);
 }
 
 int triangulated_cloud(s2pb_ctx *ctx, HostCall &L, const float *dispx, const float *dispy, const float *msk, int nx, int ny,
@@ -62,15 +55,16 @@ int triangulated_cloud(s2pb_ctx *ctx, HostCall &L, const float *dispx, const flo
                        const s2pb_rpc *rpcb, const float bbox[4], int zone, int south, double **d_xyz, float **d_err)
 {
     if (!dispx || !dispy || !msk || !msk_orig) return fail(S2PB_ERR_ARG, "bad argument");
-    if (int rc = triangulated_cloud_args_ok(nx, ny, w, h, ha, hb, rpca, rpcb, bbox, zone)) return rc;
+    if (int rc = triangulated_cloud_args_ok(ctx, nx, ny, w, h, ha, hb, rpca, rpcb, bbox, zone)) return rc;
     const size_t npix = (size_t)nx * ny, nm = (size_t)w * h;
     float *d_dx = L.upload(dispx, npix * 4), *d_dy = L.upload(dispy, npix * 4), *d_m = L.upload(msk, npix * 4);
     float *d_mo = L.upload(msk_orig, nm * 4);
     return triangulated_cloud_device(ctx, L, d_dx, d_dy, d_m, nx, ny, d_mo, w, h, ha, hb, rpca, rpcb, bbox, zone, south, d_xyz, d_err);
 }
 
-// s2p.triangulation.disp_to_xyz (s2p/triangulation.py:85-162) with a UTM (or no) output CRS: disp_to_lonlatalt, then the
-// projection (projection.cu) in place on the device cloud; only the projected cloud and the error come back.
+// s2p.triangulation.disp_to_xyz (s2p/triangulation.py:85-162) with a UTM (or no) output CRS, heights optionally above EGM96:
+// disp_to_lonlatalt, then the projection (projection.cu) in place on the device cloud; only the projected cloud and the error
+// come back.
 extern "C" int s2pb_disp_to_xyz(s2pb_ctx *ctx, double *xyz, float *err, const float *dispx, const float *dispy, const float *msk,
                                 int nx, int ny, const float *msk_orig, int w, int h, const double ha[9], const double hb[9],
                                 const s2pb_rpc *rpca, const s2pb_rpc *rpcb, const float bbox[4], int zone, int south)
@@ -104,9 +98,7 @@ int localised_cloud_device(s2pb_ctx *ctx, HostCall &L, const double *d_z, int w,
     const dim3 b2(32, 4);
     launch(ctx, height_map_to_xyz_kernel, grid2d(w, h, b2), b2, 0, L.st, P);
     CK(cudaGetLastError());
-    if (zone) {
-        if (int rc = launch_utm_project(ctx, L.st, zone, south != 0, *d_xyz, *d_xyz, npix)) return rc;
-    }
+    if (int rc = launch_cloud_project(ctx, L.st, zone, south != 0, *d_xyz, *d_xyz, npix)) return rc;
     int capped = 0;
     L.download(&capped, d_capped, 4);
     if (int rc = L.finish()) return rc;
@@ -114,23 +106,24 @@ int localised_cloud_device(s2pb_ctx *ctx, HostCall &L, const double *d_z, int w,
     return S2PB_OK;
 }
 
-int localised_cloud_args_ok(int w, int h, const s2pb_rpc *rpc, int zone)
+int localised_cloud_args_ok(const s2pb_ctx *ctx, int w, int h, const s2pb_rpc *rpc, int zone)
 {
     if (!rpc || w < 1 || h < 1) return fail(S2PB_ERR_ARG, "bad argument");
-    return cloud_zone_ok(zone);
+    return cloud_crs_ok(ctx, zone, true);
 }
 
 int localised_cloud(s2pb_ctx *ctx, HostCall &L, const double *heights, int w, int h, const s2pb_rpc *rpc, double off_x,
                     double off_y, int zone, int south, double **d_xyz)
 {
     if (!heights) return fail(S2PB_ERR_ARG, "bad argument");
-    if (int rc = localised_cloud_args_ok(w, h, rpc, zone)) return rc;
+    if (int rc = localised_cloud_args_ok(ctx, w, h, rpc, zone)) return rc;
     double *d_z = L.upload(heights, (size_t)w * h * 8);
     return localised_cloud_device(ctx, L, d_z, w, h, rpc, off_x, off_y, zone, south, d_xyz);
 }
 
-// s2p.triangulation.height_map_to_xyz (s2p/triangulation.py:165-217) with a UTM (or no) output CRS: every pixel of the height
-// map localised by the camera, then the projection (projection.cu) in place on the device cloud.
+// s2p.triangulation.height_map_to_xyz (s2p/triangulation.py:165-217) with a UTM (or no) output CRS, heights optionally above
+// EGM96: every pixel of the height map localised by the camera, then the projection (projection.cu) in place on the device
+// cloud.
 extern "C" int s2pb_height_map_to_xyz(s2pb_ctx *ctx, double *xyz, const double *heights, int w, int h, const s2pb_rpc *rpc,
                                       double off_x, double off_y, int zone, int south)
 {

@@ -6,6 +6,7 @@
 #pragma once
 #include "../../include/s2pb200.h"
 #include "agg_kernel.cuh"          // kMaxPasses
+#include "projection_kernels.cuh"  // GeoidGrid
 
 #include <cuda_runtime.h>
 #include <algorithm>
@@ -94,6 +95,7 @@ struct s2pb_ctx {
     // that s2pb_mgm_batch's worker threads run may take from it.
     struct PoolBuf { void *p; size_t bytes; bool used; };
     std::vector<PoolBuf> pool;
+    GeoidGrid geoid{};              // s2pb_set_geoid: the EGM96 grid of S2PB_ZONE_EGM96 (geoid.g null: none), owned
 };
 
 // nothing declared from here on is part of the library's exported interface
@@ -255,10 +257,15 @@ void launch_erode_mask(s2pb_ctx *ctx, const uint8_t *in, uint8_t *out, int w, in
 int mgm_match_device(s2pb_ctx *ctx, cudaStream_t st, const float *d_im1, const float *d_im2, int w, int h, int dmin, int dmax,
                      const s2pb_mgm_params *p, const float *d_wl, const float *d_wr, float *d_disp, float *d_conf, uint8_t *d_mask,
                      float *d_dispR);
-// projection.cu: (lon, lat, alt) -> UTM zone `zone` (1..60) of n device points, in place when d_in == d_out
-int launch_utm_project(s2pb_ctx *ctx, cudaStream_t st, int zone, bool south, const double *d_in, double *d_out, size_t n);
+// projection.cu: the output CRS of a cloud, `zone` as the C ABI takes it (a UTM zone, 0 for none when zone0 is true, optionally
+// with S2PB_ZONE_EGM96 when the context holds a geoid grid): its check, and the projection of n device points (lon, lat, alt)
+// to it, in place when d_in == d_out (nothing to launch for zone 0 without the geoid)
+int cloud_crs_ok(const s2pb_ctx *ctx, int zone, bool zone0);
+int launch_cloud_project(s2pb_ctx *ctx, cudaStream_t st, int zone, bool south, const double *d_in, double *d_out, size_t n);
+// the context's geoid grid back to the device (s2pb_destroy, s2pb_set_geoid)
+void geoid_free(s2pb_ctx *ctx);
 // geometry.cu: the two clouds of a host call, each from host buffers into scratch of L after the checks of its arguments, then
-// projected in place to UTM zone `zone` (0: none).  triangulated_cloud: disp_to_lonlatalt of s2pb_disp_to_xyz's inputs, *d_xyz
+// projected in place to the output CRS `zone` (launch_cloud_project).  triangulated_cloud: disp_to_lonlatalt of s2pb_disp_to_xyz's inputs, *d_xyz
 // nx*ny*3 doubles and *d_err nx*ny floats, still in flight on L.st.  localised_cloud: s2pb_height_map_to_xyz's localisation,
 // *d_xyz w*h*3 doubles, complete on return (the pixels whose iteration hit its cap are an error).  remove_isolated_3d_points
 // (n > 0; d_work: 3 * nx * ny ints) on device buffers.
@@ -266,7 +273,7 @@ int triangulated_cloud(s2pb_ctx *ctx, HostCall &L, const float *dispx, const flo
                        const float *msk_orig, int w, int h, const double ha[9], const double hb[9], const s2pb_rpc *rpca,
                        const s2pb_rpc *rpcb, const float bbox[4], int zone, int south, double **d_xyz, float **d_err);
 // triangulated_cloud_device: the same from device disparities and masks, after triangulated_cloud_args_ok checked the rest.
-int triangulated_cloud_args_ok(int nx, int ny, int w, int h, const double ha[9], const double hb[9], const s2pb_rpc *rpca,
+int triangulated_cloud_args_ok(const s2pb_ctx *ctx, int nx, int ny, int w, int h, const double ha[9], const double hb[9], const s2pb_rpc *rpca,
                                const s2pb_rpc *rpcb, const float bbox[4], int zone);
 int triangulated_cloud_device(s2pb_ctx *ctx, HostCall &L, const float *d_dx, const float *d_dy, const float *d_m, int nx, int ny,
                               const float *d_mo, int w, int h, const double ha[9], const double hb[9], const s2pb_rpc *rpca,
@@ -274,7 +281,7 @@ int triangulated_cloud_device(s2pb_ctx *ctx, HostCall &L, const float *d_dx, con
 int localised_cloud(s2pb_ctx *ctx, HostCall &L, const double *heights, int w, int h, const s2pb_rpc *rpc, double off_x,
                     double off_y, int zone, int south, double **d_xyz);
 // localised_cloud_device: the same from device heights d_z, after localised_cloud_args_ok checked the rest.
-int localised_cloud_args_ok(int w, int h, const s2pb_rpc *rpc, int zone);
+int localised_cloud_args_ok(const s2pb_ctx *ctx, int w, int h, const s2pb_rpc *rpc, int zone);
 int localised_cloud_device(s2pb_ctx *ctx, HostCall &L, const double *d_z, int w, int h, const s2pb_rpc *rpc, double off_x,
                            double off_y, int zone, int south, double **d_xyz);
 // s2pb_height_map from the device disparity d_dx and mask d_m (nx*ny) and the unpadded device mask_orig d_mo0 (mw*mh) into the

@@ -1,6 +1,8 @@
-// projection.cu -- the change of coordinates of s2p.triangulation.disp_to_xyz: WGS84 (lon, lat, alt) -> UTM.
+// projection.cu -- the change of coordinates of s2p.triangulation.disp_to_xyz: WGS84 (lon, lat, alt) -> UTM, and the EGM96
+// geoid heights of the compound targets (EPSG:326zz+5773, 327zz+5773, 4326+5773).
 #include "host.h"
-#include "projection_kernels.cuh"
+
+#include <cmath>
 
 // The coefficients of projection_kernels.cuh for UTM zone `zone` (1..60) of WGS84, in double.  The series in the third
 // flattening n are those of Karney (2011), eq. (35) for alpha (Krueger's series, ellipsoid <- sphere) and the conformal-latitude
@@ -37,12 +39,26 @@ static UtmParams utm_params(int zone, bool south)
     return P;
 }
 
-int launch_utm_project(s2pb_ctx *ctx, cudaStream_t st, int zone, bool south, const double *d_in, double *d_out, size_t n)
+int cloud_crs_ok(const s2pb_ctx *ctx, int zone, bool zone0)
 {
-    if (n == 0) return S2PB_OK;
+    const int utm = zone & ~S2PB_ZONE_EGM96;
+    if (utm < (zone0 ? 0 : 1) || utm > 60)
+        return fail(S2PB_ERR_ARG, "zone %d: a UTM zone 1 to 60%s, optionally OR S2PB_ZONE_EGM96", zone, zone0 ? ", or 0 for lon, lat" : "");
+    if ((zone & S2PB_ZONE_EGM96) && !ctx->geoid.g) return fail(S2PB_ERR_ARG, "S2PB_ZONE_EGM96 on a context without a geoid grid");
+    return S2PB_OK;
+}
+
+int launch_cloud_project(s2pb_ctx *ctx, cudaStream_t st, int zone, bool south, const double *d_in, double *d_out, size_t n)
+{
+    const int utm = zone & ~S2PB_ZONE_EGM96;
+    const bool geoid = (zone & S2PB_ZONE_EGM96) != 0;
+    if (n == 0 || (!utm && !geoid)) return S2PB_OK;
     const unsigned b = 256;
-    launch(ctx, utm_project_kernel, dim3((unsigned)((n + b - 1) / b)), dim3(b), 0, st, utm_params(zone, south), d_in, d_out,
-           (long long)n);
+    const dim3 g((unsigned)((n + b - 1) / b));
+    const UtmParams P = utm_params(utm, south);
+    if (!geoid) launch(ctx, cloud_project_kernel<true, false>, g, dim3(b), 0, st, P, ctx->geoid, d_in, d_out, (long long)n);
+    else if (utm) launch(ctx, cloud_project_kernel<true, true>, g, dim3(b), 0, st, P, ctx->geoid, d_in, d_out, (long long)n);
+    else launch(ctx, cloud_project_kernel<false, true>, g, dim3(b), 0, st, P, ctx->geoid, d_in, d_out, (long long)n);
     CK(cudaGetLastError());
     return S2PB_OK;
 }
@@ -50,14 +66,51 @@ int launch_utm_project(s2pb_ctx *ctx, cudaStream_t st, int zone, bool south, con
 extern "C" int s2pb_lonlat_to_utm(s2pb_ctx *ctx, double *xyz, const double *lonlatalt, int64_t n, int zone, int south)
 {
     if (!ctx || n < 0 || (n > 0 && (!xyz || !lonlatalt))) return fail(S2PB_ERR_ARG, "bad argument");
-    if (zone < 1 || zone > 60) return fail(S2PB_ERR_ARG, "UTM zone %d (1 to 60)", zone);
+    if (int rc = cloud_crs_ok(ctx, zone, false)) return rc;
     if (n == 0) return S2PB_OK;
     const size_t bytes = (size_t)n * 24;
     HostCall L(ctx, "the projection");
     double *d = L.upload(lonlatalt, bytes);
     if (int rc = L.error()) return rc;
-    int rc = launch_utm_project(ctx, L.st, zone, south != 0, d, d, (size_t)n);
+    int rc = launch_cloud_project(ctx, L.st, zone, south != 0, d, d, (size_t)n);
     if (rc != S2PB_OK) return rc;
     L.download(xyz, d, bytes);
     return L.finish();
+}
+
+void geoid_free(s2pb_ctx *ctx)
+{
+    if (ctx->geoid.g) cudaFree((void *)ctx->geoid.g);
+    ctx->geoid = GeoidGrid{};
+}
+
+// The grid must be global (GeoidGrid): no point of a cloud falls outside it.
+extern "C" int s2pb_set_geoid(s2pb_ctx *ctx, const float *grid, int w, int h, double lon0, double lat0, double dlon, double dlat)
+{
+    if (!ctx) return fail(S2PB_ERR_ARG, "bad argument");
+    CK(cudaSetDevice(ctx->device));
+    if (!grid) {
+        geoid_free(ctx);
+        return S2PB_OK;
+    }
+    if (w < 2 || h < 2 || (int64_t)w * h > INT32_MAX || !std::isfinite(lon0) || !std::isfinite(lat0) || !(dlon > 0.0) ||
+        !(dlat > 0.0) || !std::isfinite(dlon) || !std::isfinite(dlat))
+        return fail(S2PB_ERR_ARG, "bad geoid grid: %d x %d nodes, origin (%g, %g), spacing (%g, %g)", w, h, lon0, lat0, dlon, dlat);
+    const double eps = 1e-9;
+    if (w * dlon < 360.0 - eps || lat0 < 90.0 - eps || lat0 - (h - 1) * dlat > -90.0 + eps)
+        return fail(S2PB_ERR_ARG, "the geoid grid is not global: %d x %d nodes from (%g, %g) by (%g, %g) degrees", w, h, lon0, lat0,
+                    dlon, dlat);
+    const size_t bytes = (size_t)w * h * sizeof(float);
+    float *d = nullptr;
+    if (cudaMalloc(&d, bytes) != cudaSuccess) {
+        cudaGetLastError();
+        return fail(S2PB_ERR_NOMEM, "cudaMalloc of %zu bytes failed for the geoid grid", bytes);
+    }
+    if (cudaError_t e = cudaMemcpy(d, grid, bytes, cudaMemcpyHostToDevice)) {
+        cudaFree(d);
+        return fail(S2PB_ERR_CUDA, "copy of the geoid grid failed: %s", cudaGetErrorString(e));
+    }
+    geoid_free(ctx);
+    ctx->geoid = GeoidGrid{d, w, h, lon0, lat0, dlon, dlat};
+    return S2PB_OK;
 }

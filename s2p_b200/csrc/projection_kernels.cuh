@@ -1,4 +1,5 @@
-// projection_kernels.cuh -- WGS84 (lon, lat, alt) -> UTM (easting, northing, alt), forward, one thread per point.
+// projection_kernels.cuh -- WGS84 (lon, lat, alt) -> UTM (easting, northing, alt), forward, one thread per point, and the
+// EGM96 geoid heights of a compound target such as EPSG:326zz+5773 (GeoidGrid below).
 //
 // The map is the one PROJ runs for `+proj=utm` unless `+approx` is given: the "exact" transverse Mercator of Poder and
 // Engsager (K. Engsager, K. Poder, "A highly accurate world wide algorithm for the transverse Mercator mapping (almost)",
@@ -81,9 +82,42 @@ __device__ __forceinline__ void utm_forward(const UtmParams &P, double lon, doub
     y = P.qa * xi + P.y0;
 }
 
-// out[i] = (x, y, alt) of in[i] = (lon, lat, alt), n points of three doubles; in == out is allowed.  A point with a NaN
-// coordinate becomes NaN in all three; a point outside the domain becomes +inf in all three.
-__global__ void utm_project_kernel(const __grid_constant__ UtmParams P, const double *in, double *out, long long n)
+// The vertical datum of a cloud: heights above the EGM96 geoid instead of the WGS84 ellipsoid, H = h - N(lon, lat), the
+// step PROJ's `+proj=vgridshift` runs for a target such as EPSG:326zz+5773.  N is interpolated bilinearly in a float32 grid
+// of h rows of w nodes: node (i, j) lies at (lon0 + i dlon, lat0 - j dlat), row 0 northernmost.  The grid is global: it spans
+// at least 360 degrees of longitude, which wraps (column w - 1 is followed by column 0), and every latitude from 90 to -90.
+struct GeoidGrid {
+    const float *g;                       // h * w nodes, row-major; device memory
+    int w, h;
+    double lon0, lat0;                    // node (0, 0), degrees
+    double dlon, dlat;                    // node spacing, degrees, both > 0
+};
+
+// N(lon, lat) for |lat| <= 90 and a finite lon: bilinear in the four float32 nodes around the point, in float64, as two
+// interpolations along the row and one across (tests/geoid_oracle.py restates it in numpy).  This form gives a node's value
+// at the node and a constant grid's value everywhere exactly; it differs from PROJ's sum of four weighted nodes by rounding
+// only.  The last row stands in for the row below it, as PROJ clamps it.
+__device__ __forceinline__ double geoid_undulation(const GeoidGrid &G, double lon, double lat)
+{
+    double t = fmod(lon - G.lon0, 360.0);
+    if (t < 0.0) t += 360.0;
+    const double x = t / G.dlon, y = (G.lat0 - lat) / G.dlat;
+    const int i = min((int)floor(x), G.w - 1), j = max(0, min((int)floor(y), G.h - 1));
+    const double fx = x - i, fy = y - j;
+    const int i2 = i + 1 < G.w ? i + 1 : 0, j2 = min(j + 1, G.h - 1);
+    const double a = G.g[(size_t)j * G.w + i], b = G.g[(size_t)j * G.w + i2];
+    const double c = G.g[(size_t)j2 * G.w + i], d = G.g[(size_t)j2 * G.w + i2];
+    const double top = a + fx * (b - a), bottom = c + fx * (d - c);
+    return top + fy * (bottom - top);
+}
+
+// out[i] = (x, y, z) of in[i] = (lon, lat, alt), n points of three doubles; in == out is allowed.  kUtm: (x, y) the UTM map
+// of (lon, lat), else (lon, lat) as they are; kGeoid: z = alt - N(lon, lat) in float64, else alt.  A point with a NaN
+// coordinate becomes NaN in all three; a point outside the domain (of the UTM map, or |lat| > 90 / an infinite lon for the
+// geoid) becomes +inf in all three.
+template <bool kUtm, bool kGeoid>
+__global__ void cloud_project_kernel(const __grid_constant__ UtmParams P, const __grid_constant__ GeoidGrid G, const double *in,
+                                     double *out, long long n)
 {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
@@ -92,8 +126,19 @@ __global__ void utm_project_kernel(const __grid_constant__ UtmParams P, const do
     if (isnan(lon) || isnan(lat) || isnan(alt)) {
         x = y = z = __longlong_as_double(0x7ff8000000000000LL);
     } else {
-        utm_forward(P, lon, lat, x, y);
-        if (isinf(x)) z = x;
+        bool outside = false;
+        if (kUtm) {
+            utm_forward(P, lon, lat, x, y);
+            outside = isinf(x);
+        } else {
+            x = lon;
+            y = lat;
+        }
+        if (kGeoid && !outside) {
+            if (fabs(lat) <= 90.0 && isfinite(lon)) z = alt - geoid_undulation(G, lon, lat);
+            else outside = true;
+        }
+        if (outside) x = y = z = __longlong_as_double(0x7ff0000000000000LL);
     }
     out[3 * i] = x;
     out[3 * i + 1] = y;

@@ -272,6 +272,7 @@ extern "C" void s2pb_destroy(s2pb_ctx *ctx)
     }
     for (auto &b : ctx->pool) cudaFree(b.p);
     for (auto &t : ctx->dct) for (double *q : {t.T10, t.T01, t.TR01, t.mc, t.ms}) if (q) cudaFree(q);
+    geoid_free(ctx);
     if (ctx->abort_words) cudaFreeHost(ctx->abort_words);
     delete ctx;
 }

@@ -357,7 +357,8 @@ class Engine:
         return (h, w), (_dp(z), w, h, _rpc(rpc), float(off_x), float(off_y), int(zone), int(bool(south)))
 
     def disp_to_xyz(self, disp, mask_rect, mask_orig, H1, H2, rpc1, rpc2, img_bbx, zone=0, south=False, dispy=None):
-        """disp_to_lonlatalt and the projection to UTM zone `zone` (1..60; 0: lon, lat, alt as they are) in one device call
+        """disp_to_lonlatalt and the projection to UTM zone `zone` (1..60; 0: lon, lat, alt as they are; with _lib.ZONE_EGM96
+        OR'ed in, heights above the geoid of set_geoid) in one device call
         -> (xyz (h, w, 3) float64, err (h, w) float32).  rpc1 / rpc2: ctypes structures with the layout of
         ``triangulation.RPCStruct``; H2 already carries the pointing correction."""
         (h, w), args = self._triangulation(disp, mask_rect, mask_orig, H1, H2, rpc1, rpc2, img_bbx, zone, south, dispy)
@@ -366,9 +367,26 @@ class Engine:
         _lib.check(self._L.s2pb_disp_to_xyz(self._ctx, _dp(xyz), _fp(err), *args))
         return xyz, err
 
+    def set_geoid(self, grid):
+        """Hold ``grid`` (projection.GeoidGrid, or None to drop it) on the device for the zones with _lib.ZONE_EGM96 OR'ed in,
+        which every cloud, tile and projection method then takes: heights above the geoid, z - N(lon, lat) (s2pb_set_geoid).
+        Uploads only when the grid is not the one the engine already holds."""
+        if grid is getattr(self, "_geoid", None):
+            return
+        if grid is None:
+            _lib.check(self._L.s2pb_set_geoid(self._ctx, None, 0, 0, 0.0, 0.0, 0.0, 0.0))
+        else:
+            v = _f32(grid.values)
+            if v.ndim != 2:
+                raise ValueError("the geoid grid must be a 2-D array")
+            _lib.check(self._L.s2pb_set_geoid(self._ctx, _fp(v), v.shape[1], v.shape[0], float(grid.lon0), float(grid.lat0),
+                                              float(grid.dlon), float(grid.dlat)))
+        self._geoid = grid
+
     def lonlat_to_utm(self, lonlatalt, zone, south=False):
         """(..., 3) float64 (lon, lat in degrees, alt) -> (..., 3) float64 (easting, northing, alt) in UTM zone `zone` (1..60)
-        of WGS84, north or south (EPSG 326zz / 327zz).  NaN in any coordinate gives NaN in all three."""
+        of WGS84, north or south (EPSG 326zz / 327zz); with _lib.ZONE_EGM96 OR'ed into the zone, alt - N(lon, lat) in the geoid
+        of set_geoid.  NaN in any coordinate gives NaN in all three."""
         a = np.ascontiguousarray(lonlatalt, np.float64)
         if a.ndim < 1 or a.shape[-1] != 3:
             raise ValueError("expecting points of three coordinates, got shape %s" % (a.shape,))
@@ -378,7 +396,7 @@ class Engine:
 
     def height_map_to_xyz(self, heights, rpc, off_x, off_y, zone=0, south=False):
         """The localisation of every pixel of a (h, w) height map and the projection to UTM zone `zone` (1..60; 0: lon, lat,
-        alt as they are) in one device call -> (h, w, 3) float64.  Pixel (i, j) is image pixel (j + off_x, i + off_y) of the
+        alt as they are; _lib.ZONE_EGM96 as in disp_to_xyz) in one device call -> (h, w, 3) float64.  Pixel (i, j) is image pixel (j + off_x, i + off_y) of the
         camera ``rpc`` (a ctypes structure with the layout of ``triangulation.RPCStruct``); its third coordinate is the height
         converted to float64.  NaN heights give NaN in all three.  Pixels whose localisation does not converge raise
         S2pbError(ERR_ARG)."""

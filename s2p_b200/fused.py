@@ -80,7 +80,7 @@ def fall_through_reason(cfg):
     if cfg['matching_algorithm'] not in SERVED:
         return "algo %r is not served" % cfg['matching_algorithm']
     if projection.utm_target(cfg['out_crs']) is None:
-        return "output CRS %r is not a UTM zone of WGS84" % cfg['out_crs']
+        return projection.unserved_reason(cfg['out_crs'])
     if not cloud.numpy_stretch_is_float64():
         return "NumPy < 2 stretches the colours in float32"
     clr = cfg['images'][0]['clr']
@@ -184,7 +184,7 @@ def pair_tile(tile, engine=None):
         records, out = eng.pair_tile_to_ply(
             src1, H1c, src2, H2c, w, h, disp_min, disp_max, rio.read_stored(mask_orig).squeeze(), H_ref, H_sec,
             triangulation._rpc_struct(cfg['images'][0]['rpcm']), triangulation._rpc_struct(cfg['images'][1]['rpcm']),
-            (x, x + tw, y, y + th), *projection.utm_target(cfg['out_crs']), params=params, weights=weights,
+            (x, x + tw, y, y + th), *projection.utm_target(cfg['out_crs'], eng), params=params, weights=weights,
             erode_radius=erosion_radius(cfg['msk_erosion']), r=r, p=p, n=n, clr=clr, hc=hc,
             confidence=algo in CONFIDENCE_COLUMN, want=want)
     except S2pbError as e:
@@ -296,7 +296,7 @@ def heights_tile_fall_through_reason(cfg):
     """Why ``heights_tile`` hands the tile to ``s2p.heights_to_ply`` for this configuration, or None (the colours are looked
     at in ``heights_tile``, as ``cloud.heights_to_ply`` looks at them)."""
     if projection.utm_target(cfg['out_crs']) is None:
-        return "output CRS %r is not a UTM zone of WGS84" % cfg['out_crs']
+        return projection.unserved_reason(cfg['out_crs'])
     if not cloud.numpy_stretch_is_float64():
         return "NumPy < 2 stretches the colours in float32"
     if _fusion_operator(cfg['fusion_operator']) not in Engine.FUSION_OPS:
@@ -343,9 +343,10 @@ def heights_tile(tile, engine=None):
     want = () if clean else ("merged",) + (("cleaned",) if basura else ())
     r, p, n = cloud._filter_args(cfg)
     ply_file = os.path.join(out_dir, 'cloud.ply')
+    eng = engine or get_engine()
     try:
-        records, out = (engine or get_engine()).heights_tile_to_ply(
-            maps, offsets, triangulation._rpc_struct(cfg['images'][0]['rpcm']), x, y, *projection.utm_target(cfg['out_crs']),
+        records, out = eng.heights_tile_to_ply(
+            maps, offsets, triangulation._rpc_struct(cfg['images'][0]['rpcm']), x, y, *projection.utm_target(cfg['out_crs'], eng),
             cargarse_basura=basura, averaging=_fusion_operator(cfg['fusion_operator']), threshold=cfg['fusion_thresh'], r=r, p=p,
             n=n, colors=None if clr else colors, clr=colors if clr else None, want=want)
     except S2pbError as e:
