@@ -78,7 +78,7 @@ enum {
 typedef struct s2pb_mgm_params {
     int32_t ndir;            /* -O           number of scan passes: 2, 4 or 8            */
     int32_t tsgm;            /* TSGM         neighbours mixed per pass: 1..4             */
-    int32_t census_win;      /* CENSUS_NCC_WIN  census window side: 3, 5 or 7            */
+    int32_t census_win;      /* CENSUS_NCC_WIN  2..11: side 2*(win/2)+1; <= 1 ARG, >= 12 UNSUPPORTED */
     float   P1;              /* -P1                                                       */
     float   P2;              /* -P2                                                       */
     int32_t median;          /* MEDIAN       radius of the median post-filter, 0 = off    */

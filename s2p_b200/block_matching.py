@@ -4,7 +4,7 @@
 (s2p/block_matching.py:35-336) but, for ``algo in {'mgm', 'mgm_multi', 'mgm_multi_lsd'}``, runs the H100 engine
 through the C ABI instead of spawning the ``mgm`` / ``mgm_multi`` binaries and the three
 ``plambda`` / ``backflow`` processes of ``create_rejection_mask`` (and, for ``mgm_multi_lsd``, the two five-command
-weight-map pipelines, see ``lsd_weight_map``).  ``algo == 'sgbm'`` with both
+weight-map pipelines, see ``lsd_weight_map``).  The matcher serves ``census_ncc_win`` 2 to 11; any other window goes to s2p as well.  ``algo == 'sgbm'`` with both
 disparity bounds given (as s2p always passes them) runs the engine's bit-exact restatement of the
 ``sgbm`` binary with s2p's arguments (win 3, P1 8, P2 32, lr 1) and writes no confidence file, as the
 reference does.  Any other ``algo`` (and ``sgbm`` with a bound of None) is handed to the original s2p
@@ -24,7 +24,7 @@ import numpy as np
 
 from . import _lib, rasterio_compat as rio
 from .config import cfg
-from .engine import S2pbError, default_params, get_engine
+from .engine import S2pbError, census_window_served, default_params, get_engine
 
 try:  # share the exception class with a real s2p so that its `except` clauses keep matching
     from s2p.block_matching import MaxDisparityRangeError  # pragma: no cover
@@ -107,11 +107,12 @@ def compute_disparity_map(im1, im2, disp, mask, algo, disp_min=None, disp_max=No
     """
     if algo == "sgbm" and disp_min is not None and disp_max is not None:
         return _sgbm(im1, im2, disp, mask, disp_min, disp_max, max_disp_range)
-    if algo not in _NATIVE:
+    if algo not in _NATIVE or not census_window_served(cfg["census_ncc_win"]):
         fn = _original_compute_disparity_map()
         if fn is None:
-            raise NotImplementedError("algo %r is not served by the H100 engine and the s2p package "
-                                      "is not importable to fall through to" % algo)
+            what = ("algo %r" % algo) if algo not in _NATIVE else ("census_ncc_win %r" % cfg["census_ncc_win"])
+            raise NotImplementedError("%s is not served by the H100 engine and the s2p package "
+                                      "is not importable to fall through to" % what)
         return fn(im1, im2, disp, mask, algo, disp_min, disp_max, timeout, max_disp_range, extra_params)
 
     width, _ = rio.image_size(im1)

@@ -294,7 +294,7 @@ __device__ __forceinline__ void run_band_chunked(const PassDesc &pd, const FoldV
                     if constexpr (GEN) c = cp[kk];
                     else {
                         c = cost_decode(cp[kk]);
-                        if (SCALED) { if (c >= 0.f && c < 64.f) c = lut[(int)c]; }
+                        if (SCALED) { if (c >= 0.f && c < (float)kCostLut) c = lut[(int)c]; }
                     }
                     L = c;
                     if (!border) {

@@ -138,12 +138,20 @@ template <int LPL> __device__ __forceinline__ void st_vec(float *p, const float 
 }
 // ------------------------------------------------------------------ 8-bit census cost codes
 //
-// The census cost volume stores one byte per slot: code = the popcount (0..127; census windows give at most 48),
+// The census cost volume stores one byte per slot: code = the popcount (0..127; census windows give at most 120),
 // kCostInf (0xFF) = +INF.  Any code with its top bit set decodes to +INF, which lets the packed decoder find INF slots
 // with one sign-replicating byte permute.  Every producer and consumer goes through the helpers below; decoding gives
 // exactly (float)code.
 constexpr unsigned kCostInf = 0xFFu;
 constexpr int kCostMaxCode = 127;     // largest finite cost the format holds
+constexpr int kCostLut = kCostMaxCode + 1;   // entries of the popcount -> cost table of the scaled census costs
+// census_tools.cc:38-57,76-99: a window of side 2 (win / 2) + 1 gives side^2 - 1 code bits (at most 120 up to win 11, which the
+// format holds); above 64 bits a code takes a second 64-bit word
+__host__ __device__ constexpr int census_side(int win) { return 2 * (win / 2) + 1; }
+__host__ __device__ constexpr int census_bits(int win) { return census_side(win) * census_side(win) - 1; }
+__host__ __device__ constexpr int census_words(int win) { return census_bits(win) > 64 ? 2 : 1; }
+// the two-word code (hi : lo) shifted left by one with `bit` in
+__device__ __forceinline__ void census_push(uint64_t &lo, uint64_t &hi, unsigned bit) { hi = (hi << 1) | (lo >> 63); lo = (lo << 1) | bit; }
 __host__ __device__ __forceinline__ unsigned cost_encode(unsigned cnt, bool finite) { return finite ? cnt : kCostInf; }
 __device__ __forceinline__ unsigned char cost_encode_f(float c) { return isinf(c) ? (unsigned char)kCostInf : (unsigned char)(int)c; }
 __device__ __forceinline__ float cost_decode(unsigned code) { return (code & 0x80u) ? S2PB_INF : (float)code; }
@@ -249,10 +257,10 @@ template <int LPL> __device__ __forceinline__ void st_cost(uint8_t *p, const Cos
     }
 }
 // cost value of a stored code: the popcount itself (census 5x5: ratio = 1, one code word) or
-// the reference's scaled cost through a 64-entry table (mgm_costvolume.h:90-91)
+// the reference's scaled cost through a kCostLut-entry table (mgm_costvolume.h:90-91)
 __device__ __forceinline__ float cost_scaled(float c, const float *__restrict__ lut)
 {
-    if (lut != nullptr && c >= 0.f && c < 64.f) c = lut[(int)c];
+    if (lut != nullptr && c >= 0.f && c < (float)kCostLut) c = lut[(int)c];
     return c;
 }
 __device__ __forceinline__ float cost_value(unsigned code, const float *__restrict__ lut) { return cost_scaled(cost_decode(code), lut); }
@@ -567,7 +575,7 @@ __device__ __forceinline__ void run_band(const PassDesc &pd, const FoldView &fv,
             if (SCALED) {
 #pragma unroll
                 for (int e = 0; e < LPL; e++)
-                    if (c[e] >= 0.f && c[e] < 64.f) c[e] = lut[(int)c[e]];   // an idle scanline reads unstaged shared memory: never index with it
+                    if (c[e] >= 0.f && c[e] < (float)kCostLut) c[e] = lut[(int)c[e]];   // an idle scanline reads unstaged shared memory: never index with it
             }
         }
     };

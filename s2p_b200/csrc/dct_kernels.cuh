@@ -20,6 +20,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include "agg_kernel.cuh"      // census_push
 
 namespace s2pb {
 
@@ -243,15 +244,18 @@ __global__ void dct_combine_kernel(const double *__restrict__ sym, const double 
 }
 
 // census of the image and of its round-tripped copy in one pass; when no row needed the transform the second code is
-// the first (saves the second evaluation on tiles without no-data)
+// the first (saves the second evaluation on tiles without no-data).  NW = 2: codes of more than 64 bits, the second words
+// in codes_hi / codes_rt_hi (census_kernel)
+template <int NW>
 __global__ void census_pair_kernel(const float *__restrict__ img, const float *__restrict__ rt, const RtState *st, int w, int h, int r,
-                                   uint64_t *__restrict__ codes, uint64_t *__restrict__ codes_rt)
+                                   uint64_t *__restrict__ codes, uint64_t *__restrict__ codes_rt, uint64_t *__restrict__ codes_hi,
+                                   uint64_t *__restrict__ codes_rt_hi)
 {
     int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
     if (x >= w || y >= h) return;
     const bool both = st->nrows > 0;
     float c = img[(size_t)y * w + x], c2 = both ? rt[(size_t)y * w + x] : 0.f;
-    uint64_t code = 0, code2 = 0;
+    uint64_t code = 0, code2 = 0, hi = 0, hi2 = 0;
     for (int j = -r; j <= r; j++)
         for (int i = -r; i <= r; i++) {
             if (i == 0 && j == 0) continue;
@@ -261,11 +265,20 @@ __global__ void census_pair_kernel(const float *__restrict__ img, const float *_
                 bit = c < img[(size_t)yy * w + xx];
                 if (both) bit2 = c2 < rt[(size_t)yy * w + xx];
             }
-            code = (code << 1) | bit;
-            code2 = (code2 << 1) | bit2;
+            if constexpr (NW == 2) {
+                census_push(code, hi, bit);
+                census_push(code2, hi2, bit2);
+            } else {
+                code = (code << 1) | bit;
+                code2 = (code2 << 1) | bit2;
+            }
         }
     codes[(size_t)y * w + x] = code;
     codes_rt[(size_t)y * w + x] = both ? code2 : code;
+    if constexpr (NW == 2) {
+        codes_hi[(size_t)y * w + x] = hi;
+        codes_rt_hi[(size_t)y * w + x] = both ? hi2 : hi;
+    }
 }
 
 }  // namespace s2pb

@@ -9,21 +9,26 @@ namespace s2pb {
 
 // census_tools.cc:38-57: neighbours in row-major window order, centre skipped,
 // bit = (centre < neighbour), out-of-image neighbour compares as NaN -> 0.
-__global__ void census_kernel(const float *__restrict__ img, int w, int h, int r, uint64_t *__restrict__ codes)
+// NW = census_words(win): 2 for the codes of more than 64 bits (sides 9 and 11), shifted through the pair (codes_hi : codes);
+// the Hamming distance does not depend on where a bit sits as long as both codes put it in the same place.
+template <int NW>
+__global__ void census_kernel(const float *__restrict__ img, int w, int h, int r, uint64_t *__restrict__ codes, uint64_t *__restrict__ codes_hi)
 {
     int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
     if (x >= w || y >= h) return;
     float c = img[(size_t)y * w + x];
-    uint64_t code = 0;
+    uint64_t code = 0, hi = 0;
     for (int j = -r; j <= r; j++)
         for (int i = -r; i <= r; i++) {
             if (i == 0 && j == 0) continue;
             int xx = x + i, yy = y + j;
             unsigned bit = 0;
             if (xx >= 0 && xx < w && yy >= 0 && yy < h) bit = c < img[(size_t)yy * w + xx];
-            code = (code << 1) | bit;
+            if constexpr (NW == 2) census_push(code, hi, bit);
+            else code = (code << 1) | bit;
         }
     codes[(size_t)y * w + x] = code;
+    if constexpr (NW == 2) codes_hi[(size_t)y * w + x] = hi;
 }
 
 // main_mgm.cc:172-173,178,207,210-216: NaN -> 0 and the per-pixel label range of one view.
@@ -56,13 +61,15 @@ __global__ void has_nan_kernel(const float *__restrict__ in, int n, int *flag)
 // finite, the whole range is set to 0.  Slots outside [lo,hi] stay +INF.
 // With ZOOMFACTOR = 2 (mgm_costvolume.cc:145-154) label o compares cu(x) with the census of the matched image
 // shifted by (o mod 2)/2 pixel, at column x + floor(o/2): cv = shift 0, cv1 = shift 1/2.
-// NARROW: the census codes fit 32 bits (3x3 and 5x5 windows: 8 and 24 bits), so one POPC on the low words does it.
+// BITS, the width of the census codes: 32 when they fit the low words (3x3 and 5x5 windows: 8 and 24 bits), so one POPC on
+// those does it; 64 (7x7: 48 bits); 128 (9x9 and 11x11: 80 and 120 bits), the second words in cuh / cvh / cv1h.
 // The Hamming distance is stored as its 8-bit code (agg_kernel.cuh), four labels per 32-bit word, with no conversion
 // instruction on the quarter-rate pipe that POPC uses.
-template <int LPL, bool ZOOM2, bool NARROW>
+template <int LPL, bool ZOOM2, int BITS>
 __global__ void cost_kernel(const uint64_t *__restrict__ cu, const uint64_t *__restrict__ cv, const uint64_t *__restrict__ cv1,
                             int w, int h,
-                            const short *__restrict__ lo, const short *__restrict__ hi, int gmin, uint8_t *__restrict__ C)
+                            const short *__restrict__ lo, const short *__restrict__ hi, int gmin, uint8_t *__restrict__ C,
+                            const uint64_t *__restrict__ cuh, const uint64_t *__restrict__ cvh, const uint64_t *__restrict__ cv1h)
 {
     constexpr int DP = 32 * LPL;
     int lane = threadIdx.x & 31;
@@ -71,7 +78,7 @@ __global__ void cost_kernel(const uint64_t *__restrict__ cu, const uint64_t *__r
     for (size_t p = warp; p < npix; p += nwarps) {
         int x = (int)(p % w);
         size_t row = p - x;
-        const uint64_t a = cu[p];
+        const uint64_t a = cu[p], ah = BITS == 128 ? cuh[p] : 0;
         const int l = lo[p], hgh = hi[p];
         unsigned cnt[LPL];                   // Hamming distance where the label has one, else 0
         unsigned okm = 0, inm = 0;           // bit e: label e has a distance / lies in the pixel's range
@@ -82,11 +89,12 @@ __global__ void cost_kernel(const uint64_t *__restrict__ cu, const uint64_t *__r
             if (o >= l && o <= hgh) {
                 inm |= 1u << e;
                 int q = x + o;
-                const uint64_t *codes = cv;
-                if (ZOOM2) { q = x + (o >> 1); if (o & 1) codes = cv1; }          // floor(o/2), goodmod(o,2)
+                const uint64_t *codes = cv, *codes_hi = cvh;
+                if (ZOOM2) { q = x + (o >> 1); if (o & 1) { codes = cv1; codes_hi = cv1h; } }     // floor(o/2), goodmod(o,2)
                 if (q >= 0 && q < w) {
-                    if constexpr (NARROW) cnt[e] = __popc((unsigned)a ^ reinterpret_cast<const unsigned *>(codes)[2 * (row + q)]);
+                    if constexpr (BITS == 32) cnt[e] = __popc((unsigned)a ^ reinterpret_cast<const unsigned *>(codes)[2 * (row + q)]);
                     else cnt[e] = __popcll(a ^ codes[row + q]);
+                    if constexpr (BITS == 128) cnt[e] += __popcll(ah ^ codes_hi[row + q]);
                     okm |= 1u << e;
                 }
             }
@@ -186,6 +194,7 @@ struct CostGenParams {
     const short *lo, *hi;
     int w, h, gmin, cost, win, zoom;
     float *C;
+    const uint64_t *cuh, *cv0h, *cv1h; // the second words of the census codes of more than 64 bits (census_words(win) = 2), else null
 };
 
 __device__ __forceinline__ float bt_cost(const float *__restrict__ u, const float *__restrict__ v, int w, size_t row, int x, int qx)
@@ -274,7 +283,7 @@ __device__ __forceinline__ bool cost_gen_labels(const CostGenParams &P, size_t p
                 for (int e = 0; e < LPL; e++)
                     if (ok[e]) c[e] = fmaf(ut, vq[e][r + q[e] + i], c[e]);
             }
-        const float n = (float)(P.win * P.win);
+        const float n = (float)((2 * hw + 1) * (2 * hw + 1));        // the taps (mgm_costvolume.h:152-180)
         const float2 sa = pin ? P.su[p] : make_float2(0.f, 0.f);
 #pragma unroll
         for (int e = 0; e < LPL; e++)
@@ -295,7 +304,9 @@ __device__ __forceinline__ bool cost_gen_labels(const CostGenParams &P, size_t p
             if (q >= 0 && q < w) {
                 if (P.cost == kCostCensus) {
                     const uint64_t *codes = half ? P.cv1 : P.cv0;
-                    val = P.lut[__popcll(P.cu[p] ^ codes[row + q])];
+                    int r = __popcll(P.cu[p] ^ codes[row + q]);
+                    if (P.cuh) r += __popcll(P.cuh[p] ^ (half ? P.cv1h : P.cv0h)[row + q]);
+                    val = P.lut[r];
                 } else {
                     const float *v = half ? P.v1 : P.v0;
                     if (P.cost == kCostBTAD || P.cost == kCostBTSD) {
@@ -358,10 +369,12 @@ __global__ void unpad_cost_kernel(const float *__restrict__ C, size_t npix, int 
 // chunks [ea, eb] that hold a pixel's label range (slot 32*e + lane); the chunk-skipping aggregation and WTA never
 // read the others.  Same values as cost_kernel on those chunks, including +INF on the slots of an active chunk that
 // lie outside the range and the all-invalid -> 0 rule (mgm_costvolume.cc:166-171).
-template <bool ZOOM2>
+// BITS: 64, or 128 with the codes' second words in cuh / cvh / cv1h (as cost_kernel).
+template <bool ZOOM2, int BITS>
 __global__ void cost_chunked_kernel(const uint64_t *__restrict__ cu, const uint64_t *__restrict__ cv, const uint64_t *__restrict__ cv1,
                                     int w, int h, const short *__restrict__ lo, const short *__restrict__ hi, int gmin, int DP,
-                                    uint8_t *__restrict__ C)
+                                    uint8_t *__restrict__ C, const uint64_t *__restrict__ cuh, const uint64_t *__restrict__ cvh,
+                                    const uint64_t *__restrict__ cv1h)
 {
     const int lane = threadIdx.x & 31;
     const size_t npix = (size_t)w * h;
@@ -369,7 +382,7 @@ __global__ void cost_chunked_kernel(const uint64_t *__restrict__ cu, const uint6
     for (size_t p = warp; p < npix; p += nwarps) {
         const int x = (int)(p % w);
         const size_t row = p - x;
-        const uint64_t a = cu[p];
+        const uint64_t a = cu[p], ah = BITS == 128 ? cuh[p] : 0;
         const int l = lo[p], hgh = hi[p];
         const int ea = (l - gmin) >> 5, eb = (hgh - gmin) >> 5;
         uint8_t *dst = C + p * DP;
@@ -380,9 +393,13 @@ __global__ void cost_chunked_kernel(const uint64_t *__restrict__ cu, const uint6
             bool ok = false;
             if (o >= l && o <= hgh) {
                 int q = x + o;
-                const uint64_t *codes = cv;
-                if (ZOOM2) { q = x + (o >> 1); if (o & 1) codes = cv1; }
-                if (q >= 0 && q < w) { cnt = __popcll(a ^ codes[row + q]); ok = anyfinite = true; }
+                const uint64_t *codes = cv, *codes_hi = cvh;
+                if (ZOOM2) { q = x + (o >> 1); if (o & 1) { codes = cv1; codes_hi = cv1h; } }
+                if (q >= 0 && q < w) {
+                    cnt = __popcll(a ^ codes[row + q]);
+                    if constexpr (BITS == 128) cnt += __popcll(ah ^ codes_hi[row + q]);
+                    ok = anyfinite = true;
+                }
             }
             dst[32 * e + lane] = (uint8_t)cost_encode(cnt, ok);
         }

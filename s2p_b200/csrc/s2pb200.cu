@@ -93,6 +93,9 @@ static int slot_layout(Slot &s, int w, int h, int DP, int ndir, int cbytes, bool
     }
     size_t o;
     o = take(256); if (allocate) s.next_item = (int *)(b + o);
+    // the popcount -> cost table (kCostLut floats) runs on into the head of Ydct (256 bytes or more), which only the round trips
+    // at the start of mgm_call use: mgm_call uploads the table after them
+    static_assert(kCostLut * sizeof(float) <= 512, "the cost table overflows lut + the head of Ydct");
     o = take(256); if (allocate) s.lut = (float *)(b + o);
     o = take(npix * 8); if (allocate) s.Ydct = (double *)(b + o);
     if (!allocate) s.bytes = off;
@@ -390,14 +393,25 @@ static bool other_aggregation_pending(s2pb_ctx *ctx, const Slot &me)
 
 // ------------------------------------------------------------------ stage launchers
 
+// CENSUS_NCC_WIN: the reference takes any win and uses win / 2 as the radius (mgm_costvolume.cc:109).  win <= 1 gives codes
+// of no bit, whose cost is 0 / 0; from 12 on (side 13) the popcount overflows the 8-bit cost codes (agg_kernel.cuh)
+static int census_win_ok(int win)
+{
+    if (win < 2) return fail(S2PB_ERR_ARG, "census window must be at least 2 (got %d)", win);
+    if (win > 11) return fail(S2PB_ERR_UNSUPPORTED, "census windows wider than 11 are not supported (got %d)", win);
+    return S2PB_OK;
+}
+
 static int check_params(const s2pb_mgm_params *p, int w, int h, int dmin, int dmax)
 {
     if (!p) return fail(S2PB_ERR_ARG, "null params");
+    int rc;
     if (w < 2 || h < 2) return fail(S2PB_ERR_ARG, "image too small (%dx%d)", w, h);
     if (dmax <= dmin) return fail(S2PB_ERR_ARG, "need dmin < dmax (got %d, %d)", dmin, dmax);
     if (p->ndir != 2 && p->ndir != 4 && p->ndir != 8) return fail(S2PB_ERR_ARG, "ndir must be 2, 4 or 8");
     if (p->tsgm < 1 || p->tsgm > 4) return fail(S2PB_ERR_ARG, "tsgm must be 1..4");
-    if (p->census_win != 3 && p->census_win != 5 && p->census_win != 7) return fail(S2PB_ERR_ARG, "census_win must be 3, 5 or 7");
+    rc = census_win_ok(p->census_win);
+    if (rc != S2PB_OK) return rc;
     if (p->median < 0 || p->median > 2) return fail(S2PB_ERR_ARG, "median radius must be 0..2");
     if (p->refine < 0 || p->refine > 2) return fail(S2PB_ERR_ARG, "refine must be 0 (none), 1 (vfit) or 2 (parabola)");
     if (p->subpix != 1 && p->subpix != 2) return fail(S2PB_ERR_UNSUPPORTED, "SUBPIX must be 1 or 2");
@@ -411,13 +425,14 @@ static int check_params(const s2pb_mgm_params *p, int w, int h, int dmin, int dm
     return S2PB_OK;
 }
 
-// cost LUT for scaled census costs: cost(r) = (float)((double)r * ratio / nch), mgm_costvolume.h:90-91
-static bool cost_lut(int win, float lut[64])
+// cost LUT for scaled census costs: cost(r) = (float)((double)r * ratio / nch), mgm_costvolume.h:90-91.  The code's bits and
+// its float channels nch come from the window's side (census_tools.cc:76-99), the ratio 25 / win^2 from win itself.
+static bool cost_lut(int win, float lut[kCostLut])
 {
-    int nbits = win * win - 1, nch = (nbits / 8 + 3) / 4;
+    const int nbits = census_bits(win), nch = (nbits / 8 + 3) / 4;
     const float ratio = (float)(5 * 5 / ((double)win * win));
     bool identity = true;
-    for (int r = 0; r < 64; r++) {
+    for (int r = 0; r < kCostLut; r++) {
         float fr = (float)r;
         lut[r] = (float)((double)fr * 1.0 * (double)ratio / nch);
         if (lut[r] != fr) identity = false;
@@ -564,23 +579,26 @@ template <class F> static int with_lpl(int LPL, F &&f)
     return fail(S2PB_ERR_UNSUPPORTED, "unsupported labels-per-lane %d", LPL);
 }
 
-// census 3x3 / 5x5 up to 8 labels per lane: the strip-staged kernel; 7x7, the half-pixel pass and 12 / 16 labels per lane: the
-// per-pixel one
-template <int LPL> static void launch_cost_t(s2pb_ctx *ctx, const uint64_t *cu, const uint64_t *cv, const uint64_t *cv1, int zoom, bool narrow,
-                                             int w, int h, const short *lo, const short *hi, int gmin, uint8_t *C, cudaStream_t st)
+// census 3x3 / 5x5 up to 8 labels per lane: the strip-staged kernel; wider windows, the half-pixel pass and 12 / 16 labels per
+// lane: the per-pixel one, for codes of `bits` bits (cost_kernel's BITS)
+template <int LPL> static void launch_cost_t(s2pb_ctx *ctx, const CostGenParams &G, int bits, uint8_t *C, cudaStream_t st)
 {
     const int sm = ctx->sm_count;
-    if (zoom == 2) {
-        if (narrow) launch(ctx, cost_kernel<LPL, true, true>, sm * 8, 256, 0, st, cu, cv, cv1, w, h, lo, hi, gmin, C);
-        else launch(ctx, cost_kernel<LPL, true, false>, sm * 8, 256, 0, st, cu, cv, cv1, w, h, lo, hi, gmin, C);
-    } else if (!narrow) launch(ctx, cost_kernel<LPL, false, false>, sm * 8, 256, 0, st, cu, cv, cv1, w, h, lo, hi, gmin, C);
-    else if constexpr (LPL <= 8) launch(ctx, cost_strip_kernel<LPL>, sm * 16, kCostStripThreads, 0, st, cu, cv, w, h, lo, hi, gmin, C);
-    else launch(ctx, cost_kernel<LPL, false, true>, sm * 8, 256, 0, st, cu, cv, cv1, w, h, lo, hi, gmin, C);
+    auto go = [&](auto kernel) { launch(ctx, kernel, sm * 8, 256, 0, st, G.cu, G.cv0, G.cv1, G.w, G.h, G.lo, G.hi, G.gmin, C, G.cuh, G.cv0h, G.cv1h); };
+    if (G.zoom == 2) {
+        if (bits == 32) go(cost_kernel<LPL, true, 32>);
+        else if (bits == 64) go(cost_kernel<LPL, true, 64>);
+        else go(cost_kernel<LPL, true, 128>);
+    } else if (bits == 64) go(cost_kernel<LPL, false, 64>);
+    else if (bits == 128) go(cost_kernel<LPL, false, 128>);
+    else if constexpr (LPL <= 8) launch(ctx, cost_strip_kernel<LPL>, sm * 16, kCostStripThreads, 0, st, G.cu, G.cv0, G.w, G.h, G.lo, G.hi, G.gmin, C);
+    else go(cost_kernel<LPL, false, 32>);
 }
 
 // The cost volume of one view into G.C.  general: float costs of G.cost (census through G.lut included); else the 8-bit census
 // codes of G.cu against G.cv0 (G.cv1 at odd labels when G.zoom = 2), read as bytes from G.C, where G.win <= 5 leaves the high
-// word of a code zero.  A wide slab (wide_slab) is written only on the chunks of each pixel's span.
+// half of a code zero and G.win >= 8 puts its second word in G.cuh / G.cv0h / G.cv1h.  A wide slab (wide_slab) is written only
+// on the chunks of each pixel's span.
 static int launch_cost(s2pb_ctx *ctx, int LPL, bool general, const CostGenParams &G, cudaStream_t st)
 {
     const int sm = ctx->sm_count;
@@ -588,14 +606,19 @@ static int launch_cost(s2pb_ctx *ctx, int LPL, bool general, const CostGenParams
     int rc = S2PB_OK;
     if (wide_slab(LPL)) {
         if (general) launch(ctx, cost_gen_chunked_kernel, sm * 8, 256, 0, st, G, 32 * LPL);
-        else if (G.zoom == 2) launch(ctx, cost_chunked_kernel<true>, sm * 8, 256, 0, st, G.cu, G.cv0, G.cv1, G.w, G.h, G.lo, G.hi, G.gmin, 32 * LPL, C8);
-        else launch(ctx, cost_chunked_kernel<false>, sm * 8, 256, 0, st, G.cu, G.cv0, nullptr, G.w, G.h, G.lo, G.hi, G.gmin, 32 * LPL, C8);
+        else {
+            auto go = [&](auto kernel) { launch(ctx, kernel, sm * 8, 256, 0, st, G.cu, G.cv0, G.cv1, G.w, G.h, G.lo, G.hi, G.gmin, 32 * LPL, C8, G.cuh, G.cv0h, G.cv1h); };
+            const bool wide = census_words(G.win) == 2;
+            if (G.zoom == 2) { if (wide) go(cost_chunked_kernel<true, 128>); else go(cost_chunked_kernel<true, 64>); }
+            else if (wide) go(cost_chunked_kernel<false, 128>);
+            else go(cost_chunked_kernel<false, 64>);
+        }
     } else if (general) {
         rc = with_lpl(LPL, [&](auto k) { constexpr int K = decltype(k)::value; launch(ctx, cost_gen_kernel<K>, sm * 8, 256, 0, st, G); });
     } else {
         rc = with_lpl(LPL, [&](auto k) {
             constexpr int K = decltype(k)::value;
-            launch_cost_t<K>(ctx, G.cu, G.cv0, G.cv1, G.zoom, G.win <= 5, G.w, G.h, G.lo, G.hi, G.gmin, C8, st);
+            launch_cost_t<K>(ctx, G, G.win <= 5 ? 32 : census_words(G.win) == 2 ? 128 : 64, C8, st);
         });
     }
     if (rc != S2PB_OK) return rc;
@@ -852,9 +875,13 @@ static int mgm_call(s2pb_ctx *ctx, const MatchCall &c, int w, int h, const float
     const size_t npix = (size_t)w * h;
     dim3 b2(32, 8);
     int rc;
-    float lut_h[64];
-    const float *lut = nullptr;
-    if (cost_lut(p->census_win, lut_h) || general) { CK(cudaMemcpyAsync(s.lut, lut_h, sizeof lut_h, cudaMemcpyHostToDevice, st)); lut = s.lut; }
+    // codes of more than 64 bits (census_words): the second words of each view's two codes go to the head of the view's last pass
+    // volume (resident) or of its S (folded), 16 bytes a pixel of a region of at least 128 that the aggregation writes only
+    // after the cost stage has read them
+    const bool wide = census && census_words(p->census_win) == 2;
+    uint64_t *hi_words[2] = {nullptr, nullptr};
+    if (wide)
+        for (int vi = 0; vi < 2; vi++) hi_words[vi] = (uint64_t *)(s.folded ? s.v[vi].S : s.v[vi].L[p->ndir - 1]);
     // ---- census of both images and of the copies the other view matches against
     for (int vi = 0; vi < 2; vi++) {
         ViewWS &v = s.v[vi];
@@ -862,26 +889,40 @@ static int mgm_call(s2pb_ctx *ctx, const MatchCall &c, int w, int h, const float
         // v.rt = shift(img[vi], 0): the reference's DCT round trip (mgm_costvolume.cc:50-60)
         rc = round_trip_zero(ctx, img[vi], w, h, v.rt, v.rtstate, v.rowlist, v.rowthr, s.Ydct, st);
         if (rc != S2PB_OK) return rc;
-        if (census) launch(ctx, census_pair_kernel, grid2d(w, h, b2), b2, 0, st, img[vi], v.rt, v.rtstate, w, h, p->census_win / 2, v.census, v.census_rt);
+        if (census && wide)
+            launch(ctx, census_pair_kernel<2>, grid2d(w, h, b2), b2, 0, st, img[vi], v.rt, v.rtstate, w, h, p->census_win / 2, v.census,
+                   v.census_rt, hi_words[vi], hi_words[vi] + npix);
+        else if (census)
+            launch(ctx, census_pair_kernel<1>, grid2d(w, h, b2), b2, 0, st, img[vi], v.rt, v.rtstate, w, h, p->census_win / 2, v.census,
+                   v.census_rt, nullptr, nullptr);
         if (ncc) {     // window statistics in the (then unused) census buffers: 8 B / pixel
             launch(ctx, ncc_stats_kernel, grid2d(w, h, b2), b2, 0, st, img[vi], w, h, p->census_win / 2, (float2 *)v.census);
             launch(ctx, ncc_stats_kernel, grid2d(w, h, b2), b2, 0, st, v.rt, w, h, p->census_win / 2, (float2 *)v.census_rt);
         }
     }
     // ZOOMFACTOR 2: shf[vi] = shift(img[vi], 1/2) (kept for the image-domain distances) and its census, in the pyramid arena
+    // (mgm_multi_enqueue sizes it for two full-size mgm_calls: the half-pixel pass, second words included, takes less than one)
     float *shf[2] = {nullptr, nullptr};
-    uint64_t *cen_half[2] = {nullptr, nullptr};
+    uint64_t *cen_half[2] = {nullptr, nullptr}, *cen_half_hi[2] = {nullptr, nullptr};
     if (zoom == 2) {
-        for (int vi = 0; vi < 2; vi++) { shf[vi] = arena_take<float>(s, npix); cen_half[vi] = arena_take<uint64_t>(s, npix); }
+        for (int vi = 0; vi < 2; vi++) {
+            shf[vi] = arena_take<float>(s, npix); cen_half[vi] = arena_take<uint64_t>(s, npix);
+            if (wide) cen_half_hi[vi] = arena_take<uint64_t>(s, npix);
+        }
         double *scratch = arena_take<double>(s, npix * 4);
         if (!scratch) return fail(S2PB_ERR_NOMEM, "pyramid arena exhausted");
         for (int vi = 0; vi < 2; vi++) {
             rc = shift_half(ctx, img[vi], w, h, shf[vi], scratch, st);
             if (rc != S2PB_OK) return rc;
-            if (census) launch(ctx, census_kernel, grid2d(w, h, b2), b2, 0, st, shf[vi], w, h, p->census_win / 2, cen_half[vi]);
+            if (census && wide) launch(ctx, census_kernel<2>, grid2d(w, h, b2), b2, 0, st, shf[vi], w, h, p->census_win / 2, cen_half[vi], cen_half_hi[vi]);
+            else if (census) launch(ctx, census_kernel<1>, grid2d(w, h, b2), b2, 0, st, shf[vi], w, h, p->census_win / 2, cen_half[vi], nullptr);
             if (ncc) launch(ctx, ncc_stats_kernel, grid2d(w, h, b2), b2, 0, st, shf[vi], w, h, p->census_win / 2, (float2 *)cen_half[vi]);
         }
     }
+    // the round trips are done with Ydct, whose head the cost table takes (slot_layout)
+    float lut_h[kCostLut];
+    const float *lut = nullptr;
+    if (cost_lut(p->census_win, lut_h) || general) { CK(cudaMemcpyAsync(s.lut, lut_h, sizeof lut_h, cudaMemcpyHostToDevice, st)); lut = s.lut; }
     CK(cudaGetLastError());
     if (timed) CK(cudaEventRecord(s.ev[1], st));
     // ---- cost volumes: view 0 = left reference, view 1 = right reference (mgm_multiscale.cc:222,270)
@@ -891,6 +932,7 @@ static int mgm_call(s2pb_ctx *ctx, const MatchCall &c, int w, int h, const float
         memset(&G, 0, sizeof G);
         G.u = img[vi]; G.v0 = o.rt; G.v1 = shf[1 - vi];
         G.cu = v.census; G.cv0 = o.census_rt; G.cv1 = cen_half[1 - vi];
+        if (wide) { G.cuh = hi_words[vi]; G.cv0h = hi_words[1 - vi] + npix; G.cv1h = cen_half_hi[1 - vi]; }
         G.su = (const float2 *)G.cu; G.sv0 = (const float2 *)G.cv0; G.sv1 = (const float2 *)G.cv1;
         G.lut = s.lut; G.lo = lo[vi]; G.hi = hi[vi];
         G.w = w; G.h = h; G.gmin = gminv[vi]; G.cost = p->cost; G.win = p->census_win; G.zoom = zoom;
@@ -1444,7 +1486,7 @@ extern "C" int s2pb_census(s2pb_ctx *ctx, const float *img, int w, int h, int wi
     uint64_t *b = L.take<uint64_t>(npix * 8);
     if (int rc = L.error()) return rc;
     dim3 b2(32, 8);
-    launch(ctx, census_kernel, grid2d(w, h, b2), b2, 0, L.st, a, w, h, win / 2, b);
+    launch(ctx, census_kernel<1>, grid2d(w, h, b2), b2, 0, L.st, a, w, h, win / 2, b, nullptr);
     CK(cudaGetLastError());
     L.download(codes, b, npix * 8);
     return L.finish();
@@ -1470,20 +1512,24 @@ static int stage_costvolume(s2pb_ctx *ctx, const float *u, const float *v, int w
                             int gmin, int D, int win, int cost, bool codes, float *C)
 {
     if (!ctx || !u || !v || !lo || !hi || !C || w < 1 || h < 1 || D < 1) return fail(S2PB_ERR_ARG, "bad argument");
-    if (win != 3 && win != 5 && win != 7) return fail(S2PB_ERR_ARG, "window must be 3, 5 or 7");
+    int rc = census_win_ok(win);
+    if (rc != S2PB_OK) return rc;
     if (cost < 0 || cost >= S2PB_COST_COUNT) return fail(S2PB_ERR_ARG, "cost must be one of S2PB_COST_*");
-    int LPL, rc = slab_lpl(D, &LPL);      // the stage entry points run the register-resident kernels only
+    int LPL;
+    rc = slab_lpl(D, &LPL);               // the stage entry points run the register-resident kernels only
     if (rc == S2PB_OK && wide_slab(LPL)) rc = fail(S2PB_ERR_UNSUPPORTED, "the stage entry points take at most 512 labels, not %d", D);
     if (rc != S2PB_OK) return rc;
     const int DP = 32 * LPL;
     size_t npix = (size_t)w * h, tot = npix * D;
-    float lut_h[64];
+    float lut_h[kCostLut];
     const bool scaled = cost_lut(win, lut_h);
+    const bool wide = cost == S2PB_COST_CENSUS && census_words(win) == 2;
     HostCall L(ctx, "the cost volume");
     float *du = L.upload(u, npix * 4), *dv = L.upload(v, npix * 4);
-    uint64_t *cu = L.take<uint64_t>(npix * 8), *cv = L.take<uint64_t>(npix * 8);      // census codes or NCC window statistics
+    // census codes (their second words after the first npix when wide) or NCC window statistics
+    uint64_t *cu = L.take<uint64_t>(npix * 8 * (wide ? 2 : 1)), *cv = L.take<uint64_t>(npix * 8 * (wide ? 2 : 1));
     void *dC = L.take<void>(npix * DP * (codes ? 1 : 4));
-    float *dCf = L.take<float>(tot * 4), *dlut = L.upload(lut_h, 256);
+    float *dCf = L.take<float>(tot * 4), *dlut = L.upload(lut_h, sizeof lut_h);
     short *dlo, *dhi;
     rc = upload_ranges(L, lo, hi, npix, gmin, D, &dlo, &dhi);
     if (rc == S2PB_OK) rc = L.error();
@@ -1492,9 +1538,12 @@ static int stage_costvolume(s2pb_ctx *ctx, const float *u, const float *v, int w
     rc = stage_round_trip(ctx, L, dv, w, h, L.st, &rt);
     if (rc != S2PB_OK) return rc;
     dim3 b2(32, 8);
-    if (cost == S2PB_COST_CENSUS) {
-        launch(ctx, census_kernel, grid2d(w, h, b2), b2, 0, L.st, du, w, h, win / 2, cu);
-        launch(ctx, census_kernel, grid2d(w, h, b2), b2, 0, L.st, rt, w, h, win / 2, cv);
+    if (wide) {
+        launch(ctx, census_kernel<2>, grid2d(w, h, b2), b2, 0, L.st, du, w, h, win / 2, cu, cu + npix);
+        launch(ctx, census_kernel<2>, grid2d(w, h, b2), b2, 0, L.st, rt, w, h, win / 2, cv, cv + npix);
+    } else if (cost == S2PB_COST_CENSUS) {
+        launch(ctx, census_kernel<1>, grid2d(w, h, b2), b2, 0, L.st, du, w, h, win / 2, cu, nullptr);
+        launch(ctx, census_kernel<1>, grid2d(w, h, b2), b2, 0, L.st, rt, w, h, win / 2, cv, nullptr);
     }
     if (cost == S2PB_COST_NCC) {
         launch(ctx, ncc_stats_kernel, grid2d(w, h, b2), b2, 0, L.st, du, w, h, win / 2, (float2 *)cu);
@@ -1503,6 +1552,7 @@ static int stage_costvolume(s2pb_ctx *ctx, const float *u, const float *v, int w
     CostGenParams G;
     memset(&G, 0, sizeof G);
     G.u = du; G.v0 = rt; G.cu = cu; G.cv0 = cv;
+    if (wide) { G.cuh = cu + npix; G.cv0h = cv + npix; }
     G.su = (float2 *)cu; G.sv0 = (float2 *)cv;
     G.lut = dlut; G.lo = dlo; G.hi = dhi;
     G.w = w; G.h = h; G.gmin = gmin; G.cost = cost; G.win = win; G.zoom = 1; G.C = (float *)dC;

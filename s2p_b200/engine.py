@@ -32,6 +32,13 @@ def default_params(algo="mgm", **overrides):
     return p
 
 
+def census_window_served(win):
+    """Whether the device matcher serves CENSUS_NCC_WIN = ``win`` (s2p's ``census_ncc_win``): 2 to 11, windows of side 3 to 11.
+    The reference takes win / 2 as the radius of any win; win <= 1 gives codes of no bit (every cost 0 / 0) and from 12 on the
+    popcount no longer fits the 8-bit cost codes, so those windows go to the reference's own binaries."""
+    return 2 <= int(win) <= 11
+
+
 def device_count():
     return _lib.lib().s2pb_device_count()
 

@@ -24,7 +24,7 @@ import numpy as np
 from . import _lib, cloud, common, projection, rasterio_compat as rio, triangulation
 from .block_matching import _NATIVE, SGBM_ARGS, confidence_path, disparity_bounds, matcher_params
 from .common import needed_roi
-from .engine import Engine, S2pbError, get_engine
+from .engine import Engine, S2pbError, census_window_served, get_engine
 
 
 def _crop(im, H, w, h):
@@ -79,6 +79,9 @@ def fall_through_reason(cfg):
         return "not a two-view run"
     if cfg['matching_algorithm'] not in SERVED:
         return "algo %r is not served" % cfg['matching_algorithm']
+    window = _window_unserved(cfg)
+    if window:
+        return window
     if projection.utm_target(cfg['out_crs']) is None:
         return projection.unserved_reason(cfg['out_crs'])
     if not cloud.numpy_stretch_is_float64():
@@ -86,6 +89,15 @@ def fall_through_reason(cfg):
     clr = cfg['images'][0]['clr']
     if clr and not cloud._clr_bands_ok(clr):
         return "the clr image does not open with 1, 3 or 4 bands"
+    return None
+
+
+def _window_unserved(cfg):
+    """the reason when the matcher's census window (the mgm algos' CENSUS_NCC_WIN; s2p's default is 5) is one the device does
+    not serve, or None"""
+    win = cfg.get('census_ncc_win', 5)
+    if cfg['matching_algorithm'] in _NATIVE and not census_window_served(win):
+        return "census_ncc_win %r is not served" % win
     return None
 
 
@@ -220,7 +232,7 @@ def pair_heights_fall_through_reason(cfg):
         return "not a tri-stereo run"
     if cfg['matching_algorithm'] not in SERVED:
         return "algo %r is not served" % cfg['matching_algorithm']
-    return None
+    return _window_unserved(cfg)
 
 
 def pair_heights(tile, i, engine=None):
