@@ -259,7 +259,7 @@ typedef struct s2pb_rpc {
  * (1..60, or 0: the output is lon, lat, alt as disp_to_lonlatalt writes them) and south (non-zero: false northing
  * 10 000 000 m).  The cloud is triangulated and projected as s2pb_lonlat_to_utm projects it on the device; xyz (nx*ny*3
  * float64) and err (nx*ny float32) come back.
- * S2PB_ERR_ARG: a null pointer, a size below 1, a zone outside 0..60 (S2PB_ZONE_EGM96 aside). */
+ * S2PB_ERR_ARG: a null pointer, a size below 1, a zone outside 0..60 (S2PB_ZONE_EGM96 and S2PB_ZONE_PROJ aside). */
 int s2pb_disp_to_xyz(s2pb_ctx *ctx, double *xyz, float *err, const float *dispx, const float *dispy, const float *msk, int nx,
                      int ny, const float *msk_orig, int w, int h, const double ha[9], const double hb[9], const s2pb_rpc *rpca,
                      const s2pb_rpc *rpcb, const float orig_img_bounding_box[4], int zone, int south);
@@ -291,6 +291,44 @@ int s2pb_lonlat_to_utm(s2pb_ctx *ctx, double *xyz, const double *lonlatalt, int6
  * S2PB_ERR_ARG: w or h below 2, w * h above 2^31 - 1, a non-finite origin, a spacing that is not positive and finite, a grid
  * that is not global.  S2PB_ERR_NOMEM: the grid does not fit the device. */
 int s2pb_set_geoid(s2pb_ctx *ctx, const float *grid, int w, int h, double lon0, double lat0, double dlon, double dlat);
+
+/* Map projections other than the UTM zones of WGS84, for output CRSs whose datum reaches WGS84 through a null
+ * transformation, so that the cloud is the map of the triangulated WGS84 (lon, lat) and the altitude passes through: the
+ * ETRS89 UTM zones (EPSG 25828-25838, S2PB_PROJ_TM on GRS80) and RGF93 v1 / Lambert-93 and CC42-CC50 (EPSG 2154,
+ * 3942-3950, S2PB_PROJ_LCC on GRS80).  Angles in degrees, lengths in metres.
+ *   S2PB_PROJ_TM: transverse Mercator, the map of s2pb_lonlat_to_utm on the given ellipsoid, central meridian lon0, scale k0,
+ *     false easting x0 and northing y0; lat0 must be 0 (northings count from the equator); lat1 and lat2 are not read.
+ *   S2PB_PROJ_LCC: Lambert conic conformal with two standard parallels lat1 and lat2 (EPSG method 9802), false origin
+ *     (lon0, lat0) at (x0, y0); k0 is not read.  lat1 == lat2 gives the one-parallel cone.  In this operation order, with
+ *     psi(phi) = asinh(tan phi) - e atanh(e sin phi) and the host's n, a F and r_F (IOGP Guidance Note 7-2, 3.1.1.1):
+ *     lam = lon - lon0 reduced to [-180, 180], rho = a F exp(-(n psi)), theta = n lam, x = x0 + rho sin theta,
+ *     y = y0 + (r_F - rho cos theta).  A pole on the side the cone opens to maps to the apex (rho = 0); the other pole
+ *     gives +inf in all three coordinates. */
+#define S2PB_PROJ_TM 1
+#define S2PB_PROJ_LCC 2
+typedef struct s2pb_projection {
+    int32_t method;              /* S2PB_PROJ_TM or S2PB_PROJ_LCC */
+    double a, rf;                /* ellipsoid: semi-major axis, inverse flattening */
+    double lon0, lat0;           /* natural origin (TM) or false origin (LCC) */
+    double lat1, lat2;           /* standard parallels (LCC) */
+    double k0;                   /* scale factor on the central meridian (TM) */
+    double x0, y0;               /* false easting and northing */
+} s2pb_projection;
+/* OR S2PB_ZONE_PROJ, instead of a UTM zone, into the `zone` argument of s2pb_disp_to_xyz, s2pb_height_map_to_xyz and the PLY
+ * calls, or into the zone field of s2pb_pair_tile and s2pb_heights_tile: every point of that call then goes through the
+ * context's projection (s2pb_set_projection).  S2PB_ZONE_EGM96 may be OR'ed in too (heights above the geoid, then the map).
+ * S2PB_ERR_ARG: the flag on a context without a projection, with a nonzero south, or with any bit other than S2PB_ZONE_EGM96. */
+#define S2PB_ZONE_PROJ 0x200
+/* Hold *proj on the context for S2PB_ZONE_PROJ, replacing the one it holds (proj NULL: drop it).  Nothing is uploaded.
+ * S2PB_ERR_ARG: an unknown method; a, rf, k0 (TM), an angle, x0 or y0 not finite; a <= 0, rf <= 1; TM: k0 <= 0 or lat0 != 0;
+ * LCC: a standard parallel outside (-90, 90), lat1 == -lat2 (no cone), |lat0| > 90, lat0 the pole the cone does not reach.
+ * A refused projection leaves the one held in place. */
+int s2pb_set_projection(s2pb_ctx *ctx, const s2pb_projection *proj);
+/* EPSG:4979 -> the map *proj (checked as s2pb_set_projection checks it) for n points of three float64 (lon and lat in degrees,
+ * alt), host buffers (xyz may be lonlatalt).  The altitude passes through.  A point with a NaN coordinate becomes NaN in all
+ * three; a point the map cannot project (|lat| > 90, outside the TM domain of s2pb_lonlat_to_utm, the LCC pole away from
+ * the cone) +inf in all three.  S2PB_ERR_ARG: a null pointer with n > 0, n < 0, a refused projection. */
+int s2pb_lonlat_to_proj(s2pb_ctx *ctx, double *xyz, const double *lonlatalt, int64_t n, const s2pb_projection *proj);
 
 /* ---- tri-stereo height maps (s2p/__init__.py disparity_to_height and heights_fusion) ---- */
 /* s2p.triangulation.height_map (s2p/triangulation.py:346-389) in one call.  disp, msk: the rectified disparity and mask,
@@ -324,7 +362,7 @@ int s2pb_cargarse_basura(s2pb_ctx *ctx, const float *in, float *out, int w, int 
  * lat, alt as they are) north or south (south != 0) as s2pb_lonlat_to_utm projects it; xyz (w*h*3 float64) comes back.
  * The third coordinate is z bit for bit.  A NaN height gives NaN in all three (the reference leaves lon and lat undefined
  * there); an iteration whose residual turns NaN stops, as the reference's does, with a NaN lon and lat.
- * S2PB_ERR_ARG: a null pointer, a size below 1, a zone outside 0..60 (S2PB_ZONE_EGM96 aside), or pixels whose iteration did not meet the
+ * S2PB_ERR_ARG: a null pointer, a size below 1, a zone outside 0..60 (S2PB_ZONE_EGM96 and S2PB_ZONE_PROJ aside), or pixels whose iteration did not meet the
  * reference's stopping test within 1000 steps (the reference would not return; the message gives their number). */
 int s2pb_height_map_to_xyz(s2pb_ctx *ctx, double *xyz, const double *heights, int w, int h, const s2pb_rpc *rpc, double off_x,
                            double off_y, int zone, int south);
@@ -515,7 +553,7 @@ typedef struct s2pb_heights_tile {
     int32_t cargarse_basura, op;
     double threshold;
     /* height_map_to_xyz: the reference image's camera, the tile's origin in that image, the output UTM zone (0: lon, lat, alt;
-     * S2PB_ZONE_EGM96 may be OR'ed in) */
+     * S2PB_ZONE_PROJ instead: the context's projection; S2PB_ZONE_EGM96 may be OR'ed in) */
     const s2pb_rpc *rpc;
     double off_x, off_y;
     int32_t zone, south;

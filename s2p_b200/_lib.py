@@ -47,6 +47,14 @@ class PairTile(ctypes.Structure):
 
 MATCHER_MGM, MATCHER_SGBM = 0, 1     # S2PB_MATCHER_*
 ZONE_EGM96 = 0x100                   # S2PB_ZONE_EGM96
+ZONE_PROJ = 0x200                    # S2PB_ZONE_PROJ
+PROJ_TM, PROJ_LCC = 1, 2             # S2PB_PROJ_*
+
+
+class Projection(ctypes.Structure):
+    """Mirror of ``s2pb_projection``: a map projection for S2PB_ZONE_PROJ (angles in degrees, lengths in metres)."""
+    _fields_ = [("method", c_int32), ("a", c_double), ("rf", c_double), ("lon0", c_double), ("lat0", c_double), ("lat1", c_double),
+                ("lat2", c_double), ("k0", c_double), ("x0", c_double), ("y0", c_double)]
 MAX_FUSION = 16                      # S2PB_MAX_FUSION
 
 
@@ -113,6 +121,8 @@ _SIGNATURES = {
                                  POINTER(c_double), POINTER(c_double), c_void_p, c_void_p, _f, c_int, c_int]),
     "s2pb_lonlat_to_utm": (c_int, [c_void_p, POINTER(c_double), POINTER(c_double), c_int64, c_int, c_int]),
     "s2pb_set_geoid": (c_int, [c_void_p, _f, c_int, c_int, c_double, c_double, c_double, c_double]),
+    "s2pb_set_projection": (c_int, [c_void_p, POINTER(Projection)]),
+    "s2pb_lonlat_to_proj": (c_int, [c_void_p, POINTER(c_double), POINTER(c_double), c_int64, POINTER(Projection)]),
     "s2pb_height_map_to_xyz": (c_int, [c_void_p, POINTER(c_double), POINTER(c_double), c_int, c_int, c_void_p, c_double, c_double,
                                        c_int, c_int]),
     "s2pb_height_map": (c_int, [c_void_p, POINTER(c_double), _f, _f, c_int, c_int, _f, c_int, c_int, c_int, c_int, c_int, c_int,

@@ -12,8 +12,9 @@ with no temporary file; for tri-stereo, the tile's window of the image in its st
 ``s2pb_height_map_to_ply_clr``).
 
 The steps fall through to the original when the device path would not write the reference's file:
-- an output CRS other than WGS84 and its UTM zones, with or without EGM96 heights (those only where the grid is found; the
-  original then uses the installed ``disp_to_xyz`` / filter drop-ins);
+- an output CRS other than WGS84, its UTM zones, the ETRS89 UTM zones and the RGF93 v1 Lambert grids, with or without EGM96
+  heights (those only where the grid is found; ``projection.output_target``; the original then uses the installed
+  ``disp_to_xyz`` / filter drop-ins);
 - NumPy < 2, whose casting rules make the stretch float32;
 - colours whose band count the reference refuses, or whose type does not convert exactly to float32 (the original raises or
   stretches them itself);
@@ -109,7 +110,7 @@ def disparity_to_ply(tile, engine=None):
     import s2p
     from s2p.config import cfg
     original = getattr(s2p, "_s2pb_original_disparity_to_ply", None)
-    target = projection.utm_target(cfg['out_crs'])
+    target = projection.output_target(cfg['out_crs'])
     clr = cfg['images'][0]['clr']
     if original is not None and (target is None or not numpy_stretch_is_float64() or (clr and not _clr_bands_ok(clr))):
         return original(tile)
@@ -151,7 +152,7 @@ def disparity_to_ply(tile, engine=None):
     r, p, n = _filter_args(cfg)
     eng = engine or get_engine()
     cloud = (disp_img, mask_rect_img, mask_orig_img, H1, H2, triangulation._rpc_struct(rpc1), triangulation._rpc_struct(rpc2),
-             (x, x + w, y, y + h), *projection.utm_target(cfg['out_crs'], eng))
+             (x, x + w, y, y + h), *projection.output_target(cfg['out_crs'], eng))
     if clr:
         crop, hc = common.homography_crop(clr, H1, ww, hh, common.homography_cmd("<colours of %s>" % ply_file, clr, H1, ww, hh))
         records = eng.disp_to_ply_clr(*cloud, r=r, p=p, n=n, clr=crop, hc=hc, confidence=confidence)
@@ -174,7 +175,7 @@ def heights_to_ply(tile, engine=None):
     import s2p
     from s2p.config import cfg
     original = getattr(s2p, "_s2pb_original_heights_to_ply", None)
-    target = projection.utm_target(cfg['out_crs'])
+    target = projection.output_target(cfg['out_crs'])
     if original is not None and (target is None or not numpy_stretch_is_float64()):
         return original(tile)
     out_dir = tile['dir']
@@ -199,7 +200,7 @@ def heights_to_ply(tile, engine=None):
     heights = rasterio_compat.read_band_stored(height_map)
     r, p, n = _filter_args(cfg)
     eng = engine or get_engine()
-    cloud = (heights, triangulation._rpc_struct(cfg['images'][0]['rpcm']), x, y, *projection.utm_target(cfg['out_crs'], eng))
+    cloud = (heights, triangulation._rpc_struct(cfg['images'][0]['rpcm']), x, y, *projection.output_target(cfg['out_crs'], eng))
     if clr:
         records = eng.height_map_to_ply_clr(*cloud, r=r, p=p, n=n, colors=colors)
     else:

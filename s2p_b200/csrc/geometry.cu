@@ -44,10 +44,10 @@ int triangulated_cloud_device(s2pb_ctx *ctx, HostCall &L, const float *d_dx, con
 }
 
 int triangulated_cloud_args_ok(const s2pb_ctx *ctx, int nx, int ny, int w, int h, const double ha[9], const double hb[9],
-                               const s2pb_rpc *rpca, const s2pb_rpc *rpcb, const float bbox[4], int zone)
+                               const s2pb_rpc *rpca, const s2pb_rpc *rpcb, const float bbox[4], int zone, int south)
 {
     if (!ha || !hb || !rpca || !rpcb || !bbox || nx < 1 || ny < 1 || w < 1 || h < 1) return fail(S2PB_ERR_ARG, "bad argument");
-    return cloud_crs_ok(ctx, zone, true);
+    return cloud_crs_ok(ctx, zone, south, true);
 }
 
 int triangulated_cloud(s2pb_ctx *ctx, HostCall &L, const float *dispx, const float *dispy, const float *msk, int nx, int ny,
@@ -55,16 +55,16 @@ int triangulated_cloud(s2pb_ctx *ctx, HostCall &L, const float *dispx, const flo
                        const s2pb_rpc *rpcb, const float bbox[4], int zone, int south, double **d_xyz, float **d_err)
 {
     if (!dispx || !dispy || !msk || !msk_orig) return fail(S2PB_ERR_ARG, "bad argument");
-    if (int rc = triangulated_cloud_args_ok(ctx, nx, ny, w, h, ha, hb, rpca, rpcb, bbox, zone)) return rc;
+    if (int rc = triangulated_cloud_args_ok(ctx, nx, ny, w, h, ha, hb, rpca, rpcb, bbox, zone, south)) return rc;
     const size_t npix = (size_t)nx * ny, nm = (size_t)w * h;
     float *d_dx = L.upload(dispx, npix * 4), *d_dy = L.upload(dispy, npix * 4), *d_m = L.upload(msk, npix * 4);
     float *d_mo = L.upload(msk_orig, nm * 4);
     return triangulated_cloud_device(ctx, L, d_dx, d_dy, d_m, nx, ny, d_mo, w, h, ha, hb, rpca, rpcb, bbox, zone, south, d_xyz, d_err);
 }
 
-// s2p.triangulation.disp_to_xyz (s2p/triangulation.py:85-162) with a UTM (or no) output CRS, heights optionally above EGM96:
-// disp_to_lonlatalt, then the projection (projection.cu) in place on the device cloud; only the projected cloud and the error
-// come back.
+// s2p.triangulation.disp_to_xyz (s2p/triangulation.py:85-162) with a UTM, another projected (S2PB_ZONE_PROJ) or no output
+// CRS, heights optionally above EGM96: disp_to_lonlatalt, then the projection (projection.cu) in place on the device cloud;
+// only the projected cloud and the error come back.
 extern "C" int s2pb_disp_to_xyz(s2pb_ctx *ctx, double *xyz, float *err, const float *dispx, const float *dispy, const float *msk,
                                 int nx, int ny, const float *msk_orig, int w, int h, const double ha[9], const double hb[9],
                                 const s2pb_rpc *rpca, const s2pb_rpc *rpcb, const float bbox[4], int zone, int south)
@@ -106,22 +106,22 @@ int localised_cloud_device(s2pb_ctx *ctx, HostCall &L, const double *d_z, int w,
     return S2PB_OK;
 }
 
-int localised_cloud_args_ok(const s2pb_ctx *ctx, int w, int h, const s2pb_rpc *rpc, int zone)
+int localised_cloud_args_ok(const s2pb_ctx *ctx, int w, int h, const s2pb_rpc *rpc, int zone, int south)
 {
     if (!rpc || w < 1 || h < 1) return fail(S2PB_ERR_ARG, "bad argument");
-    return cloud_crs_ok(ctx, zone, true);
+    return cloud_crs_ok(ctx, zone, south, true);
 }
 
 int localised_cloud(s2pb_ctx *ctx, HostCall &L, const double *heights, int w, int h, const s2pb_rpc *rpc, double off_x,
                     double off_y, int zone, int south, double **d_xyz)
 {
     if (!heights) return fail(S2PB_ERR_ARG, "bad argument");
-    if (int rc = localised_cloud_args_ok(ctx, w, h, rpc, zone)) return rc;
+    if (int rc = localised_cloud_args_ok(ctx, w, h, rpc, zone, south)) return rc;
     double *d_z = L.upload(heights, (size_t)w * h * 8);
     return localised_cloud_device(ctx, L, d_z, w, h, rpc, off_x, off_y, zone, south, d_xyz);
 }
 
-// s2p.triangulation.height_map_to_xyz (s2p/triangulation.py:165-217) with a UTM (or no) output CRS, heights optionally above
+// s2p.triangulation.height_map_to_xyz (s2p/triangulation.py:165-217) with a UTM, another projected or no output CRS, heights optionally above
 // EGM96: every pixel of the height map localised by the camera, then the projection (projection.cu) in place on the device
 // cloud.
 extern "C" int s2pb_height_map_to_xyz(s2pb_ctx *ctx, double *xyz, const double *heights, int w, int h, const s2pb_rpc *rpc,

@@ -30,7 +30,7 @@ static int heights_tile_args_ok(s2pb_ctx *ctx, const s2pb_heights_tile *t, uint8
     if (t->cargarse_basura) {
         if (int rc = basura_args_ok(t->w, t->h)) return rc;
     }
-    if (int rc = localised_cloud_args_ok(ctx, t->w, t->h, t->rpc, t->zone)) return rc;
+    if (int rc = localised_cloud_args_ok(ctx, t->w, t->h, t->rpc, t->zone, t->south)) return rc;
     if (t->stretch) return tail_args_ok(ctx, t->w, t->h, (const float *)t->colors, t->nbands, t->pct, records, npoints);
     if (int rc = tail_args_ok(ctx, t->w, t->h, (const float *)t->colors, t->nbands, 0.0, records, npoints)) return rc;
     return typed_colours_ok(t->nbands, t->color_type);

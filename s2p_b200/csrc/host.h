@@ -96,6 +96,8 @@ struct s2pb_ctx {
     struct PoolBuf { void *p; size_t bytes; bool used; };
     std::vector<PoolBuf> pool;
     GeoidGrid geoid{};              // s2pb_set_geoid: the EGM96 grid of S2PB_ZONE_EGM96 (geoid.g null: none), owned
+    MapKind proj_kind = MapKind::kNone;   // s2pb_set_projection: the map of S2PB_ZONE_PROJ (kNone: none) and its parameters
+    MapParams proj{};
 };
 
 // nothing declared from here on is part of the library's exported interface
@@ -257,10 +259,11 @@ void launch_erode_mask(s2pb_ctx *ctx, const uint8_t *in, uint8_t *out, int w, in
 int mgm_match_device(s2pb_ctx *ctx, cudaStream_t st, const float *d_im1, const float *d_im2, int w, int h, int dmin, int dmax,
                      const s2pb_mgm_params *p, const float *d_wl, const float *d_wr, float *d_disp, float *d_conf, uint8_t *d_mask,
                      float *d_dispR);
-// projection.cu: the output CRS of a cloud, `zone` as the C ABI takes it (a UTM zone, 0 for none when zone0 is true, optionally
-// with S2PB_ZONE_EGM96 when the context holds a geoid grid): its check, and the projection of n device points (lon, lat, alt)
-// to it, in place when d_in == d_out (nothing to launch for zone 0 without the geoid)
-int cloud_crs_ok(const s2pb_ctx *ctx, int zone, bool zone0);
+// projection.cu: the output CRS of a cloud, `zone` and `south` as the C ABI takes them (a UTM zone, 0 for none when zone0 is
+// true, or S2PB_ZONE_PROJ with south 0 when zone0 is true and the context holds a projection; optionally with S2PB_ZONE_EGM96
+// when it holds a geoid grid): its check, and the projection of n device points (lon, lat, alt) to it, in place when
+// d_in == d_out (nothing to launch for zone 0 without the geoid)
+int cloud_crs_ok(const s2pb_ctx *ctx, int zone, int south, bool zone0);
 int launch_cloud_project(s2pb_ctx *ctx, cudaStream_t st, int zone, bool south, const double *d_in, double *d_out, size_t n);
 // the context's geoid grid back to the device (s2pb_destroy, s2pb_set_geoid)
 void geoid_free(s2pb_ctx *ctx);
@@ -274,14 +277,14 @@ int triangulated_cloud(s2pb_ctx *ctx, HostCall &L, const float *dispx, const flo
                        const s2pb_rpc *rpcb, const float bbox[4], int zone, int south, double **d_xyz, float **d_err);
 // triangulated_cloud_device: the same from device disparities and masks, after triangulated_cloud_args_ok checked the rest.
 int triangulated_cloud_args_ok(const s2pb_ctx *ctx, int nx, int ny, int w, int h, const double ha[9], const double hb[9], const s2pb_rpc *rpca,
-                               const s2pb_rpc *rpcb, const float bbox[4], int zone);
+                               const s2pb_rpc *rpcb, const float bbox[4], int zone, int south);
 int triangulated_cloud_device(s2pb_ctx *ctx, HostCall &L, const float *d_dx, const float *d_dy, const float *d_m, int nx, int ny,
                               const float *d_mo, int w, int h, const double ha[9], const double hb[9], const s2pb_rpc *rpca,
                               const s2pb_rpc *rpcb, const float bbox[4], int zone, int south, double **d_xyz, float **d_err);
 int localised_cloud(s2pb_ctx *ctx, HostCall &L, const double *heights, int w, int h, const s2pb_rpc *rpc, double off_x,
                     double off_y, int zone, int south, double **d_xyz);
 // localised_cloud_device: the same from device heights d_z, after localised_cloud_args_ok checked the rest.
-int localised_cloud_args_ok(const s2pb_ctx *ctx, int w, int h, const s2pb_rpc *rpc, int zone);
+int localised_cloud_args_ok(const s2pb_ctx *ctx, int w, int h, const s2pb_rpc *rpc, int zone, int south);
 int localised_cloud_device(s2pb_ctx *ctx, HostCall &L, const double *d_z, int w, int h, const s2pb_rpc *rpc, double off_x,
                            double off_y, int zone, int south, double **d_xyz);
 // s2pb_height_map from the device disparity d_dx and mask d_m (nx*ny) and the unpadded device mask_orig d_mo0 (mw*mh) into the

@@ -126,7 +126,8 @@ static int pair_tile_args_ok(s2pb_ctx *ctx, const s2pb_pair_tile *t, uint8_t *re
 {
     if (!ctx || !t) return fail(S2PB_ERR_ARG, "bad argument");
     if (int rc = pair_match_args_ok(t, conf, disp_right, t->with_conf != 0)) return rc;
-    if (int rc = triangulated_cloud_args_ok(ctx, t->w, t->h, t->mw, t->mh, t->ha, t->hb, t->rpc1, t->rpc2, t->bbox, t->zone)) return rc;
+    if (int rc = triangulated_cloud_args_ok(ctx, t->w, t->h, t->mw, t->mh, t->ha, t->hb, t->rpc1, t->rpc2, t->bbox, t->zone, t->south))
+        return rc;
     if (t->clr) {
         if (int rc = tail_args_ok(ctx, t->w, t->h, t->clr, t->clr_bands, 0.0, records, npoints)) return rc;
         if (int rc = typed_colours_ok(t->clr_bands, S2PB_PLY_F32)) return rc;

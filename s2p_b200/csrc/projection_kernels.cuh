@@ -1,5 +1,6 @@
-// projection_kernels.cuh -- WGS84 (lon, lat, alt) -> UTM (easting, northing, alt), forward, one thread per point, and the
-// EGM96 geoid heights of a compound target such as EPSG:326zz+5773 (GeoidGrid below).
+// projection_kernels.cuh -- WGS84 (lon, lat, alt) -> UTM (easting, northing, alt), forward, one thread per point; the
+// Lambert conic conformal map of the French grids (lcc_forward below); and the EGM96 geoid heights of a compound target such
+// as EPSG:326zz+5773 (GeoidGrid below).
 //
 // The map is the one PROJ runs for `+proj=utm` unless `+approx` is given: the "exact" transverse Mercator of Poder and
 // Engsager (K. Engsager, K. Poder, "A highly accurate world wide algorithm for the transverse Mercator mapping (almost)",
@@ -14,7 +15,8 @@
 //      sin / cos 2xi' and sinh / cosh 2eta' come from the quantities of step 2 without further transcendental calls;
 //   4. scale by k0 times the rectifying radius and add the false easting / northing.
 // The coefficients depend on the ellipsoid only; the host computes them in double (projection.cu) and they travel as a
-// __grid_constant__ kernel parameter, in the constant bank, as the triangulation kernels pass their camera models.
+// __grid_constant__ kernel parameter, in the constant bank, as the triangulation kernels pass their camera models.  The same
+// map on GRS80 gives the ETRS89 UTM zones (EPSG 25828-25838): only the coefficients, qa and the origin differ.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -82,6 +84,66 @@ __device__ __forceinline__ void utm_forward(const UtmParams &P, double lon, doub
     y = P.qa * xi + P.y0;
 }
 
+// The Lambert conic conformal map with two standard parallels (EPSG method 9802, IOGP Guidance Note 7-2 sec. 3.1.1.1) of
+// RGF93 v1 / Lambert-93 (EPSG:2154) and the nine zones CC42-CC50 (EPSG 3942-3950), on GRS80.  With the isometric latitude
+// psi(phi) = asinh(tan phi) - e atanh(e sin phi), the note's t(phi) is exp(-psi), so the radius r = a F t^n is a F exp(-n psi).
+// The host computes the cone constant n, a F and r_F = a F t(phi_F)^n (projection.cu).
+struct LccParams {
+    double lon0;                          // longitude of the false origin, degrees
+    double e;                             // first eccentricity
+    double n;                             // cone constant
+    double aF;                            // a F, metres
+    double rho0;                          // r_F: radius at the latitude of the false origin, metres
+    double x0, y0;                        // easting, northing at the false origin, metres
+};
+
+// (lon, lat) in degrees -> (x, y) in metres, in this operation order (tests/lcc_oracle.py restates it in numpy):
+//   lam = (lon - lon0) d2r, reduced to [-pi, pi] as utm_forward reduces it; phi = lat d2r;
+//   psi = asinh(tan phi) - e atanh(e sin phi);  rho = aF exp(-(n psi));  theta = n lam;
+//   x = x0 + rho sin theta;  y = y0 + (rho0 - rho cos theta).
+// A pole (| |phi| - pi/2 | < 1e-10 rad) is the apex of the cone, rho = 0, on the side the cone opens to (phi n > 0); on the
+// other side, and for |lat| > 90, the point cannot be projected and gives +inf, as PROJ flags it with HUGE_VAL.
+__device__ __forceinline__ void lcc_forward(const LccParams &P, double lon, double lat, double &x, double &y)
+{
+    const double d2r = 0.017453292519943295;      // pi / 180
+    double lam = (lon - P.lon0) * d2r;
+    if (fabs(lam) > 3.141592653589793) lam -= 6.283185307179586 * floor((lam + 3.141592653589793) / 6.283185307179586);
+    const double phi = lat * d2r;
+    const bool pole = fabs(fabs(phi) - 1.5707963267948966) < 1e-10;
+    if (!(fabs(lat) <= 90.0) || (pole && phi * P.n <= 0.0)) {
+        x = y = __longlong_as_double(0x7ff0000000000000LL);
+        return;
+    }
+    double rho = 0.0;
+    if (!pole) {
+        const double psi = asinh(tan(phi)) - P.e * atanh(P.e * sin(phi));
+        rho = P.aF * exp(-(P.n * psi));
+    }
+    const double theta = P.n * lam;
+    x = P.x0 + rho * sin(theta);
+    y = P.y0 + (P.rho0 - rho * cos(theta));
+}
+
+// The map of a cloud's output CRS: which one is a template parameter of cloud_project_kernel, and its parameters, which the
+// host keeps in the union MapParams, travel as the struct of that map (MapArg), so that the UTM instantiations take the
+// UtmParams they always took.
+enum class MapKind { kNone, kTm, kLcc };
+union MapParams {
+    UtmParams tm;                         // kTm (and kNone): utm_forward (WGS84 UTM, ETRS89 UTM)
+    LccParams lcc;                        // kLcc: lcc_forward
+};
+template <MapKind kMap> struct MapArgOf { using type = UtmParams; };
+template <> struct MapArgOf<MapKind::kLcc> { using type = LccParams; };
+template <MapKind kMap> using MapArg = typename MapArgOf<kMap>::type;
+__device__ __forceinline__ void map_forward(const UtmParams &P, double lon, double lat, double &x, double &y)
+{
+    utm_forward(P, lon, lat, x, y);
+}
+__device__ __forceinline__ void map_forward(const LccParams &P, double lon, double lat, double &x, double &y)
+{
+    lcc_forward(P, lon, lat, x, y);
+}
+
 // The vertical datum of a cloud: heights above the EGM96 geoid instead of the WGS84 ellipsoid, H = h - N(lon, lat), the
 // step PROJ's `+proj=vgridshift` runs for a target such as EPSG:326zz+5773.  N is interpolated bilinearly in a float32 grid
 // of h rows of w nodes: node (i, j) lies at (lon0 + i dlon, lat0 - j dlat), row 0 northernmost.  The grid is global: it spans
@@ -111,12 +173,12 @@ __device__ __forceinline__ double geoid_undulation(const GeoidGrid &G, double lo
     return top + fy * (bottom - top);
 }
 
-// out[i] = (x, y, z) of in[i] = (lon, lat, alt), n points of three doubles; in == out is allowed.  kUtm: (x, y) the UTM map
-// of (lon, lat), else (lon, lat) as they are; kGeoid: z = alt - N(lon, lat) in float64, else alt.  A point with a NaN
-// coordinate becomes NaN in all three; a point outside the domain (of the UTM map, or |lat| > 90 / an infinite lon for the
-// geoid) becomes +inf in all three.
-template <bool kUtm, bool kGeoid>
-__global__ void cloud_project_kernel(const __grid_constant__ UtmParams P, const __grid_constant__ GeoidGrid G, const double *in,
+// out[i] = (x, y, z) of in[i] = (lon, lat, alt), n points of three doubles; in == out is allowed.  kMap: (x, y) the map of
+// (lon, lat) (kTm: utm_forward, kLcc: lcc_forward), kNone: (lon, lat) as they are; kGeoid: z = alt - N(lon,
+// lat) in float64, else alt.  A point with a NaN coordinate becomes NaN in all three; a point outside the domain (of the map,
+// or |lat| > 90 / an infinite lon for the geoid) becomes +inf in all three.
+template <MapKind kMap, bool kGeoid>
+__global__ void cloud_project_kernel(const __grid_constant__ MapArg<kMap> P, const __grid_constant__ GeoidGrid G, const double *in,
                                      double *out, long long n)
 {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -127,8 +189,8 @@ __global__ void cloud_project_kernel(const __grid_constant__ UtmParams P, const 
         x = y = z = __longlong_as_double(0x7ff8000000000000LL);
     } else {
         bool outside = false;
-        if (kUtm) {
-            utm_forward(P, lon, lat, x, y);
+        if constexpr (kMap != MapKind::kNone) {
+            map_forward(P, lon, lat, x, y);
             outside = isinf(x);
         } else {
             x = lon;

@@ -89,6 +89,11 @@ def _rpc(rpc):
     return ctypes.cast(ctypes.pointer(rpc), ctypes.c_void_p)
 
 
+def _projection(proj):
+    """projection.Projection (any object with its fields) as the ``s2pb_projection`` of the C ABI"""
+    return _lib.Projection(*(getattr(proj, name) for name, _ in _lib.Projection._fields_))
+
+
 class Engine:
     def __init__(self, device=0):
         L = _lib.lib()
@@ -389,6 +394,25 @@ class Engine:
             _lib.check(self._L.s2pb_set_geoid(self._ctx, _fp(v), v.shape[1], v.shape[0], float(grid.lon0), float(grid.lat0),
                                               float(grid.dlon), float(grid.dlat)))
         self._geoid = grid
+
+    def set_projection(self, proj):
+        """Hold ``proj`` (projection.Projection, or None to drop it) on the context for the zone _lib.ZONE_PROJ, which every
+        cloud and tile method then takes: the map of that projection instead of a UTM zone (s2pb_set_projection)."""
+        if proj == getattr(self, "_projection", None):
+            return
+        _lib.check(self._L.s2pb_set_projection(self._ctx, None if proj is None else ctypes.byref(_projection(proj))))
+        self._projection = proj
+
+    def lonlat_to_proj(self, lonlatalt, proj):
+        """(..., 3) float64 (lon, lat in degrees, alt) -> (..., 3) float64 (x, y, alt) in the map ``proj``
+        (projection.Projection; s2pb_lonlat_to_proj).  NaN in any coordinate gives NaN in all three, a point the map cannot
+        project +inf in all three."""
+        a = np.ascontiguousarray(lonlatalt, np.float64)
+        if a.ndim < 1 or a.shape[-1] != 3:
+            raise ValueError("expecting points of three coordinates, got shape %s" % (a.shape,))
+        out = np.empty_like(a)
+        _lib.check(self._L.s2pb_lonlat_to_proj(self._ctx, _dp(out), _dp(a), a.size // 3, ctypes.byref(_projection(proj))))
+        return out
 
     def lonlat_to_utm(self, lonlatalt, zone, south=False):
         """(..., 3) float64 (lon, lat in degrees, alt) -> (..., 3) float64 (easting, northing, alt) in UTM zone `zone` (1..60)

@@ -82,7 +82,7 @@ def fall_through_reason(cfg):
     window = _window_unserved(cfg)
     if window:
         return window
-    if projection.utm_target(cfg['out_crs']) is None:
+    if projection.output_target(cfg['out_crs']) is None:
         return projection.unserved_reason(cfg['out_crs'])
     if not cloud.numpy_stretch_is_float64():
         return "NumPy < 2 stretches the colours in float32"
@@ -196,7 +196,7 @@ def pair_tile(tile, engine=None):
         records, out = eng.pair_tile_to_ply(
             src1, H1c, src2, H2c, w, h, disp_min, disp_max, rio.read_stored(mask_orig).squeeze(), H_ref, H_sec,
             triangulation._rpc_struct(cfg['images'][0]['rpcm']), triangulation._rpc_struct(cfg['images'][1]['rpcm']),
-            (x, x + tw, y, y + th), *projection.utm_target(cfg['out_crs'], eng), params=params, weights=weights,
+            (x, x + tw, y, y + th), *projection.output_target(cfg['out_crs'], eng), params=params, weights=weights,
             erode_radius=erosion_radius(cfg['msk_erosion']), r=r, p=p, n=n, clr=clr, hc=hc,
             confidence=algo in CONFIDENCE_COLUMN, want=want)
     except S2pbError as e:
@@ -307,7 +307,7 @@ def _fusion_operator(name):
 def heights_tile_fall_through_reason(cfg):
     """Why ``heights_tile`` hands the tile to ``s2p.heights_to_ply`` for this configuration, or None (the colours are looked
     at in ``heights_tile``, as ``cloud.heights_to_ply`` looks at them)."""
-    if projection.utm_target(cfg['out_crs']) is None:
+    if projection.output_target(cfg['out_crs']) is None:
         return projection.unserved_reason(cfg['out_crs'])
     if not cloud.numpy_stretch_is_float64():
         return "NumPy < 2 stretches the colours in float32"
@@ -358,7 +358,7 @@ def heights_tile(tile, engine=None):
     eng = engine or get_engine()
     try:
         records, out = eng.heights_tile_to_ply(
-            maps, offsets, triangulation._rpc_struct(cfg['images'][0]['rpcm']), x, y, *projection.utm_target(cfg['out_crs'], eng),
+            maps, offsets, triangulation._rpc_struct(cfg['images'][0]['rpcm']), x, y, *projection.output_target(cfg['out_crs'], eng),
             cargarse_basura=basura, averaging=_fusion_operator(cfg['fusion_operator']), threshold=cfg['fusion_thresh'], r=r, p=p,
             n=n, colors=None if clr else colors, clr=colors if clr else None, want=want)
     except S2pbError as e:

@@ -6,8 +6,19 @@ s2p triangulates to WGS84 (lon, lat, alt), EPSG:4979, and projects the cloud to 
 projects to the UTM zones of WGS84, EPSG 32601-32660 (north) and 32701-32760 (south), with PROJ's exact transverse Mercator
 (``csrc/projection_kernels.cuh``).  No output CRS, 4979 and 4326 leave (lon, lat, alt) as they are, as pyproj does.
 
-The compound targets 326zz+5773, 327zz+5773 and 4326+5773 differ from those only in z: PROJ subtracts the EGM96 undulation
-N(lon, lat), interpolated bilinearly in its grid ``us_nga_egm96_15.tif``, from the ellipsoidal height.  The device does the
+The device also projects to the ETRS89 UTM zones 28N-38N (EPSG 25828-25838) and to RGF93 v1 / Lambert-93 (2154) and its nine
+conic zones CC42-CC50 (3942-3950), the national grids s2p's users in Europe and France set most often (``PROJECTED``, the one
+table of their map parameters, with ``S2PB_ZONE_PROJ``).  All of them are on GRS80, and their datums reach WGS84 through the
+null transformations "ETRS89 to WGS 84 (1)" and "RGF93 v1 to WGS 84 (1)" of the EPSG dataset, the operation PROJ applies
+where no grid applies: the cloud is the pure map of the triangulated (lon, lat) and the altitude passes through, as for UTM.
+They are served where PROJ itself agrees (``proj_agrees``): pyproj is importable and its transformation from EPSG:4979 of
+reference points over the area of use lands within 1 mm of the same map (``map_lonlat``), the altitude unchanged.  A PROJ
+whose database or grids apply another operation, or no pyproj (which the reference's own path needs too), keeps the
+reference's path.
+
+The compound targets 326zz+5773, 327zz+5773 and 4326+5773 (and those grids +5773) differ from those only in z: PROJ
+subtracts the EGM96 undulation N(lon, lat), interpolated bilinearly in its grid ``us_nga_egm96_15.tif``, from the ellipsoidal
+height.  The device does the
 same (``S2PB_ZONE_EGM96``) with the grid file PROJ would open, found by ``locate_egm96`` and read by ``read_geoid_grid``
 without GDAL; where there is no such file, or it is not a global north-up float32 grid interpolated bilinearly, the target is
 not served.  Any target not served -- those, another geoid, datum or projection -- goes through the reference's pyproj code
@@ -89,12 +100,154 @@ def utm_target(crs, engine=None):
     return target[0] | _lib.ZONE_EGM96, target[1]
 
 
-def unserved_reason(crs):
-    """why utm_target(crs) is None, for the fall-through messages"""
+# ------------------------------------------------------------------ the other projected targets (S2PB_ZONE_PROJ)
+
+Projection = collections.namedtuple("Projection", "method a rf lon0 lat0 lat1 lat2 k0 x0 y0")
+Projection.__doc__ = """the fields of s2pb_projection: method _lib.PROJ_TM or _lib.PROJ_LCC, the ellipsoid (semi-major axis a in
+metres, inverse flattening rf), the origin (lon0, lat0), the standard parallels lat1, lat2 (LCC), the scale k0 (TM), degrees,
+and the false easting and northing x0, y0 in metres"""
+
+GRS80 = (6378137.0, 298.257222101)          # EPSG:7019 GRS 1980, the ellipsoid of ETRS89 (EPSG:6258) and RGF93 v1 (EPSG:6171)
+
+
+def _etrs89_utm(zone):
+    """EPSG 25800 + zone, ETRS89 / UTM zone zoneN: Transverse Mercator (EPSG method 9807), latitude of natural origin 0,
+    longitude 6 zone - 183, scale 0.9996, false easting 500 000 m, false northing 0"""
+    return Projection(_lib.PROJ_TM, *GRS80, 6.0 * zone - 183.0, 0.0, 0.0, 0.0, 0.9996, 500000.0, 0.0)
+
+
+def _rgf93_cc(lat):
+    """EPSG 3900 + lat, RGF93 v1 / CC<lat>: Lambert Conic Conformal (2SP) (EPSG method 9802), false origin (3 E, lat N) at
+    (1 700 000, 1 200 000 + (lat - 42) 1 000 000) m, standard parallels lat - 0.75 and lat + 0.75"""
+    return Projection(_lib.PROJ_LCC, *GRS80, 3.0, float(lat), lat - 0.75, lat + 0.75, 0.0, 1700000.0,
+                      1200000.0 + (lat - 42) * 1000000.0)
+
+
+# EPSG code -> the map the device runs for it (the single rule of which projected CRSs other than WGS84 UTM are served)
+PROJECTED = {
+    **{25800 + zone: _etrs89_utm(zone) for zone in range(28, 39)},
+    # EPSG:2154 RGF93 v1 / Lambert-93: LCC 2SP, false origin (3 E, 46.5 N) at (700 000, 6 600 000) m, parallels 49 and 44
+    2154: Projection(_lib.PROJ_LCC, *GRS80, 3.0, 46.5, 49.0, 44.0, 0.0, 700000.0, 6600000.0),
+    **{3900 + lat: _rgf93_cc(lat) for lat in range(42, 51)},
+}
+
+
+# ------------------------------------------------------------------ PROJ's consent
+
+def map_lonlat(proj, lon, lat):
+    """(x, y) in metres of (lon, lat) in degrees by the map proj in float64 numpy: the Lambert conic conformal of lcc_forward,
+    or the transverse Mercator of utm_forward (Krueger's series to order n^6, the coefficients of projection.cu's tm_params).
+    For the agreement check below; the device's maps are pinned to 50-digit truths by the tests."""
+    lon, lat = np.asarray(lon, np.float64), np.asarray(lat, np.float64)
+    f = 1.0 / proj.rf
+    lam = np.radians(lon - proj.lon0)
+    lam = lam - 2 * np.pi * np.floor((lam + np.pi) / (2 * np.pi))
+    phi = np.radians(lat)
+    if proj.method == _lib.PROJ_LCC:
+        e = np.sqrt(f * (2.0 - f))
+        m = lambda p: np.cos(p) / np.sqrt(1.0 - (e * np.sin(p)) ** 2)                          # noqa: E731
+        psi = lambda p: np.arcsinh(np.tan(p)) - e * np.arctanh(e * np.sin(p))                  # noqa: E731
+        p1, p2, p0 = np.radians(proj.lat1), np.radians(proj.lat2), np.radians(proj.lat0)
+        n = np.sin(p1) if proj.lat1 == proj.lat2 else (np.log(m(p1)) - np.log(m(p2))) / (psi(p2) - psi(p1))
+        aF = proj.a * m(p1) * np.exp(n * psi(p1)) / n
+        rho, theta = aF * np.exp(-n * psi(phi)), n * lam
+        return proj.x0 + rho * np.sin(theta), proj.y0 + aF * np.exp(-n * psi(p0)) - rho * np.cos(theta)
+    n = f / (2.0 - f)
+    cbg = [n * (-2 + n * (2 / 3 + n * (4 / 3 + n * (-82 / 45 + n * (32 / 45 + n * 4642 / 4725))))),
+           n ** 2 * (5 / 3 + n * (-16 / 15 + n * (-13 / 9 + n * (904 / 315 + n * -1522 / 945)))),
+           n ** 3 * (-26 / 15 + n * (34 / 21 + n * (8 / 5 + n * -12686 / 2835))),
+           n ** 4 * (1237 / 630 + n * (-12 / 5 + n * -24832 / 14175)), n ** 5 * (-734 / 315 + n * 109598 / 31185),
+           n ** 6 * 444337 / 155925]
+    gtu = [n * (1 / 2 + n * (-2 / 3 + n * (5 / 16 + n * (41 / 180 + n * (-127 / 288 + n * 7891 / 37800))))),
+           n ** 2 * (13 / 48 + n * (-3 / 5 + n * (557 / 1440 + n * (281 / 630 + n * -1983433 / 1935360)))),
+           n ** 3 * (61 / 240 + n * (-103 / 140 + n * (15061 / 26880 + n * 167603 / 181440))),
+           n ** 4 * (49561 / 161280 + n * (-179 / 168 + n * 6601661 / 7257600)), n ** 5 * (34729 / 80640 + n * -3418889 / 1995840),
+           n ** 6 * 212378941 / 319334400]
+    chi = phi + sum(c * np.sin(2 * (k + 1) * phi) for k, c in enumerate(cbg))
+    zeta = np.arctan2(np.sin(chi), np.cos(chi) * np.cos(lam)) + 1j * np.arcsinh(
+        np.sin(lam) * np.cos(chi) / np.hypot(np.sin(chi), np.cos(chi) * np.cos(lam)))
+    zeta = zeta + sum(c * np.sin(2 * (k + 1) * zeta) for k, c in enumerate(gtu))
+    qa = proj.a * proj.k0 / (1 + n) * (1 + n ** 2 / 4 + n ** 4 / 64 + n ** 6 / 256)
+    return proj.x0 + qa * zeta.imag, proj.y0 + qa * zeta.real
+
+
+AGREE_M = 1e-3      # PROJ against map_lonlat: far above rounding, far below any datum shift ETRS89 / RGF93 v1 could have
+
+
+def _reference_points(proj):
+    """3 x 3 (lon, lat) over the CRS's area of use, degrees"""
+    if proj.method == _lib.PROJ_LCC:
+        lons, lats = (-4.0, 3.0, 9.0), (proj.lat0 - 2.0, proj.lat0, proj.lat0 + 2.0)
+    else:
+        lons, lats = (proj.lon0 - 3.0, proj.lon0, proj.lon0 + 3.0), (36.0, 50.0, 70.0)
+    lon, lat = np.meshgrid(lons, lats)
+    return lon.ravel(), lat.ravel()
+
+
+_consent = {}
+
+
+def proj_agrees(code):
+    """Whether PROJ, through pyproj, takes EPSG:4979 to EPSG ``code`` of PROJECTED as the device does: its transformation of
+    reference points over the area of use within AGREE_M of map_lonlat in x and y, the altitude unchanged.  The device
+    serves these CRSs only then, so that a PROJ whose database or grids would apply another operation (a datum shift) keeps the
+    reference's path; without pyproj the reference's path cannot run either, and the steps fall through as before.  Asked
+    once per code and pyproj module."""
+    try:
+        import pyproj
+    except ImportError:
+        return False
+    key = (code, pyproj)
+    if key not in _consent:
+        proj = PROJECTED[code]
+        lon, lat = _reference_points(proj)
+        h = np.linspace(-100.0, 4000.0, lon.size)
+        try:
+            t = pyproj.Transformer.from_crs("epsg:4979", "epsg:%d" % code, always_xy=True)
+            x, y, z = (np.asarray(v, np.float64) for v in t.transform(lon, lat, h))
+        except Exception:       # pyproj's errors (CRSError, ProjError) and a PROJ without the code
+            _consent[key] = False
+        else:
+            wx, wy = map_lonlat(proj, lon, lat)
+            _consent[key] = bool(np.all(np.abs(x - wx) <= AGREE_M) and np.all(np.abs(y - wy) <= AGREE_M) and
+                                 np.all(np.abs(z - h) <= 1e-6))
+    return _consent[key]
+
+
+def output_target(crs, engine=None):
+    """The zone argument of the device's cloud calls for crs -> (zone, south): utm_target's for WGS84 and its UTM zones;
+    (_lib.ZONE_PROJ, False) for a code of PROJECTED that proj_agrees with, whose map is then registered on ``engine`` (when
+    given); either with _lib.ZONE_EGM96 OR'ed in for a +5773 target when ``egm96_grid()`` finds the grid, registered as
+    utm_target registers it; None for any other target"""
+    target = utm_target(crs, engine)
+    if target is not None:
+        return target
     codes = _codes(crs)
-    if codes and codes[1] == EGM96_HEIGHT and (codes[0] == 4326 or _zone_of(codes[0])):
+    if codes is None or codes[0] not in PROJECTED or codes[1] not in (None, EGM96_HEIGHT) or not proj_agrees(codes[0]):
+        return None
+    zone = _lib.ZONE_PROJ
+    if codes[1] == EGM96_HEIGHT:
+        grid = egm96_grid()
+        if grid is None:
+            return None
+        if engine is not None:
+            engine.set_geoid(grid)
+        zone |= _lib.ZONE_EGM96
+    if engine is not None:
+        engine.set_projection(PROJECTED[codes[0]])
+    return zone, False
+
+
+def unserved_reason(crs):
+    """why output_target(crs) is None, for the fall-through messages"""
+    codes = _codes(crs)
+    if codes and codes[0] in PROJECTED and codes[1] in (None, EGM96_HEIGHT) and not proj_agrees(codes[0]):
+        return ("output CRS %r is not a UTM zone of WGS84, and the device serves it as an ETRS89 / RGF93 v1 grid only where pyproj "
+                "is importable and PROJ's own transformation from EPSG:4979 agrees with the device's map" % (crs,))
+    if codes and codes[1] == EGM96_HEIGHT and (codes[0] == 4326 or _zone_of(codes[0]) or codes[0] in PROJECTED):
         return "output CRS %r needs the EGM96 grid %s, which was not found or is not one the device reads" % (crs, EGM96_FILE)
-    return "output CRS %r is not a UTM zone of WGS84" % (crs,)
+    return ("output CRS %r is not a UTM zone of WGS84, nor an ETRS89 UTM zone (EPSG 25828-25838) or RGF93 v1 Lambert grid "
+            "(2154, 3942-3950)" % (crs,))
 
 
 # ------------------------------------------------------------------ the EGM96 grid
@@ -272,15 +425,15 @@ def lonlat_to_utm(lonlatalt, zone, south=False, engine=None):
 
 
 def pyproj_original(lonlatalt, out_crs):
-    """The reference's change of coordinates (s2p/triangulation.py:147-160) for the targets the device does not serve:
+    """The reference's change of coordinates (s2p/triangulation.py:147-160) for the targets output_target does not serve:
     s2p.geographiclib's pyproj wrappers when they are importable, S2pbError(ERR_UNSUPPORTED) otherwise."""
     try:
         from s2p import geographiclib
         in_crs = geographiclib.pyproj_crs("epsg:4979")
     except ImportError:
-        raise _lib.S2pbError(_lib.ERR_UNSUPPORTED, "output CRS %r: only WGS84 (EPSG 4979, 4326) and its UTM zones, with EGM96 heights "
-                             "when %s is found, are projected on the device, and s2p.geographiclib (pyproj) is not importable"
-                             % (out_crs, EGM96_FILE)) from None
+        raise _lib.S2pbError(_lib.ERR_UNSUPPORTED, "output CRS %r: only WGS84 (EPSG 4979, 4326), its UTM zones, the ETRS89 UTM zones "
+                             "and the RGF93 v1 Lambert grids, with EGM96 heights when %s is found, are projected on the device, "
+                             "and s2p.geographiclib (pyproj) is not importable" % (out_crs, EGM96_FILE)) from None
     if not (out_crs and out_crs != in_crs):
         return lonlatalt
     h, w = lonlatalt.shape[:2]

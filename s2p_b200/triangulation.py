@@ -11,7 +11,8 @@ The 3D outlier filter of the same library, ``count_3d_neighbors`` and ``remove_i
 which ``filter_xyz`` runs on the cloud of a tile (s2p/triangulation.py:275-343), goes through the adapter too.
 
 ``disp_to_xyz`` (s2p/triangulation.py:85-162) triangulates and projects the cloud to its output CRS in one device call
-(``s2pb_disp_to_xyz``) when that CRS is WGS84 or one of its UTM zones (``projection``); ``install()`` replaces the reference's
+(``s2pb_disp_to_xyz``) when that CRS is WGS84, one of its UTM zones, an ETRS89 UTM zone or an RGF93 v1 Lambert grid
+(``projection.output_target``); ``install()`` replaces the reference's
 function with it.
 
 ``height_map`` (s2p/triangulation.py:346-389), the tri-stereo step that triangulates a pair and resamples the altitude onto the
@@ -69,13 +70,13 @@ def disp_to_lonlatalt(disp, mask_rect, mask_orig, H1, H2, rpc1, rpc2, img_bbx, d
 def disp_to_xyz(rpc1, rpc2, H1, H2, disp, mask_rect, img_bbx, mask_orig, A=None, out_crs=None, engine=None):
     """s2p.triangulation.disp_to_xyz (s2p/triangulation.py:85-162): -> (xyz (h, w, 3) float64 in the coordinates of
     out_crs, err (h, w) float32).  rpc1 / rpc2 are wrapped as the reference wraps them (``RPCStruct(rpc)``); ctypes
-    structures pass as they are.  No out_crs, EPSG 4979 / 4326 and the UTM zones of WGS84, and those with EGM96 heights
-    (+5773) when the grid is found, run on the device in one call; any other out_crs is triangulated on the device and projected by the reference's pyproj code (``projection``)."""
+    structures pass as they are.  No out_crs, EPSG 4979 / 4326, the UTM zones of WGS84 and ETRS89 and the RGF93 v1 Lambert
+    grids, and those with EGM96 heights (+5773) when the grid is found, run on the device in one call; any other out_crs is triangulated on the device and projected by the reference's pyproj code (``projection``)."""
     r1, r2 = _rpc_struct(rpc1), _rpc_struct(rpc2)
     if A is not None:                                       # pointing correction (s2p/triangulation.py:114-115)
         H2 = np.dot(H2, np.linalg.inv(A))
     eng = engine or get_engine()
-    target = projection.utm_target(out_crs, eng)
+    target = projection.output_target(out_crs, eng)
     if target is None:
         lla, err = disp_to_lonlatalt(disp, mask_rect, mask_orig, H1, H2, r1, r2, img_bbx, engine=eng)
         return projection.pyproj_original(lla, out_crs), err
@@ -87,13 +88,13 @@ def height_map_to_xyz(heights, rpc, off_x=0, off_y=0, out_crs=None, engine=None)
     map at ``heights`` (a raster file; band 1, read in its stored dtype) localised by the camera ``rpc`` at image pixel
     (col + off_x, row + off_y) and its height, in the coordinates of out_crs.  rpc is wrapped as the reference wraps it
     (``RPCStruct(rpc)``); ctypes structures pass as they are.  NaN heights give NaN in all three coordinates (the reference
-    leaves lon and lat undefined there).  No out_crs, EPSG 4979 / 4326 and the UTM zones of WGS84, and those with EGM96
-    heights (+5773) when the grid is found, run on the device in one call; any other out_crs is localised on the device and projected by the reference's pyproj code (``projection``)."""
+    leaves lon and lat undefined there).  No out_crs, EPSG 4979 / 4326, the UTM zones of WGS84 and ETRS89 and the RGF93 v1
+    Lambert grids, and those with EGM96 heights (+5773) when the grid is found, run on the device in one call; any other out_crs is localised on the device and projected by the reference's pyproj code (``projection``)."""
     from . import rasterio_compat
     h_map = rasterio_compat.read_band_stored(heights)
     r = _rpc_struct(rpc)
     eng = engine or get_engine()
-    target = projection.utm_target(out_crs, eng)
+    target = projection.output_target(out_crs, eng)
     if target is None:
         return projection.pyproj_original(eng.height_map_to_xyz(h_map, r, off_x, off_y), out_crs)
     return eng.height_map_to_xyz(h_map, r, off_x, off_y, *target)
