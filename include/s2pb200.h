@@ -195,6 +195,17 @@ long long s2pb_workspace_bytes(int w, int h, int D, int ndir, int cost_bytes, in
 int s2pb_workspace_layout(int w, int h, int D, int ndir, int cost_bytes, long long limit);
 /* number of mgm calls the context has run in the folded layout */
 long long s2pb_folded_calls(const s2pb_ctx *ctx);
+/* ---- DCT coefficient tables ---------------------------------------------------------
+ * The matched image's DCT round trip (and the half-pixel shift of mgm_multi) multiplies each image row by n x n double tables
+ * computed on the host with libm.  Up to 8192 px they stay on the device once per width.  Wider rows keep a table there while
+ * the context's tables of such widths stay within this limit -- and within the workspace limit, when one is set -- and
+ * otherwise stream it in K-panels through pinned staging buffers, with the same results, bit for bit.  Default 8 GiB;
+ * 0 streams every table of rows wider than 8192 px.  Tables already on the device stay.  S2PB_ERR_ARG: bytes < 0. */
+int s2pb_set_dct_table_limit(s2pb_ctx *ctx, long long bytes);
+/* out[r][c] (nrows x ncols, row-major) = the coefficients (row0 + r, col0 + c) of a table for rows of n pixels, as the engine
+ * computes them: kind 0 REDFT10 [k][j] = 2 cos(pi (j + 1/2) k / n), 1 REDFT01 [i][k] = 1 for k = 0, else 2 cos(pi k (i + 1/2) / n),
+ * 2 RODFT01 [i][k] = (-1)^i for k = n - 1, else 2 sin(pi (k + 1) (i + 1/2) / n).  No device needed. */
+int s2pb_dct_coefficients(int kind, int n, int row0, int nrows, int col0, int ncols, double *out);
 
 /* ---- the `sgbm` matcher (3rdparty/sgbm/sgbm.cpp + stereosgbm.cpp) ----------------- */
 /* The binary's argv after dmin dmax (`sgbm im1 im2 disp cost dmin dmax win P1 P2 lr`).  What it hardcodes stays

@@ -111,6 +111,8 @@ _SIGNATURES = {
     "s2pb_workspace_bytes": (c_longlong, [c_int, c_int, c_int, c_int, c_int, c_int]),
     "s2pb_workspace_layout": (c_int, [c_int, c_int, c_int, c_int, c_int, c_longlong]),
     "s2pb_folded_calls": (c_longlong, [c_void_p]),
+    "s2pb_set_dct_table_limit": (c_int, [c_void_p, c_longlong]),
+    "s2pb_dct_coefficients": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, POINTER(c_double)]),
     "s2pb_homography": (c_int, [c_void_p, _f, c_int, c_int, POINTER(c_double), _f, c_int, c_int]),
     "s2pb_rectify_match": (c_int, [c_void_p, _f, c_int, c_int, POINTER(c_double), _f, c_int, c_int, POINTER(c_double), c_int, c_int,
                                    c_int, c_int, POINTER(MgmParams), _f, _f, _f, _f, POINTER(c_uint8), _f]),

@@ -236,6 +236,94 @@ __global__ void __launch_bounds__(kGemmThreads) rt_inverse_gemm_kernel(const dou
     }
 }
 
+// The K-panel form of dct_gemm_kernel (INV = false) and rt_inverse_gemm_kernel (INV = true), for rows wider than the resident
+// tables serve (dct_tables): one launch adds the terms of inputs [k0, k1) through a panel of the table, P[q][k - k0], q the
+// output (INV: q the position in the column list; the host builds the listed columns' rows only).  Each output's running sum
+// waits in `acc` ([row][n] doubles, row-major like Y) between the launches: the first panel starts it from 0.0, the last one
+// applies the resident kernel's epilogue instead of storing it.  Within a panel and across the panels the terms are added in
+// ascending k with the same separately rounded operations, and a double survives the store and the load exactly, so every
+// output is the resident kernel's sum bit for bit.  Forward: `acc` may be Y itself (each output is read and then written by
+// the thread that owns it).
+template <typename IN, bool DIVN, bool INV>
+__global__ void __launch_bounds__(kGemmThreads) dct_panel_gemm_kernel(const double *__restrict__ P, int k0, int k1, const IN *__restrict__ X, int n,
+                                                                      int nrows_all, const RtState *st, const int *__restrict__ rowlist,
+                                                                      const int *__restrict__ collist, double *acc, bool first, bool last,
+                                                                      double *Y, const double *__restrict__ mul, const double *__restrict__ mul2,
+                                                                      double *__restrict__ Y2, const float *__restrict__ rowthr,
+                                                                      const float *__restrict__ img, float *__restrict__ rt)
+{
+    constexpr int TO = kGemmTO, TR = kGemmTR, TK = kGemmTK;
+    __shared__ __align__(16) double Ts[TK][TO + 2];
+    __shared__ __align__(16) double Xs[TK][TR + 2];
+    __shared__ int rows_s[TR], cols_s[TO];
+    const int nrows = rowlist ? st->nrows : nrows_all, nout = INV ? st->ncols : n, kp = k1 - k0;
+    const int otiles = (nout + TO - 1) / TO, rtiles = (nrows + TR - 1) / TR;
+    const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
+    for (int item = blockIdx.x; item < otiles * rtiles; item += gridDim.x) {
+        const int o0 = (item % otiles) * TO, r0 = (item / otiles) * TR;
+        __syncthreads();
+        if (threadIdx.x < TR) {
+            const int rr = r0 + threadIdx.x;
+            rows_s[threadIdx.x] = rr < nrows ? (rowlist ? rowlist[rr] : rr) : -1;
+        } else if (threadIdx.x < TR + TO) {
+            const int q = threadIdx.x - TR;
+            cols_s[q] = o0 + q >= nout ? -1 : INV ? collist[o0 + q] : o0 + q;
+        }
+        __syncthreads();                                             // rows_s, cols_s are visible
+        double acc_r[4][4];
+#pragma unroll
+        for (int qa = 0; qa < 4; qa++)
+#pragma unroll
+            for (int qb = 0; qb < 4; qb++) {
+                const int row = rows_s[4 * ty + qb], col = cols_s[gemm_out(tx, qa)];
+                acc_r[qa][qb] = (!first && row >= 0 && col >= 0) ? acc[(size_t)row * n + col] : 0.0;
+            }
+        const int tq = o0 + (threadIdx.x >> 1), tkk = 8 * (threadIdx.x & 1);
+        const int xrow = rows_s[threadIdx.x >> 2], xkk = 4 * (threadIdx.x & 3);
+        double tv[8], xv[4];
+        auto fetch = [&](int kb) {                                   // (register prefetch of the next tiles, as in dct_gemm_kernel)
+#pragma unroll
+            for (int q = 0; q < 8; q++) { const int k = kb + tkk + q; tv[q] = (tq < nout && k < k1) ? P[(size_t)tq * kp + (k - k0)] : 0.0; }
+#pragma unroll
+            for (int q = 0; q < 4; q++) { const int k = kb + xkk + q; xv[q] = (xrow >= 0 && k < k1) ? (double)X[(size_t)xrow * n + k] : 0.0; }
+        };
+        fetch(k0);
+        for (int kb = k0; kb < k1; kb += TK) {
+            __syncthreads();
+#pragma unroll
+            for (int q = 0; q < 8; q++) Ts[tkk + q][threadIdx.x >> 1] = tv[q];
+#pragma unroll
+            for (int q = 0; q < 4; q++) Xs[xkk + q][threadIdx.x >> 2] = xv[q];
+            __syncthreads();
+            if (kb + TK < k1) fetch(kb + TK);
+            gemm_tile_fp64(Ts, Xs, (k1 - kb < TK) ? k1 - kb : TK, tx, ty, acc_r);
+        }
+#pragma unroll
+        for (int qb = 0; qb < 4; qb++) {
+            const int row = rows_s[4 * ty + qb];
+            if (row < 0) continue;
+#pragma unroll
+            for (int qa = 0; qa < 4; qa++) {
+                const int col = cols_s[gemm_out(tx, qa)];
+                if (col < 0) continue;
+                const size_t p = (size_t)row * n + col;
+                double y = acc_r[qa][qb];
+                if (!last) { acc[p] = y; continue; }
+                if (INV) {
+                    if (fabsf(img[p]) <= rowthr[row]) rt[p] = (float)__dmul_rn(0.5, __dadd_rn(y, 0.0));
+                    continue;
+                }
+                if (DIVN) y = __ddiv_rn(y, (double)n);
+                if (Y2) {
+                    if (col >= 1) Y2[p - 1] = __dmul_rn(y, mul2[col]);
+                    if (col == n - 1) Y2[p] = 0.0;
+                }
+                Y[p] = mul ? __dmul_rn(y, mul[col]) : y;
+            }
+        }
+    }
+}
+
 // q != 0: out = (float)(0.5 * (sym + antisym)) on every pixel (shear.c:88-89)
 __global__ void dct_combine_kernel(const double *__restrict__ sym, const double *__restrict__ anti, size_t n, float *__restrict__ out)
 {

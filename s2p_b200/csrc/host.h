@@ -73,6 +73,17 @@ struct Slot {
     int *abort = nullptr;         // this slot's word of s2pb_ctx::abort_words: a timeout of a call on this slot raises it
     bool timed = false;
     bool direct_out = false;      // the last host-API call wrote its results straight into the caller's pinned buffers
+    // K-panels of the DCT tables of rows wider than the resident tables serve (dct_tables, stream_panels): two pinned staging
+    // buffers and two device panels of `panel` doubles each, the copy stream and its events, and the running sums of the round
+    // trip's inverse product (acc_pix doubles); allocated on first use
+    struct DctStream {
+        double *h[2] = {nullptr, nullptr}, *d[2] = {nullptr, nullptr};
+        size_t panel = 0;
+        cudaStream_t copy = nullptr;
+        cudaEvent_t copied[2] = {}, consumed[2] = {};
+        double *acc = nullptr;
+        size_t acc_pix = 0;
+    } dcts;
 };
 struct s2pb_ctx {
     int device = 0;
@@ -86,8 +97,11 @@ struct s2pb_ctx {
     std::atomic<long long> launches{0};   // (mgm_multi tiles of a batch are enqueued from several host threads)
     size_t ws_limit = 0;                  // s2pb_set_workspace_limit: bytes per workspace, 0 = none
     std::atomic<long long> folded_calls{0};   // mgm_calls that ran in the folded layout (s2pb_folded_calls)
-    // DCT coefficient tables of the matched image's round trip, one entry per image width (dct_tables)
+    // DCT coefficient tables of the matched image's round trip, one entry per image width (dct_tables); a null table of a width
+    // above kDctDenseWidth is streamed in K-panels
     struct DctTab { int n; double *T10, *T01, *TR01, *mc, *ms; };
+    size_t dct_limit = (size_t)8 << 30;   // s2pb_set_dct_table_limit: device bytes of resident tables above kDctDenseWidth
+    size_t dct_wide_bytes = 0;            // ... held now
     std::list<DctTab> dct;          // a list: entries stay put while other host threads hold pointers to them
     std::mutex dct_mu;
     // scratch pool of the host-buffer entry points: device buffers are kept between calls (a cudaMalloc / cudaFree pair per

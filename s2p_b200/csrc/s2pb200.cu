@@ -13,6 +13,7 @@
 #include "agg_chunked.cuh"
 
 #include <chrono>
+#include <climits>
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
@@ -275,6 +276,17 @@ extern "C" void s2pb_destroy(s2pb_ctx *ctx)
     }
     for (auto &b : ctx->pool) cudaFree(b.p);
     for (auto &t : ctx->dct) for (double *q : {t.T10, t.T01, t.TR01, t.mc, t.ms}) if (q) cudaFree(q);
+    for (auto &s : ctx->slots) {
+        Slot::DctStream &S = s.dcts;
+        if (S.copy) { cudaStreamSynchronize(S.copy); cudaStreamDestroy(S.copy); }
+        for (int b = 0; b < 2; b++) {
+            if (S.h[b]) cudaFreeHost(S.h[b]);
+            if (S.d[b]) cudaFree(S.d[b]);
+            if (S.copied[b]) cudaEventDestroy(S.copied[b]);
+            if (S.consumed[b]) cudaEventDestroy(S.consumed[b]);
+        }
+        if (S.acc) cudaFree(S.acc);
+    }
     geoid_free(ctx);
     if (ctx->abort_words) cudaFreeHost(ctx->abort_words);
     delete ctx;
@@ -419,7 +431,8 @@ static int check_params(const s2pb_mgm_params *p, int w, int h, int dmin, int dm
     if (p->scales < 0 && p->remove_small_cc > 0) return fail(S2PB_ERR_UNSUPPORTED, "REMOVESMALLCC is only wired into the mgm_multi path");
     if (p->lr_mode < 0 || p->lr_mode > 2) return fail(S2PB_ERR_ARG, "TESTLRRL must be 0, 1 or 2");
     if (p->scales < 0 && p->lr_mode == 2) return fail(S2PB_ERR_ARG, "TESTLRRL=2 only exists in mgm_multi");
-    if (p->scales >= 0 && w > 4000) return fail(S2PB_ERR_UNSUPPORTED, "mgm_multi tiles wider than 4000 px are not supported");
+    // pixel indices of the pyramid, the label ranges and the post filters are 32-bit
+    if ((long long)w * h > INT_MAX) return fail(S2PB_ERR_UNSUPPORTED, "tiles of more than 2^31 - 1 pixels are not supported (%dx%d)", w, h);
     if (abs(dmin) > 16000 || abs(dmax) > 16000) return fail(S2PB_ERR_ARG, "disparity bounds out of the int16 label range");
     if (p->cost < 0 || p->cost >= S2PB_COST_COUNT) return fail(S2PB_ERR_ARG, "cost must be one of S2PB_COST_* (got %d)", p->cost);
     return S2PB_OK;
@@ -689,21 +702,81 @@ static void fill_wta(WtaParams &P, const ViewWS &v, int ndir, int gmin, const s2
 
 // ------------------------------------------------------------------ the matched image's DCT round trip (dct_kernels.cuh)
 
-// Coefficient tables for rows of n pixels, computed once per width on the host (libm, like the reference's DCT) and
-// kept on the device.  FFTW's unnormalised definitions:
+// Coefficient tables for rows of n pixels, computed on the host (libm, like the reference's DCT: device cos / sin differ in the
+// last bit).  FFTW's unnormalised definitions, each table [output][input] row-major:
 //   REDFT10  Y[k] = sum_j 2 cos(pi (j + 1/2) k / n) X[j]
 //   REDFT01  Y[i] = X[0] + sum_{k>=1} 2 cos(pi k (i + 1/2) / n) X[k]
 //   RODFT01  Y[i] = (-1)^i X[n-1] + sum_{k<n-1} 2 sin(pi (k + 1) (i + 1/2) / n) X[k]
-// half = true adds what the half-pixel shift of SUBPIX = 2 needs (both inverse tables row-major and the phase factors
-// cos(k a), sin(k a), a = (pi / n) * (-1/2), shear.c:66-79).
+// Up to kDctDenseWidth they are kept on the device, once per width, whatever they take (1.5 GiB at 8192 with the half shift).
+// Wider rows keep a table resident while the context's resident wide tables stay within its table budget (dct_budget), and
+// stream it in K-panels otherwise (stream_panels).
+constexpr int kDctDenseWidth = 8192;
+enum DctKind { kDctT10 = 0, kDctT01 = 1, kDctTR01 = 2 };
+
+static double dct_coef(int kind, int n, int r, int c)
+{
+    const double pi = 3.14159265358979323846264338327950288;
+    if (kind == kDctT10) return 2.0 * cos(pi * (c + 0.5) * r / n);
+    if (kind == kDctT01) return (c == 0) ? 1.0 : 2.0 * cos(pi * c * (r + 0.5) / n);
+    return (c == n - 1) ? ((r & 1) ? -1.0 : 1.0) : 2.0 * sin(pi * (c + 1) * (r + 0.5) / n);
+}
+
+// dst[q][c - c0] = coefficient (rows[q], c) of table `kind` (rows == nullptr: row q), c in [c0, c0 + ncols), on a pool of host
+// threads (one block of rows each)
+static void dct_fill(int kind, int n, const int *rows, int nrows, int c0, int ncols, double *dst)
+{
+    auto work = [=](int q0, int q1) {
+        for (int q = q0; q < q1; q++) {
+            const int r = rows ? rows[q] : q;
+            double *o = dst + (size_t)q * ncols;
+            for (int c = 0; c < ncols; c++) o[c] = dct_coef(kind, n, r, c0 + c);
+        }
+    };
+    const long long terms = (long long)nrows * ncols;
+    int nt = (int)std::min<long long>(std::max(1u, std::thread::hardware_concurrency()), std::min<long long>(64, terms / 65536 + 1));
+    nt = std::min(nt, nrows);
+    if (nt <= 1) { work(0, nrows); return; }
+    std::vector<std::thread> pool;
+    for (int t = 0; t < nt; t++) pool.emplace_back(work, (int)((long long)nrows * t / nt), (int)((long long)nrows * (t + 1) / nt));
+    for (auto &th : pool) th.join();
+}
+
+extern "C" int s2pb_dct_coefficients(int kind, int n, int row0, int nrows, int col0, int ncols, double *out)
+{
+    if (kind < kDctT10 || kind > kDctTR01 || n < 1 || !out || row0 < 0 || nrows < 0 || col0 < 0 || ncols < 0 || row0 + nrows > n ||
+        col0 + ncols > n)
+        return fail(S2PB_ERR_ARG, "bad argument");
+    std::vector<int> rows(nrows);
+    for (int q = 0; q < nrows; q++) rows[q] = row0 + q;
+    dct_fill(kind, n, rows.data(), nrows, col0, ncols, out);
+    return S2PB_OK;
+}
+
+extern "C" int s2pb_set_dct_table_limit(s2pb_ctx *ctx, long long bytes)
+{
+    if (!ctx || bytes < 0) return fail(S2PB_ERR_ARG, "bad argument");
+    std::lock_guard<std::mutex> lock(ctx->dct_mu);
+    ctx->dct_limit = (size_t)bytes;
+    return S2PB_OK;
+}
+
+// the device bytes the context may hold in resident tables wider than kDctDenseWidth: its table limit, and no more than its
+// workspace limit when one is set
+static size_t dct_budget(const s2pb_ctx *ctx)
+{
+    return ctx->ws_limit ? std::min(ctx->dct_limit, ctx->ws_limit) : ctx->dct_limit;
+}
+
+// The tables of rows of n pixels (half: with what the half-pixel shift of SUBPIX = 2 needs, RODFT01 and the phase factors
+// cos(k a), sin(k a), a = (pi / n) * (-1/2), shear.c:66-79).  Above kDctDenseWidth a table that the budget or the device
+// cannot hold stays null: the caller streams it.
 static int dct_tables(s2pb_ctx *ctx, int n, bool half, const s2pb_ctx::DctTab **out)
 {
-    if (n > 8192) return fail(S2PB_ERR_UNSUPPORTED, "tiles wider than 8192 px are not supported (DCT tables of %d x %d doubles)", n, n);
     std::lock_guard<std::mutex> lock(ctx->dct_mu);
     s2pb_ctx::DctTab *t = nullptr;
     for (auto &e : ctx->dct) if (e.n == n) t = &e;
     if (!t) { ctx->dct.push_back({n, nullptr, nullptr, nullptr, nullptr, nullptr}); t = &ctx->dct.back(); }
-    const double pi = 3.14159265358979323846264338327950288;
+    const bool wide = n > kDctDenseWidth;
     const size_t nn = (size_t)n * n;
     std::vector<double> h;
     auto upload = [&](double **dst, size_t count) -> int {
@@ -712,24 +785,21 @@ static int dct_tables(s2pb_ctx *ctx, int n, bool half, const s2pb_ctx::DctTab **
         CK(cudaMemcpy(*dst, h.data(), count * sizeof(double), cudaMemcpyHostToDevice));
         return S2PB_OK;
     };
+    auto table = [&](double **dst, int kind) -> int {
+        if (*dst) return S2PB_OK;
+        if (wide && ctx->dct_wide_bytes + nn * 8 > dct_budget(ctx)) return S2PB_OK;       // streamed
+        h.resize(nn);
+        dct_fill(kind, n, nullptr, n, 0, n, h.data());
+        int rc = upload(dst, nn);
+        if (!wide || rc == S2PB_ERR_CUDA) return rc;
+        if (*dst) ctx->dct_wide_bytes += nn * 8;
+        return S2PB_OK;                                                                      // (out of memory: streamed)
+    };
     int rc;
-    if (!t->T10) {
-        h.resize(nn);
-        for (int k = 0; k < n; k++)
-            for (int j = 0; j < n; j++) h[(size_t)k * n + j] = 2.0 * cos(pi * (j + 0.5) * k / n);
-        if ((rc = upload(&t->T10, nn)) != S2PB_OK) return rc;
-    }
-    if (!t->T01) {
-        h.resize(nn);
-        for (int i = 0; i < n; i++)
-            for (int k = 0; k < n; k++) h[(size_t)i * n + k] = (k == 0) ? 1.0 : 2.0 * cos(pi * k * (i + 0.5) / n);
-        if ((rc = upload(&t->T01, nn)) != S2PB_OK) return rc;
-    }
-    if (half && !t->TR01) {
-        h.resize(nn);
-        for (int i = 0; i < n; i++)
-            for (int k = 0; k < n; k++) h[(size_t)i * n + k] = (k == n - 1) ? ((i & 1) ? -1.0 : 1.0) : 2.0 * sin(pi * (k + 1) * (i + 0.5) / n);
-        if ((rc = upload(&t->TR01, nn)) != S2PB_OK) return rc;
+    if ((rc = table(&t->T10, kDctT10)) != S2PB_OK) return rc;
+    if ((rc = table(&t->T01, kDctT01)) != S2PB_OK) return rc;
+    if (half && (rc = table(&t->TR01, kDctTR01)) != S2PB_OK) return rc;
+    if (half && !t->mc) {
         const float q = 0.5f, translation = -q;                  // shift() passes (0., -q) as floats, mgm_costvolume.cc:35
         const double tt = 0 * 0.0f + translation, a = (M_PI / n) * tt;
         h.resize(n);
@@ -742,9 +812,83 @@ static int dct_tables(s2pb_ctx *ctx, int n, bool half, const s2pb_ctx::DctTab **
     return S2PB_OK;
 }
 
-// rt = shift(img, 0) of the reference: see dct_kernels.cuh.  Asynchronous; when no row needs it the kernels return at once.
+// Columns per K-panel of a table streamed for rows of n pixels: panels of about 64 MiB, a multiple of the products' K tile
+static int dct_panel_cols(int n)
+{
+    const size_t cols = ((size_t)64 << 20) / 8 / (size_t)n / kGemmTK * kGemmTK;
+    return (int)std::max<size_t>(kGemmTK, std::min<size_t>(cols, (size_t)n));
+}
+
+// the staging of slot s's streamed products for panels of `panel` doubles and, when acc_pix > 0, that many running sums
+static int dct_stream_ensure(Slot &s, size_t panel, size_t acc_pix)
+{
+    Slot::DctStream &S = s.dcts;
+    if (!S.copy) {
+        CK(cudaStreamCreateWithFlags(&S.copy, cudaStreamNonBlocking));
+        for (int b = 0; b < 2; b++) {
+            CK(cudaEventCreateWithFlags(&S.copied[b], cudaEventDisableTiming));
+            CK(cudaEventCreateWithFlags(&S.consumed[b], cudaEventDisableTiming));
+        }
+    }
+    // the buffers are replaced only after the products that read them: each panel's product records consumed[b]
+    if (S.panel < panel || S.acc_pix < acc_pix)
+        for (int b = 0; b < 2; b++) { CK(cudaEventSynchronize(S.consumed[b])); CK(cudaEventSynchronize(S.copied[b])); }
+    if (S.panel < panel) {
+        for (int b = 0; b < 2; b++) {
+            if (S.h[b]) { cudaFreeHost(S.h[b]); S.h[b] = nullptr; }
+            if (S.d[b]) { cudaFree(S.d[b]); S.d[b] = nullptr; }
+        }
+        S.panel = 0;
+        for (int b = 0; b < 2; b++) {
+            if (cudaMallocHost((void **)&S.h[b], panel * 8) != cudaSuccess || cudaMalloc((void **)&S.d[b], panel * 8) != cudaSuccess) {
+                cudaGetLastError();
+                return fail(S2PB_ERR_NOMEM, "staging of the streamed DCT tables (2 x %zu bytes pinned and on the device)", panel * 8);
+            }
+        }
+        S.panel = panel;
+    }
+    if (S.acc_pix < acc_pix) {
+        if (S.acc) { CK(cudaFree(S.acc)); S.acc = nullptr; S.acc_pix = 0; }
+        if (cudaMalloc((void **)&S.acc, acc_pix * 8) != cudaSuccess) {
+            cudaGetLastError();
+            return fail(S2PB_ERR_NOMEM, "running sums of the streamed DCT round trip (%zu bytes)", acc_pix * 8);
+        }
+        S.acc_pix = acc_pix;
+    }
+    return S2PB_OK;
+}
+
+// One product through the K-panels of table `kind` for rows of n pixels, restricted to the table rows `rows` (nullptr: all n;
+// nrows of them).  Panel p is built on the host into staging buffer p % 2 while the device multiplies panel p - 1, uploaded on
+// the slot's copy stream once the product of panel p - 2 is done with device buffer p % 2, and multiplied on st by
+// product(panel, k0, k1) (dct_panel_gemm_kernel).  Returns once the last panel is enqueued.
+template <class F>
+static int stream_panels(Slot &s, cudaStream_t st, int kind, int n, const int *rows, int nrows, F &&product)
+{
+    const int kp = dct_panel_cols(n);
+    int rc = dct_stream_ensure(s, (size_t)nrows * kp, 0);
+    if (rc != S2PB_OK) return rc;
+    Slot::DctStream &S = s.dcts;
+    for (int k0 = 0, p = 0; k0 < n; k0 += kp, p++) {
+        const int b = p & 1, k1 = std::min(n, k0 + kp);
+        CK(cudaEventSynchronize(S.copied[b]));                   // the upload of panel p - 2 has left the staging buffer
+        dct_fill(kind, n, rows, nrows, k0, k1 - k0, S.h[b]);
+        CK(cudaStreamWaitEvent(S.copy, S.consumed[b], 0));       // the product of panel p - 2 is done with the device buffer
+        CK(cudaMemcpyAsync(S.d[b], S.h[b], (size_t)nrows * (k1 - k0) * 8, cudaMemcpyHostToDevice, S.copy));
+        CK(cudaEventRecord(S.copied[b], S.copy));
+        CK(cudaStreamWaitEvent(st, S.copied[b], 0));
+        product((const double *)S.d[b], k0, k1);
+        CK(cudaEventRecord(S.consumed[b], st));
+    }
+    CK(cudaGetLastError());
+    return S2PB_OK;
+}
+
+// rt = shift(img, 0) of the reference: see dct_kernels.cuh.  Asynchronous with resident tables; when no row needs it the
+// kernels return at once.  A streamed table (rows wider than kDctDenseWidth) first waits for the row and column lists: with no
+// listed row nothing is streamed, and the inverse streams the listed columns' rows of its table only.
 // Y: [h][w] doubles of scratch.  rowlist: room for h + w ints and w bytes (row list, column list, column flags).
-static int round_trip_zero(s2pb_ctx *ctx, const float *img, int w, int h, float *rt, RtState *state, int *rowlist, float *rowthr,
+static int round_trip_zero(s2pb_ctx *ctx, Slot &s, const float *img, int w, int h, float *rt, RtState *state, int *rowlist, float *rowthr,
                            double *Y, cudaStream_t st)
 {
     int *collist = rowlist + h;
@@ -756,14 +900,43 @@ static int round_trip_zero(s2pb_ctx *ctx, const float *img, int w, int h, float 
     CK(cudaMemsetAsync(colflag, 0, (size_t)w, st));
     launch(ctx, rt_flag_kernel, h, 256, 0, st, img, w, h, rt, state, rowlist, rowthr, colflag);
     launch(ctx, rt_collist_kernel, 1, 1024, 0, st, colflag, w, state, collist);
-    launch(ctx, dct_gemm_kernel<float, true>, ctx->sm_count * 4, kGemmThreads, 0, st, t->T10, img, w, h, state, rowlist, Y, nullptr, nullptr, nullptr);
-    launch(ctx, rt_inverse_gemm_kernel, ctx->sm_count * 4, kGemmThreads, 0, st, t->T01, Y, w, state, rowlist, collist, rowthr, img, rt);
+    const int g = ctx->sm_count * 4;
+    if (t->T10 && t->T01) {
+        launch(ctx, dct_gemm_kernel<float, true>, g, kGemmThreads, 0, st, t->T10, img, w, h, state, rowlist, Y, nullptr, nullptr, nullptr);
+        launch(ctx, rt_inverse_gemm_kernel, g, kGemmThreads, 0, st, t->T01, Y, w, state, rowlist, collist, rowthr, img, rt);
+        CK(cudaGetLastError());
+        return S2PB_OK;
+    }
+    RtState hs;
+    std::vector<int> cols(w);
+    CK(cudaMemcpyAsync(&hs, state, sizeof hs, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(cols.data(), collist, (size_t)w * 4, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (hs.nrows == 0) return S2PB_OK;
+    if (t->T10)
+        launch(ctx, dct_gemm_kernel<float, true>, g, kGemmThreads, 0, st, t->T10, img, w, h, state, rowlist, Y, nullptr, nullptr, nullptr);
+    else
+        rc = stream_panels(s, st, kDctT10, w, nullptr, w, [&](const double *P, int k0, int k1) {
+            launch(ctx, dct_panel_gemm_kernel<float, true, false>, g, kGemmThreads, 0, st, P, k0, k1, img, w, h, state, rowlist, nullptr, Y,
+                   k0 == 0, k1 == w, Y, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
+        });
+    if (rc != S2PB_OK) return rc;
+    if (t->T01) {
+        launch(ctx, rt_inverse_gemm_kernel, g, kGemmThreads, 0, st, t->T01, Y, w, state, rowlist, collist, rowthr, img, rt);
+    } else {
+        if ((rc = dct_stream_ensure(s, 0, (size_t)w * h)) != S2PB_OK) return rc;
+        double *acc = s.dcts.acc;
+        rc = stream_panels(s, st, kDctT01, w, cols.data(), hs.ncols, [&](const double *P, int k0, int k1) {
+            launch(ctx, dct_panel_gemm_kernel<double, false, true>, g, kGemmThreads, 0, st, P, k0, k1, (const double *)Y, w, 0, state, rowlist,
+                   collist, acc, k0 == 0, k1 == w, nullptr, nullptr, nullptr, nullptr, rowthr, img, rt);
+        });
+    }
     CK(cudaGetLastError());
-    return S2PB_OK;
+    return rc;
 }
 
 // out = shift(img, 1/2) of the reference (SUBPIX = 2).  scratch: 4 x [h][w] doubles.
-static int shift_half(s2pb_ctx *ctx, const float *img, int w, int h, float *out, double *scratch, cudaStream_t st)
+static int shift_half(s2pb_ctx *ctx, Slot &s, const float *img, int w, int h, float *out, double *scratch, cudaStream_t st)
 {
     const s2pb_ctx::DctTab *t;
     int rc = dct_tables(ctx, w, true, &t);
@@ -771,9 +944,29 @@ static int shift_half(s2pb_ctx *ctx, const float *img, int w, int h, float *out,
     const size_t npix = (size_t)w * h;
     double *ck = scratch, *sk = scratch + npix, *sym = scratch + 2 * npix, *anti = scratch + 3 * npix;
     const int g = ctx->sm_count * 4;
-    launch(ctx, dct_gemm_kernel<float, true>, g, kGemmThreads, 0, st, t->T10, img, w, h, nullptr, nullptr, ck, t->mc, t->ms, sk);
-    launch(ctx, dct_gemm_kernel<double, false>, g, kGemmThreads, 0, st, t->T01, ck, w, h, nullptr, nullptr, sym, nullptr, nullptr, nullptr);
-    launch(ctx, dct_gemm_kernel<double, false>, g, kGemmThreads, 0, st, t->TR01, sk, w, h, nullptr, nullptr, anti, nullptr, nullptr, nullptr);
+    if (t->T10)
+        launch(ctx, dct_gemm_kernel<float, true>, g, kGemmThreads, 0, st, t->T10, img, w, h, nullptr, nullptr, ck, t->mc, t->ms, sk);
+    else
+        rc = stream_panels(s, st, kDctT10, w, nullptr, w, [&](const double *P, int k0, int k1) {
+            launch(ctx, dct_panel_gemm_kernel<float, true, false>, g, kGemmThreads, 0, st, P, k0, k1, img, w, h, nullptr, nullptr, nullptr,
+                   ck, k0 == 0, k1 == w, ck, (const double *)t->mc, (const double *)t->ms, sk, nullptr, nullptr, nullptr);
+        });
+    if (rc != S2PB_OK) return rc;
+    const double *inv_tab[2] = {t->T01, t->TR01};
+    const double *inv_in[2] = {ck, sk};
+    double *inv_out[2] = {sym, anti};
+    for (int i = 0; i < 2; i++) {
+        if (inv_tab[i]) {
+            launch(ctx, dct_gemm_kernel<double, false>, g, kGemmThreads, 0, st, inv_tab[i], inv_in[i], w, h, nullptr, nullptr, inv_out[i],
+                   nullptr, nullptr, nullptr);
+            continue;
+        }
+        rc = stream_panels(s, st, i ? kDctTR01 : kDctT01, w, nullptr, w, [&](const double *P, int k0, int k1) {
+            launch(ctx, dct_panel_gemm_kernel<double, false, false>, g, kGemmThreads, 0, st, P, k0, k1, inv_in[i], w, h, nullptr, nullptr,
+                   nullptr, inv_out[i], k0 == 0, k1 == w, inv_out[i], nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
+        });
+        if (rc != S2PB_OK) return rc;
+    }
     launch(ctx, dct_combine_kernel, (unsigned)((npix + 255) / 256), 256, 0, st, sym, anti, npix, out);
     CK(cudaGetLastError());
     return S2PB_OK;
@@ -887,7 +1080,7 @@ static int mgm_call(s2pb_ctx *ctx, const MatchCall &c, int w, int h, const float
         ViewWS &v = s.v[vi];
         v.lo = lo[vi]; v.hi = hi[vi];
         // v.rt = shift(img[vi], 0): the reference's DCT round trip (mgm_costvolume.cc:50-60)
-        rc = round_trip_zero(ctx, img[vi], w, h, v.rt, v.rtstate, v.rowlist, v.rowthr, s.Ydct, st);
+        rc = round_trip_zero(ctx, s, img[vi], w, h, v.rt, v.rtstate, v.rowlist, v.rowthr, s.Ydct, st);
         if (rc != S2PB_OK) return rc;
         if (census && wide)
             launch(ctx, census_pair_kernel<2>, grid2d(w, h, b2), b2, 0, st, img[vi], v.rt, v.rtstate, w, h, p->census_win / 2, v.census,
@@ -912,7 +1105,7 @@ static int mgm_call(s2pb_ctx *ctx, const MatchCall &c, int w, int h, const float
         double *scratch = arena_take<double>(s, npix * 4);
         if (!scratch) return fail(S2PB_ERR_NOMEM, "pyramid arena exhausted");
         for (int vi = 0; vi < 2; vi++) {
-            rc = shift_half(ctx, img[vi], w, h, shf[vi], scratch, st);
+            rc = shift_half(ctx, s, img[vi], w, h, shf[vi], scratch, st);
             if (rc != S2PB_OK) return rc;
             if (census && wide) launch(ctx, census_kernel<2>, grid2d(w, h, b2), b2, 0, st, shf[vi], w, h, p->census_win / 2, cen_half[vi], cen_half_hi[vi]);
             else if (census) launch(ctx, census_kernel<1>, grid2d(w, h, b2), b2, 0, st, shf[vi], w, h, p->census_win / 2, cen_half[vi], nullptr);
@@ -1470,7 +1663,7 @@ static int stage_round_trip(s2pb_ctx *ctx, ScratchLease &L, const float *dv, int
     char *aux = L.take<char>(lists + (size_t)h * 4 + 256);
     double *Y = L.take<double>(npix * 8);
     if (!out || !aux || !Y) return L.nomem("the round trip");
-    int rc = round_trip_zero(ctx, dv, w, h, out, (RtState *)(aux + lists + (size_t)h * 4), (int *)aux, (float *)(aux + lists), Y, st);
+    int rc = round_trip_zero(ctx, ctx->slots[0], dv, w, h, out, (RtState *)(aux + lists + (size_t)h * 4), (int *)aux, (float *)(aux + lists), Y, st);
     if (rc != S2PB_OK) return rc;
     *rt = out;
     return S2PB_OK;

@@ -59,6 +59,17 @@ def workspace_layout(w, h, nlabels, ndir=8, cost_bytes=1, limit=0):
     return "folded" if r == 1 else "resident"
 
 
+def dct_coefficients(kind, n, rows, cols):
+    """The engine's DCT coefficient table ``kind`` (0 REDFT10, 1 REDFT01, 2 RODFT01) for rows of n pixels, on the row range
+    ``rows`` and the column range ``cols`` (Python ranges of step 1), float64 (s2pb_dct_coefficients; no device needed)."""
+    out = np.empty((len(rows), len(cols)), np.float64)
+    r0 = rows.start if len(rows) else 0
+    c0 = cols.start if len(cols) else 0
+    _lib.check(_lib.lib().s2pb_dct_coefficients(int(kind), int(n), int(r0), len(rows), int(c0), len(cols),
+                                                out.ctypes.data_as(ctypes.POINTER(ctypes.c_double))))
+    return out
+
+
 def _f32(a):
     return np.ascontiguousarray(a, dtype=np.float32)
 
@@ -233,6 +244,12 @@ class Engine:
         """Cap each workspace of this engine at ``nbytes`` (0: no cap).  A tile whose resident workspace exceeds the cap runs in the
         folded layout, with the same results (s2pb_set_workspace_limit)."""
         _lib.check(self._L.s2pb_set_workspace_limit(self._ctx, int(nbytes)))
+
+    def set_dct_table_limit(self, nbytes):
+        """Keep the DCT tables of rows wider than 8192 px on the device up to ``nbytes`` in all (default 8 GiB, and no more
+        than the workspace limit when one is set); wider tables are streamed in panels, with the same results
+        (s2pb_set_dct_table_limit)."""
+        _lib.check(self._L.s2pb_set_dct_table_limit(self._ctx, int(nbytes)))
 
     def folded_calls(self):
         """matcher calls (pyramid levels of mgm_multi included) that ran in the folded layout"""
