@@ -64,16 +64,6 @@ __global__ void rt_flag_kernel(const float *__restrict__ img, int w, int h, floa
     }
 }
 
-// Y[r][o] = (sum_{i=0}^{n-1} T[o][i] * X[r][i]) * scale-by-division, r over the listed rows (or all rows when
-// rowlist == nullptr).  The sum runs in ascending i with separately rounded multiply and add, from 0.0, like a plain C
-// loop compiled without contraction.  T is [n][n] row-major.  64 outputs x 32 rows per block of 128 threads, 4 x 4 per
-// thread: a thread's four T values and four X values of one i are two 16-byte shared loads each, i.e. four loads per
-// sixteen multiply-add pairs (a 4 x 2 tile with 8-byte loads needs six per eight and is bound by them).  512 work items on a
-// 1024 x 1024 image for the 132 SMs.
-// IN = float (image rows) or double.  DIVN: divide the sum by n (the forward transform's normalisation, shear.c:62-63).
-// `mul` (optional, [n]): the output is multiplied by mul[o] (the phase factor cos(o a));
-// `mul2`/`Y2` (optional): a second output Y2[r][o-1] = y * mul2[o] for o >= 1 and Y2[r][n-1] = 0 (the antisymmetric
-// part's input, shear.c:71-79).
 constexpr int kGemmThreads = 128, kGemmTO = 64, kGemmTR = 32, kGemmTK = 16;
 // one tile product: acc[qa][qb] += Ts[kk][gemm_out(tx, qa)] * Xs[kk][4 ty + qb] for kk < kmax, in ascending kk.  A thread's four
 // outputs are two adjacent pairs 32 apart (2 tx, 2 tx + 1, 32 + 2 tx, 33 + 2 tx): the lanes' 16-byte loads are then contiguous
@@ -92,74 +82,6 @@ __device__ __forceinline__ void gemm_tile_fp64(const double (*Ts)[kGemmTO + 2], 
             for (int qb = 0; qb < 4; qb++) acc[qa][qb] = __dadd_rn(acc[qa][qb], __dmul_rn(a[qa], b[qb]));
     }
 }
-template <typename IN, bool DIVN>
-__global__ void __launch_bounds__(kGemmThreads) dct_gemm_kernel(const double *__restrict__ T, const IN *__restrict__ X, int n, int nrows_all,
-                                                                const RtState *st, const int *__restrict__ rowlist,
-                                                                double *__restrict__ Y, const double *__restrict__ mul,
-                                                                const double *__restrict__ mul2, double *__restrict__ Y2)
-{
-    constexpr int TO = kGemmTO, TR = kGemmTR, TK = kGemmTK;
-    __shared__ __align__(16) double Ts[TK][TO + 2];
-    __shared__ __align__(16) double Xs[TK][TR + 2];
-    __shared__ int rows_s[TR];
-    const int nrows = rowlist ? st->nrows : nrows_all;
-    const int otiles = (n + TO - 1) / TO, rtiles = (nrows + TR - 1) / TR;
-    const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;         // outputs gemm_out(tx, 0..3), rows 4 ty .. +3
-    for (int item = blockIdx.x; item < otiles * rtiles; item += gridDim.x) {
-        const int o0 = (item % otiles) * TO, r0 = (item / otiles) * TR;
-        __syncthreads();
-        if (threadIdx.x < TR) {
-            const int rr = r0 + threadIdx.x;
-            rows_s[threadIdx.x] = rr < nrows ? (rowlist ? rowlist[rr] : rr) : -1;
-        }
-        double acc[4][4];
-#pragma unroll
-        for (int qa = 0; qa < 4; qa++)
-#pragma unroll
-            for (int qb = 0; qb < 4; qb++) acc[qa][qb] = 0.0;
-        // T tile: 64 outputs x 16 inputs, thread t holds output (t >> 1), inputs 8 (t & 1) .. +7; X tile: 32 rows x 16 inputs, thread t
-        // holds row (t >> 2), inputs 4 (t & 3) .. +3.  The next tile's values are fetched into registers before the current tile's
-        // product, so the global-load latency hides behind 16 x 32 FP64 instructions instead of standing between two barriers.
-        __syncthreads();                                             // rows_s is visible
-        const int to = o0 + (threadIdx.x >> 1), tkk = 8 * (threadIdx.x & 1);
-        const int xrow = rows_s[threadIdx.x >> 2], xkk = 4 * (threadIdx.x & 3);
-        double tv[8], xv[4];
-        auto fetch = [&](int k0) {
-#pragma unroll
-            for (int q = 0; q < 8; q++) { const int k = k0 + tkk + q; tv[q] = (to < n && k < n) ? T[(size_t)to * n + k] : 0.0; }
-#pragma unroll
-            for (int q = 0; q < 4; q++) { const int k = k0 + xkk + q; xv[q] = (xrow >= 0 && k < n) ? (double)X[(size_t)xrow * n + k] : 0.0; }
-        };
-        fetch(0);
-        for (int k0 = 0; k0 < n; k0 += TK) {
-            __syncthreads();                                         // the previous product is done with the tiles
-#pragma unroll
-            for (int q = 0; q < 8; q++) Ts[tkk + q][threadIdx.x >> 1] = tv[q];
-#pragma unroll
-            for (int q = 0; q < 4; q++) Xs[xkk + q][threadIdx.x >> 2] = xv[q];
-            __syncthreads();
-            if (k0 + TK < n) fetch(k0 + TK);
-            gemm_tile_fp64(Ts, Xs, (n - k0 < TK) ? n - k0 : TK, tx, ty, acc);
-        }
-#pragma unroll
-        for (int qb = 0; qb < 4; qb++) {
-            const int row = rows_s[4 * ty + qb];
-            if (row < 0) continue;
-#pragma unroll
-            for (int qa = 0; qa < 4; qa++) {
-                const int o = o0 + gemm_out(tx, qa);
-                if (o >= n) continue;
-                double y = acc[qa][qb];
-                if (DIVN) y = __ddiv_rn(y, (double)n);
-                if (Y2) {
-                    if (o >= 1) Y2[(size_t)row * n + o - 1] = __dmul_rn(y, mul2[o]);
-                    if (o == n - 1) Y2[(size_t)row * n + n - 1] = 0.0;
-                }
-                Y[(size_t)row * n + o] = mul ? __dmul_rn(y, mul[o]) : y;
-            }
-        }
-    }
-}
 
 // the columns that hold a flagged pixel, compacted (one block; the order is irrelevant)
 __global__ void rt_collist_kernel(const unsigned char *__restrict__ colflag, int w, RtState *st, int *__restrict__ collist)
@@ -173,92 +95,44 @@ __global__ void rt_collist_kernel(const unsigned char *__restrict__ colflag, int
     if (threadIdx.x == 0) st->ncols = count;
 }
 
-// q = 0, inverse: rt[r][i] = (float)(0.5 * (sum_k T01[i][k] Y[r][k] + 0.0)) for the FLAGGED pixels of the listed rows (the
-// antisymmetric part is identically +0: its inputs are Y[k] sin(0) = +-0).  The same tiled product as dct_gemm_kernel, over
-// the listed rows x the listed columns only -- a no-data margin is a few percent of the columns, so the inverse costs a few
-// percent of the forward transform; with a ragged mask the column list grows towards the full width and the cost towards
-// that of the forward one.  T01 is [n][n] row-major (output pixel, coefficient).
-__global__ void __launch_bounds__(kGemmThreads) rt_inverse_gemm_kernel(const double *__restrict__ T01, const double *__restrict__ Y, int n,
-                                                                       const RtState *st, const int *__restrict__ rowlist, const int *__restrict__ collist,
-                                                                       const float *__restrict__ rowthr, const float *__restrict__ img, float *__restrict__ rt)
-{
-    constexpr int TO = kGemmTO, TR = kGemmTR, TK = kGemmTK;
-    __shared__ __align__(16) double Ts[TK][TO + 2];
-    __shared__ __align__(16) double Xs[TK][TR + 2];
-    __shared__ int rows_s[TR], cols_s[TO];
-    const int nrows = st->nrows, ncols = st->ncols;
-    const int otiles = (ncols + TO - 1) / TO, rtiles = (nrows + TR - 1) / TR;
-    const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
-    for (int item = blockIdx.x; item < otiles * rtiles; item += gridDim.x) {
-        const int o0 = (item % otiles) * TO, r0 = (item / otiles) * TR;
-        __syncthreads();
-        if (threadIdx.x < TR) rows_s[threadIdx.x] = (r0 + (int)threadIdx.x < nrows) ? rowlist[r0 + threadIdx.x] : -1;
-        else if (threadIdx.x < TR + TO) { const int q = threadIdx.x - TR; cols_s[q] = (o0 + q < ncols) ? collist[o0 + q] : -1; }
-        double acc[4][4];
-#pragma unroll
-        for (int qa = 0; qa < 4; qa++)
-#pragma unroll
-            for (int qb = 0; qb < 4; qb++) acc[qa][qb] = 0.0;
-        __syncthreads();                                             // rows_s, cols_s are visible
-        const int tcol = cols_s[threadIdx.x >> 1], tkk = 8 * (threadIdx.x & 1);
-        const int xrow = rows_s[threadIdx.x >> 2], xkk = 4 * (threadIdx.x & 3);
-        double tv[8], xv[4];
-        auto fetch = [&](int k0) {                                   // (register prefetch of the next tiles, as in dct_gemm_kernel)
-#pragma unroll
-            for (int q = 0; q < 8; q++) { const int k = k0 + tkk + q; tv[q] = (tcol >= 0 && k < n) ? T01[(size_t)tcol * n + k] : 0.0; }
-#pragma unroll
-            for (int q = 0; q < 4; q++) { const int k = k0 + xkk + q; xv[q] = (xrow >= 0 && k < n) ? Y[(size_t)xrow * n + k] : 0.0; }
-        };
-        fetch(0);
-        for (int k0 = 0; k0 < n; k0 += TK) {
-            __syncthreads();
-#pragma unroll
-            for (int q = 0; q < 8; q++) Ts[tkk + q][threadIdx.x >> 1] = tv[q];
-#pragma unroll
-            for (int q = 0; q < 4; q++) Xs[xkk + q][threadIdx.x >> 2] = xv[q];
-            __syncthreads();
-            if (k0 + TK < n) fetch(k0 + TK);
-            gemm_tile_fp64(Ts, Xs, (n - k0 < TK) ? n - k0 : TK, tx, ty, acc);
-        }
-#pragma unroll
-        for (int qb = 0; qb < 4; qb++) {
-            const int row = rows_s[4 * ty + qb];
-            if (row < 0) continue;
-            const float thr = rowthr[row];
-#pragma unroll
-            for (int qa = 0; qa < 4; qa++) {
-                const int col = cols_s[gemm_out(tx, qa)];
-                if (col < 0) continue;
-                const size_t p = (size_t)row * n + col;
-                if (fabsf(img[p]) <= thr) rt[p] = (float)__dmul_rn(0.5, __dadd_rn(acc[qa][qb], 0.0));
-            }
-        }
-    }
-}
-
-// The K-panel form of dct_gemm_kernel (INV = false) and rt_inverse_gemm_kernel (INV = true), for rows wider than the resident
-// tables serve (dct_tables): one launch adds the terms of inputs [k0, k1) through a panel of the table, P[q][k - k0], q the
-// output (INV: q the position in the column list; the host builds the listed columns' rows only).  Each output's running sum
-// waits in `acc` ([row][n] doubles, row-major like Y) between the launches: the first panel starts it from 0.0, the last one
-// applies the resident kernel's epilogue instead of storing it.  Within a panel and across the panels the terms are added in
-// ascending k with the same separately rounded operations, and a double survives the store and the load exactly, so every
-// output is the resident kernel's sum bit for bit.  Forward: `acc` may be Y itself (each output is read and then written by
-// the thread that owns it).
+// Every table product of the round trip and of the half shift:
+//   forward (INV = false): Y[r][o] = sum_k T[o][k] X[r][k], then the epilogue below, r over the listed rows (all rows when
+//     rowlist == nullptr);
+//   inverse of q = 0 (INV = true): rt[r][i] = (float)(0.5 * (sum_k T01[i][k] Y[r][k] + 0.0)) for the FLAGGED pixels of the
+//     listed rows, i over the listed columns (the antisymmetric part is identically +0: its inputs are Y[k] sin(0) = +-0).  A
+//     no-data margin is a few percent of the columns, so the inverse costs a few percent of the forward transform; with a
+//     ragged mask the column list grows towards the full width and the cost towards that of the forward one.
+// One launch adds the terms of inputs [k0, k1) through a panel of the table, P[j][k - k0] with leading dimension ldp, j the
+// output -- or, when `listed`, the output's position in the column list (the host built the listed columns' rows only).  A
+// resident [n][n] table is one panel: k0 = 0, k1 = n, ldp = n, first and last.  A streamed table (dct_tables) takes one launch
+// per K-panel, and each output's running sum waits in `acc` ([row][n] doubles, row-major like Y) between the launches: the
+// first panel starts it from 0.0, the last one applies the epilogue instead of storing it.  Within a panel and across the
+// panels the terms are added in ascending k with separately rounded multiply and add, from 0.0, like a plain C loop compiled
+// without contraction, and a double survives the store and the load exactly, so every output is the same sum however the table
+// is cut.  Forward: `acc` may be Y itself (each output is read and then written by the thread that owns it).
+// 64 outputs x 32 rows per block of 128 threads, 4 x 4 per thread: a thread's four T values and four X values of one k are two
+// 16-byte shared loads each, i.e. four loads per sixteen multiply-add pairs (a 4 x 2 tile with 8-byte loads needs six per eight
+// and is bound by them).  512 work items on a 1024 x 1024 image for the 132 SMs.
+// IN = float (image rows) or double.  DIVN: divide the sum by n (the forward transform's normalisation, shear.c:62-63).
+// `mul` (optional, [n]): the output is multiplied by mul[o] (the phase factor cos(o a));
+// `mul2`/`Y2` (optional): a second output Y2[r][o-1] = y * mul2[o] for o >= 1 and Y2[r][n-1] = 0 (the antisymmetric
+// part's input, shear.c:71-79).
 template <typename IN, bool DIVN, bool INV>
-__global__ void __launch_bounds__(kGemmThreads) dct_panel_gemm_kernel(const double *__restrict__ P, int k0, int k1, const IN *__restrict__ X, int n,
-                                                                      int nrows_all, const RtState *st, const int *__restrict__ rowlist,
-                                                                      const int *__restrict__ collist, double *acc, bool first, bool last,
-                                                                      double *Y, const double *__restrict__ mul, const double *__restrict__ mul2,
-                                                                      double *__restrict__ Y2, const float *__restrict__ rowthr,
-                                                                      const float *__restrict__ img, float *__restrict__ rt)
+__global__ void __launch_bounds__(kGemmThreads) dct_gemm_kernel(const double *__restrict__ P, int ldp, bool listed, int k0, int k1,
+                                                                const IN *__restrict__ X, int n, int nrows_all, const RtState *st,
+                                                                const int *__restrict__ rowlist, const int *__restrict__ collist, double *acc,
+                                                                bool first, bool last, double *Y, const double *__restrict__ mul,
+                                                                const double *__restrict__ mul2, double *__restrict__ Y2,
+                                                                const float *__restrict__ rowthr, const float *__restrict__ img,
+                                                                float *__restrict__ rt)
 {
     constexpr int TO = kGemmTO, TR = kGemmTR, TK = kGemmTK;
     __shared__ __align__(16) double Ts[TK][TO + 2];
     __shared__ __align__(16) double Xs[TK][TR + 2];
     __shared__ int rows_s[TR], cols_s[TO];
-    const int nrows = rowlist ? st->nrows : nrows_all, nout = INV ? st->ncols : n, kp = k1 - k0;
+    const int nrows = rowlist ? st->nrows : nrows_all, nout = INV ? st->ncols : n;
     const int otiles = (nout + TO - 1) / TO, rtiles = (nrows + TR - 1) / TR;
-    const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
+    const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;         // outputs gemm_out(tx, 0..3), rows 4 ty .. +3
     for (int item = blockIdx.x; item < otiles * rtiles; item += gridDim.x) {
         const int o0 = (item % otiles) * TO, r0 = (item / otiles) * TR;
         __syncthreads();
@@ -278,18 +152,21 @@ __global__ void __launch_bounds__(kGemmThreads) dct_panel_gemm_kernel(const doub
                 const int row = rows_s[4 * ty + qb], col = cols_s[gemm_out(tx, qa)];
                 acc_r[qa][qb] = (!first && row >= 0 && col >= 0) ? acc[(size_t)row * n + col] : 0.0;
             }
-        const int tq = o0 + (threadIdx.x >> 1), tkk = 8 * (threadIdx.x & 1);
+        // T tile: 64 outputs x 16 inputs, thread t holds output (t >> 1), inputs 8 (t & 1) .. +7; X tile: 32 rows x 16 inputs, thread t
+        // holds row (t >> 2), inputs 4 (t & 3) .. +3.  The next tile's values are fetched into registers before the current tile's
+        // product, so the global-load latency hides behind 16 x 32 FP64 instructions instead of standing between two barriers.
+        const int tcol = cols_s[threadIdx.x >> 1], tq = listed ? o0 + (threadIdx.x >> 1) : tcol, tkk = 8 * (threadIdx.x & 1);
         const int xrow = rows_s[threadIdx.x >> 2], xkk = 4 * (threadIdx.x & 3);
         double tv[8], xv[4];
-        auto fetch = [&](int kb) {                                   // (register prefetch of the next tiles, as in dct_gemm_kernel)
+        auto fetch = [&](int kb) {
 #pragma unroll
-            for (int q = 0; q < 8; q++) { const int k = kb + tkk + q; tv[q] = (tq < nout && k < k1) ? P[(size_t)tq * kp + (k - k0)] : 0.0; }
+            for (int q = 0; q < 8; q++) { const int k = kb + tkk + q; tv[q] = (tcol >= 0 && k < k1) ? P[(size_t)tq * ldp + (k - k0)] : 0.0; }
 #pragma unroll
             for (int q = 0; q < 4; q++) { const int k = kb + xkk + q; xv[q] = (xrow >= 0 && k < k1) ? (double)X[(size_t)xrow * n + k] : 0.0; }
         };
         fetch(k0);
         for (int kb = k0; kb < k1; kb += TK) {
-            __syncthreads();
+            __syncthreads();                                         // the previous product is done with the tiles
 #pragma unroll
             for (int q = 0; q < 8; q++) Ts[tkk + q][threadIdx.x >> 1] = tv[q];
 #pragma unroll

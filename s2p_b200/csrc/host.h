@@ -73,9 +73,9 @@ struct Slot {
     int *abort = nullptr;         // this slot's word of s2pb_ctx::abort_words: a timeout of a call on this slot raises it
     bool timed = false;
     bool direct_out = false;      // the last host-API call wrote its results straight into the caller's pinned buffers
-    // K-panels of the DCT tables of rows wider than the resident tables serve (dct_tables, stream_panels): two pinned staging
-    // buffers and two device panels of `panel` doubles each, the copy stream and its events, and the running sums of the round
-    // trip's inverse product (acc_pix doubles); allocated on first use
+    // K-panels of the DCT tables that are not resident (dct_tables, dct_product; a resident table is multiplied as one panel):
+    // two pinned staging buffers and two device panels of `panel` doubles each, the copy stream and its events, and the running
+    // sums of the round trip's inverse product (acc_pix doubles); allocated on first use
     struct DctStream {
         double *h[2] = {nullptr, nullptr}, *d[2] = {nullptr, nullptr};
         size_t panel = 0;
@@ -97,8 +97,8 @@ struct s2pb_ctx {
     std::atomic<long long> launches{0};   // (mgm_multi tiles of a batch are enqueued from several host threads)
     size_t ws_limit = 0;                  // s2pb_set_workspace_limit: bytes per workspace, 0 = none
     std::atomic<long long> folded_calls{0};   // mgm_calls that ran in the folded layout (s2pb_folded_calls)
-    // DCT coefficient tables of the matched image's round trip, one entry per image width (dct_tables); a null table of a width
-    // above kDctDenseWidth is streamed in K-panels
+    // DCT coefficient tables of the matched image's round trip, one entry per image width (dct_tables); every product runs
+    // through dct_gemm_kernel, a table held here as one panel, a null table (only above kDctDenseWidth) streamed in K-panels
     struct DctTab { int n; double *T10, *T01, *TR01, *mc, *ms; };
     size_t dct_limit = (size_t)8 << 30;   // s2pb_set_dct_table_limit: device bytes of resident tables above kDctDenseWidth
     size_t dct_wide_bytes = 0;            // ... held now

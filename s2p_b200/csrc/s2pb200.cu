@@ -709,7 +709,8 @@ static void fill_wta(WtaParams &P, const ViewWS &v, int ndir, int gmin, const s2
 //   RODFT01  Y[i] = (-1)^i X[n-1] + sum_{k<n-1} 2 sin(pi (k + 1) (i + 1/2) / n) X[k]
 // Up to kDctDenseWidth they are kept on the device, once per width, whatever they take (1.5 GiB at 8192 with the half shift).
 // Wider rows keep a table resident while the context's resident wide tables stay within its table budget (dct_budget), and
-// stream it in K-panels otherwise (stream_panels).
+// stream it in K-panels otherwise.  Either way every product runs through dct_gemm_kernel (dct_product): a resident table is
+// one panel.
 constexpr int kDctDenseWidth = 8192;
 enum DctKind { kDctT10 = 0, kDctT01 = 1, kDctTR01 = 2 };
 
@@ -858,13 +859,18 @@ static int dct_stream_ensure(Slot &s, size_t panel, size_t acc_pix)
     return S2PB_OK;
 }
 
-// One product through the K-panels of table `kind` for rows of n pixels, restricted to the table rows `rows` (nullptr: all n;
-// nrows of them).  Panel p is built on the host into staging buffer p % 2 while the device multiplies panel p - 1, uploaded on
-// the slot's copy stream once the product of panel p - 2 is done with device buffer p % 2, and multiplied on st by
-// product(panel, k0, k1) (dct_panel_gemm_kernel).  Returns once the last panel is enqueued.
+// One product through table `kind` for rows of n pixels, restricted to the table rows `rows` (nullptr: all n; nrows of them):
+// product(P, ldp, listed, k0, k1) multiplies by the panel P of the table's inputs [k0, k1) (dct_gemm_kernel).  A resident
+// table T is one panel, product(T, n, false, 0, n).  A streamed one (T null) goes in K-panels of the listed rows: panel p is
+// built on the host into staging buffer p % 2 while the device multiplies panel p - 1, uploaded on the slot's copy stream once
+// the product of panel p - 2 is done with device buffer p % 2, and multiplied on st.  Returns once the last panel is enqueued.
 template <class F>
-static int stream_panels(Slot &s, cudaStream_t st, int kind, int n, const int *rows, int nrows, F &&product)
+static int dct_product(Slot &s, cudaStream_t st, const double *T, int kind, int n, const int *rows, int nrows, F &&product)
 {
+    if (T) {
+        product(T, n, false, 0, n);
+        return S2PB_OK;
+    }
     const int kp = dct_panel_cols(n);
     int rc = dct_stream_ensure(s, (size_t)nrows * kp, 0);
     if (rc != S2PB_OK) return rc;
@@ -877,7 +883,7 @@ static int stream_panels(Slot &s, cudaStream_t st, int kind, int n, const int *r
         CK(cudaMemcpyAsync(S.d[b], S.h[b], (size_t)nrows * (k1 - k0) * 8, cudaMemcpyHostToDevice, S.copy));
         CK(cudaEventRecord(S.copied[b], S.copy));
         CK(cudaStreamWaitEvent(st, S.copied[b], 0));
-        product((const double *)S.d[b], k0, k1);
+        product((const double *)S.d[b], k1 - k0, rows != nullptr, k0, k1);
         CK(cudaEventRecord(S.consumed[b], st));
     }
     CK(cudaGetLastError());
@@ -900,37 +906,26 @@ static int round_trip_zero(s2pb_ctx *ctx, Slot &s, const float *img, int w, int 
     CK(cudaMemsetAsync(colflag, 0, (size_t)w, st));
     launch(ctx, rt_flag_kernel, h, 256, 0, st, img, w, h, rt, state, rowlist, rowthr, colflag);
     launch(ctx, rt_collist_kernel, 1, 1024, 0, st, colflag, w, state, collist);
+    RtState hs{};
+    std::vector<int> cols;
+    if (!t->T10 || !t->T01) {
+        cols.resize(w);
+        CK(cudaMemcpyAsync(&hs, state, sizeof hs, cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(cols.data(), collist, (size_t)w * 4, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        if (hs.nrows == 0) return S2PB_OK;
+    }
     const int g = ctx->sm_count * 4;
-    if (t->T10 && t->T01) {
-        launch(ctx, dct_gemm_kernel<float, true>, g, kGemmThreads, 0, st, t->T10, img, w, h, state, rowlist, Y, nullptr, nullptr, nullptr);
-        launch(ctx, rt_inverse_gemm_kernel, g, kGemmThreads, 0, st, t->T01, Y, w, state, rowlist, collist, rowthr, img, rt);
-        CK(cudaGetLastError());
-        return S2PB_OK;
-    }
-    RtState hs;
-    std::vector<int> cols(w);
-    CK(cudaMemcpyAsync(&hs, state, sizeof hs, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(cols.data(), collist, (size_t)w * 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    if (hs.nrows == 0) return S2PB_OK;
-    if (t->T10)
-        launch(ctx, dct_gemm_kernel<float, true>, g, kGemmThreads, 0, st, t->T10, img, w, h, state, rowlist, Y, nullptr, nullptr, nullptr);
-    else
-        rc = stream_panels(s, st, kDctT10, w, nullptr, w, [&](const double *P, int k0, int k1) {
-            launch(ctx, dct_panel_gemm_kernel<float, true, false>, g, kGemmThreads, 0, st, P, k0, k1, img, w, h, state, rowlist, nullptr, Y,
-                   k0 == 0, k1 == w, Y, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
-        });
+    rc = dct_product(s, st, t->T10, kDctT10, w, nullptr, w, [&](const double *P, int ldp, bool listed, int k0, int k1) {
+        launch(ctx, dct_gemm_kernel<float, true, false>, g, kGemmThreads, 0, st, P, ldp, listed, k0, k1, img, w, h, state, rowlist, nullptr,
+               Y, k0 == 0, k1 == w, Y, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
+    });
     if (rc != S2PB_OK) return rc;
-    if (t->T01) {
-        launch(ctx, rt_inverse_gemm_kernel, g, kGemmThreads, 0, st, t->T01, Y, w, state, rowlist, collist, rowthr, img, rt);
-    } else {
-        if ((rc = dct_stream_ensure(s, 0, (size_t)w * h)) != S2PB_OK) return rc;
-        double *acc = s.dcts.acc;
-        rc = stream_panels(s, st, kDctT01, w, cols.data(), hs.ncols, [&](const double *P, int k0, int k1) {
-            launch(ctx, dct_panel_gemm_kernel<double, false, true>, g, kGemmThreads, 0, st, P, k0, k1, (const double *)Y, w, 0, state, rowlist,
-                   collist, acc, k0 == 0, k1 == w, nullptr, nullptr, nullptr, nullptr, rowthr, img, rt);
-        });
-    }
+    if (!t->T01 && (rc = dct_stream_ensure(s, 0, (size_t)w * h)) != S2PB_OK) return rc;
+    rc = dct_product(s, st, t->T01, kDctT01, w, cols.data(), hs.ncols, [&](const double *P, int ldp, bool listed, int k0, int k1) {
+        launch(ctx, dct_gemm_kernel<double, false, true>, g, kGemmThreads, 0, st, P, ldp, listed, k0, k1, (const double *)Y, w, 0, state,
+               rowlist, collist, s.dcts.acc, k0 == 0, k1 == w, nullptr, nullptr, nullptr, nullptr, rowthr, img, rt);
+    });
     CK(cudaGetLastError());
     return rc;
 }
@@ -944,26 +939,18 @@ static int shift_half(s2pb_ctx *ctx, Slot &s, const float *img, int w, int h, fl
     const size_t npix = (size_t)w * h;
     double *ck = scratch, *sk = scratch + npix, *sym = scratch + 2 * npix, *anti = scratch + 3 * npix;
     const int g = ctx->sm_count * 4;
-    if (t->T10)
-        launch(ctx, dct_gemm_kernel<float, true>, g, kGemmThreads, 0, st, t->T10, img, w, h, nullptr, nullptr, ck, t->mc, t->ms, sk);
-    else
-        rc = stream_panels(s, st, kDctT10, w, nullptr, w, [&](const double *P, int k0, int k1) {
-            launch(ctx, dct_panel_gemm_kernel<float, true, false>, g, kGemmThreads, 0, st, P, k0, k1, img, w, h, nullptr, nullptr, nullptr,
-                   ck, k0 == 0, k1 == w, ck, (const double *)t->mc, (const double *)t->ms, sk, nullptr, nullptr, nullptr);
-        });
+    rc = dct_product(s, st, t->T10, kDctT10, w, nullptr, w, [&](const double *P, int ldp, bool listed, int k0, int k1) {
+        launch(ctx, dct_gemm_kernel<float, true, false>, g, kGemmThreads, 0, st, P, ldp, listed, k0, k1, img, w, h, nullptr, nullptr, nullptr,
+               ck, k0 == 0, k1 == w, ck, (const double *)t->mc, (const double *)t->ms, sk, nullptr, nullptr, nullptr);
+    });
     if (rc != S2PB_OK) return rc;
     const double *inv_tab[2] = {t->T01, t->TR01};
     const double *inv_in[2] = {ck, sk};
     double *inv_out[2] = {sym, anti};
     for (int i = 0; i < 2; i++) {
-        if (inv_tab[i]) {
-            launch(ctx, dct_gemm_kernel<double, false>, g, kGemmThreads, 0, st, inv_tab[i], inv_in[i], w, h, nullptr, nullptr, inv_out[i],
-                   nullptr, nullptr, nullptr);
-            continue;
-        }
-        rc = stream_panels(s, st, i ? kDctTR01 : kDctT01, w, nullptr, w, [&](const double *P, int k0, int k1) {
-            launch(ctx, dct_panel_gemm_kernel<double, false, false>, g, kGemmThreads, 0, st, P, k0, k1, inv_in[i], w, h, nullptr, nullptr,
-                   nullptr, inv_out[i], k0 == 0, k1 == w, inv_out[i], nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
+        rc = dct_product(s, st, inv_tab[i], i ? kDctTR01 : kDctT01, w, nullptr, w, [&](const double *P, int ldp, bool listed, int k0, int k1) {
+            launch(ctx, dct_gemm_kernel<double, false, false>, g, kGemmThreads, 0, st, P, ldp, listed, k0, k1, inv_in[i], w, h, nullptr,
+                   nullptr, nullptr, inv_out[i], k0 == 0, k1 == w, inv_out[i], nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
         });
         if (rc != S2PB_OK) return rc;
     }
